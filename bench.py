@@ -90,12 +90,16 @@ def parse():
                     help="untimed adaptive iterations run as setup, before "
                          "the W warm-up steps (covers both step-size searches)")
     ap.add_argument("--dense-impl", type=int, default=None,
-                    help="0 SIMT fp32, 1 tcgen05 3xTF32, 2 tcgen05 fp16-split per "
-                         "pass, 4 cluster-of-8 trajectory, 5 L2-resident trajectory "
-                         "(default: see DEFAULT_DENSE_IMPL)")
+                    help="0 SIMT fp32, 1 wgmma 3xTF32, 2 wgmma fp16-split per pass, "
+                         "3 fp16-split with in-kernel operand split, 4 / 5 trajectory entry "
+                         "points (default: see DEFAULT_DENSE_IMPL)")
     ap.add_argument("--cpu-chains", type=int, default=4096)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed path computed in its "
+                         "last step to DIR/<name>.npy (float32; a fixed, seeded row sample "
+                         "of outputs over 64 MB)")
     ap.add_argument("--no-adapt", action="store_true",
                     help="kernel-timing experiments only: fixed step size, no "
                          "adaptation (not the benchmark configuration)")
@@ -109,7 +113,8 @@ def load_peaks():
         return {"hbm_gbs": d["hbm_gbs"], "tf": d.get("bf16_tflops_sustained",
                                                      d["bf16_tflops"]),
                 "tf_burst": d["bf16_tflops"], "src": "measured"}
-    return {"hbm_gbs": 6650.0, "tf": 1400.0, "tf_burst": 1590.0,
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s
+    return {"hbm_gbs": 3350.0, "tf": 989.0, "tf_burst": 989.0,
             "src": "fallback"}
 
 
@@ -247,6 +252,31 @@ def time_cpu_iwae(args, n_iters=3):
             "host_cpu_count": os.cpu_count()}, 1e3 * dt
 
 
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Write {name: tensor} as float32 .npy files under out_dir.  An array whose rows do not
+    all fit the 64 MB budget is reduced to a fixed row sample (seed 0, sorted), and the chosen
+    row indices are written beside it as <name>_rows.npy (float64)."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    budget = DUMP_MAX_BYTES
+    for name, t in arrays.items():
+        a = torch.as_tensor(t).detach().to("cpu", torch.float32).numpy()
+        a = np.atleast_1d(a)
+        if a.nbytes > budget // 2:
+            row_bytes = a.nbytes // a.shape[0]
+            n = max(1, min(a.shape[0], (budget // 2) // row_bytes))
+            rows = np.sort(np.random.Generator(np.random.PCG64(0)).choice(
+                a.shape[0], size=n, replace=False))
+            a = a[rows]
+            np.save(os.path.join(out_dir, name + "_rows.npy"), rows.astype(np.float64))
+            budget -= rows.size * 8
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+        budget -= a.nbytes
+
+
 def run_reference(args):
     """--impl reference: the reference's own CPU path.  TensorFlow (and so zhusuan) cannot be
     installed here, so this arm times the torch-CPU restatement (kind "port") with all physical
@@ -298,7 +328,7 @@ def run_iwae(args):
     """--workload iwae: the second half of BASELINE.json's metric, particle-ELBOs/s on config 3
     (VAE 784-(500,500)-40, IWAE K=64, batch 4096 per GPU, forward + SGVB reparameterised
     backward; examples/variational_autoencoders/iwae.py:23-78).  Every dense layer runs on the
-    tcgen05 fp16-split kernel (fp32 accuracy), the decoder output fused with the Bernoulli
+    wgmma fp16-split kernel (fp32 accuracy), the decoder output fused with the Bernoulli
     log-likelihood; the batch axis shards over ranks, particles stay local, ONE packed gradient
     all-reduce per step."""
     import torch
@@ -388,6 +418,9 @@ def run_iwae(args):
     ms_per_step = float(ms.item()) / args.steps
     value = world * K * N / (ms_per_step * 1e-3)
     bound = float(-cost.detach())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dict(
+            [("cost", cost)] + [("grad_%02d" % i, t) for i, t in enumerate(g)]))
 
     # e2e: per step, H2D of the step's batch from pinned memory, the step, D2H of the bound
     e2e = None
@@ -547,6 +580,10 @@ def run_hmc(args):
     value = C * world * L * args.steps / (total_ms * 1e-3)
     acc_mean = float(info.acceptance_rate.mean())
     step_size = float(info.updated_step_size)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"samples_x": info.samples["x"],
+                                         "acceptance_rate": info.acceptance_rate,
+                                         "updated_step_size": info.updated_step_size})
 
     # ---------------- e2e: host buffers through the public API ---------------
     # Every step: H2D of the step's chain state from pinned host memory, one
@@ -696,7 +733,7 @@ def run_hmc(args):
                            if args.no_adapt else "step-size + mass adaptation on"),
             "chains_per_gpu": C, "dim": D, "n_leapfrogs": L,
             "burnin_iters": args.burnin, "dense_impl": impl,
-            "l2": "inputs larger than L2 (q,p = %.0f MB each per GPU vs 126 "
+            "l2": "inputs larger than L2 (q,p = %.0f MB each per GPU vs 50 "
                   "MB L2)" % (C * D * 4 / 1e6),
             "rng": "in-kernel Philox4x32-10",
             "cuda_graph": bool(args.cuda_graph),

@@ -1,4 +1,4 @@
-/* zsb200.h -- C ABI of libzsb200.so, the B200 (sm_100a) kernels behind zhusuan's
+/* zsb200.h -- C ABI of libzsb200.so, the H100 (sm_90a) kernels behind zhusuan's
  * HMC / SG-MCMC / ELBO-IWAE hot path.
  *
  * The reference (thu-ml/zhusuan) has NO native boundary: its arithmetic is TensorFlow-1.x graph
@@ -154,7 +154,7 @@ int zsb_vimco_signal_f32(const float* x, float* signal, float* lme, int64_t oute
 int zsb_normalized_weights_f32(const float* x, float* w, int64_t outer, int64_t K, int64_t inner,
                                void* stream);
 
-/* ---- K8: dense layer of a VAE/BNN log-joint on tcgen05 with the likelihood fused into the GEMM
+/* ---- K8: dense layer of a VAE/BNN log-joint on wgmma with the likelihood fused into the GEMM
  * epilogue (the model code of examples/variational_autoencoders/iwae.py:23-32: tf.layers.dense +
  * bn.bernoulli('x', logits, group_ndims=1)); fp32 accuracy from a 3-product fp16 hi/lo split.
  * Operands are fp16 plane pairs [2][rows][Kp], Kp = zsb_linear_tc_kpad(K), produced by
@@ -212,7 +212,7 @@ int zsb_linear_tc_dgrad_f32(const void* w_planes, const float* scale_w, const vo
 /* Weight gradient of the dense layer, dW [J, K] = g^T h = sum_r g[r, j] * h[r, k] (the
  * tf.gradients of tf.layers.dense w.r.t. its kernel, iwae.py:23-44), read straight from the
  * ROW-MAJOR planes h_planes [2][R][kpad(K)] and g_planes [2][R][kpad(J)]: the contraction runs
- * over the rows, so both operands are MN-major tcgen05 operands and no transposed copy of an
+ * over the rows, so both operands are MN-major wgmma operands and no transposed copy of an
  * activation is ever written.  part = zsb_linear_tc_slices(J, K, R) * J * K floats of split-K
  * scratch (NULL: one slice). */
 int zsb_linear_tc_wgrad_f32(const void* h_planes, const float* scale_h, int K,
@@ -287,7 +287,7 @@ int zsb_hmc_diag_normal_step_f32(float* q, const float* noise, const float* u, c
  * while-loop body (hmc.py:352-364): g = b - q_cur P; p_out = p_in + p_scale*eps*g;
  * q_next = q_cur + eps*p_out/mass (skipped if NULL); lp_part/k_part [ntiles, chains] partials.
  * impl 0 = SIMT fp32 (P full fp32; *_lo ignored).
- * impl 1 = tcgen05.mma kind::tf32, 3xTF32 split: P = hi part (low 13 mantissa bits cleared),
+ * impl 1 = wgmma TF32, 3xTF32 split: P = hi part (low 13 mantissa bits cleared),
  *          P_lo = P - hi; q_cur_lo = residual of q_cur (zsb_hmc_dense_split_lo_f32 for the first
  *          pass), q_next_lo receives the residual of q_next. */
 int zsb_hmc_dense_ntiles(int64_t D, int impl);
@@ -297,9 +297,9 @@ int zsb_hmc_dense_leapfrog_f32(const float* q_cur, const float* q_cur_lo, float*
                                const float* mu, const float* mass, const float* state,
                                float p_scale, float* lp_part, float* k_part, int64_t chains,
                                int64_t D, int impl, void* stream);
-int zsb_hmc_dense_tc_config(int bk);   /* impl-1 pipeline shape: 32 (2x96 KB) or 16 (4x48 KB) */
+int zsb_hmc_dense_tc_config(int bk);   /* impl-1 pipeline shape: 32 (2x64 KB) or 16 (4x32 KB) */
 int zsb_hmc_dense_split_lo_f32(const float* q, float* lo, int64_t n, void* stream);
-/* impl 2: fp16-split tensor-core path (3 kind::f16 MMAs per k-step at twice the TF32 rate).
+/* impl 2: fp16-split tensor-core path (3 fp16 wgmma products per k-step at twice the TF32 rate).
  * P_h16/P_l16: [D,D] __half hi/lo of P*sP; q_*_planes: [2][chains][D] __half hi/lo of q*sq;
  * scales: device float[4] = {sq, 1/(sP*sq), scratch, sP}.  D % 64 == 0. */
 int zsb_hmc_dense_h16_prepare_f32(const float* q, void* planes, float* scales, int64_t n,
@@ -310,8 +310,8 @@ int zsb_hmc_dense_leapfrog_h16_f32(const float* q_cur, const void* q_cur_planes,
                                    const float* bvec, const float* mu, const float* mass,
                                    const float* state, float p_scale, float* lp_part,
                                    float* k_part, int64_t chains, int64_t D, void* stream);
-/* impl 3: impl 2 with the fp16 planes of q produced inside the kernel (converter warps between
- * TMA and MMA): HBM traffic per pass = the algorithmic 16*D bytes per chain.  scales: device
+/* impl 3: impl 2 with the fp16 planes of q produced inside the kernel (by the MMA warpgroup from
+ * the fp32 rows): HBM traffic per pass = the algorithmic 16*D bytes per chain.  scales: device
  * float[8], [3] = sP, [4..6] rotating max|q| slots; prepare before pass 0 of each trajectory. */
 int zsb_hmc_dense_h16i_prepare_f32(const float* q, float* scales, int64_t n, void* stream);
 int zsb_hmc_dense_leapfrog_h16i_f32(const float* q_cur, float* q_next, const float* p_in,
@@ -320,10 +320,8 @@ int zsb_hmc_dense_leapfrog_h16i_f32(const float* q_cur, float* q_next, const flo
                                     const float* mu, const float* mass, const float* state,
                                     float p_scale, float* lp_part, float* k_part, int64_t chains,
                                     int64_t D, void* stream);
-/* impl 4 -- first trajectory-fused design (validated in round 2: correct, but 2x slower than impl 2:
- * only 8 clusters of 8 CTAs become co-resident and MMA N = 128 saturates the L2->SM port; kept as a
- * cross-check of impl 5): the whole leapfrog `while_loop` of hmc.py:347-372 (L+1 passes) in one
- * launch; a cluster of 8 CTAs keeps a 256-chain block's q / p / planes in L2.  D == 1024, L >= 1.
+/* impl 4: the whole leapfrog `while_loop` of hmc.py:347-372 (L+1 passes) through one entry point
+ * with impl 2's buffers and ping-pong schedule.  D == 1024, L >= 1.
  * Buffers as impl 2 (planes0 from zsb_hmc_dense_h16_prepare_f32); the proposal ends in qa when
  * L - 1 is even, else in qb; pw holds the final momentum. */
 int zsb_hmc_dense_trajectory_h16_f32(const float* q0, const void* planes0, float* qa,
@@ -334,15 +332,13 @@ int zsb_hmc_dense_trajectory_h16_f32(const float* q0, const void* planes0, float
                                      float* lp1_part, float* k_part, int64_t chains, int64_t D,
                                      int n_leapfrogs, void* stream);
 /* impl 5: the whole leapfrog `while_loop` of hmc.py:347-372 (L+1 passes, body = leapfrog_integrator
- * hmc.py:38-43, plus the log p / kinetic terms of hamiltonian() hmc.py:30-35) in ONE persistent
- * launch whose chain groups stay resident in the 126 MB L2: CTA pairs, N = 256 chains per unit,
- * group-major order (zsb_hmc_dense_resident_group(D) 256-chain blocks per group), pass-to-pass
- * dependencies through the int32 `flags` counters (zsb_hmc_dense_resident_flags(chains) words).
- * Inside the trajectory the state of q is its fp16 hi/lo plane pair (planes0 from
- * zsb_hmc_dense_h16_prepare_f32; planes1 = work buffer, same size); the proposal's planes end in
- * buffer (n_leapfrogs & 1) and zsb_hmc_dense_select_planes_f32 assigns them to the accepted
- * chains (the `tf.where` + assign of hmc.py:488-497).  planes1 == planes0 selects the in-place
- * variant (proposal in planes0; smaller L2 footprint).  D % 64 == 0, n_leapfrogs >= 1. */
+ * hmc.py:38-43, plus the log p / kinetic terms of hamiltonian() hmc.py:30-35) with the fp16 hi/lo
+ * plane pair of q*sq as the state of q inside the trajectory (planes0 from
+ * zsb_hmc_dense_h16_prepare_f32; planes1 = work buffer of the same size, distinct from planes0);
+ * the proposal's planes end in buffer (n_leapfrogs & 1) and zsb_hmc_dense_select_planes_f32
+ * assigns them to the accepted chains (the `tf.where` + assign of hmc.py:488-497).  `flags`
+ * (zsb_hmc_dense_resident_flags(chains) int32 words) is reserved scratch.  D % 64 == 0,
+ * n_leapfrogs >= 1. */
 int zsb_hmc_dense_resident_flags(int64_t chains);
 int zsb_hmc_dense_resident_group(int64_t D);
 int zsb_hmc_dense_resident_h16_f32(void* planes0, void* planes1, const float* p0, float* pw,

@@ -41,7 +41,7 @@ def build(dev, seed=5, x_dim=784, z_dim=40, h=500):
 def step_fn(W, x, K, dev, fused=False):
     n, x_dim = x.shape
     z_dim = W["em"].shape[0]
-    if fused:      # every dense layer on the tcgen05 kernel; Bernoulli fused into the last GEMM
+    if fused:      # every dense layer on the wgmma kernel; Bernoulli fused into the last GEMM
         lin = lambda h, w, b, relu=False: zs.fused.linear(h, w, b, relu=relu)
     else:
         lin = lambda h, w, b, relu=False: (F.relu(F.linear(h, w, b)) if relu
@@ -99,12 +99,12 @@ def main():
     x = torch.tensor(rng.random((N, 784)) < 0.13, dtype=torch.int32, device=dev)
     out = {"n_gpus": world, "batch_per_gpu": N}
     grads = {}
-    for mode in ("fp32_matmul", "tf32_matmul", "tcgen05_split_fused"):
+    for mode in ("fp32_matmul", "tf32_matmul", "wgmma_split_fused"):
         tf32 = mode == "tf32_matmul"
         torch.backends.cuda.matmul.allow_tf32 = tf32
         W = build(dev)
         zs.set_random_seed(1234)           # same eps in every mode
-        local_step = step_fn(W, x, K, dev, fused=(mode == "tcgen05_split_fused"))
+        local_step = step_fn(W, x, K, dev, fused=(mode == "wgmma_split_fused"))
 
         def step():
             cost, g = local_step()
@@ -132,7 +132,7 @@ def main():
             "tflops_dense_layers": world * 3.97e6 * K * N / (ms * 1e-3) / 1e12,
             "bound_value": float(-cost)}
     ref = grads["fp32_matmul"]
-    for mode in ("tf32_matmul", "tcgen05_split_fused"):
+    for mode in ("tf32_matmul", "wgmma_split_fused"):
         out[mode]["grad_rel_err_vs_fp32"] = float((grads[mode] - ref).norm() / ref.norm())
     if rank != 0:
         td.destroy_process_group()

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Micro-benchmarks of the HBM-bound kernels vs the measured copy bandwidth
 (MEASURED_PEAKS.json hbm_gbs).  Each line: algorithmic bytes / CUDA-event time.
-Inputs are > L2 (126 MB) so nothing is cache-resident."""
+Inputs are > L2 (50 MB) so nothing is cache-resident."""
 import ctypes
 import json
 import os
@@ -100,7 +100,7 @@ def main():
     report("normal_log_prob group=16 (268 MB)", 4 * big.numel(), ms)
     lw = torch.randn(64, 4096 * 256, device=dev)
     ms = timeit(lambda: zs.log_mean_exp(lw, 0))
-    report("log_mean_exp [64, 1M] axis 0", 4 * lw.numel(), ms, "two passes over x, second from L2 only if < 126 MB")
+    report("log_mean_exp [64, 1M] axis 0", 4 * lw.numel(), ms, "two passes over x, second from L2 only if < 50 MB")
     # fused diag-normal HMC iteration, C1' = 1M chains x 100
     C1, D1, L = 1 << 20, 100, 10
     std = torch.tensor(1.0 / (1.0 + np.arange(D1)), dtype=torch.float32, device=dev)

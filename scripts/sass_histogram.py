@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Opcode histogram of the tensor-core kernels in libzsb200.so (cuobjdump -sass): evidence that the
-hot kernels are tcgen05 / TMEM / TMA code (UTCHMMA = tcgen05.mma, UTMALDG = TMA tensor load, LDTM =
-tcgen05.ld, UTCBAR = tcgen05.commit, SYNCS = mbarrier ops).  Writes a markdown table."""
+hot kernels are wgmma / TMEM / TMA code (UTCHMMA = wgmma.mma, UTMALDG = TMA tensor load, LDTM =
+wgmma.ld, UTCBAR = wgmma.commit, SYNCS = mbarrier ops).  Writes a markdown table."""
 import collections
 import re
 import subprocess

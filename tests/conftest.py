@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 def pytest_configure(config):
     config.addinivalue_line(
-        "markers", "gpu: test needs a CUDA device (run on the B200 box with "
+        "markers", "gpu: test needs a CUDA device (an H100; select with "
                    "`-m gpu`); everything else runs on CPU")
 
 

@@ -220,7 +220,7 @@ def test_vae_objectives_match_reference_run(zs, fused):
     the REFERENCE'S OWN BayesianNet / Normal / Bernoulli / importance_weighted_objective / elbo /
     .sgvb() / .reinforce() (executed on the NumPy TF stand-in, oracle/tf_shim/make_ref_golden.py).
     The same model written against this package -- generic path (registry kernels + torch linear)
-    and the K8 path (tcgen05 dense layers, Bernoulli epilogue) -- must reproduce the per-datum
+    and the K8 path (wgmma dense layers, Bernoulli epilogue) -- must reproduce the per-datum
     bounds, the costs and the gradient of every weight; the injected eps enters through a
     user-defined Distribution subclass (the plugin contract, bn.stochastic)."""
     import torch.nn.functional as F

@@ -1,4 +1,4 @@
-"""GPU parity: K8 dense-layer kernels on tcgen05 (gemm_logjoint_tc.cu) -- the decoder output layer
+"""GPU parity: K8 dense-layer kernels on wgmma (gemm_logjoint_tc.cu) -- the decoder output layer
 of examples/variational_autoencoders/iwae.py:23-32 with the Bernoulli likelihood
 (univariate.py:398-403, group_ndims=1) fused into the GEMM epilogue -- against float64 matmul,
 the NumPy oracle and the unfused path of this repo."""
@@ -75,7 +75,7 @@ def test_linear_backward_on_tensor_cores(zs, R, K, J, relu):
 @pytest.mark.parametrize("R,K,J", [(1000, 500, 784), (63, 1, 5), (4097, 130, 257), (64, 64, 128),
                                    (20000, 40, 500)])
 def test_weight_gradient_from_row_major_planes(zs, R, K, J):
-    """zsb_linear_tc_wgrad_f32: dW = g^T h with both operands read as MN-major tcgen05 operands
+    """zsb_linear_tc_wgrad_f32: dW = g^T h with both operands read as MN-major wgmma operands
     from the ROW-MAJOR planes (no transposed copy) against float64 and against the transposed-plane
     product of zsb_linear_tc_f32; ragged contraction length (TMA zero fill of the last 64-row box),
     odd / tiny widths, feature counts that are not multiples of the 64-column box."""

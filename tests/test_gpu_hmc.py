@@ -299,7 +299,7 @@ def _dense_pass_reference(q, p, P, b, mu, mass, eps, scale):
                                  (130, 64), (515, 192)])
 def test_dense_single_pass_vs_float64(zs, impl, C, D):
     """One fused GEMM+leapfrog pass through the C ABI vs float64, for the SIMT
-    (impl 0) and tcgen05 3xTF32 (impl 1) kernels, including ragged M / N tiles.
+    (impl 0) and wgmma 3xTF32 (impl 1) kernels, including ragged M / N tiles.
     Bar: per-evaluation log-prob and gradient-derived p within 1e-5 relative."""
     from zhusuan_b200._lib import lib, ptr, stream
     if impl >= 2 and D % 64:

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libzsb200 (sm_100a only).
+// Shared device/host helpers for libzsb200 (sm_90a, H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -25,8 +25,8 @@ const uint32_t* zsb_epoch_ptr();   // device draw epoch (api.cu), NULL when not 
 
 static inline int64_t zsb_ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
-// Number of SMs on B200; grids of grid-stride kernels are sized in multiples of this.
-#define ZSB_NUM_SMS 148
+// Number of SMs on H100 SXM; grids of grid-stride kernels are sized in multiples of this.
+#define ZSB_NUM_SMS 132
 
 // ---- device state of one HMC sampler (all float32, lives in HBM; hmc.py:258-264, 82-87, 118) ----
 // Layout is part of the C ABI (include/zsb200.h: ZSB_HMC_STATE_*).

@@ -15,218 +15,95 @@
 //          is known BEFORE the GEMM: |dl| <= max|g| * (1 + max|x|)  (sigmoid in (0, 1)).
 //
 // fp32 accuracy on fp16 tensor cores: both operands are pre-split into scaled fp16 hi + lo planes
-// (zsb_split16_pad_f32), three kind::f16 tcgen05.mma per k-step accumulate hi*hi + hi*lo + lo*hi
-// in fp32 in TMEM (dropped term ~2^-22 relative) -- the scheme of the dense-Gaussian HMC kernel
-// (hmc_dense_tc.cu), whose pipeline this kernel shares: CTA pairs (cta_group::2, M = 256
-// features x N = 256 rows per unit), TMA producer warp, single-thread MMA issuer, 8 epilogue
-// warps, double-buffered TMEM accumulators.  As there, the product is computed transposed
-// (TMEM lane = feature j, column = row r) so an epilogue warp touches 32 consecutive features of
-// one row per instruction: coalesced x loads and out stores.
+// (zsb_split16_pad_f32), three fp16 wgmma products per k-step accumulate hi*hi + hi*lo + lo*hi
+// in fp32 (dropped term ~2^-22 relative) -- the scheme of the dense-Gaussian HMC kernel
+// (hmc_dense_tc.cu), whose persistent pipeline (tc_pipeline_kernel: TMA producer warp, MMA
+// warpgroup, 4 epilogue warps, 128 features x 128 rows per unit) this product shares.  As there,
+// the product is computed transposed (accumulator row = feature j, column = row r) so an epilogue
+// warp touches 32 consecutive features of one row per instruction: coalesced x loads and out stores.
 #include "tc_common.cuh"
 
 namespace {
-
-constexpr int GBK = 32;                       // 64 halves = 128 B per smem row (SWIZZLE_128B)
-using GC = Cfg2<GBK>;
 
 __device__ __forceinline__ float bern_lp(float x, float l) {   // -sigmoid_cross_entropy(x, l)
   return -(fmaxf(l, 0.f) - l * x + __logf(1.f + __expf(-fabsf(l))));
 }
 
 // MN (bit 0: operand A, bit 1: operand B; EPI 0 only): the operand is read in a row-major plane
-// layout [contraction rows, features] -- MN-major for the tensor core (instruction-descriptor bits
-// 15 / 16).  MN = 3: weight gradient dW = g^T h from the row-major planes of g and h; MN = 1: input
-// gradient dh = g W with A = the FORWARD planes of W [J, K] (no W^T copy): no product of a dense
-// layer needs a transposed copy of anything.  A stage then holds, per
-// plane, two TMA boxes of 64 contraction rows x 64 features (128-byte rows, SWIZZLE_128B): the
-// canonical MN-major tile ((8,8,m),(8,k)) : ((1,8,LBO),(64,SBO)) in fp16 elements with
-// SBO = 1 KB (next 8 contraction rows) and LBO = 8 KB (next 64 features); one k-step of 16
-// contraction rows advances the start address by 2 KB.  `Kp` is the padded contraction length.
-__device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);            // start address       bits [0,14)
-  d |= (uint64_t)(8192 >> 4) << 16;                   // leading byte offset bits [16,30)
-  d |= (uint64_t)(1024 >> 4) << 32;                   // stride byte offset  bits [32,46)
-  d |= (uint64_t)1 << 46;                             // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                             // SWIZZLE_128B
-  return d;
-}
+// layout [contraction rows, features] -- MN-major (transposed) wgmma operand.  MN = 3: weight
+// gradient dW = g^T h from the row-major planes of g and h; MN = 1: input gradient dh = g W with
+// A = the FORWARD planes of W [J, K] (no W^T copy): no product of a dense layer needs a transposed
+// copy of anything.  A stage then holds, per plane, two TMA boxes of 64 contraction rows x 64
+// features (128-byte rows, SWIZZLE_128B; see gmma_desc).  `Kp` is the padded contraction length.
+// GL: the epi 2 / 3 epilogues load the upstream gradient per row instead of broadcasting it.
+template <int EPI, int MN, int GL>
+struct LinW {
+  static constexpr int KIND = 1, RB = 128, MNA = MN & 1, MNB = (MN >> 1) & 1, CVT = 0;
+  static constexpr uint32_t TX = Cfg<RB>::STAGE;
+  CUtensorMap map_whi, map_wlo, map_hhi, map_hlo;
+  const float* bias; const float* x_obs; int64_t n_x; const float* gout;
+  float* out; float* part; int64_t R; int J; int Kp; int relu;
+  const float* scale_w; const float* scale_h; int k_slices; float* amax_scale;
+  int n_blk; int64_t n_tiles; int n_kb_all; int kb_per;
+  struct EpiState { float amax = 0.f; };
 
-template <int EPI, int MN = 0, int GL = 0>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS, 1)
-linear_tc2_kernel(const __grid_constant__ CUtensorMap map_whi,
-                  const __grid_constant__ CUtensorMap map_wlo,
-                  const __grid_constant__ CUtensorMap map_hhi,
-                  const __grid_constant__ CUtensorMap map_hlo, const float* __restrict__ bias,
-                  const float* __restrict__ x_obs, int64_t n_x, const float* __restrict__ gout,
-                  float* __restrict__ out, float* __restrict__ part, int64_t R, int J, int Kp,
-                  int relu, const float* __restrict__ scale_w, const float* __restrict__ scale_h,
-                  int k_slices, float* __restrict__ amax_scale) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bars = smem_base + GC::STAGES * GC::STAGE;
-  const uint32_t full_bar = bars;
-  const uint32_t empty_bar = bars + 8 * GC::STAGES;
-  const uint32_t tfull_bar = bars + 16 * GC::STAGES;
-  const uint32_t tempty_bar = bars + 16 * GC::STAGES + 16;
-  const uint32_t tmem_slot = bars + 16 * GC::STAGES + 32;
-  uint32_t* tmem_slot_ptr =
-      reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int n_blk = (J + BM - 1) / BM;                     // 128-feature blocks
-  const int n_pair = (n_blk + 1) / 2;
-  const int64_t c_blk = (R + BN - 1) / BN;                 // 256-row blocks
-  // work unit = (tile, k-slice): split-K (EPI 0 only) keeps all CTA pairs busy when the output
-  // is small and the contraction is long (dW = dl^T h: 784 x 500 outputs, K = 262 144 rows)
-  const int64_t n_tiles = c_blk * n_pair;
-  const int64_t n_units = n_tiles * k_slices;
-  const int64_t unit0 = blockIdx.x >> 1, unit_step = gridDim.x >> 1;
-  const int n_kb_all = Kp / (2 * GBK);
-  const int kb_per = (n_kb_all + k_slices - 1) / k_slices;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < GC::STAGES; ++s) {
-      mbar_init(full_bar + 8 * s, 1);
-      mbar_init(empty_bar + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar + 8 * a, 1);
-      mbar_init(tempty_bar + 8 * a, 2 * 32 * NUM_EPI_WARPS);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  __host__ __device__ __forceinline__ int64_t units() const { return n_tiles * k_slices; }
+  __device__ __forceinline__ void kb_range(int64_t uu, int& kb0, int& kb1) const {
+    kb0 = (int)(uu / n_tiles) * kb_per;
+    kb1 = min(kb0 + kb_per, n_kb_all);
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;"
-                 ::"r"(tmem_slot), "n"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
+  __device__ __forceinline__ void prefetch() const {
+    tma_prefetch_desc(&map_whi); tma_prefetch_desc(&map_wlo);
+    tma_prefetch_desc(&map_hhi); tma_prefetch_desc(&map_hlo);
   }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    if (lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_whi) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_wlo) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_hhi) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_hlo) : "memory");
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int64_t uu = unit0; uu < n_units; uu += unit_step) {
-        const int64_t u = uu % n_tiles;
-        const int kb0 = (int)(uu / n_tiles) * kb_per;
-        const int kb1 = min(kb0 + kb_per, n_kb_all);
-        const int j0 = ((int)(u % n_pair) * 2 + (int)rank) * BM;         // own feature block
-        const int r0 = (int)((u / n_pair) * BN) + (int)rank * (BN / 2);  // own half of the rows
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(empty_bar + 8 * stage, phase ^ 1);
-          const uint32_t fb = full_bar + 8 * stage;
-          const uint32_t sa = smem_base + stage * GC::STAGE;
-          if (leader) mbar_expect_tx(fb, 2 * GC::STAGE);
-          // MN-major operand: two boxes of 64 features (c0) x 64 contraction rows (c1), 8 KB each
-          if (MN & 1) {
+  __device__ __forceinline__ void load(int64_t uu, int kb, uint32_t sa, uint32_t fb) const {
+    using C = Cfg<RB>;
+    const int64_t u = uu % n_tiles;
+    const int j0 = (int)(u % n_blk) * BM;                  // feature block
+    const int r0 = (int)((u / n_blk) * BN);                // row block
+    if (MN & 1) {        // MN-major operand: two boxes of 64 features (c0) x 64 contraction rows
 #pragma unroll
-            for (int b = 0; b < 2; ++b) {
-              const uint32_t o = (uint32_t)b * 8192u;
-              tma_load_2d_2sm(sa + o, &map_whi, fb, j0 + 64 * b, kb * 64);
-              tma_load_2d_2sm(sa + GC::A_TILE + o, &map_wlo, fb, j0 + 64 * b, kb * 64);
-            }
-          } else {
-            tma_load_2d_2sm(sa, &map_whi, fb, kb * 2 * GBK, j0);
-            tma_load_2d_2sm(sa + GC::A_TILE, &map_wlo, fb, kb * 2 * GBK, j0);
-          }
-          if (MN & 2) {
-#pragma unroll
-            for (int b = 0; b < 2; ++b) {
-              const uint32_t o = (uint32_t)b * 8192u;
-              tma_load_2d_2sm(sa + 2 * GC::A_TILE + o, &map_hhi, fb, r0 + 64 * b, kb * 64);
-              tma_load_2d_2sm(sa + 2 * GC::A_TILE + GC::B_TILE + o, &map_hlo, fb, r0 + 64 * b,
-                              kb * 64);
-            }
-          } else {
-            tma_load_2d_2sm(sa + 2 * GC::A_TILE, &map_hhi, fb, kb * 2 * GBK, r0);
-            tma_load_2d_2sm(sa + 2 * GC::A_TILE + GC::B_TILE, &map_hlo, fb, kb * 2 * GBK, r0);
-          }
-          if (++stage == GC::STAGES) { stage = 0; phase ^= 1; }
-        }
+      for (int b = 0; b < 2; ++b) {
+        const uint32_t o = (uint32_t)b * 8192u;
+        tma_load_2d(sa + o, &map_whi, fb, j0 + 64 * b, kb * 64);
+        tma_load_2d(sa + C::A_TILE + o, &map_wlo, fb, j0 + 64 * b, kb * 64);
       }
+    } else {
+      tma_load_2d(sa, &map_whi, fb, kb * 64, j0);
+      tma_load_2d(sa + C::A_TILE, &map_wlo, fb, kb * 64, j0);
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (leader && lane == 0) {
-      const uint32_t idesc = make_idesc_2sm_f16() | ((MN & 1) ? (1u << 15) : 0u) |
-                             ((MN & 2) ? (1u << 16) : 0u);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int64_t uu = unit0; uu < n_units; uu += unit_step) {
-        const int kb0 = (int)(uu / n_tiles) * kb_per;
-        const int kb1 = min(kb0 + kb_per, n_kb_all);
-        mbar_wait(tempty_bar + 8 * acc, acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(full_bar + 8 * stage, phase);
-          tc_fence_after();
-          const uint32_t sa = smem_base + stage * GC::STAGE;
-          const uint64_t a_hi = (MN & 1) ? make_smem_desc_mn(sa) : make_smem_desc<GBK>(sa);
-          const uint64_t a_lo = (MN & 1) ? make_smem_desc_mn(sa + GC::A_TILE)
-                                         : make_smem_desc<GBK>(sa + GC::A_TILE);
-          const uint64_t b_hi = (MN & 2) ? make_smem_desc_mn(sa + 2 * GC::A_TILE)
-                                         : make_smem_desc<GBK>(sa + 2 * GC::A_TILE);
-          const uint64_t b_lo = (MN & 2) ? make_smem_desc_mn(sa + 2 * GC::A_TILE + GC::B_TILE)
-                                         : make_smem_desc<GBK>(sa + 2 * GC::A_TILE + GC::B_TILE);
+    if (MN & 2) {
 #pragma unroll
-          for (int k = 0; k < GBK / 8; ++k) {     // K-major: 16 halves = 32 B; MN-major: 2 KB
-            const uint64_t ka = (MN & 1) ? (uint64_t)((k * 2048) >> 4) : (uint64_t)((k * 8 * 4) >> 4);
-            const uint64_t kk = (MN & 2) ? (uint64_t)((k * 2048) >> 4) : (uint64_t)((k * 8 * 4) >> 4);
-            const uint32_t first = ((kb - kb0) | k) != 0 ? 1u : 0u;
-            umma_f16_2sm(d_tmem, a_lo + ka, b_hi + kk, idesc, first);
-            umma_f16_2sm(d_tmem, a_hi + ka, b_lo + kk, idesc, 1u);
-            umma_f16_2sm(d_tmem, a_hi + ka, b_hi + kk, idesc, 1u);
-          }
-          umma_commit_2sm(empty_bar + 8 * stage);
-          if (++stage == GC::STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit_2sm(tfull_bar + 8 * acc);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      for (int b = 0; b < 2; ++b) {
+        const uint32_t o = (uint32_t)b * 8192u;
+        tma_load_2d(sa + 2 * C::A_TILE + o, &map_hhi, fb, r0 + 64 * b, kb * 64);
+        tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE + o, &map_hlo, fb, r0 + 64 * b, kb * 64);
       }
+    } else {
+      tma_load_2d(sa + 2 * C::A_TILE, &map_hhi, fb, kb * 64, r0);
+      tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE, &map_hlo, fb, kb * 64, r0);
     }
-  } else {
-    // ===================== epilogue (warps 2..9, both CTAs) =====================
-    const int quarter = warp & 3;
-    const int half = (warp - 2) >> 2;
+  }
+  __device__ __forceinline__ void convert(int64_t, int, uint8_t*, int) const {}
+  __device__ __forceinline__ void epilogue(int64_t uu, uint32_t trow, int quarter, int lane,
+                                           EpiState& st) const {
+    float& amax = st.amax;   // max |stored output| (EPI 0 / 2): the consumer's fp16-split scale
     const float acc_scale = 1.f / (scale_w[0] * scale_h[0]);   // powers of two: exact
     // EPI 3: `out` = the fp16 plane pair [2][R][Jp_out], amax_scale[0] = their (a-priori) scale
     __half* __restrict__ pl_out = reinterpret_cast<__half*>(out);
     const int Jp_out = ((J + 63) / 64) * 64;
     const float s_out = (EPI == 3) ? amax_scale[0] : 1.f;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    float amax = 0.f;        // max |stored output| (EPI 0 / 2): the consumer's fp16-split scale
-    for (int64_t uu = unit0; uu < n_units; uu += unit_step) {
-      const int64_t u = uu % n_tiles;
-      const int slice = (int)(uu / n_tiles);
-      const bool empty_slice = slice * kb_per >= n_kb_all;   // accumulator never written
-      float* __restrict__ out_s = (EPI == 0 && out) ? out + (int64_t)slice * R * J : out;
-      const int nb = (int)(u % n_pair) * 2 + (int)rank;
-      const int j = nb * BM + quarter * 32 + lane;
-      const bool j_ok = j < J;
-      const float b_j = (j_ok && bias) ? bias[j] : 0.f;
-      const int64_t r0 = (u / n_pair) * BN + half * (BN / 2);
-      mbar_wait(tfull_bar + 8 * acc, acc_phase);
-      tc_fence_after();
-      const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16) +
-                            (uint32_t)(acc * BN + half * (BN / 2));
-      const int64_t part_row = (int64_t)(nb * 4 + quarter) * R;
-      const float b_use = (slice == 0) ? b_j : 0.f;           // bias once across the slices
+    const int64_t u = uu % n_tiles;
+    const int slice = (int)(uu / n_tiles);
+    const bool empty_slice = slice * kb_per >= n_kb_all;   // accumulator never written
+    float* __restrict__ out_s = (EPI == 0 && out) ? out + (int64_t)slice * R * J : out;
+    const int nb = (int)(u % n_blk);
+    const int j = nb * BM + quarter * 32 + lane;
+    const bool j_ok = j < J;
+    const float b_j = (j_ok && bias) ? bias[j] : 0.f;
+    const int64_t r0 = (u / n_blk) * BN;
+    const int64_t part_row = (int64_t)(nb * 4 + quarter) * R;
+    const float b_use = (slice == 0) ? b_j : 0.f;           // bias once across the slices
       const bool warp_j_ok = __all_sync(0xffffffffu, j_ok);
       float csum = 0.f;                                       // EPI 3: column sum of this lane's j
       // observations of one 16-column block (rows rbase .. rbase+15, this lane's feature j); all
@@ -306,46 +183,48 @@ linear_tc2_kernel(const __grid_constant__ CUtensorMap map_whi,
         }
         if (EPI == 1) {
           const float sum = warp_transpose_sum16(lpv, lane);
-          if (nb < n_blk && lane < 16 && rbase + lane < R) part[part_row + rbase + lane] = sum;
+          if (lane < 16 && rbase + lane < R) part[part_row + rbase + lane] = sum;
         }
       };
-      // the TMEM load and the observation loads of block i+1 are in flight while block i is
-      // processed
+      // the observation loads of block i+1 are in flight while block i is processed
       uint32_t va[16], vb[16];
       float xa[EPI ? 16 : 1], xb[EPI ? 16 : 1], ga = 0.f, gb = 0.f;
       load_x(xa, ga, 0);
-      tmem_ld16(trow, va);
 #pragma unroll 1
-      for (int c = 0; c < BN / 2; c += 32) {
+      for (int c = 0; c < BN; c += 32) {
         load_x(xb, gb, c + 16);
-        tmem_ld_wait();
-        tmem_ld16(trow + (uint32_t)(c + 16), vb);
+        acc_ld16(trow + 4u * (uint32_t)c, va);
         process(va, xa, ga, c);
-        if (c + 32 < BN / 2) load_x(xa, ga, c + 32);
-        tmem_ld_wait();
-        if (c + 32 < BN / 2) tmem_ld16(trow + (uint32_t)(c + 32), va);
+        if (c + 32 < BN) load_x(xa, ga, c + 32);
+        acc_ld16(trow + 4u * (uint32_t)(c + 16), vb);
         process(vb, xb, gb, c + 16);
       }
-      tc_fence_before();
-      if (leader) mbar_arrive(tempty_bar + 8 * acc);
-      else mbar_arrive_remote(tempty_bar + 8 * acc, 0);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
       if (EPI == 3 && part && j_ok) atomicAdd(part + j, csum);   // bias gradient (part = col_sum)
-    }
+  }
+  __device__ __forceinline__ void epi_finish(EpiState& st, int, int lane) const {
     if ((EPI == 0 || EPI == 2) && amax_scale) {   // NaN / inf never win the max (fmaxf drops NaN)
-      amax = warp_max(amax <= 3.0e38f ? amax : 0.f);
-      if (lane == 0 && amax > 0.f)
-        atomicMax(reinterpret_cast<unsigned int*>(amax_scale) + 2, __float_as_uint(amax));
+      const float m = warp_max(st.amax <= 3.0e38f ? st.amax : 0.f);
+      if (lane == 0 && m > 0.f)
+        atomicMax(reinterpret_cast<unsigned int*>(amax_scale) + 2, __float_as_uint(m));
     }
   }
+};
 
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;"
-                 ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
-  }
+// one product on the tensor cores: A = w planes (J_ features), B = h planes (R rows)
+template <int EPI, int MN, int GL>
+int launch_linear(const CUtensorMap& whi, const CUtensorMap& wlo, const CUtensorMap& hhi,
+                  const CUtensorMap& hlo, const float* bias, const float* x_obs, int64_t n_x,
+                  const float* gout, float* out, float* part, int64_t R, int J_, int Kp, int relu,
+                  const float* scale_w, const float* scale_h, int k_slices, float* amax_scale,
+                  cudaStream_t st, const char* what) {
+  const int n_blk = (J_ + BM - 1) / BM;
+  const int64_t n_tiles = ((R + BN - 1) / BN) * n_blk;
+  const int n_kb_all = Kp / 64;
+  const int kb_per = (n_kb_all + k_slices - 1) / k_slices;
+  const LinW<EPI, MN, GL> w{whi, wlo, hhi, hlo, bias, x_obs, n_x, gout, out, part, R, J_, Kp,
+                            relu, scale_w, scale_h, k_slices, amax_scale, n_blk, n_tiles,
+                            n_kb_all, kb_per};
+  return tc_launch(w, st, what);
 }
 
 // One pass over an activation / gradient matrix that produces BOTH operand layouts of the dense
@@ -592,12 +471,6 @@ __global__ void __launch_bounds__(256) part_sum_kernel(const float* __restrict__
   }
 }
 
-template <int EPI, int MN = 0, int GL = 0>
-cudaError_t linear_prepare() {
-  static const cudaError_t e = cudaFuncSetAttribute(
-      linear_tc2_kernel<EPI, MN, GL>, cudaFuncAttributeMaxDynamicSharedMemorySize, GC::SMEM);
-  return e;
-}
 // ZSB_EPI_GLOAD=1: the epi 2 / 3 epilogues load the upstream gradient per row (warp-uniform loads)
 // instead of broadcasting it by shuffle (A/B switch of an experiment; default = shuffle)
 int epi_gload() {
@@ -611,7 +484,7 @@ extern "C" {
 
 int zsb_linear_tc_kpad(int K) { return ((K + 63) / 64) * 64; }
 // rows of the partial-sum scratch of epi 1 (each [R] floats)
-int zsb_linear_tc_nparts(int J) { return 4 * 2 * ((((J + BM - 1) / BM) + 1) / 2); }
+int zsb_linear_tc_nparts(int J) { return 4 * ((J + BM - 1) / BM); }
 
 // Operand preparation: src [rows, K] fp32 -> planes [2][rows][Kp] fp16 (Kp = zsb_linear_tc_kpad(K))
 // and scale[0] (device float[4] scratch, zero-initialised once by the caller).
@@ -683,14 +556,14 @@ int zsb_split16_dual_f32(const float* src, const float* mask_src, int64_t R, int
 //   epi 1: out [R] = sum_j Bernoulli(logits = h W^T + bias).log_prob(x[r % n_x, j]);
 //          part = scratch of zsb_linear_tc_nparts(J) * R floats
 //   epi 2: out [R, J] = gout[r] * (x - sigmoid(logits))
-// Split-K (epi 0 only): when the output has fewer than one 256 x 256 tile per CTA pair and `part`
-// is given (zsb_linear_tc_slices(R, J, K) * R * J floats), the contraction is cut into slices that
-// run on different CTA pairs and are summed afterwards (the weight-gradient shape dW = dl^T h).
+// Split-K (epi 0 only): when the output has fewer than one 128 x 128 tile per SM and `part` is
+// given (zsb_linear_tc_slices(R, J, K) * R * J floats), the contraction is cut into slices that
+// run on different SMs and are summed afterwards (the weight-gradient shape dW = dl^T h).
 int zsb_linear_tc_slices(int64_t R, int J, int K) {
   const int n_blk = (J + BM - 1) / BM;
-  const int64_t tiles = ((R + BN - 1) / BN) * ((n_blk + 1) / 2);
+  const int64_t tiles = ((R + BN - 1) / BN) * n_blk;
   const int n_kb = zsb_linear_tc_kpad(K) / 64;
-  int64_t want = (ZSB_NUM_SMS / 2) / tiles;                 // CTA pairs per tile
+  int64_t want = ZSB_NUM_SMS / tiles;                       // CTAs per tile
   if (want < 1) want = 1;
   if (want > n_kb / 8) want = n_kb / 8;                      // >= 8 k-blocks per slice
   if (want < 1) want = 1;
@@ -730,18 +603,12 @@ int zsb_linear_tc_amax_f32(int epi, const void* w_planes, const float* scale_w,
   const __half* hp = reinterpret_cast<const __half*>(h_planes);
   CUtensorMap m_whi, m_wlo, m_hhi, m_hlo;
   int rc;
-  if ((rc = make_map(&m_whi, wp, (uint64_t)J, (uint64_t)Kp, BM, GBK, 1))) return rc;
-  if ((rc = make_map(&m_wlo, wp + (int64_t)J * Kp, (uint64_t)J, (uint64_t)Kp, BM, GBK, 1)))
+  if ((rc = make_map(&m_whi, wp, (uint64_t)J, (uint64_t)Kp, BM, 128, 1))) return rc;
+  if ((rc = make_map(&m_wlo, wp + (int64_t)J * Kp, (uint64_t)J, (uint64_t)Kp, BM, 128, 1)))
     return rc;
-  if ((rc = make_map(&m_hhi, hp, (uint64_t)R, (uint64_t)Kp, BN / 2, GBK, 1))) return rc;
-  if ((rc = make_map(&m_hlo, hp + R * Kp, (uint64_t)R, (uint64_t)Kp, BN / 2, GBK, 1))) return rc;
+  if ((rc = make_map(&m_hhi, hp, (uint64_t)R, (uint64_t)Kp, BN, 128, 1))) return rc;
+  if ((rc = make_map(&m_hlo, hp + R * Kp, (uint64_t)R, (uint64_t)Kp, BN, 128, 1))) return rc;
   const int n_blk = (J + BM - 1) / BM;
-  const int64_t n_units = ((R + BN - 1) / BN) * ((n_blk + 1) / 2);
-  int dev = 0, sms = ZSB_NUM_SMS;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  int64_t pairs = sms / 2;
-  if (n_units < pairs) pairs = n_units;
   int k_slices = 1;
   if (epi == 0 && part) {
     k_slices = zsb_linear_tc_slices(R, J, K);
@@ -750,36 +617,25 @@ int zsb_linear_tc_amax_f32(int epi, const void* w_planes, const float* scale_w,
       return ZSB_ERR_INVALID;
     }
   }
-  pairs = sms / 2;
-  if (n_units * k_slices < pairs) pairs = n_units * k_slices;
-  const unsigned grid = (unsigned)(2 * pairs);
   float* out_k = (k_slices > 1) ? part : out;
-  cudaError_t prep;
-#define ZSB_LIN(EPI)                                                                           \
-  do {                                                                                         \
-    prep = linear_prepare<EPI>();                                                              \
-    if (prep == cudaSuccess)                                                                   \
-      linear_tc2_kernel<EPI><<<grid, NUM_THREADS, GC::SMEM, st>>>(                             \
-          m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, epi == 1 ? nullptr : out_k,      \
-          part, R, J, Kp, relu, scale_w, scale_h, k_slices,                                    \
-          k_slices > 1 ? nullptr : amax_scale);                                                \
-  } while (0)
-  if (epi == 0) ZSB_LIN(0);
-  else if (epi == 1) ZSB_LIN(1);
-  else if (!epi_gload()) ZSB_LIN(2);
-  else {
-    prep = linear_prepare<2, 0, 1>();
-    if (prep == cudaSuccess)
-      linear_tc2_kernel<2, 0, 1><<<grid, NUM_THREADS, GC::SMEM, st>>>(
-          m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out_k, part, R, J, Kp, relu, scale_w,
-          scale_h, k_slices, amax_scale);
-  }
-#undef ZSB_LIN
-  if (prep != cudaSuccess) {
-    zsb_set_error("linear_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(prep));
-    return ZSB_ERR_CUDA;
-  }
-  rc = zsb_check_launch("linear_tc");
+  float* amax_k = k_slices > 1 ? nullptr : amax_scale;
+  if (epi == 0)
+    rc = launch_linear<0, 0, 0>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out_k, part,
+                                R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
+                                "linear_tc");
+  else if (epi == 1)
+    rc = launch_linear<1, 0, 0>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, nullptr,
+                                part, R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
+                                "linear_tc");
+  else if (!epi_gload())
+    rc = launch_linear<2, 0, 0>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out_k, part,
+                                R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
+                                "linear_tc");
+  else
+    rc = launch_linear<2, 0, 1>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out_k, part,
+                                R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
+                                "linear_tc");
+
   if (rc == ZSB_OK && k_slices > 1) {
     const int64_t n = R * (int64_t)J;
     int64_t blocks = zsb_ceil_div(n, 256);
@@ -823,34 +679,20 @@ int zsb_linear_tc_bern_grad_planes_f32(const void* w_planes, const float* scale_
   const __half* hp = reinterpret_cast<const __half*>(h_planes);
   CUtensorMap m_whi, m_wlo, m_hhi, m_hlo;
   int rc;
-  if ((rc = make_map(&m_whi, wp, (uint64_t)J, (uint64_t)Kp, BM, GBK, 1))) return rc;
-  if ((rc = make_map(&m_wlo, wp + (int64_t)J * Kp, (uint64_t)J, (uint64_t)Kp, BM, GBK, 1)))
+  if ((rc = make_map(&m_whi, wp, (uint64_t)J, (uint64_t)Kp, BM, 128, 1))) return rc;
+  if ((rc = make_map(&m_wlo, wp + (int64_t)J * Kp, (uint64_t)J, (uint64_t)Kp, BM, 128, 1)))
     return rc;
-  if ((rc = make_map(&m_hhi, hp, (uint64_t)R, (uint64_t)Kp, BN / 2, GBK, 1))) return rc;
-  if ((rc = make_map(&m_hlo, hp + R * Kp, (uint64_t)R, (uint64_t)Kp, BN / 2, GBK, 1))) return rc;
-  const int n_blk = (J + BM - 1) / BM;
-  const int64_t n_units = ((R + BN - 1) / BN) * ((n_blk + 1) / 2);
-  int dev = 0, sms = ZSB_NUM_SMS;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  int64_t pairs = sms / 2;
-  if (n_units < pairs) pairs = n_units;
-  const unsigned grid = (unsigned)(2 * pairs);
-  const cudaError_t prep = epi_gload() ? linear_prepare<3, 0, 1>() : linear_prepare<3>();
-  if (prep != cudaSuccess) {
-    zsb_set_error("linear_tc_bern_grad_planes: cudaFuncSetAttribute: %s",
-                  cudaGetErrorString(prep));
-    return ZSB_ERR_CUDA;
-  }
+  if ((rc = make_map(&m_hhi, hp, (uint64_t)R, (uint64_t)Kp, BN, 128, 1))) return rc;
+  if ((rc = make_map(&m_hlo, hp + R * Kp, (uint64_t)R, (uint64_t)Kp, BN, 128, 1))) return rc;
   if (epi_gload())
-    linear_tc2_kernel<3, 0, 1><<<grid, NUM_THREADS, GC::SMEM, st>>>(
-        m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, reinterpret_cast<float*>(dl_planes),
-        col_sum, R, J, Kp, 0, scale_w, scale_h, 1, scale_out);
-  else
-    linear_tc2_kernel<3><<<grid, NUM_THREADS, GC::SMEM, st>>>(
-        m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, reinterpret_cast<float*>(dl_planes),
-        col_sum, R, J, Kp, 0, scale_w, scale_h, 1, scale_out);
-  return zsb_check_launch("linear_tc_bern_grad_planes");
+    return launch_linear<3, 0, 1>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout,
+                                  reinterpret_cast<float*>(dl_planes), col_sum, R, J, Kp, 0,
+                                  scale_w, scale_h, 1, scale_out, st,
+                                  "linear_tc_bern_grad_planes");
+  return launch_linear<3, 0, 0>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout,
+                                reinterpret_cast<float*>(dl_planes), col_sum, R, J, Kp, 0,
+                                scale_w, scale_h, 1, scale_out, st, "linear_tc_bern_grad_planes");
+
 }
 
 // Input gradient of a dense layer from the FORWARD weight planes:
@@ -870,36 +712,23 @@ int zsb_linear_tc_dgrad_f32(const void* w_planes, const float* scale_w, const vo
   const __half* gp = reinterpret_cast<const __half*>(g_planes);
   CUtensorMap m_whi, m_wlo, m_hhi, m_hlo;
   int rc;
-  if ((rc = make_map(&m_whi, wp, (uint64_t)J, (uint64_t)Kp_w, 64, GBK, 1))) return rc;
-  if ((rc = make_map(&m_wlo, wp + (int64_t)J * Kp_w, (uint64_t)J, (uint64_t)Kp_w, 64, GBK, 1)))
+  if ((rc = make_map(&m_whi, wp, (uint64_t)J, (uint64_t)Kp_w, 64, 128, 1))) return rc;
+  if ((rc = make_map(&m_wlo, wp + (int64_t)J * Kp_w, (uint64_t)J, (uint64_t)Kp_w, 64, 128, 1)))
     return rc;
-  if ((rc = make_map(&m_hhi, gp, (uint64_t)R, (uint64_t)Jp, BN / 2, GBK, 1))) return rc;
-  if ((rc = make_map(&m_hlo, gp + R * Jp, (uint64_t)R, (uint64_t)Jp, BN / 2, GBK, 1))) return rc;
-  const int n_blk = (K + BM - 1) / BM;
-  const int64_t n_units = ((R + BN - 1) / BN) * ((n_blk + 1) / 2);
-  int dev = 0, sms = ZSB_NUM_SMS;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  int64_t pairs = sms / 2;
-  if (n_units < pairs) pairs = n_units;
-  const unsigned grid = (unsigned)(2 * pairs);
-  const cudaError_t prep = linear_prepare<0, 1>();
-  if (prep != cudaSuccess) {
-    zsb_set_error("linear_tc_dgrad: cudaFuncSetAttribute: %s", cudaGetErrorString(prep));
-    return ZSB_ERR_CUDA;
-  }
-  linear_tc2_kernel<0, 1><<<grid, NUM_THREADS, GC::SMEM, st>>>(
-      m_whi, m_wlo, m_hhi, m_hlo, nullptr, nullptr, 0, nullptr, out, nullptr, R, K, Jp, 0,
-      scale_w, scale_g, 1, amax_scale);
-  return zsb_check_launch("linear_tc_dgrad");
+  if ((rc = make_map(&m_hhi, gp, (uint64_t)R, (uint64_t)Jp, BN, 128, 1))) return rc;
+  if ((rc = make_map(&m_hlo, gp + R * Jp, (uint64_t)R, (uint64_t)Jp, BN, 128, 1))) return rc;
+  return launch_linear<0, 1, 0>(m_whi, m_wlo, m_hhi, m_hlo, nullptr, nullptr, 0, nullptr, out,
+                                nullptr, R, K, Jp, 0, scale_w, scale_g, 1, amax_scale, st,
+                                "linear_tc_dgrad");
+
 }
 
 // Weight gradient of a dense layer WITHOUT transposed operands:
 //   out [J, K] = sum_r g[r, j] * h[r, k]            (dW = g^T h, tf.gradients of tf.layers.dense)
 // h_planes [2][R][Kp(K)], g_planes [2][R][Kp(J)]: the row-major fp16 hi/lo planes the forward /
 // input-gradient products already use (zsb_split16_pad_f32 / zsb_split16_dual_f32).  The contraction
-// runs over the rows, so both operands are MN-major for tcgen05 (see linear_tc2_kernel<0, 3>);
-// split-K over the CTA pairs as in zsb_linear_tc_f32 (part = zsb_linear_tc_slices(J, K, R) * J * K
+// runs over the rows, so both operands are MN-major wgmma operands (LinW<0, 3>);
+// split-K over the SMs as in zsb_linear_tc_f32 (part = zsb_linear_tc_slices(J, K, R) * J * K
 // floats, or NULL for a single slice).
 int zsb_linear_tc_wgrad_f32(const void* h_planes, const float* scale_h, int K,
                             const void* g_planes, const float* scale_g, int J, int64_t R,
@@ -912,30 +741,17 @@ int zsb_linear_tc_wgrad_f32(const void* h_planes, const float* scale_h, int K,
   const int Rp = zsb_linear_tc_kpad((int)R);                 // padded contraction length
   const __half* hp = reinterpret_cast<const __half*>(h_planes);
   const __half* gp = reinterpret_cast<const __half*>(g_planes);
-  CUtensorMap m_whi, m_wlo, m_hhi, m_hlo;                    // "w" = h (lanes = k), "h" = g
+  CUtensorMap m_whi, m_wlo, m_hhi, m_hlo;                    // "w" = h (rows = k), "h" = g
   int rc;
-  if ((rc = make_map(&m_whi, hp, (uint64_t)R, (uint64_t)Kp_h, 64, GBK, 1))) return rc;
-  if ((rc = make_map(&m_wlo, hp + R * Kp_h, (uint64_t)R, (uint64_t)Kp_h, 64, GBK, 1))) return rc;
-  if ((rc = make_map(&m_hhi, gp, (uint64_t)R, (uint64_t)Jp_g, 64, GBK, 1))) return rc;
-  if ((rc = make_map(&m_hlo, gp + R * Jp_g, (uint64_t)R, (uint64_t)Jp_g, 64, GBK, 1))) return rc;
-  const int n_blk = (K + BM - 1) / BM;
-  const int64_t n_units = (((int64_t)J + BN - 1) / BN) * ((n_blk + 1) / 2);
-  int dev = 0, sms = ZSB_NUM_SMS;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if ((rc = make_map(&m_whi, hp, (uint64_t)R, (uint64_t)Kp_h, 64, 128, 1))) return rc;
+  if ((rc = make_map(&m_wlo, hp + R * Kp_h, (uint64_t)R, (uint64_t)Kp_h, 64, 128, 1))) return rc;
+  if ((rc = make_map(&m_hhi, gp, (uint64_t)R, (uint64_t)Jp_g, 64, 128, 1))) return rc;
+  if ((rc = make_map(&m_hlo, gp + R * Jp_g, (uint64_t)R, (uint64_t)Jp_g, 64, 128, 1))) return rc;
   const int k_slices = part ? zsb_linear_tc_slices(J, K, (int)R) : 1;
-  int64_t pairs = sms / 2;
-  if (n_units * k_slices < pairs) pairs = n_units * k_slices;
-  const unsigned grid = (unsigned)(2 * pairs);
-  const cudaError_t prep = linear_prepare<0, 3>();
-  if (prep != cudaSuccess) {
-    zsb_set_error("linear_tc_wgrad: cudaFuncSetAttribute: %s", cudaGetErrorString(prep));
-    return ZSB_ERR_CUDA;
-  }
-  linear_tc2_kernel<0, 3><<<grid, NUM_THREADS, GC::SMEM, st>>>(
-      m_whi, m_wlo, m_hhi, m_hlo, nullptr, nullptr, 0, nullptr, k_slices > 1 ? part : out, part,
-      (int64_t)J, K, Rp, 0, scale_h, scale_g, k_slices, nullptr);
-  rc = zsb_check_launch("linear_tc_wgrad");
+  rc = launch_linear<0, 3, 0>(m_whi, m_wlo, m_hhi, m_hlo, nullptr, nullptr, 0, nullptr,
+                              k_slices > 1 ? part : out, part, (int64_t)J, K, Rp, 0, scale_h,
+                              scale_g, k_slices, nullptr, st, "linear_tc_wgrad");
+
   if (rc == ZSB_OK && k_slices > 1) {
     const int64_t n = (int64_t)J * K;
     int64_t blocks = zsb_ceil_div(n, 256);

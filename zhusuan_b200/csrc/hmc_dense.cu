@@ -13,7 +13,7 @@
 //
 // This file holds the SIMT fp32 implementation (impl 0): 128x128x16 tiles, 8x8 register micro-tile,
 // register-prefetch double buffering.  It is the always-available, any-D%16 reference kernel; the
-// tcgen05 3xTF32 tensor-core implementation (impl 1) lives in hmc_dense_tc.cu.
+// wgmma 3xTF32 tensor-core implementation (impl 1) lives in hmc_dense_tc.cu.
 #include "common.cuh"
 
 namespace {
@@ -224,7 +224,7 @@ int zsb_hmc_dense_ntiles(int64_t D, int impl) {
 }
 
 // impl 0: SIMT fp32 (P = full fp32 matrix; P_lo / q_cur_lo / q_next_lo ignored).
-// impl 1: tcgen05 3xTF32 (P = hi part, P_lo = residual; q_cur_lo = TF32 residual of q_cur on entry,
+// impl 1: wgmma 3xTF32 (P = hi part, P_lo = residual; q_cur_lo = TF32 residual of q_cur on entry,
 //         q_next_lo receives q_next's residual; D % 32 == 0).
 int zsb_hmc_dense_leapfrog_f32(const float* q_cur, const float* q_cur_lo, float* q_next,
                                float* q_next_lo, const float* p_in, float* p_out,

@@ -7,11 +7,10 @@
 
 namespace {
 
-// MODE 0: plain pass; 1: + log-prob partials (first pass); 2: + log-prob and kinetic partials.
-// Fused leapfrog epilogue for one warp's share of a tile: this thread's dimension `n` (TMEM lane)
-// against 128 chains starting at c0 (TMEM columns trow .. trow+127).  MODE 0: plain pass;
-// 1: + log-prob partials (first pass); 2: + log-prob and kinetic partials (last pass).
-// NCOL: TMEM columns (chains) this warp owns.
+// Fused leapfrog epilogue for one warp's share of a tile: this thread's dimension `n` (accumulator
+// row) against NCOL chains starting at c0 (`trow` = shared address of the row's first column).
+// MODE 0: plain pass; 1: + log-prob partials (first pass); 2: + log-prob and kinetic partials
+// (last pass).
 struct EpiArgs {
   const float* __restrict__ q_cur; float* __restrict__ q_next; float* __restrict__ q_next_lo;
   const float* __restrict__ p_in; float* __restrict__ p_out;
@@ -41,7 +40,7 @@ __device__ __forceinline__ void store_split(const EpiArgs& a, float* __restrict_
 // run-time a.D.  H16: fp16-split planes (impl 2) vs TF32 residual (impl 1).
 // COHERENT: 1 when q_cur may have been written earlier in the SAME launch (trajectory kernel): the
 // non-coherent ld.global.nc path of __ldg could then return a stale L1 line.
-template <int MODE, int NEXT, int DC, int H16, int NCOL = BN / 2, int COHERENT = 0>
+template <int MODE, int NEXT, int DC, int H16, int NCOL = BN, int COHERENT = 0>
 __device__ __forceinline__ void epilogue_half_tile(const EpiArgs& a, uint32_t trow, int n,
                                                    bool n_ok, bool parts_ok, int64_t c0,
                                                    int64_t part_row, int lane, float s2,
@@ -113,29 +112,25 @@ __device__ __forceinline__ void epilogue_half_tile(const EpiArgs& a, uint32_t tr
   };
 
   if (fast_tile) {
-    // software-pipelined: the global loads AND the TMEM load of block i+1 are in flight while
-    // block i is computed and stored (two register sets A/B, loop unrolled by two blocks)
+    // software-pipelined: the global loads of block i+1 are in flight while block i is computed
+    // and stored (two register sets A/B, loop unrolled by two blocks)
     float pa[16], qa[16], pb[16], qb[16];
     uint32_t va[16], vb[16];
     load(pa, qa, 0);
-    tmem_ld16(trow, va);
 #pragma unroll 1
     for (int c = 0; c < NCOL; c += 32) {
       load(pb, qb, c + 16);
-      tmem_ld_wait();                                   // va has landed
-      tmem_ld16(trow + (uint32_t)(c + 16), vb);
+      acc_ld16(trow + 4u * (uint32_t)c, va);
       compute(va, pa, qa, c);
       if (c + 32 < NCOL) load(pa, qa, c + 32);
-      tmem_ld_wait();                                   // vb has landed
-      if (c + 32 < NCOL) tmem_ld16(trow + (uint32_t)(c + 32), va);
+      acc_ld16(trow + 4u * (uint32_t)(c + 16), vb);
       compute(vb, pb, qb, c + 16);
     }
   } else {
 #pragma unroll 1
     for (int c = 0; c < NCOL; c += 16) {
       uint32_t v[16];
-      tmem_ld16(trow + (uint32_t)c, v);      // all 32 lanes participate (sync.aligned)
-      tmem_ld_wait();
+      acc_ld16(trow + 4u * (uint32_t)c, v);
       const int64_t cbase = c0 + c;
       if (cbase < chains && !skip) {
         const size_t cb = (size_t)c * D;

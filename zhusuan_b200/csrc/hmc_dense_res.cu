@@ -1,83 +1,21 @@
-// L2-RESIDENT whole-trajectory kernel for a dense-Gaussian log-joint (dense_impl = 5).
+// Whole-trajectory dense-Gaussian HMC with the fp16 hi/lo planes of q as the chain state
+// (dense_impl = 5).
 //
 // Replaces the L+1 iterations of the leapfrog `tf.while_loop` of zhusuan/hmc.py:347-372 (body =
-// leapfrog_integrator, hmc.py:38-43) plus the log p / kinetic terms of hamiltonian(), hmc.py:30-35,
-// in ONE persistent launch, organised so that a chain's state crosses HBM once per ITERATION
-// instead of once per leapfrog pass.
+// leapfrog_integrator, hmc.py:38-43) plus the log p / kinetic terms of hamiltonian(), hmc.py:30-35.
+// Inside a trajectory the state of q is its fp16 hi/lo plane pair of q*sq (plus fp32 p): each
+// pass reads the planes it wrote in the previous pass, reconstructs q = (hi + lo)/sq (within 2^-23
+// of the fp32 value), and writes the next planes, so no fp32 copy of q travels: 16*D bytes per
+// chain and pass, the algorithmic minimum.
 //
-// Why this shape (measured in round 2, profiles/r02_traj_v1_findings.md):
-//  * the per-pass kernel (hmc_dense_tc.cu, impl 2) streams 1.61 GB per pass through HBM and sits
-//    on the board's power cap; passes couple chains only at iteration boundaries, so a block of
-//    chains can run all its passes back to back out of the 126 MB L2;
-//  * a first trajectory kernel (hmc_dense_traj.cu, impl 4: clusters of 8 CTAs = all 1024
-//    dimensions of a 256-chain block, cluster barriers between passes, MMA N = 128) is correct but
-//    2x slower: only 8 clusters of 8 become co-resident (64 of 148 SMs busy), and N = 128 doubles
-//    the operand bytes per MMA cycle -- 62 B/clk/SM, the L2->SM port limit.
-// So this kernel keeps the per-pass kernel's proven machinery -- CTA pairs (cta_group::2, M = 256
-// dimensions), N = 256 chains per unit, fp16 hi/lo operand planes and three kind::f16 products,
-// TMA 128B-swizzle ring, two TMEM accumulators so the epilogue of one unit hides behind the MMAs
-// of the next, all 74 pairs busy -- and adds:
-//  * STATE = the fp16 hi/lo planes of q*sq (plus fp32 p): the epilogue reads the planes it wrote
-//    in the previous pass, reconstructs q = (hi + lo)/sq (within 2^-23 of the fp32 value), and
-//    writes the next planes.  No separate fp32 copy of q travels: 16*D bytes per chain-pass, the
-//    algorithmic minimum, and 12 B per element of L2 footprint (two plane buffers + p);
-//  * GROUP-MAJOR order: chains are processed in groups of `group_blocks` 256-chain blocks (37 at
-//    D = 1024: 148 units = 2 per CTA pair per pass); a group runs all L+1 passes before the next
-//    group starts, so its state (9 472 chains x 12 KB = 116 MB) stays in the L2;
-//  * pass-to-pass dependencies through global counters instead of cluster barriers: every epilogue
-//    warp of every dimension tile of chain block c bumps flags[c] once per pass (release, after
-//    __threadfence + fence.proxy.async); the TMA producer of a unit of pass i+1 spins (acquire)
-//    until flags[c] == (i+1) * n_pair * 2 CTAs * 8 warps.  A pair processes the SAME units in
-//    every pass, two units apart, so the wait is normally already satisfied.
-// All CTAs must be co-resident (grid <= one CTA per SM); waits trap after ~2 s instead of hanging.
+// On H100 one pass of the benchmark shape (65 536 chains x 1024 dimensions) executes ~0.4 TFLOP of
+// fp16 products against ~1 GB of operand and state traffic, so the pass is bound by the tensor
+// cores, not by HBM: the passes run as L+1 launches of the persistent tensor-core kernel
+// (tc_pipeline_kernel) on alternating plane buffers, and the sampler state never leaves the plane
+// format between the prepare and the select.
 #include "tc_common.cuh"
 
 namespace {
-
-using CR = Cfg2<32>;                 // 128 x 64-half A tile + own 128 x 64-half B tile, 3 stages
-
-struct ResMaps {
-  CUtensorMap p_hi, p_lo;            // P planes [D, D] fp16; box 128 rows (MC: 64 rows)
-  CUtensorMap q_hi[2], q_lo[2];      // state planes, buffers 0 / 1: [chains, D] fp16 each
-};
-
-__device__ __forceinline__ int flag_load_acquire(const int* f) {
-  int v;
-  asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(f) : "memory");
-  return v;
-}
-__device__ __forceinline__ void flag_add_release(int* f, int v) {
-  asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(f), "r"(v) : "memory");
-}
-__device__ __forceinline__ void flag_wait(const int* f, int target) {
-  if (flag_load_acquire(f) >= target) return;
-  const long long t0 = clock64();
-  while (flag_load_acquire(f) < target) {
-    __nanosleep(64);
-    if (clock64() - t0 > WAIT_TIMEOUT_CYCLES) {
-      printf("zsb dense_res: flag wait timeout (block %d thread %d target %d have %d)\n",
-             blockIdx.x, threadIdx.x, target, flag_load_acquire(f));
-      __trap();
-    }
-  }
-}
-
-// 2-CTA TMA load multicast to the CTAs of `mask` (same CTA-relative smem offset in each; the
-// complete_tx lands on the mbarrier of each destination CTA's pair leader)
-__device__ __forceinline__ void tma_load_2d_2sm_mc(uint32_t dst, const CUtensorMap* map,
-                                                   uint32_t bar, int c0, int c1, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      ".multicast::cluster [%0], [%1, {%4, %5}], [%2], %3;"
-      ::"r"(dst), "l"(map), "r"(bar & PEER_BIT_MASK), "h"(mask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_mask(uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64"
-      " [%0], %1;"
-      ::"r"(bar), "h"(mask) : "memory");
-}
 
 struct ResEpi {
   const __half* __restrict__ hi_cur; const __half* __restrict__ lo_cur;   // planes of q (this pass)
@@ -88,7 +26,7 @@ struct ResEpi {
   float sq, inv_sq, acc_scale;
 };
 
-// One warp's share of a unit: dimension n (TMEM lane) against NCOL chains from c0.
+// One warp's share of a unit: dimension n (accumulator row) against NCOL chains from c0.
 //   Q   = hi + lo                      (q * sq, exact to 2^-24)
 //   g   = b_n - acc_scale * acc        (acc = (P sP)(q sq) from the three products)
 //   p  += s2 * g
@@ -99,7 +37,7 @@ __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, 
                                                 bool parts_ok, int64_t c0, int64_t part_row,
                                                 int lane, float s2, float eps_over_m_sq,
                                                 float inv_m, float b_n, float mu_n, bool skip) {
-  constexpr int NCOL = BN / 2;
+  constexpr int NCOL = BN;
   const uint32_t D = DC ? (uint32_t)DC : (uint32_t)a.D;
   const int64_t chains = a.chains;
   const bool warp_n_ok = __all_sync(0xffffffffu, n_ok);
@@ -165,28 +103,24 @@ __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, 
         if (lane < 16) a.k_part[part_row + c0 + c + lane] = sum;
       }
     };
-    // software pipeline: global + TMEM loads of block i+1 in flight while block i is computed
+    // software pipeline: the global loads of block i+1 are in flight while block i is computed
     float pa[16], pb[16];
     uint32_t ha[16], hb[16], va[16], vb[16];
     load(pa, ha, 0);
-    tmem_ld16(trow, va);
 #pragma unroll 1
     for (int c = 0; c < NCOL; c += 32) {
       load(pb, hb, c + 16);
-      tmem_ld_wait();
-      tmem_ld16(trow + (uint32_t)(c + 16), vb);
+      acc_ld16(trow + 4u * (uint32_t)c, va);
       compute(va, pa, ha, c);
       if (c + 32 < NCOL) load(pa, ha, c + 32);
-      tmem_ld_wait();
-      if (c + 32 < NCOL) tmem_ld16(trow + (uint32_t)(c + 32), va);
+      acc_ld16(trow + 4u * (uint32_t)(c + 16), vb);
       compute(vb, pb, hb, c + 16);
     }
   } else {
 #pragma unroll 1
     for (int c = 0; c < NCOL; c += 16) {
       uint32_t v[16];
-      tmem_ld16(trow + (uint32_t)c, v);      // all 32 lanes participate (sync.aligned)
-      tmem_ld_wait();
+      acc_ld16(trow + 4u * (uint32_t)c, v);
       const int64_t cbase = c0 + c;
       if (cbase < chains && !skip) {
         const size_t cb = (size_t)c * D;
@@ -229,249 +163,82 @@ __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, 
   }
 }
 
-// MC = 1: clusters of 4 CTAs = two pairs working on the SAME dimension tile and two adjacent chain
-// blocks; each CTA loads half of its 128 P rows and multicasts it to its counterpart in the other
-// pair, so a P tile is read from the L2 once per two pairs (the kernel is bound by L2 read
-// throughput: 6.5 kB/clk chip-wide measured = the ~6.3 kB/clk LTS cap).
-template <int DC, int MC>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-dense_res_kernel(const __grid_constant__ ResMaps maps, __half* __restrict__ planes0,
-                 __half* __restrict__ planes1, const float* __restrict__ p0,
-                 float* __restrict__ pw, const float* __restrict__ bvec,
-                 const float* __restrict__ mu, const float* __restrict__ mass,
-                 const float* __restrict__ state, float* __restrict__ lp0_part,
-                 float* __restrict__ lp1_part, float* __restrict__ k_part, int64_t chains,
-                 int D_rt, int L, const float* __restrict__ scales, int* __restrict__ flags,
-                 int group_blocks, int dbg, int inplace) {
-  using C = CR;
-  const int D = DC ? DC : D_rt;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bars = smem_base + C::STAGES * C::STAGE;
-  const uint32_t full_bar = bars;                          // [STAGES]  leader
-  const uint32_t empty_bar = bars + 8 * C::STAGES;         // [STAGES]  each CTA
-  const uint32_t tfull_bar = bars + 16 * C::STAGES;        // [2]       each CTA
-  const uint32_t tempty_bar = bars + 16 * C::STAGES + 16;  // [2]       leader
-  const uint32_t tmem_slot = bars + 16 * C::STAGES + 32;   // u32
-  uint32_t* tmem_slot_ptr =
-      reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  const int lane = threadIdx.x & 31;
-  const uint32_t crank = cluster_ctarank();                // 0..1 (MC: 0..3)
-  const uint32_t rank = crank & 1u;                        // rank inside the CTA pair
-  const uint32_t pidx = crank >> 1;                        // pair inside the cluster (MC only)
-  const uint32_t leader_rank = crank & ~1u;
-  const bool leader = rank == 0;
-  const uint16_t pair_mask = (uint16_t)(3u << leader_rank);
-  const int n_blk = (D + BM - 1) / BM;
-  const int n_pair = (n_blk + 1) / 2;                      // dimension tiles (M = 256) per block
-  const int64_t c_blk = (chains + BN - 1) / BN;            // 256-chain blocks
-  constexpr int CL = MC ? 4 : 2;
-  const int64_t my = blockIdx.x / CL, n_clusters = gridDim.x / CL;
-  const int n_kb = D / 64;
-  const int flag_per_pass = n_pair * 2 * NUM_EPI_WARPS;    // arrivals on flags[c] per pass
+template <int MODE, int NEXT, int DC>
+struct ResW {
+  static constexpr int KIND = 1, RB = 128, MNA = 0, MNB = 0, CVT = 0;
+  static constexpr int KE = RB / 2;
+  static constexpr uint32_t TX = Cfg<RB>::STAGE;
+  CUtensorMap m_phi, m_plo, m_qhi, m_qlo;
+  ResEpi ea;
+  const float* bvec; const float* mu; const float* mass; const float* state;
+  const float* scales;
+  float p_scale;
+  int n_blk, D_rt;
+  struct EpiState {};
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < C::STAGES; ++s) {
-      mbar_init(full_bar + 8 * s, 1);
-      mbar_init(empty_bar + 8 * s, MC ? 2 : 1);    // MC: both pairs' MMAs free a slot
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar + 8 * a, 1);
-      mbar_init(tempty_bar + 8 * a, 2 * 32 * NUM_EPI_WARPS);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  __device__ __forceinline__ int D() const { return DC ? DC : D_rt; }
+  __host__ __device__ __forceinline__ int64_t units() const {
+    return ((ea.chains + BN - 1) / BN) * (int64_t)n_blk;
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;"
-                 ::"r"(tmem_slot), "n"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
+  __device__ __forceinline__ void kb_range(int64_t, int& kb0, int& kb1) const {
+    kb0 = 0;
+    kb1 = D() / KE;
   }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-
-  // Work decomposition of one pass of a group of `gb` chain blocks.  MC = 0: pair `my` takes the
-  // units u = my, my + n_clusters, ... with (block, tile) = (u / n_pair, u % n_pair).  MC = 1: the
-  // cluster takes v = my, my + n_clusters, ... with (block pair, tile) = (v / n_pair, v % n_pair)
-  // and its pair `pidx` the block 2 * (v / n_pair) + pidx -- a phantom (skipped in the epilogue,
-  // zero-filled by TMA) when that block lies beyond the group.
-#define ZSB_RES_UNITS(gb) (MC ? (((gb) + 1) / 2) * n_pair : (gb) * n_pair)
-#define ZSB_RES_BLOCK(g0, u) ((g0) + (MC ? 2 * ((u) / n_pair) + (int64_t)pidx : (u) / n_pair))
-
-  if (warp == 0) {
-    // ===================== TMA producer (every CTA) =====================
-    if (lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.p_hi) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.p_lo) : "memory");
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int64_t g0 = 0; g0 < c_blk; g0 += group_blocks) {
-        const int64_t gb = (c_blk - g0 < group_blocks) ? (c_blk - g0) : group_blocks;
-        const int64_t units = ZSB_RES_UNITS(gb);
-        for (int i = 0; i <= L; ++i) {
-          const int buf = inplace ? 0 : (i & 1);
-          for (int64_t u = my; u < units; u += n_clusters) {
-            const int64_t cb = ZSB_RES_BLOCK(g0, u);
-            const bool valid = cb < g0 + gb;
-            const int n0 = ((int)(u % n_pair) * 2 + (int)rank) * BM;         // own dimension rows
-            const int c0 = (int)(cb * BN) + (int)rank * (BN / 2);            // own chain half
-            if (i > 0 && valid && !(dbg & 4)) {  // every tile of block cb finished pass i-1
-              flag_wait(flags + cb, i * flag_per_pass);
-              asm volatile("fence.proxy.async;" ::: "memory");
-            }
-            for (int kb = 0; kb < n_kb; ++kb) {
-              mbar_wait(empty_bar + 8 * stage, phase ^ 1);
-              const uint32_t fb = full_bar + 8 * stage;
-              const uint32_t sa = smem_base + stage * C::STAGE;
-              if (leader) mbar_expect_tx(fb, 2 * C::STAGE);
-              if (MC) {     // own half (64 rows = 8 KB) of the P tile, to both pairs
-                const uint16_t mm = (uint16_t)(5u << rank);
-                const uint32_t ho = pidx * (uint32_t)(C::A_TILE / 2);
-                tma_load_2d_2sm_mc(sa + ho, &maps.p_hi, fb, kb * 64, n0 + (int)pidx * (BM / 2),
-                                   mm);
-                tma_load_2d_2sm_mc(sa + C::A_TILE + ho, &maps.p_lo, fb, kb * 64,
-                                   n0 + (int)pidx * (BM / 2), mm);
-              } else {
-                tma_load_2d_2sm(sa, &maps.p_hi, fb, kb * 64, n0);
-                tma_load_2d_2sm(sa + C::A_TILE, &maps.p_lo, fb, kb * 64, n0);
-              }
-              tma_load_2d_2sm(sa + 2 * C::A_TILE, &maps.q_hi[buf], fb, kb * 64, c0);
-              tma_load_2d_2sm(sa + 2 * C::A_TILE + C::B_TILE, &maps.q_lo[buf], fb, kb * 64, c0);
-              if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (leader && lane == 0) {
-      const uint32_t idesc = make_idesc_2sm_f16();
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int64_t g0 = 0; g0 < c_blk; g0 += group_blocks) {
-        const int64_t gb = (c_blk - g0 < group_blocks) ? (c_blk - g0) : group_blocks;
-        const int64_t units = ZSB_RES_UNITS(gb);
-        for (int i = 0; i <= L; ++i) {
-          for (int64_t u = my; u < units; u += n_clusters) {
-            mbar_wait(tempty_bar + 8 * acc, acc_phase ^ 1);
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-            for (int kb = 0; kb < n_kb; ++kb) {
-              mbar_wait(full_bar + 8 * stage, phase);
-              tc_fence_after();
-              const uint32_t sa = smem_base + stage * C::STAGE;
-              const uint64_t a_hi = make_smem_desc<32>(sa);
-              const uint64_t a_lo = make_smem_desc<32>(sa + C::A_TILE);
-              const uint64_t b_hi = make_smem_desc<32>(sa + 2 * C::A_TILE);
-              const uint64_t b_lo = make_smem_desc<32>(sa + 2 * C::A_TILE + C::B_TILE);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const uint64_t ko = (uint64_t)((k * 32) >> 4);
-                const uint32_t first = (kb | k) != 0 ? 1u : 0u;
-                if (dbg & 2) {          // timing experiment: one product instead of three
-                  umma_f16_2sm(d_tmem, a_hi + ko, b_hi + ko, idesc, first);
-                } else {
-                  umma_f16_2sm(d_tmem, a_lo + ko, b_hi + ko, idesc, first);
-                  umma_f16_2sm(d_tmem, a_hi + ko, b_lo + ko, idesc, 1u);
-                  umma_f16_2sm(d_tmem, a_hi + ko, b_hi + ko, idesc, 1u);
-                }
-              }
-              umma_commit_mask(empty_bar + 8 * stage, MC ? (uint16_t)0xF : pair_mask);
-              if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-            }
-            umma_commit_mask(tfull_bar + 8 * acc, pair_mask);
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-          }
-        }
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 2..9, both CTAs) =====================
-    const int quarter = warp & 3;
-    const int half = (warp - 2) >> 2;
+  __device__ __forceinline__ void prefetch() const {
+    tma_prefetch_desc(&m_phi); tma_prefetch_desc(&m_plo);
+    tma_prefetch_desc(&m_qhi); tma_prefetch_desc(&m_qlo);
+  }
+  __device__ __forceinline__ void load(int64_t u, int kb, uint32_t sa, uint32_t fb) const {
+    using C = Cfg<RB>;
+    const int n0 = (int)(u % n_blk) * BM;
+    const int c0 = (int)(u / n_blk) * BN;
+    tma_load_2d(sa, &m_phi, fb, kb * KE, n0);
+    tma_load_2d(sa + C::A_TILE, &m_plo, fb, kb * KE, n0);
+    tma_load_2d(sa + 2 * C::A_TILE, &m_qhi, fb, kb * KE, c0);
+    tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE, &m_qlo, fb, kb * KE, c0);
+  }
+  __device__ __forceinline__ void convert(int64_t, int, uint8_t*, int) const {}
+  __device__ __forceinline__ void epilogue(int64_t u, uint32_t trow, int quarter, int lane,
+                                           EpiState&) const {
+    const int nb = (int)(u % n_blk);
+    const int n = nb * BM + quarter * 32 + lane;
+    const int64_t c0 = (u / n_blk) * BN;
+    const bool n_ok = n < D();
     const float eps = state[ZSB_ST_EPS_USED];
+    const float s2 = mul(eps, p_scale);
     const float sq = scales[0];
-    const int64_t plane = chains * (int64_t)D;
-    __half* pl[2] = {planes0, inplace ? planes0 : planes1};
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int64_t g0 = 0; g0 < c_blk; g0 += group_blocks) {
-      const int64_t gb = (c_blk - g0 < group_blocks) ? (c_blk - g0) : group_blocks;
-      const int64_t units = ZSB_RES_UNITS(gb);
-      for (int i = 0; i <= L; ++i) {
-        const bool last = i == L;
-        const float s2 = mul(eps, (i > 0 && !last) ? 1.f : 0.5f);
-        const int buf = i & 1;
-        for (int64_t u = my; u < units; u += n_clusters) {
-          const int64_t cb = ZSB_RES_BLOCK(g0, u);
-          const bool valid = cb < g0 + gb;
-          const int nb = (int)(u % n_pair) * 2 + (int)rank;
-          const int n = nb * BM + quarter * 32 + lane;
-          const int64_t c0 = cb * BN + half * (BN / 2);
-          const bool n_ok = n < D;
-          const float m_n = n_ok ? mass[n] : 1.f;
-          const float eps_over_m_sq = mul(fdiv(eps, m_n), sq);
-          const float inv_m = fdiv(1.f, m_n);
-          const float b_n = (n_ok && bvec) ? bvec[n] : 0.f;
-          const float mu_n = (n_ok && mu) ? mu[n] : 0.f;
-          mbar_wait(tfull_bar + 8 * acc, acc_phase);
-          tc_fence_after();
-          if (inplace && valid && !last) {
-            // single plane buffer: q_next's planes overwrite q's.  This pair's MMAs of (cb, i)
-            // have completed (tfull) -> count it; nobody may overwrite the planes of block cb
-            // before EVERY dimension tile's MMAs of pass i have read them.
-            int* mma_done = flags + c_blk;
-            if (leader && warp == 2 && lane == 0) flag_add_release(mma_done + cb, 1);
-            if (lane == 0) flag_wait(mma_done + cb, (i + 1) * n_pair);
-            __syncwarp();
-          }
-          const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16) +
-                                (uint32_t)(acc * BN + half * (BN / 2));
-          const int64_t part_row = (int64_t)(nb * 4 + quarter) * chains;
-          const ResEpi ea{pl[buf], pl[buf] + plane, pl[buf ^ 1], pl[buf ^ 1] + plane,
-                          i == 0 ? p0 : pw, pw, i == 0 ? lp0_part : lp1_part, k_part,
-                          chains, D, sq, fdiv(1.f, sq), scales[1]};
-          const bool skip = (dbg & 1) != 0 || !valid;
-          if (last)
-            epilogue_planes<2, 0, DC>(ea, trow, n, n_ok, nb < n_blk, c0, part_row, lane, s2,
-                                      eps_over_m_sq, inv_m, b_n, mu_n, skip);
-          else if (i == 0)
-            epilogue_planes<1, 1, DC>(ea, trow, n, n_ok, nb < n_blk, c0, part_row, lane, s2,
-                                      eps_over_m_sq, inv_m, b_n, mu_n, skip);
-          else
-            epilogue_planes<0, 1, DC>(ea, trow, n, n_ok, nb < n_blk, c0, part_row, lane, s2,
-                                      eps_over_m_sq, inv_m, b_n, mu_n, skip);
-          tc_fence_before();
-          if (leader) mbar_arrive(tempty_bar + 8 * acc);
-          else mbar_arrive_remote(tempty_bar + 8 * acc, leader_rank);
-          if (!last && valid) {
-            // publish this warp's planes of (cb, pass i) to the TMA producers of pass i+1
-            __threadfence();
-            asm volatile("fence.proxy.async;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) flag_add_release(flags + cb, 1);
-          }
-          if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
-      }
-    }
+    const float m_n = n_ok ? mass[n] : 1.f;
+    const float eps_over_m_sq = mul(fdiv(eps, m_n), sq);
+    const float inv_m = fdiv(1.f, m_n);
+    const float b_n = (n_ok && bvec) ? bvec[n] : 0.f;
+    const float mu_n = (n_ok && mu) ? mu[n] : 0.f;
+    const int64_t part_row = (int64_t)(nb * 4 + quarter) * ea.chains;
+    ResEpi a = ea;
+    a.sq = sq;
+    a.inv_sq = fdiv(1.f, sq);
+    a.acc_scale = scales[1];
+    epilogue_planes<MODE, NEXT, DC>(a, trow, n, n_ok, true, c0, part_row, lane, s2,
+                                    eps_over_m_sq, inv_m, b_n, mu_n, false);
   }
+  __device__ __forceinline__ void epi_finish(EpiState&, int, int) const {}
+};
 
-#undef ZSB_RES_UNITS
-#undef ZSB_RES_BLOCK
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;"
-                 ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
+template <int DC>
+int res_pass(const CUtensorMap& phi, const CUtensorMap& plo, const CUtensorMap& qhi,
+             const CUtensorMap& qlo, const ResEpi& ea, const float* bvec, const float* mu,
+             const float* mass, const float* state, const float* scales, float p_scale, int n_blk,
+             int D, int mode, cudaStream_t st) {
+  if (mode == 1) {
+    const ResW<1, 1, DC> w{phi, plo, qhi, qlo, ea, bvec, mu, mass, state, scales, p_scale, n_blk, D};
+    return tc_launch(w, st, "hmc_dense_resident");
   }
+  if (mode == 0) {
+    const ResW<0, 1, DC> w{phi, plo, qhi, qlo, ea, bvec, mu, mass, state, scales, p_scale, n_blk, D};
+    return tc_launch(w, st, "hmc_dense_resident");
+  }
+  const ResW<2, 0, DC> w{phi, plo, qhi, qlo, ea, bvec, mu, mass, state, scales, p_scale, n_blk, D};
+  return tc_launch(w, st, "hmc_dense_resident");
 }
 
 // q[c, :] <- (hi + lo) / sq of the proposal planes where accept[c] (hmc.py:488-497).
@@ -521,156 +288,61 @@ __global__ void __launch_bounds__(256) select_planes_kernel(float* __restrict__ 
   }
 }
 
-template <int DC, int MC>
-cudaError_t res_prepare() {
-  static const cudaError_t e = cudaFuncSetAttribute(
-      dense_res_kernel<DC, MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, CR::SMEM);
-  return e;
-}
-
-// ZSB_RES_MC: 1 / 0 force the P-tile multicast variant (clusters of 4) on / off; unset = auto
-int res_mc_env() {
-  static const int mc = getenv("ZSB_RES_MC") ? atoi(getenv("ZSB_RES_MC")) : -1;
-  return mc;
-}
-
-// co-resident clusters of `cl` CTAs of this kernel (one CTA per SM)
-template <int DC, int MC>
-int res_max_clusters(int cl, int sms) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(cl * (sms / cl)));
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = CR::SMEM;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = (unsigned)cl; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  int n = 0;
-  if (cudaOccupancyMaxActiveClusters(&n, dense_res_kernel<DC, MC>, &cfg) != cudaSuccess || n < 1) {
-    cudaGetLastError();
-    n = sms / cl;
-  }
-  return n;
-}
-
 }  // namespace
 
-// Variant + group size for a problem.  Multicast (clusters of 4 CTAs = two pairs sharing a P tile:
-// 20 % fewer L2 reads per MAC, but only 33 such clusters = 132 of the 148 SMs are co-resident on
-// B200; measured 19.4 vs 20.1 ms per iteration at 65 536 x 1024) when the group still fills two
-// units per pair; chain blocks per group = two units per CTA pair per pass.
-void res_choose(int D, int64_t chains, int* mc_out, int* group_out) {
-  static const int env_group = getenv("ZSB_RES_GROUP") ? atoi(getenv("ZSB_RES_GROUP")) : 0;
-  int dev = 0, sms = ZSB_NUM_SMS;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int n_pair = ((D + BM - 1) / BM + 1) / 2;
-  const int64_t c_blk = (chains + BN - 1) / BN;
-  int mc = res_mc_env();
-  int max_cl4 = 0;
-  if (mc != 0 && res_prepare<0, 1>() == cudaSuccess) {
-    static const int cached = res_max_clusters<0, 1>(4, sms);
-    max_cl4 = cached;
-  }
-  if (mc < 0) mc = (max_cl4 > 0 && c_blk * n_pair >= 4 * (int64_t)max_cl4) ? 1 : 0;
-  if (mc && max_cl4 <= 0) mc = 0;
-  int g = mc ? 2 * ((2 * max_cl4) / n_pair) : (2 * (sms / 2)) / n_pair;
-  if (env_group > 0) g = env_group;
-  if (g < 1) g = 1;
-  if (getenv("ZSB_RES_VERBOSE"))
-    fprintf(stderr, "zsb dense_res: multicast %d (%d co-resident clusters of 4), group = %d blocks\n",
-            mc, max_cl4, g);
-  *mc_out = mc;
-  *group_out = g;
-}
-
+// Chain blocks per scheduling group (one group = every chain: the passes run as separate launches)
 int zsb_dense_res_group_blocks(int D) {
-  int mc, g;
-  res_choose(D, 1LL << 30, &mc, &g);
-  return g;
+  (void)D;
+  return 1 << 30;
 }
 
-// One launch = the L+1 passes of a trajectory for every chain (D % 64 == 0, L >= 1).
-//   planes0: fp16 hi/lo planes of q * sq (zsb_hmc_dense_h16_prepare_f32), planes1: work buffer;
-//   on return the proposal's planes are in buffer (L & 1); p0 -> pw (final momentum);
-//   lp0_part / lp1_part / k_part as the per-pass kernel writes them; flags: int32[2*ceil(chains/256)].
-//   planes1 == planes0 selects the IN-PLACE variant (8 instead of 12 bytes of L2 footprint per
-//   element): an epilogue then waits until every dimension tile's MMAs of the pass have read the
-//   block's planes before it overwrites them; the proposal's planes end in planes0.
+// The L+1 passes of a trajectory for every chain (D % 64 == 0, L >= 1).
+//   planes0: fp16 hi/lo planes of q * sq (zsb_hmc_dense_h16_prepare_f32), planes1: work buffer of
+//   the same size (must differ from planes0: a pass reads every dimension of a chain block's planes
+//   while other tiles of the same launch write the next ones); on return the proposal's planes are
+//   in buffer (L & 1); p0 -> pw (final momentum); lp0_part / lp1_part / k_part as the per-pass
+//   kernel writes them.  `flags` is not used.
 int zsb_dense_res_h16_launch(void* planes0, void* planes1, const float* p0, float* pw,
                              const void* P_h16, const void* P_l16, const float* scales,
                              const float* bvec, const float* mu, const float* mass,
                              const float* state, float* lp0_part, float* lp1_part, float* k_part,
                              int* flags, int64_t chains, int D, int L, cudaStream_t st) {
+  (void)flags;
   if (D % 64 != 0 || D < 64 || L < 1 || chains <= 0 || chains >= (1LL << 31)) {
     zsb_set_error("dense_res: needs D %% 64 == 0, n_leapfrogs >= 1");
     return ZSB_ERR_INVALID;
   }
-  ResMaps m;
+  if (planes0 == planes1) {
+    zsb_set_error("dense_res: planes1 must be a separate work buffer");
+    return ZSB_ERR_INVALID;
+  }
+  CUtensorMap phi, plo, qhi[2], qlo[2];
   int rc;
-  int mc = 0, group = 1;
-  res_choose(D, chains, &mc, &group);
-  const uint32_t a_rows = mc ? BM / 2 : BM;
-  if ((rc = make_map(&m.p_hi, P_h16, (uint64_t)D, (uint64_t)D, a_rows, 32, 1))) return rc;
-  if ((rc = make_map(&m.p_lo, P_l16, (uint64_t)D, (uint64_t)D, a_rows, 32, 1))) return rc;
-  const __half* pl[2] = {reinterpret_cast<const __half*>(planes0),
-                         reinterpret_cast<const __half*>(planes1)};
+  if ((rc = make_map(&phi, P_h16, (uint64_t)D, (uint64_t)D, BM, 128, 1))) return rc;
+  if ((rc = make_map(&plo, P_l16, (uint64_t)D, (uint64_t)D, BM, 128, 1))) return rc;
+  __half* pl[2] = {reinterpret_cast<__half*>(planes0), reinterpret_cast<__half*>(planes1)};
+  const int64_t plane = chains * (int64_t)D;
   for (int b = 0; b < 2; ++b) {
-    if ((rc = make_map(&m.q_hi[b], pl[b], (uint64_t)chains, (uint64_t)D, BN / 2, 32, 1)))
-      return rc;
-    if ((rc = make_map(&m.q_lo[b], pl[b] + chains * D, (uint64_t)chains, (uint64_t)D, BN / 2, 32,
-                       1)))
+    if ((rc = make_map(&qhi[b], pl[b], (uint64_t)chains, (uint64_t)D, BN, 128, 1))) return rc;
+    if ((rc = make_map(&qlo[b], pl[b] + plane, (uint64_t)chains, (uint64_t)D, BN, 128, 1)))
       return rc;
   }
-  int dev = 0, sms = ZSB_NUM_SMS;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int n_pair = ((D + BM - 1) / BM + 1) / 2;
-  const int64_t c_blk = (chains + BN - 1) / BN;
-  if (group > c_blk) group = (int)c_blk;
-  static const int env_dbg = getenv("ZSB_RES_DBG") ? atoi(getenv("ZSB_RES_DBG")) : 0;
-  const int inplace = planes0 == planes1 ? 1 : 0;
-  cudaError_t e = cudaMemsetAsync(flags, 0, sizeof(int) * (size_t)c_blk * 2, st);
-  if (e != cudaSuccess) {
-    zsb_set_error("dense_res: cudaMemsetAsync: %s", cudaGetErrorString(e));
-    return ZSB_ERR_CUDA;
+  const int n_blk = (D + BM - 1) / BM;
+  for (int i = 0; i <= L; ++i) {
+    const bool last = i == L;
+    const int buf = i & 1;
+    const ResEpi ea{pl[buf], pl[buf] + plane, pl[buf ^ 1], pl[buf ^ 1] + plane,
+                    i == 0 ? p0 : pw, pw, i == 0 ? lp0_part : lp1_part, k_part, chains, D,
+                    1.f, 1.f, 1.f};
+    const int mode = last ? 2 : (i == 0 ? 1 : 0);
+    const float p_scale = (i > 0 && !last) ? 1.f : 0.5f;
+    rc = (D == 1024) ? res_pass<1024>(phi, plo, qhi[buf], qlo[buf], ea, bvec, mu, mass, state,
+                                      scales, p_scale, n_blk, D, mode, st)
+                     : res_pass<0>(phi, plo, qhi[buf], qlo[buf], ea, bvec, mu, mass, state,
+                                   scales, p_scale, n_blk, D, mode, st);
+    if (rc != ZSB_OK) return rc;
   }
-  const int cl = mc ? 4 : 2;
-  cudaError_t prep = cudaSuccess, le = cudaSuccess;
-  __half* pl0 = reinterpret_cast<__half*>(planes0);
-  __half* pl1 = reinterpret_cast<__half*>(planes1);
-  int Di = D, Li = L, dbg = env_dbg;
-#define ZSB_RES_LAUNCH(DC, MCV)                                                                 \
-  do {                                                                                          \
-    prep = res_prepare<DC, MCV>();                                                              \
-    if (prep != cudaSuccess) break;                                                             \
-    static const int max_cl = res_max_clusters<DC, MCV>(cl, sms);                               \
-    int64_t clusters = max_cl;                                                                  \
-    const int64_t units = MCV ? (int64_t)((group + 1) / 2) * n_pair : (int64_t)group * n_pair;  \
-    if (units < clusters) clusters = units;                                                     \
-    cudaLaunchConfig_t cfg = {};                                                                \
-    cfg.gridDim = dim3((unsigned)(cl * clusters));                                              \
-    cfg.blockDim = dim3(NUM_THREADS);                                                           \
-    cfg.dynamicSmemBytes = CR::SMEM;                                                            \
-    cfg.stream = st;                                                                            \
-    cudaLaunchAttribute at[1];                                                                  \
-    at[0].id = cudaLaunchAttributeClusterDimension;                                             \
-    at[0].val.clusterDim.x = (unsigned)cl; at[0].val.clusterDim.y = 1;                          \
-    at[0].val.clusterDim.z = 1;                                                                 \
-    cfg.attrs = at; cfg.numAttrs = 1;                                                           \
-    le = cudaLaunchKernelEx(&cfg, dense_res_kernel<DC, MCV>, m, pl0, pl1, p0, pw, bvec, mu,     \
-                            mass, state, lp0_part, lp1_part, k_part, chains, Di, Li, scales,    \
-                            flags, group, dbg, inplace);                                        \
-  } while (0)
-  if (mc) { if (D == 1024) ZSB_RES_LAUNCH(1024, 1); else ZSB_RES_LAUNCH(0, 1); }
-  else { if (D == 1024) ZSB_RES_LAUNCH(1024, 0); else ZSB_RES_LAUNCH(0, 0); }
-#undef ZSB_RES_LAUNCH
-  if (prep != cudaSuccess || le != cudaSuccess) {
-    zsb_set_error("dense_res: launch setup: %s",
-                  cudaGetErrorString(prep != cudaSuccess ? prep : le));
-    return ZSB_ERR_CUDA;
-  }
-  return zsb_check_launch("hmc_dense_resident");
+  return ZSB_OK;
 }
 
 int zsb_dense_select_planes_launch(float* q, const void* planes, const float* scales,

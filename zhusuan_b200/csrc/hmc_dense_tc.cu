@@ -4,401 +4,135 @@
 // hamiltonian(), hmc.py:30-35, which get_acceptance_rate (hmc.py:46-61) would otherwise
 // recompute with two extra forward evaluations.
 //
-// Dense-Gaussian leapfrog pass on 5th-gen tensor cores (impl 1): tcgen05.mma kind::tf32 with a
-// 3xTF32 split so the fp32 gradient  g = b - P q  keeps ~fp32 accuracy:
-//     q = q_hi + q_lo,  P = P_hi + P_lo   (hi = top 19 bits, exactly what the TF32 datapath reads)
-//     P q ~= P_hi q_hi + P_hi q_lo + P_lo q_hi          (dropped term ~2^-22 relative)
-// accumulated in fp32 in TMEM.  Same fused leapfrog epilogue as the SIMT kernel (hmc_dense.cu).
-//
+// Dense-Gaussian leapfrog pass on the Hopper tensor cores (wgmma, tc_pipeline_kernel of
+// tc_common.cuh) with a three-product split so the fp32 gradient  g = b - P q  keeps ~fp32 accuracy:
+//   impl 1  TF32 operands:  q = q_hi + q_lo,  P = P_hi + P_lo  (hi = top 19 bits, what the TF32
+//           datapath reads);  P q ~= P_hi q_hi + P_hi q_lo + P_lo q_hi  (dropped term ~2^-22)
+//   impl 2  fp16 operands:  hi / lo planes of P*sP and q*sq (powers of two), three fp16 products at
+//           twice the TF32 rate; the pass writes the planes of q_next for the next pass
+//   impl 3  as impl 2, but the MMA warpgroup builds the planes of q from the fp32 rows itself
+//           (no plane buffers in HBM); sq comes from the running max|q| the previous pass left
 // The GEMM is computed TRANSPOSED, G^T[n, c] = sum_k P[n, k] q[c, k]  (A = P rows, B = chain rows,
-// both K-major), so that in TMEM a lane is a dimension n and a column is a chain c: an epilogue
-// warp then touches 32 consecutive dimensions of ONE chain per instruction -- a full 128-byte line
-// of p / q / q_next -- instead of 32 chains 4 KB apart.
-//
-// Structure (one persistent CTA per SM, 320 threads, warp-specialised):
-//   warp 0      TMA producer: cp.async.bulk.tensor swizzled tiles of P_hi, P_lo (128 x BK) and
-//               q (=q_hi), q_lo (256 x BK) into a STAGES-deep shared-memory ring (192 KB total),
-//               mbarrier complete_tx signalling
-//   warp 1      MMA issuer: one elected lane issues 3 tcgen05.mma (128x256x8) per k-step;
-//               tcgen05.commit frees the smem slot / publishes the accumulator
-//   warps 2-9   epilogue: tcgen05.ld (32x32b.x16) the fp32 accumulator, p += s2*g,
-//               q_next = q + eps*p/m, q_next_lo, warp-transpose reductions of lp and K -> HBM
-//   TMEM        2 x 256 columns: accumulator double buffer (epilogue of tile i overlaps MMA of i+1)
-// Tiles (128 dims x 256 chains) are assigned round-robin with the dimension block fastest, so the
-// CTAs running concurrently share their chain rows and the whole (8 MB hi+lo) P through the L2.
+// both K-major), so an accumulator row is a dimension n and a column a chain c: an epilogue warp
+// then touches 32 consecutive dimensions of ONE chain per instruction -- a full 128-byte line of
+// p / q / q_next -- instead of 32 chains 4 KB apart.  Tiles (128 dims x 128 chains) are assigned
+// round-robin with the dimension block fastest, so the CTAs running concurrently share their chain
+// rows and P through the L2.
 #include "hmc_dense_epilogue.cuh"
 
 namespace {
 
-template <int BK, int MODE>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-dense_leapfrog_tc_kernel(const __grid_constant__ CUtensorMap map_phi,
-                         const __grid_constant__ CUtensorMap map_plo,
-                         const __grid_constant__ CUtensorMap map_qhi,
-                         const __grid_constant__ CUtensorMap map_qlo,
-                         const float* __restrict__ q_cur, float* __restrict__ q_next,
-                         float* __restrict__ q_next_lo, const float* __restrict__ p_in,
-                         float* __restrict__ p_out, const float* __restrict__ bvec,
-                         const float* __restrict__ mu, const float* __restrict__ mass,
-                         const float* __restrict__ state, float p_scale,
-                         float* __restrict__ lp_part, float* __restrict__ k_part, int64_t chains,
-                         int D, int dbg) {
-  // dbg (timing experiments only, results are then WRONG): bit0 skip epilogue global traffic,
-  // bit1 issue only the hi*hi MMA, bit2 skip the TMA loads of the lo tiles, bit3 enable L2 prefetch (measured slower: the kernel is L2-bandwidth bound).
-  using C = Cfg<BK>;
-  extern __shared__ uint8_t smem_raw[];
-  // 1024-B alignment required by the swizzle atoms
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bars = smem_base + C::STAGES * C::STAGE;
-  const uint32_t full_bar = bars;                          // [STAGES]
-  const uint32_t empty_bar = bars + 8 * C::STAGES;         // [STAGES]
-  const uint32_t tfull_bar = bars + 16 * C::STAGES;        // [2]
-  const uint32_t tempty_bar = bars + 16 * C::STAGES + 16;  // [2]
-  const uint32_t tmem_slot = bars + 16 * C::STAGES + 32;   // u32
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(
-      smem_raw + (tmem_slot - smem_u32(smem_raw)));
+// OP 0: TF32 (impl 1), 1: fp16 planes (impl 2).  H16: epilogue flavour (0 TF32 residual, 1 fp16
+// planes, 2 in-kernel split: q_next fp32 + running max|q_next|).  RB_: smem row bytes.
+template <int OP, int RB_, int MODE, int DC, int H16>
+struct DenseW {
+  static constexpr int KIND = OP, RB = RB_, MNA = 0, MNB = 0, CVT = (H16 == 2);
+  static constexpr int KE = OP ? RB / 2 : RB / 4;          // contraction elements per k-block
+  static constexpr uint32_t TX = CVT ? 2 * Cfg<RB>::A_TILE : Cfg<RB>::STAGE;
+  CUtensorMap m_phi, m_plo, m_qhi, m_qlo;
+  EpiArgs ea;
+  const float* bvec; const float* mu; const float* mass; const float* state;
+  float* scales;                                           // OP 1: {sq, 1/(sP sq), -, sP, slots}
+  float p_scale;
+  int n_blk, D_rt, pass_index;
+  struct EpiState { float amax = 0.f; };
 
-  // broadcast so the compiler knows the role branches are warp-uniform (uniform datapath usable)
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  const int lane = threadIdx.x & 31;
-  const int n_blk = (D + BM - 1) / BM;                     // dimension blocks
-  const int64_t c_blk = (chains + BN - 1) / BN;            // chain blocks
-  const int64_t n_tiles = c_blk * n_blk;
-  const int n_kb = D / BK;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < C::STAGES; ++s) {
-      mbar_init(full_bar + 8 * s, 1);
-      mbar_init(empty_bar + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar + 8 * a, 1);
-      mbar_init(tempty_bar + 8 * a, 32 * NUM_EPI_WARPS);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  __device__ __forceinline__ int D() const { return DC ? DC : D_rt; }
+  __host__ __device__ __forceinline__ int64_t units() const {
+    return ((ea.chains + BN - 1) / BN) * (int64_t)n_blk;
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                 ::"r"(tmem_slot), "n"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+  __device__ __forceinline__ void kb_range(int64_t, int& kb0, int& kb1) const {
+    kb0 = 0;
+    kb1 = D() / KE;
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_phi) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_plo) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_qhi) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_qlo) : "memory");
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-        const int n0 = (int)(t % n_blk) * BM;
-        const int c0 = (int)((t / n_blk) * BN);
-        // L2 prefetch of the chain block this CTA needs NEXT (one CTA of the n_blk that share
-        // the block issues it), so those first-touch DRAM misses are off the TMA critical path.
-        const int64_t tn = t + gridDim.x;
-        const bool do_pf = (dbg & 8) && tn < n_tiles && (tn % n_blk) == 0;   // opt-in: measured slower
-        const int c0n = (int)((tn / n_blk) * BN);
-        for (int kb = 0; kb < n_kb; ++kb) {
-          if (do_pf) {
-            tma_prefetch_l2_2d(&map_qhi, kb * BK, c0n);
-            tma_prefetch_l2_2d(&map_qlo, kb * BK, c0n);
-          }
-          mbar_wait(empty_bar + 8 * stage, phase ^ 1);
-          const uint32_t fb = full_bar + 8 * stage;
-          const uint32_t sa = smem_base + stage * C::STAGE;
-          mbar_expect_tx(fb, (dbg & 4) ? C::STAGE / 2 : C::STAGE);
-          tma_load_2d(sa, &map_phi, fb, kb * BK, n0);
-          if (!(dbg & 4)) tma_load_2d(sa + C::A_TILE, &map_plo, fb, kb * BK, n0);
-          tma_load_2d(sa + 2 * C::A_TILE, &map_qhi, fb, kb * BK, c0);
-          if (!(dbg & 4)) tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE, &map_qlo, fb, kb * BK, c0);
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
+  __device__ __forceinline__ void prefetch() const {
+    tma_prefetch_desc(&m_phi);
+    tma_prefetch_desc(&m_plo);
+    if (!CVT) { tma_prefetch_desc(&m_qhi); tma_prefetch_desc(&m_qlo); }
+  }
+  __device__ __forceinline__ void load(int64_t u, int kb, uint32_t sa, uint32_t fb) const {
+    using C = Cfg<RB>;
+    const int n0 = (int)(u % n_blk) * BM;
+    const int c0 = (int)(u / n_blk) * BN;
+    tma_load_2d(sa, &m_phi, fb, kb * KE, n0);
+    tma_load_2d(sa + C::A_TILE, &m_plo, fb, kb * KE, n0);
+    if (!CVT) {
+      tma_load_2d(sa + 2 * C::A_TILE, &m_qhi, fb, kb * KE, c0);
+      tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE, &m_qlo, fb, kb * KE, c0);
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc();
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-        mbar_wait(tempty_bar + 8 * acc, acc_phase ^ 1);   // epilogue drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = 0; kb < n_kb; ++kb) {
-          mbar_wait(full_bar + 8 * stage, phase);         // TMA bytes have landed
-          tc_fence_after();
-          const uint32_t sa = smem_base + stage * C::STAGE;
-          const uint64_t a_hi = make_smem_desc<BK>(sa);
-          const uint64_t a_lo = make_smem_desc<BK>(sa + C::A_TILE);
-          const uint64_t b_hi = make_smem_desc<BK>(sa + 2 * C::A_TILE);
-          const uint64_t b_lo = make_smem_desc<BK>(sa + 2 * C::A_TILE + C::B_TILE);
+  }
+  // impl 3: scale of this pass's q from the running-max slot the previous pass (or prepare) filled
+  __device__ __forceinline__ float sq3() const {
+    const unsigned int* slots = reinterpret_cast<const unsigned int*>(scales) + 4;
+    const float qmax = __uint_as_float(slots[pass_index % 3]);
+    int qe = 0;
+    if (qmax > 0.f) frexpf(qmax, &qe);
+    return ldexpf(1.f, 12 - qe);                          // max|q| * sq in [2^11, 2^12)
+  }
+  // impl 3: thread `tid` converts chain c0 + tid, contraction kb*KE .. +KE, into the B planes in
+  // the SWIZZLE_128B K-major layout (16-byte chunk index XOR row % 8)
+  __device__ __forceinline__ void convert(int64_t u, int kb, uint8_t* stage, int tid) const {
+    if (!CVT) return;
+    using C = Cfg<RB>;
+    static_assert(!CVT || RB == 128, "in-kernel split uses 128-byte rows");
+    const float sq = sq3();
+    const int64_t c = (u / n_blk) * BN + tid;
+    const bool ok = c < ea.chains;
+    const float4* src = reinterpret_cast<const float4*>(ea.q_cur + (ok ? c : 0) * (int64_t)D() +
+                                                        (int64_t)kb * KE);
+    uint8_t* hi = stage + 2 * C::A_TILE + tid * RB;
+    uint8_t* lo = hi + C::B_TILE;
 #pragma unroll
-          for (int k = 0; k < BK / 8; ++k) {
-            const uint64_t ko = (uint64_t)((k * 8 * 4) >> 4);   // +32 B along K per UMMA_K=8
-            // small cross terms first, hi*hi last
-            if (dbg & 2) {
-              umma_tf32(d_tmem, a_hi + ko, b_hi + ko, idesc, (kb | k) != 0 ? 1u : 0u);
-            } else {
-              umma_tf32(d_tmem, a_lo + ko, b_hi + ko, idesc, (kb | k) != 0 ? 1u : 0u);
-              umma_tf32(d_tmem, a_hi + ko, b_lo + ko, idesc, 1u);
-              umma_tf32(d_tmem, a_hi + ko, b_hi + ko, idesc, 1u);
-            }
-          }
-          umma_commit(empty_bar + 8 * stage);             // frees the smem slot when MMAs retire
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(tfull_bar + 8 * acc);                 // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+    for (int ch = 0; ch < RB / 16; ++ch) {                 // 8 halves per 16-byte chunk
+      const float4 a = ok ? __ldg(src + 2 * ch) : make_float4(0.f, 0.f, 0.f, 0.f);
+      const float4 b = ok ? __ldg(src + 2 * ch + 1) : make_float4(0.f, 0.f, 0.f, 0.f);
+      const float x[8] = {a.x * sq, a.y * sq, a.z * sq, a.w * sq,
+                          b.x * sq, b.y * sq, b.z * sq, b.w * sq};
+      uint32_t h[4], l[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const __half2 h2 = __floats2half2_rn(x[2 * i], x[2 * i + 1]);
+        const float2 hf = __half22float2(h2);
+        const __half2 l2 = __floats2half2_rn(x[2 * i] - hf.x, x[2 * i + 1] - hf.y);
+        h[i] = *reinterpret_cast<const uint32_t*>(&h2);
+        l[i] = *reinterpret_cast<const uint32_t*>(&l2);
       }
+      const int off = ((ch ^ (tid & 7)) << 4);
+      *reinterpret_cast<uint4*>(hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
+      *reinterpret_cast<uint4*>(lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
     }
-  } else {
-    // ===================== epilogue (warps 2..9) =====================
-    // Warp w may read TMEM lanes [32*(w%4), +32).  Two warps share each lane quarter and split
-    // the tile's 256 chain columns in halves, so every scheduler has two epilogue warps to
-    // overlap the global-load latency of one with the arithmetic of the other.
-    const int quarter = warp & 3;
-    const int half = (warp - 2) >> 2;
+  }
+  __device__ __forceinline__ void epilogue(int64_t u, uint32_t trow, int quarter, int lane,
+                                           EpiState& st) const {
+    const int nb = (int)(u % n_blk);
+    const int n = nb * BM + quarter * 32 + lane;          // this thread's dimension
+    const int64_t c0 = (u / n_blk) * BN;
+    const int Dv = D();
+    const bool n_ok = n < Dv;
     const float eps = state[ZSB_ST_EPS_USED];
     const float s2 = mul(eps, p_scale);
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-      const int nb = (int)(t % n_blk);
-      const int n = nb * BM + quarter * 32 + lane;          // this thread's dimension
-      const int64_t c0 = (t / n_blk) * BN + half * (BN / 2);  // first chain of this warp's half
-      const bool n_ok = n < D;
-      const float m_n = n_ok ? mass[n] : 1.f;
-      const float eps_over_m = fdiv(eps, m_n);              // q += eps * (p / m) as p * (eps / m)
-      const float inv_m = fdiv(1.f, m_n);
-      const float b_n = (n_ok && bvec) ? bvec[n] : 0.f;
-      const float mu_n = (n_ok && mu) ? mu[n] : 0.f;
-      mbar_wait(tfull_bar + 8 * acc, acc_phase);
-      tc_fence_after();
-      const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16) +
-                            (uint32_t)(acc * BN + half * (BN / 2));
-      const int64_t part_row = (int64_t)(nb * 4 + quarter) * chains;
-      const EpiArgs ea{q_cur, q_next, q_next_lo, p_in, p_out, lp_part, k_part, chains, D,
-                       0, 1.f, 1.f};
-      float unused_amax = 0.f;
-      epilogue_half_tile<MODE, -1, 0, 0>(ea, trow, n, n_ok, true, c0, part_row, lane, s2,
-                                         eps_over_m, inv_m, b_n, mu_n, (dbg & 1) != 0,
-                                         unused_amax);
-      tc_fence_before();
-      mbar_arrive(tempty_bar + 8 * acc);               // all epilogue threads free the accumulator
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
+    const float m_n = n_ok ? mass[n] : 1.f;
+    const float eps_over_m = fdiv(eps, m_n);              // q += eps * (p / m) as p * (eps / m)
+    const float inv_m = fdiv(1.f, m_n);
+    const float b_n = (n_ok && bvec) ? bvec[n] : 0.f;
+    const float mu_n = (n_ok && mu) ? mu[n] : 0.f;
+    const int64_t part_row = (int64_t)(nb * 4 + quarter) * ea.chains;
+    EpiArgs a = ea;
+    if (H16 == 1) { a.q_scale = scales[0]; a.acc_scale = scales[1]; }
+    if (H16 == 2) a.acc_scale = 1.f / (scales[3] * sq3());   // powers of two: exact
+    epilogue_half_tile<MODE, -1, DC, H16>(a, trow, n, n_ok, true, c0, part_row, lane, s2,
+                                          eps_over_m, inv_m, b_n, mu_n, false, st.amax);
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;"
-                 ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
-  }
-}
-
-// =================================================================================================
-// cta_group::2 variant: a CTA PAIR (cluster of 2) computes a 256-dim x 256-chain tile with ONE
-// tcgen05.mma.cta_group::2 (M=256) per k-step, issued by the leader CTA.  Each CTA stages only
-// its own 128 dimension rows of P and HALF (128) of the tile's chain rows, so the operand bytes
-// per MAC pulled through the L2 drop by a third (the measured limiter of the 1-CTA kernel), and
-// the tensor core reads the shared chain operand from both CTAs' shared memory.
-//   full[s]   (leader only)  1 arrival (leader's expect_tx) + bytes of BOTH CTAs' TMA loads
-//   empty[s]  (each CTA)     1 arrival: leader's tcgen05.commit multicast to both CTAs
-//   tfull[a]  (each CTA)     1 arrival: leader's commit multicast (accumulator ready)
-//   tempty[a] (leader only)  2 x 256 arrivals: both CTAs' epilogue threads (peer arrives remotely)
-// Accumulator rows 0-127 (dimension block 2i) live in the leader's TMEM, rows 128-255 (block
-// 2i+1) in the peer's; the epilogue is the same as the 1-CTA kernel's.
-// OP 0: TF32 operands (fp32 words, 3xTF32 split).  OP 1: fp16 operands (impl 2): the operand
-// tiles hold (P*sP) and (q*sq) split as hi + lo halves, 2*BK elements per 128/64-byte row, three
-// kind::f16 MMAs per 16-element k-step; `scales` = {sq, 1/(sP*sq)} in device memory.
-template <int BK, int MODE, int OP, int NEXT, int DC>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS, 1)
-dense_leapfrog_tc2_kernel(const __grid_constant__ CUtensorMap map_phi,
-                          const __grid_constant__ CUtensorMap map_plo,
-                          const __grid_constant__ CUtensorMap map_qhi,
-                          const __grid_constant__ CUtensorMap map_qlo,
-                          const float* __restrict__ q_cur, float* __restrict__ q_next,
-                          float* __restrict__ q_next_lo, const float* __restrict__ p_in,
-                          float* __restrict__ p_out, const float* __restrict__ bvec,
-                          const float* __restrict__ mu, const float* __restrict__ mass,
-                          const float* __restrict__ state, float p_scale,
-                          float* __restrict__ lp_part, float* __restrict__ k_part, int64_t chains,
-                          int D_rt, int dbg, const float* __restrict__ scales) {
-  using C = Cfg2<BK>;
-  const int D = DC ? DC : D_rt;
-  constexpr int KELEMS = OP ? 2 * BK : BK;                 // operand elements per smem row
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bars = smem_base + C::STAGES * C::STAGE;
-  const uint32_t full_bar = bars;                          // [STAGES]
-  const uint32_t empty_bar = bars + 8 * C::STAGES;         // [STAGES]
-  const uint32_t tfull_bar = bars + 16 * C::STAGES;        // [2]
-  const uint32_t tempty_bar = bars + 16 * C::STAGES + 16;  // [2]
-  const uint32_t tmem_slot = bars + 16 * C::STAGES + 32;   // u32
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(
-      smem_raw + (tmem_slot - smem_u32(smem_raw)));
-
-  // broadcast so the compiler knows the role branches are warp-uniform (uniform datapath usable)
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();                 // 0 = leader
-  const bool leader = rank == 0;
-  const int n_blk = (D + BM - 1) / BM;
-  const int n_pair = (n_blk + 1) / 2;                      // dimension-block pairs
-  const int64_t c_blk = (chains + BN - 1) / BN;
-  const int64_t n_units = c_blk * n_pair;                  // work units of the cluster
-  const int64_t unit0 = blockIdx.x >> 1, unit_step = gridDim.x >> 1;
-  const int n_kb = D / KELEMS;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < C::STAGES; ++s) {
-      mbar_init(full_bar + 8 * s, 1);
-      mbar_init(empty_bar + 8 * s, 1);
+  __device__ __forceinline__ void epi_finish(EpiState& st, int quarter, int lane) const {
+    if (H16 != 2) return;
+    unsigned int* slots = reinterpret_cast<unsigned int*>(scales) + 4;
+    if (ea.q_next) {
+      const float m = warp_max(st.amax);
+      if (lane == 0) atomicMax(slots + (pass_index + 1) % 3, __float_as_uint(m));
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar + 8 * a, 1);
-      mbar_init(tempty_bar + 8 * a, 2 * 32 * NUM_EPI_WARPS);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    if (blockIdx.x == 0 && quarter == 0 && lane == 0) slots[(pass_index + 2) % 3] = 0u;
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;"
-                 ::"r"(tmem_slot), "n"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();            // barrier inits + TMEM allocation visible to both CTAs
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    if (lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_phi) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_plo) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_qhi) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_qlo) : "memory");
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int64_t u = unit0; u < n_units; u += unit_step) {
-        const int n0 = ((int)(u % n_pair) * 2 + (int)rank) * BM;     // own dimension block
-        const int c0 = (int)((u / n_pair) * BN) + (int)rank * (BN / 2);  // own chain half
-        for (int kb = 0; kb < n_kb; ++kb) {
-          mbar_wait(empty_bar + 8 * stage, phase ^ 1);    // own slot free (leader's commit)
-          const uint32_t fb = full_bar + 8 * stage;
-          const uint32_t sa = smem_base + stage * C::STAGE;
-          if (leader) mbar_expect_tx(fb, 2 * C::STAGE);   // bytes of both CTAs
-          tma_load_2d_2sm(sa, &map_phi, fb, kb * KELEMS, n0);
-          tma_load_2d_2sm(sa + C::A_TILE, &map_plo, fb, kb * KELEMS, n0);
-          tma_load_2d_2sm(sa + 2 * C::A_TILE, &map_qhi, fb, kb * KELEMS, c0);
-          tma_load_2d_2sm(sa + 2 * C::A_TILE + C::B_TILE, &map_qlo, fb, kb * KELEMS, c0);
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (leader && lane == 0) {
-      const uint32_t idesc = OP ? make_idesc_2sm_f16() : make_idesc_2sm();
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int64_t u = unit0; u < n_units; u += unit_step) {
-        mbar_wait(tempty_bar + 8 * acc, acc_phase ^ 1);   // both epilogues drained this buffer
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = 0; kb < n_kb; ++kb) {
-          mbar_wait(full_bar + 8 * stage, phase);         // both CTAs' TMA bytes have landed
-          tc_fence_after();
-          const uint32_t sa = smem_base + stage * C::STAGE;
-          const uint64_t a_hi = make_smem_desc<BK>(sa);
-          const uint64_t a_lo = make_smem_desc<BK>(sa + C::A_TILE);
-          const uint64_t b_hi = make_smem_desc<BK>(sa + 2 * C::A_TILE);
-          const uint64_t b_lo = make_smem_desc<BK>(sa + 2 * C::A_TILE + C::B_TILE);
-#pragma unroll
-          for (int k = 0; k < BK / 8; ++k) {
-            const uint64_t ko = (uint64_t)((k * 8 * 4) >> 4);
-            const uint32_t first = (kb | k) != 0 ? 1u : 0u;
-            if (OP && (dbg & 2)) {  // timing experiment: one product instead of three
-              umma_f16_2sm(d_tmem, a_hi + ko, b_hi + ko, idesc, first);
-            } else if (OP) {        // 32 B per k-step either way: 16 halves or 8 TF32 words
-              umma_f16_2sm(d_tmem, a_lo + ko, b_hi + ko, idesc, first);
-              umma_f16_2sm(d_tmem, a_hi + ko, b_lo + ko, idesc, 1u);
-              umma_f16_2sm(d_tmem, a_hi + ko, b_hi + ko, idesc, 1u);
-            } else if (dbg & 2) {
-              umma_tf32_2sm(d_tmem, a_hi + ko, b_hi + ko, idesc, first);
-            } else {
-              umma_tf32_2sm(d_tmem, a_lo + ko, b_hi + ko, idesc, first);
-              umma_tf32_2sm(d_tmem, a_hi + ko, b_lo + ko, idesc, 1u);
-              umma_tf32_2sm(d_tmem, a_hi + ko, b_hi + ko, idesc, 1u);
-            }
-          }
-          umma_commit_2sm(empty_bar + 8 * stage);         // frees the slot in both CTAs
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit_2sm(tfull_bar + 8 * acc);             // accumulators ready in both CTAs
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 2..9, both CTAs) =====================
-    const int quarter = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const float eps = state[ZSB_ST_EPS_USED];
-    const float s2 = mul(eps, p_scale);
-    const float q_scale = OP ? scales[0] : 1.f;
-    const float acc_scale = OP ? scales[1] : 1.f;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int64_t u = unit0; u < n_units; u += unit_step) {
-      const int nb = (int)(u % n_pair) * 2 + (int)rank;
-      const int n = nb * BM + quarter * 32 + lane;
-      const int64_t c0 = (u / n_pair) * BN + half * (BN / 2);
-      const bool n_ok = n < D;
-      const float m_n = n_ok ? mass[n] : 1.f;
-      const float eps_over_m = fdiv(eps, m_n);
-      const float inv_m = fdiv(1.f, m_n);
-      const float b_n = (n_ok && bvec) ? bvec[n] : 0.f;
-      const float mu_n = (n_ok && mu) ? mu[n] : 0.f;
-      mbar_wait(tfull_bar + 8 * acc, acc_phase);
-      tc_fence_after();
-      const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16) +
-                            (uint32_t)(acc * BN + half * (BN / 2));
-      const int64_t part_row = (int64_t)(nb * 4 + quarter) * chains;
-      const EpiArgs ea{q_cur, q_next, q_next_lo, p_in, p_out, lp_part, k_part, chains, D,
-                       OP, q_scale, acc_scale};
-      float unused_amax = 0.f;
-      epilogue_half_tile<MODE, NEXT, DC, OP>(ea, trow, n, n_ok, nb < n_blk, c0, part_row, lane,
-                                             s2, eps_over_m, inv_m, b_n, mu_n, (dbg & 1) != 0,
-                                             unused_amax);
-      tc_fence_before();
-      if (leader) mbar_arrive(tempty_bar + 8 * acc);
-      else mbar_arrive_remote(tempty_bar + 8 * acc, 0);   // leader's barrier counts both CTAs
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();            // nobody exits / frees TMEM while the peer may still use it
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;"
-                 ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
-  }
-}
+};
 
 // q_lo = q - (q with the low 13 mantissa bits cleared): the residual the TF32 datapath drops.
 __global__ void __launch_bounds__(256) split_lo_kernel(const float* __restrict__ q,
@@ -453,394 +187,6 @@ __global__ void __launch_bounds__(256) split16_kernel(const float* __restrict__ 
   }
 }
 
-int g_tc_pair = 0;  // 1: cta_group::2 CTA-pair kernel
-int g_tc_bk = 32;
-int g_tc_dbg = 0;  // timing experiments only (see kernel)   // pipeline shape: 32 -> 2 stages x 96 KB (SW128), 16 -> 4 x 48 KB (SW64)
-
-template <int BK>
-int launch_tc(const float* q_cur, const float* q_cur_lo, float* q_next, float* q_next_lo,
-              const float* p_in, float* p_out, const float* P_hi, const float* P_lo,
-              const float* bvec, const float* mu, const float* mass, const float* state,
-              float p_scale, float* lp_part, float* k_part, int64_t chains, int D,
-              cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(dense_leapfrog_tc_kernel<BK, 0>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg<BK>::SMEM);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(dense_leapfrog_tc_kernel<BK, 1>,
-                               cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BK>::SMEM);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(dense_leapfrog_tc_kernel<BK, 2>,
-                               cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BK>::SMEM);
-    if (e != cudaSuccess) {
-      zsb_set_error("dense_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-      return ZSB_ERR_CUDA;
-    }
-    attr_set = true;
-  }
-  if (k_part && !lp_part) {
-    zsb_set_error("dense_tc: k_part requires lp_part");
-    return ZSB_ERR_INVALID;
-  }
-  CUtensorMap m_phi, m_plo, m_qhi, m_qlo;
-  int rc;
-  if ((rc = make_map(&m_phi, P_hi, (uint64_t)D, (uint64_t)D, BM, BK))) return rc;
-  if ((rc = make_map(&m_plo, P_lo, (uint64_t)D, (uint64_t)D, BM, BK))) return rc;
-  if ((rc = make_map(&m_qhi, q_cur, (uint64_t)chains, (uint64_t)D, BN, BK))) return rc;
-  if ((rc = make_map(&m_qlo, q_cur_lo, (uint64_t)chains, (uint64_t)D, BN, BK))) return rc;
-  const int64_t n_tiles = ((chains + BN - 1) / BN) * ((D + BM - 1) / BM);
-  int dev = 0, sms = ZSB_NUM_SMS;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const unsigned grid = (unsigned)(n_tiles < sms ? n_tiles : sms);
-#define ZSB_TC_LAUNCH(MODE)                                                                  \
-  dense_leapfrog_tc_kernel<BK, MODE><<<grid, NUM_THREADS, Cfg<BK>::SMEM, st>>>(                \
-      m_phi, m_plo, m_qhi, m_qlo, q_cur, q_next, q_next_lo, p_in, p_out, bvec, mu, mass, state, \
-      p_scale, lp_part, k_part, chains, D, g_tc_dbg)
-  if (k_part) ZSB_TC_LAUNCH(2);
-  else if (lp_part) ZSB_TC_LAUNCH(1);
-  else ZSB_TC_LAUNCH(0);
-#undef ZSB_TC_LAUNCH
-  return zsb_check_launch("hmc_dense_leapfrog_tc");
-}
-
-// ------------------------------------------------------------------------------------------------
-// impl 3: the fp16 hi/lo planes of q are produced INSIDE the kernel.  HBM traffic per launch drops
-// from 24*D to the algorithmic 16*D bytes per chain (read q, p; write q_next, p_out): the planes of
-// q_next are no longer written by one pass and read back by the next.
-//
-//   warp 0        TMA producer of the P planes (as the pair kernel)          -> a_full  (leader)
-//   warp 1        MMA issuer (leader): waits a_full + cvt_full               -> op_empty (both CTAs)
-//   warp 2        TMA producer of the fp32 q tile [128 chains x 64] (unswizzled staging ring,
-//                 3 deep: this is the HBM stream)                            -> raw_full (local)
-//   warps 3-6     converters: q * sq -> fp16 hi + lo, written in the SWIZZLE_128B K-major operand
-//                 layout (16-byte chunk index XOR row % 8); fence.proxy.async -> cvt_full (leader,
-//                 remote arrive from the peer), raw_empty (local)
-//   warps 7-14    epilogue (as the pair kernel, without the plane stores); tracks max|q_next|
-// The scale sq of a pass is derived from max|q_cur|, which the PREVIOUS pass's epilogue left in
-// one of three rotating device slots (pass k reads slot k%3, accumulates max|q_next| into slot
-// (k+1)%3 and clears slot (k+2)%3); zsb_hmc_dense_h16i_prepare_f32 seeds slot 0 from q itself.
-struct Cfg3 {
-  static constexpr int A_TILE = BM * 128;                    // 128 rows x 64 halves
-  static constexpr int B_TILE = (BN / 2) * 128;
-  static constexpr int OP_STAGE = 2 * A_TILE + 2 * B_TILE;   // 64 KB
-  static constexpr int OP_STAGES = 2;
-  static constexpr int RAW_STAGE = (BN / 2) * 64 * 4;        // 32 KB: 128 chains x 64 fp32
-  static constexpr int RAW_STAGES = 3;
-  static constexpr int BARS = OP_STAGES * OP_STAGE + RAW_STAGES * RAW_STAGE;   // 224 KB
-  static constexpr int SMEM = BARS + 256 + 1024;
-  static constexpr int CVT_WARPS = 4;
-  static constexpr int EPI_WARP0 = 3 + CVT_WARPS;            // first epilogue warp
-  static constexpr int THREADS = 32 * (EPI_WARP0 + NUM_EPI_WARPS);   // 480
-};
-
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(bar), "r"(cta) : "memory");
-}
-
-template <int MODE, int NEXT, int DC>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(Cfg3::THREADS, 1)
-dense_leapfrog_tc3_kernel(const __grid_constant__ CUtensorMap map_phi,
-                          const __grid_constant__ CUtensorMap map_plo,
-                          const __grid_constant__ CUtensorMap map_q32,
-                          const float* __restrict__ q_cur, float* __restrict__ q_next,
-                          const float* __restrict__ p_in, float* __restrict__ p_out,
-                          const float* __restrict__ bvec, const float* __restrict__ mu,
-                          const float* __restrict__ mass, const float* __restrict__ state,
-                          float p_scale, float* __restrict__ lp_part, float* __restrict__ k_part,
-                          int64_t chains, int D_rt, float* __restrict__ scales, int pass_index) {
-  using C = Cfg3;
-  const int D = DC ? DC : D_rt;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t raw_base = smem_base + C::OP_STAGES * C::OP_STAGE;
-  const uint32_t bars = smem_base + C::BARS;
-  const uint32_t a_full = bars;               // [2]  leader: bytes of both CTAs' P tiles
-  const uint32_t op_empty = bars + 16;        // [2]  each CTA: MMA commit (multicast)
-  const uint32_t raw_full = bars + 32;        // [3]  local: fp32 q tile landed
-  const uint32_t raw_empty = bars + 56;       // [3]  local: converters done with the tile
-  const uint32_t cvt_full = bars + 80;        // [2]  leader: both CTAs' planes written
-  const uint32_t tfull_bar = bars + 96;       // [2]
-  const uint32_t tempty_bar = bars + 112;     // [2]
-  const uint32_t tmem_slot = bars + 128;
-  uint32_t* tmem_slot_ptr =
-      reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int n_blk = (D + BM - 1) / BM;
-  const int n_pair = (n_blk + 1) / 2;
-  const int64_t c_blk = (chains + BN - 1) / BN;
-  const int64_t n_units = c_blk * n_pair;
-  const int64_t unit0 = blockIdx.x >> 1, unit_step = gridDim.x >> 1;
-  const int n_kb = D / 64;
-
-  // scale of this pass's q_cur from the running-max slot the previous pass (or prepare) filled
-  unsigned int* slots = reinterpret_cast<unsigned int*>(scales) + 4;      // scales[4..6]
-  const float qmax = __uint_as_float(slots[pass_index % 3]);
-  int qe = 0;
-  if (qmax > 0.f) frexpf(qmax, &qe);
-  const float sq = ldexpf(1.f, 12 - qe);                                 // max|q| * sq in [2^11, 2^12)
-  if (blockIdx.x == 0 && threadIdx.x == 0) slots[(pass_index + 2) % 3] = 0u;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < C::OP_STAGES; ++s) {
-      mbar_init(a_full + 8 * s, 1);
-      mbar_init(op_empty + 8 * s, 1);
-      mbar_init(cvt_full + 8 * s, 2 * C::CVT_WARPS);
-    }
-    for (int s = 0; s < C::RAW_STAGES; ++s) {
-      mbar_init(raw_full + 8 * s, 1);
-      mbar_init(raw_empty + 8 * s, C::CVT_WARPS);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar + 8 * a, 1);
-      mbar_init(tempty_bar + 8 * a, 2 * 32 * NUM_EPI_WARPS);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;"
-                 ::"r"(tmem_slot), "n"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-
-  if (warp == 0) {
-    // ===================== TMA producer: P planes (both CTAs) =====================
-    if (lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_phi) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_plo) : "memory");
-      int os = 0;
-      uint32_t oph = 0;
-      for (int64_t u = unit0; u < n_units; u += unit_step) {
-        const int n0 = ((int)(u % n_pair) * 2 + (int)rank) * BM;
-        for (int kb = 0; kb < n_kb; ++kb) {
-          mbar_wait(op_empty + 8 * os, oph ^ 1);
-          const uint32_t fb = a_full + 8 * os;
-          const uint32_t sa = smem_base + os * C::OP_STAGE;
-          if (leader) mbar_expect_tx(fb, 2 * 2 * C::A_TILE);
-          tma_load_2d_2sm(sa, &map_phi, fb, kb * 64, n0);
-          tma_load_2d_2sm(sa + C::A_TILE, &map_plo, fb, kb * 64, n0);
-          if (++os == C::OP_STAGES) { os = 0; oph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (leader && lane == 0) {
-      const uint32_t idesc = make_idesc_2sm_f16();
-      int os = 0;
-      uint32_t oph = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int64_t u = unit0; u < n_units; u += unit_step) {
-        mbar_wait(tempty_bar + 8 * acc, acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = 0; kb < n_kb; ++kb) {
-          mbar_wait(a_full + 8 * os, oph);            // both CTAs' P tiles have landed
-          mbar_wait(cvt_full + 8 * os, oph);          // both CTAs' q planes are written
-          tc_fence_after();
-          const uint32_t sa = smem_base + os * C::OP_STAGE;
-          const uint64_t a_hi = make_smem_desc<32>(sa);
-          const uint64_t a_lo = make_smem_desc<32>(sa + C::A_TILE);
-          const uint64_t b_hi = make_smem_desc<32>(sa + 2 * C::A_TILE);
-          const uint64_t b_lo = make_smem_desc<32>(sa + 2 * C::A_TILE + C::B_TILE);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {                 // 16 halves = 32 B per k-step
-            const uint64_t ko = (uint64_t)((k * 32) >> 4);
-            const uint32_t first = (kb | k) != 0 ? 1u : 0u;
-            umma_f16_2sm(d_tmem, a_lo + ko, b_hi + ko, idesc, first);
-            umma_f16_2sm(d_tmem, a_hi + ko, b_lo + ko, idesc, 1u);
-            umma_f16_2sm(d_tmem, a_hi + ko, b_hi + ko, idesc, 1u);
-          }
-          umma_commit_2sm(op_empty + 8 * os);
-          if (++os == C::OP_STAGES) { os = 0; oph ^= 1; }
-        }
-        umma_commit_2sm(tfull_bar + 8 * acc);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp == 2) {
-    // ===================== TMA producer: fp32 q tiles (both CTAs, local barriers) ==============
-    if (lane == 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q32) : "memory");
-      int rs = 0;
-      uint32_t rph = 0;
-      for (int64_t u = unit0; u < n_units; u += unit_step) {
-        const int c0 = (int)((u / n_pair) * BN) + (int)rank * (BN / 2);   // own chain half
-        for (int kb = 0; kb < n_kb; ++kb) {
-          mbar_wait(raw_empty + 8 * rs, rph ^ 1);
-          const uint32_t fb = raw_full + 8 * rs;
-          mbar_expect_tx(fb, C::RAW_STAGE);
-          tma_load_2d(raw_base + rs * C::RAW_STAGE, &map_q32, fb, kb * 64, c0);
-          if (++rs == C::RAW_STAGES) { rs = 0; rph ^= 1; }
-        }
-      }
-    }
-  } else if (warp < C::EPI_WARP0) {
-    // ===================== converters (warps 3..6, both CTAs) =====================
-    const int cw = warp - 3;                              // rows cw*32 .. cw*32+31 of the tile
-    int os = 0, rs = 0;
-    uint32_t oph = 0, rph = 0;
-    const uint32_t chunk = (uint32_t)lane >> 2, sub = ((uint32_t)lane & 3u) << 2;
-    for (int64_t u = unit0; u < n_units; u += unit_step) {
-      for (int kb = 0; kb < n_kb; ++kb) {
-        mbar_wait(raw_full + 8 * rs, rph);                // fp32 tile landed (async proxy write)
-        mbar_wait(op_empty + 8 * os, oph ^ 1);            // plane slot drained by the MMAs
-        const uint8_t* src = smem_raw + (raw_base - smem_u32(smem_raw)) + rs * C::RAW_STAGE;
-        uint8_t* dst_hi = smem_raw + (smem_base - smem_u32(smem_raw)) + os * C::OP_STAGE +
-                          2 * C::A_TILE;
-        uint8_t* dst_lo = dst_hi + C::B_TILE;
-#pragma unroll 8
-        for (int i = 0; i < 32; ++i) {
-          const int r = cw * 32 + i;
-          const float2 v = *reinterpret_cast<const float2*>(src + r * 256 + lane * 8);
-          const float x0 = v.x * sq, x1 = v.y * sq;
-          const __half h0 = __float2half_rn(x0), h1 = __float2half_rn(x1);
-          const __half l0 = __float2half_rn(x0 - __half2float(h0));
-          const __half l1 = __float2half_rn(x1 - __half2float(h1));
-          const uint32_t off = (uint32_t)(r >> 3) * 1024u + (uint32_t)(r & 7) * 128u +
-                               ((chunk ^ (uint32_t)(r & 7)) << 4) + sub;
-          *reinterpret_cast<__half2*>(dst_hi + off) = __halves2half2(h0, h1);
-          *reinterpret_cast<__half2*>(dst_lo + off) = __halves2half2(l0, l1);
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // visible to the MMA proxy
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(raw_empty + 8 * rs);
-          if (leader) mbar_arrive(cvt_full + 8 * os);
-          else mbar_arrive_cluster(cvt_full + 8 * os, 0);
-        }
-        if (++os == C::OP_STAGES) { os = 0; oph ^= 1; }
-        if (++rs == C::RAW_STAGES) { rs = 0; rph ^= 1; }
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 7..14, both CTAs) =====================
-    const int quarter = warp & 3;
-    const int half = (warp - C::EPI_WARP0) >> 2;
-    const float eps = state[ZSB_ST_EPS_USED];
-    const float s2 = mul(eps, p_scale);
-    const float acc_scale = 1.f / (scales[3] * sq);      // powers of two: exact
-    float amax = 0.f;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int64_t u = unit0; u < n_units; u += unit_step) {
-      const int nb = (int)(u % n_pair) * 2 + (int)rank;
-      const int n = nb * BM + quarter * 32 + lane;
-      const int64_t c0 = (u / n_pair) * BN + half * (BN / 2);
-      const bool n_ok = n < D;
-      const float m_n = n_ok ? mass[n] : 1.f;
-      const float eps_over_m = fdiv(eps, m_n);
-      const float inv_m = fdiv(1.f, m_n);
-      const float b_n = (n_ok && bvec) ? bvec[n] : 0.f;
-      const float mu_n = (n_ok && mu) ? mu[n] : 0.f;
-      mbar_wait(tfull_bar + 8 * acc, acc_phase);
-      tc_fence_after();
-      const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16) +
-                            (uint32_t)(acc * BN + half * (BN / 2));
-      const int64_t part_row = (int64_t)(nb * 4 + quarter) * chains;
-      const EpiArgs ea{q_cur, q_next, nullptr, p_in, p_out, lp_part, k_part, chains, D,
-                       2, 1.f, acc_scale};
-      epilogue_half_tile<MODE, NEXT, DC, 2>(ea, trow, n, n_ok, nb < n_blk, c0, part_row, lane,
-                                            s2, eps_over_m, inv_m, b_n, mu_n, false, amax);
-      tc_fence_before();
-      if (leader) mbar_arrive(tempty_bar + 8 * acc);
-      else mbar_arrive_remote(tempty_bar + 8 * acc, 0);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-    if (NEXT) {
-      amax = warp_max(amax);
-      if (lane == 0) atomicMax(slots + (pass_index + 1) % 3, __float_as_uint(amax));
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;"
-                 ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
-  }
-}
-
-template <int MODE, int NEXT, int DC>
-struct Tc3Inst {
-  static cudaError_t prepare() {
-    static const cudaError_t e = cudaFuncSetAttribute(
-        dense_leapfrog_tc3_kernel<MODE, NEXT, DC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-        Cfg3::SMEM);
-    return e;
-  }
-};
-
-int launch_tc3(const float* q_cur, float* q_next, const float* p_in, float* p_out,
-               const void* P_h16, const void* P_l16, const float* bvec, const float* mu,
-               const float* mass, const float* state, float p_scale, float* lp_part,
-               float* k_part, int64_t chains, int D, float* scales, int pass_index,
-               cudaStream_t st) {
-  if (k_part && !lp_part) {
-    zsb_set_error("dense_tc3: k_part requires lp_part");
-    return ZSB_ERR_INVALID;
-  }
-  CUtensorMap m_phi, m_plo, m_q32;
-  int rc;
-  if ((rc = make_map(&m_phi, P_h16, (uint64_t)D, (uint64_t)D, BM, 32, 1))) return rc;
-  if ((rc = make_map(&m_plo, P_l16, (uint64_t)D, (uint64_t)D, BM, 32, 1))) return rc;
-  if ((rc = make_map_plain(&m_q32, q_cur, (uint64_t)chains, (uint64_t)D, BN / 2, 64))) return rc;
-  const int n_blk = (D + BM - 1) / BM;
-  const int64_t n_units = ((chains + BN - 1) / BN) * ((n_blk + 1) / 2);
-  int dev = 0, sms = ZSB_NUM_SMS;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  int64_t pairs = sms / 2;
-  if (n_units < pairs) pairs = n_units;
-  const unsigned grid = (unsigned)(2 * pairs);
-  cudaError_t prep = cudaSuccess;
-#define ZSB_TC3_LAUNCH(MODE, NEXT, DC)                                                         \
-  do {                                                                                         \
-    prep = Tc3Inst<MODE, NEXT, DC>::prepare();                                                 \
-    if (prep == cudaSuccess)                                                                   \
-      dense_leapfrog_tc3_kernel<MODE, NEXT, DC><<<grid, Cfg3::THREADS, Cfg3::SMEM, st>>>(      \
-          m_phi, m_plo, m_q32, q_cur, q_next, p_in, p_out, bvec, mu, mass, state, p_scale,     \
-          lp_part, k_part, chains, D, scales, pass_index);                                     \
-  } while (0)
-#define ZSB_TC3_MODE(NEXT, DC)                                                                 \
-  do {                                                                                         \
-    if (k_part) ZSB_TC3_LAUNCH(2, NEXT, DC);                                                   \
-    else if (lp_part) ZSB_TC3_LAUNCH(1, NEXT, DC);                                             \
-    else ZSB_TC3_LAUNCH(0, NEXT, DC);                                                          \
-  } while (0)
-#define ZSB_TC3_NEXT(DC)                                                                       \
-  do {                                                                                         \
-    if (q_next) ZSB_TC3_MODE(1, DC);                                                           \
-    else ZSB_TC3_MODE(0, DC);                                                                  \
-  } while (0)
-  if (D == 1024) ZSB_TC3_NEXT(1024);
-  else ZSB_TC3_NEXT(0);
-#undef ZSB_TC3_NEXT
-#undef ZSB_TC3_MODE
-#undef ZSB_TC3_LAUNCH
-  if (prep != cudaSuccess) {
-    zsb_set_error("dense_tc3: cudaFuncSetAttribute: %s", cudaGetErrorString(prep));
-    return ZSB_ERR_CUDA;
-  }
-  return zsb_check_launch("hmc_dense_leapfrog_tc3");
-}
-
 // seeds running-max slot 0 with max|q| and clears slots 1, 2 (scales[4..6])
 __global__ void __launch_bounds__(256) absmax_slot_kernel(const float* __restrict__ q, int64_t n,
                                                           float* __restrict__ scales) {
@@ -858,103 +204,65 @@ __global__ void clear_slots_kernel(float* __restrict__ scales) {
   if (threadIdx.x < 3 && blockIdx.x == 0) reinterpret_cast<unsigned int*>(scales)[4 + threadIdx.x] = 0u;
 }
 
-// one instantiation of the pair kernel: opt in to the dynamic shared memory once, then launch
-template <int BK, int MODE, int OP, int NEXT, int DC>
-struct Tc2Inst {
-  static cudaError_t prepare() {
-    static const cudaError_t e = cudaFuncSetAttribute(
-        dense_leapfrog_tc2_kernel<BK, MODE, OP, NEXT, DC>,
-        cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg2<BK>::SMEM);
-    return e;
-  }
-};
 
-template <int BK, int OP>
-int launch_tc2(const float* q_cur, const float* q_cur_lo, float* q_next, float* q_next_lo,
-               const float* p_in, float* p_out, const float* P_hi, const float* P_lo,
-               const float* bvec, const float* mu, const float* mass, const float* state,
-               float p_scale, float* lp_part, float* k_part, int64_t chains, int D,
-               const float* scales, cudaStream_t st) {
+int g_tc_bk = 32;   // impl-1 pipeline shape: 32 -> 128-byte rows (2 stages), 16 -> 64-byte (4)
+
+// one pass on the tensor cores; q_lo: impl 1 TF32 residual of q_cur / impl 2 its fp16 planes
+template <int OP, int RB, int H16>
+int launch_dense(const float* q_cur, const void* q_lo, float* q_next, void* q_next_lo,
+                 const float* p_in, float* p_out, const void* P_hi, const void* P_lo,
+                 const float* bvec, const float* mu, const float* mass, const float* state,
+                 float p_scale, float* lp_part, float* k_part, int64_t chains, int D, float* scales,
+                 int pass_index, cudaStream_t st, const char* what) {
   if (k_part && !lp_part) {
-    zsb_set_error("dense_tc2: k_part requires lp_part");
+    zsb_set_error("%s: k_part requires lp_part", what);
     return ZSB_ERR_INVALID;
   }
   CUtensorMap m_phi, m_plo, m_qhi, m_qlo;
   int rc;
-  if (OP) {
-    // fp16 planes: P_hi / P_lo are [D, D] __half matrices; q_cur_lo is a [2][chains][D] __half
-    // buffer holding the hi plane then the lo plane of q_cur * sq.
-    const __half* qp = reinterpret_cast<const __half*>(q_cur_lo);
-    if ((rc = make_map(&m_phi, P_hi, (uint64_t)D, (uint64_t)D, BM, BK, 1))) return rc;
-    if ((rc = make_map(&m_plo, P_lo, (uint64_t)D, (uint64_t)D, BM, BK, 1))) return rc;
-    if ((rc = make_map(&m_qhi, qp, (uint64_t)chains, (uint64_t)D, BN / 2, BK, 1))) return rc;
-    if ((rc = make_map(&m_qlo, qp + chains * D, (uint64_t)chains, (uint64_t)D, BN / 2, BK, 1)))
-      return rc;
-  } else {
-  if ((rc = make_map(&m_phi, P_hi, (uint64_t)D, (uint64_t)D, BM, BK))) return rc;
-  if ((rc = make_map(&m_plo, P_lo, (uint64_t)D, (uint64_t)D, BM, BK))) return rc;
-  if ((rc = make_map(&m_qhi, q_cur, (uint64_t)chains, (uint64_t)D, BN / 2, BK))) return rc;
-  if ((rc = make_map(&m_qlo, q_cur_lo, (uint64_t)chains, (uint64_t)D, BN / 2, BK))) return rc;
+  if ((rc = make_map(&m_phi, P_hi, (uint64_t)D, (uint64_t)D, BM, RB, OP))) return rc;
+  if ((rc = make_map(&m_plo, P_lo, (uint64_t)D, (uint64_t)D, BM, RB, OP))) return rc;
+  m_qhi = m_phi;
+  m_qlo = m_plo;
+  if (H16 != 2) {
+    const void* qh = OP ? q_lo : (const void*)q_cur;
+    const void* ql = OP ? (const void*)(reinterpret_cast<const __half*>(q_lo) + chains * D) : q_lo;
+    if ((rc = make_map(&m_qhi, qh, (uint64_t)chains, (uint64_t)D, BN, RB, OP))) return rc;
+    if ((rc = make_map(&m_qlo, ql, (uint64_t)chains, (uint64_t)D, BN, RB, OP))) return rc;
   }
+  const EpiArgs ea{q_cur, q_next, reinterpret_cast<float*>(q_next_lo), p_in, p_out, lp_part,
+                   k_part, chains, D, H16, 1.f, 1.f};
   const int n_blk = (D + BM - 1) / BM;
-  const int64_t n_units = ((chains + BN - 1) / BN) * ((n_blk + 1) / 2);
-  int dev = 0, sms = ZSB_NUM_SMS;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  int64_t pairs = sms / 2;
-  if (n_units < pairs) pairs = n_units;
-  const unsigned grid = (unsigned)(2 * pairs);
-  cudaError_t prep = cudaSuccess;
-#define ZSB_TC2_LAUNCH(MODE, NEXT, DC)                                                         \
+#define ZSB_DENSE(MODE, DCV)                                                                   \
   do {                                                                                         \
-    prep = Tc2Inst<BK, MODE, OP, NEXT, DC>::prepare();                                         \
-    if (prep == cudaSuccess)                                                                   \
-      dense_leapfrog_tc2_kernel<BK, MODE, OP, NEXT, DC>                                        \
-          <<<grid, NUM_THREADS, Cfg2<BK>::SMEM, st>>>(                                         \
-              m_phi, m_plo, m_qhi, m_qlo, q_cur, q_next, q_next_lo, p_in, p_out, bvec, mu,     \
-              mass, state, p_scale, lp_part, k_part, chains, D, g_tc_dbg, scales);             \
+    const DenseW<OP, RB, MODE, DCV, H16> w{m_phi, m_plo, m_qhi, m_qlo, ea, bvec, mu, mass,     \
+                                           state, scales, p_scale, n_blk, D, pass_index};      \
+    return tc_launch(w, st, what);                                                             \
   } while (0)
-#define ZSB_TC2_MODE(NEXT, DC)                                                                 \
+#define ZSB_DENSE_MODE(DCV)                                                                    \
   do {                                                                                         \
-    if (k_part) ZSB_TC2_LAUNCH(2, NEXT, DC);                                                   \
-    else if (lp_part) ZSB_TC2_LAUNCH(1, NEXT, DC);                                             \
-    else ZSB_TC2_LAUNCH(0, NEXT, DC);                                                          \
+    if (k_part) ZSB_DENSE(2, DCV);                                                             \
+    else if (lp_part) ZSB_DENSE(1, DCV);                                                       \
+    else ZSB_DENSE(0, DCV);                                                                    \
   } while (0)
-#define ZSB_TC2_NEXT(DC)                                                                       \
-  do {                                                                                         \
-    if (q_next) ZSB_TC2_MODE(1, DC);                                                           \
-    else ZSB_TC2_MODE(0, DC);                                                                  \
-  } while (0)
-  // the default configuration (fp16 split, BK = 32) is also compiled with the dimension count as
-  // a constant for the common sizes: the epilogue's per-column offsets become immediates
-  bool done = false;
-  if constexpr (OP == 1 && BK == 32) {
-    if (D == 1024) { ZSB_TC2_NEXT(1024); done = true; }
-    else if (D == 512) { ZSB_TC2_NEXT(512); done = true; }
-    else if (D == 2048) { ZSB_TC2_NEXT(2048); done = true; }
-  }
-  if (!done) ZSB_TC2_NEXT(0);
-  if (prep != cudaSuccess) {
-    zsb_set_error("dense_tc2: cudaFuncSetAttribute: %s", cudaGetErrorString(prep));
-    return ZSB_ERR_CUDA;
-  }
-#undef ZSB_TC2_NEXT
-#undef ZSB_TC2_MODE
-#undef ZSB_TC2_LAUNCH
-  return zsb_check_launch("hmc_dense_leapfrog_tc2");
+  // the benchmark's dimension count is also compiled as a constant: the epilogue's per-column
+  // offsets become immediates
+  if constexpr (OP == 1 && H16 == 1)
+    if (D == 1024) ZSB_DENSE_MODE(1024);
+  ZSB_DENSE_MODE(0);
+#undef ZSB_DENSE_MODE
+#undef ZSB_DENSE
 }
 
 }  // namespace
 
 // rows of the [parts, chains] lp/K partial scratch: 4 warp-quarters per 128-dimension block
-int zsb_dense_tc_ntiles(int D) { return 4 * (2 * (((D + BM - 1) / BM + 1) / 2)); }
+int zsb_dense_tc_ntiles(int D) { return 4 * ((D + BM - 1) / BM); }
 
 int zsb_dense_tc_set_bk(int cfg) {
   const int bk = cfg & 0xFF;
   if (bk != 16 && bk != 32) return ZSB_ERR_INVALID;
   g_tc_bk = bk;
-  g_tc_dbg = (cfg >> 8) & 0xFF;   // undocumented timing-experiment flags
-  g_tc_pair = (cfg >> 16) & 1;    // 1: cta_group::2 CTA-pair kernel
   return ZSB_OK;
 }
 
@@ -974,18 +282,13 @@ int zsb_dense_leapfrog_tc_launch(const float* q_cur, const float* q_cur_lo, floa
     zsb_set_error("dense_tc: bad arguments");
     return ZSB_ERR_INVALID;
   }
-  if (g_tc_pair) {
-    if (g_tc_bk == 16)
-      return launch_tc2<16, 0>(q_cur, q_cur_lo, q_next, q_next_lo, p_in, p_out, P_hi, P_lo, bvec,
-                               mu, mass, state, p_scale, lp_part, k_part, chains, D, nullptr, st);
-    return launch_tc2<32, 0>(q_cur, q_cur_lo, q_next, q_next_lo, p_in, p_out, P_hi, P_lo, bvec, mu,
-                             mass, state, p_scale, lp_part, k_part, chains, D, nullptr, st);
-  }
   if (g_tc_bk == 16)
-    return launch_tc<16>(q_cur, q_cur_lo, q_next, q_next_lo, p_in, p_out, P_hi, P_lo, bvec, mu,
-                         mass, state, p_scale, lp_part, k_part, chains, D, st);
-  return launch_tc<32>(q_cur, q_cur_lo, q_next, q_next_lo, p_in, p_out, P_hi, P_lo, bvec, mu, mass,
-                       state, p_scale, lp_part, k_part, chains, D, st);
+    return launch_dense<0, 64, 0>(q_cur, q_cur_lo, q_next, q_next_lo, p_in, p_out, P_hi, P_lo,
+                                  bvec, mu, mass, state, p_scale, lp_part, k_part, chains, D,
+                                  nullptr, 0, st, "hmc_dense_leapfrog_tc");
+  return launch_dense<0, 128, 0>(q_cur, q_cur_lo, q_next, q_next_lo, p_in, p_out, P_hi, P_lo,
+                                 bvec, mu, mass, state, p_scale, lp_part, k_part, chains, D,
+                                 nullptr, 0, st, "hmc_dense_leapfrog_tc");
 }
 
 int zsb_dense_split_lo_launch(const float* q, float* lo, int64_t n, cudaStream_t st) {
@@ -1001,7 +304,7 @@ int zsb_dense_split_lo_launch(const float* q, float* lo, int64_t n, cudaStream_t
   return zsb_check_launch("hmc_dense_split_lo");
 }
 
-// ---- impl 2: fp16-split operands (see dense_leapfrog_tc2_kernel OP=1) ----
+// ---- impl 2: fp16-split operands ----
 int zsb_dense_leapfrog_h16_launch(const float* q_cur, const void* q_cur_planes, float* q_next,
                                   void* q_next_planes, const float* p_in, float* p_out,
                                   const void* P_h16, const void* P_l16, const float* scales,
@@ -1016,11 +319,9 @@ int zsb_dense_leapfrog_h16_launch(const float* q_cur, const void* q_cur_planes, 
     zsb_set_error("dense_h16: bad arguments");
     return ZSB_ERR_INVALID;
   }
-  return launch_tc2<32, 1>(q_cur, reinterpret_cast<const float*>(q_cur_planes), q_next,
-                           reinterpret_cast<float*>(q_next_planes), p_in, p_out,
-                           reinterpret_cast<const float*>(P_h16),
-                           reinterpret_cast<const float*>(P_l16), bvec, mu, mass, state, p_scale,
-                           lp_part, k_part, chains, D, scales, st);
+  return launch_dense<1, 128, 1>(q_cur, q_cur_planes, q_next, q_next_planes, p_in, p_out, P_h16,
+                                 P_l16, bvec, mu, mass, state, p_scale, lp_part, k_part, chains, D,
+                                 const_cast<float*>(scales), 0, st, "hmc_dense_leapfrog_h16");
 }
 
 // impl 3 (in-kernel split).  scales: float[8] device scratch with scales[3] = sP.
@@ -1038,8 +339,9 @@ int zsb_dense_leapfrog_h16i_launch(const float* q_cur, float* q_next, const floa
     zsb_set_error("dense_h16i: bad arguments");
     return ZSB_ERR_INVALID;
   }
-  return launch_tc3(q_cur, q_next, p_in, p_out, P_h16, P_l16, bvec, mu, mass, state, p_scale,
-                    lp_part, k_part, chains, D, scales, pass_index, st);
+  return launch_dense<1, 128, 2>(q_cur, nullptr, q_next, nullptr, p_in, p_out, P_h16, P_l16, bvec,
+                                 mu, mass, state, p_scale, lp_part, k_part, chains, D, scales,
+                                 pass_index, st, "hmc_dense_leapfrog_h16i");
 }
 int zsb_dense_h16i_prepare_launch(const float* q, float* scales, int64_t n, cudaStream_t st) {
   int64_t blocks = zsb_ceil_div(n, 256 * 8);

@@ -1,305 +1,17 @@
-// EXPERIMENTAL (written at the end of round 1, compiled, NOT yet run on hardware; opt-in only:
-// dense_impl=4, tests skipped unless ZSB_EXPERIMENTAL=1).  DESIGN.md section 6, roadmap item 1.
-//
-// A whole HMC leapfrog trajectory (zhusuan/hmc.py:347-372: the L+1 iterations of the
-// `tf.while_loop` in HMC._leapfrog, body = leapfrog_integrator hmc.py:38-43) for a dense-Gaussian
-// log-joint in ONE persistent launch, so that a chain's q / p / fp16 planes stay resident in the
-// 126 MB L2 across the passes instead of crossing HBM 51 times per iteration.
-//
-// Passes couple chains only at iteration boundaries, never inside a trajectory.  A cluster of 8
-// CTAs = four cta_group::2 pairs = all 1024 dimensions owns a block of 256 chains and runs every
-// pass of it back to back; per cluster the block's state is 256 x 1024 x 20 B = 5 MB, 16 clusters
-// = 80 MB of L2.  Inside a block the two 128-chain halves alternate (TMEM accumulator h = half):
-//
-//   MMA(h0, i)   MMA(h1, i)      MMA(h0, i+1)    MMA(h1, i+1)   ...
-//                epi(h0, i)      epi(h1, i)      epi(h0, i+1)
-//                     \-- qready[h0]: every epilogue warp of all 8 CTAs has written q_next and
-//                         its fp16 planes for half h0 --> the TMA producers may load pass i+1
-//
-// so the epilogue of one half hides behind the MMAs of the other, exactly like the two-unit
-// pipeline of the per-pass kernel (hmc_dense_tc.cu), whose operand format (fp16 hi/lo planes,
-// three kind::f16 products), tile shape per CTA pair (M = 256 dimensions) and fused epilogue
-// (hmc_dense_epilogue.cuh) it reuses; the MMA N is 128 instead of 256.
-//
-// Cross-CTA visibility of the planes: epilogue lanes store, `__threadfence()`,
-// `fence.proxy.async` (generic -> async proxy), then one lane per warp arrives (release.cluster)
-// on `qready[h]` of every CTA of the cluster; a producer waits with acquire.cluster before it
-// issues the TMA loads of that half's next pass.
-#include "hmc_dense_epilogue.cuh"
+// Trajectory entry point of dense_impl = 4: the L+1 leapfrog passes of zhusuan/hmc.py:347-372
+// (body = leapfrog_integrator, hmc.py:38-43, plus the log p / kinetic terms of hamiltonian(),
+// hmc.py:30-35) for every chain, with the buffers and operand planes of the per-pass fp16-split
+// kernel (impl 2, hmc_dense_tc.cu) and the ping-pong schedule of the per-pass host loop
+// (zhusuan_b200/hmc.py: q0 -> qa -> qb -> qa ...).  Each pass is one launch of that kernel.
+#include "common.cuh"
 
-namespace {
+int zsb_dense_leapfrog_h16_launch(const float* q_cur, const void* q_cur_planes, float* q_next,
+                                  void* q_next_planes, const float* p_in, float* p_out,
+                                  const void* P_h16, const void* P_l16, const float* scales,
+                                  const float* bvec, const float* mu, const float* mass,
+                                  const float* state, float p_scale, float* lp_part, float* k_part,
+                                  int64_t chains, int D, cudaStream_t st);
 
-constexpr int TN = 128;                    // chains per half-unit (MMA N)
-constexpr int TBLOCK = 2 * TN;             // chains per block (two halves)
-constexpr int CLUSTER = 8;                 // 4 pairs x 256 dimensions = D = 1024
-
-struct CfgT {
-  static constexpr int A_TILE = BM * 128;                     // 128 rows x 64 halves (16 KB)
-  static constexpr int B_TILE = (TN / 2) * 128;               // own 64 chain rows (8 KB)
-  static constexpr int STAGE = 2 * A_TILE + 2 * B_TILE;       // 48 KB
-  static constexpr int STAGES = 4;                            // 192 KB
-  static constexpr int SMEM = STAGES * STAGE + 1024 + 256;
-};
-
-__device__ __forceinline__ uint32_t make_idesc_2sm_f16_n128() {   // F16 x F16 -> F32, M=256, N=128
-  return (1u << 4) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-}
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64"
-      " [%0], %1;"
-      ::"r"(bar), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_release_cluster(uint32_t bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(bar), "r"(cta) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P1, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, P1;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait_cluster(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait_cluster(bar, parity)) {
-    if (clock64() - t0 > WAIT_TIMEOUT_CYCLES) {
-      printf("zsb dense_traj: qready wait timeout (block %d thread %d)\n", blockIdx.x,
-             threadIdx.x);
-      __trap();
-    }
-  }
-}
-
-struct TrajMaps {
-  CUtensorMap p_hi, p_lo;        // P planes [D, D] fp16
-  CUtensorMap q_hi[3], q_lo[3];  // planes of q0, qa, qb: [chains, D] fp16 each
-};
-
-// Buffer schedule of pass i (0..L): reads buffer cur(i), writes buffer nxt(i) (none on the last).
-//   i = 0: q0 -> qa;  i odd: qa -> qb;  i even > 0: qb -> qa.
-__device__ __forceinline__ int traj_cur(int i) { return i == 0 ? 0 : ((i & 1) ? 1 : 2); }
-__device__ __forceinline__ int traj_nxt(int i) { return (i & 1) ? 2 : 1; }
-
-template <int DC>
-__global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(NUM_THREADS, 1)
-dense_traj_kernel(const __grid_constant__ TrajMaps maps, const float* __restrict__ q0,
-                  float* __restrict__ qa, float* __restrict__ qb, void* planes_a, void* planes_b,
-                  const float* __restrict__ p0, float* __restrict__ pw,
-                  const float* __restrict__ bvec, const float* __restrict__ mu,
-                  const float* __restrict__ mass, const float* __restrict__ state,
-                  float* __restrict__ lp0_part, float* __restrict__ lp1_part,
-                  float* __restrict__ k_part, int64_t chains, int L,
-                  const float* __restrict__ scales, int dbg) {
-  using C = CfgT;
-  constexpr int D = DC;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bars = smem_base + C::STAGES * C::STAGE;
-  const uint32_t full_bar = bars;                          // [4]  leader of the pair
-  const uint32_t empty_bar = bars + 32;                    // [4]  each CTA
-  const uint32_t tfull_bar = bars + 64;                    // [2]  each CTA (accumulator = half)
-  const uint32_t tempty_bar = bars + 80;                   // [2]  leader of the pair
-  const uint32_t qready_bar = bars + 96;                   // [2]  each CTA: planes of half h ready
-  const uint32_t tmem_slot = bars + 112;
-  uint32_t* tmem_slot_ptr =
-      reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
-  const int lane = threadIdx.x & 31;
-  const uint32_t crank = cluster_ctarank();                // 0..7
-  const uint32_t pair = crank >> 1, prank = crank & 1;     // pair 0..3, rank inside the pair
-  const bool leader = prank == 0;
-  const uint32_t leader_rank = crank & ~1u;
-  const uint16_t pair_mask = (uint16_t)(3u << leader_rank);
-  const int64_t n_blocks = (chains + TBLOCK - 1) / TBLOCK;
-  const int64_t blk0 = blockIdx.x / CLUSTER, blk_step = gridDim.x / CLUSTER;
-  constexpr int n_kb = D / 64;
-  const int n0 = (int)(2 * pair + prank) * BM;             // own 128 dimension rows
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < C::STAGES; ++s) {
-      mbar_init(full_bar + 8 * s, 1);
-      mbar_init(empty_bar + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar + 8 * a, 1);
-      mbar_init(tempty_bar + 8 * a, 2 * 32 * NUM_EPI_WARPS);
-      mbar_init(qready_bar + 8 * a, CLUSTER * NUM_EPI_WARPS);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;"
-                 ::"r"(tmem_slot), "n"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-
-  if (warp == 0) {
-    // ===================== TMA producer (every CTA) =====================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t qphase[2] = {0, 0};
-      for (int64_t blk = blk0; blk < n_blocks; blk += blk_step) {
-        for (int i = 0; i <= L; ++i) {
-          const int cb = traj_cur(i);
-          for (int h = 0; h < 2; ++h) {
-            if (i > 0 && !(dbg & 4)) {                    // planes of (h, i) come from pass i-1
-              mbar_wait_cluster(qready_bar + 8 * h, qphase[h]);
-              qphase[h] ^= 1;
-              asm volatile("fence.proxy.async;" ::: "memory");
-            }
-            const int c0 = (int)(blk * TBLOCK) + h * TN + (int)prank * (TN / 2);
-            for (int kb = 0; kb < n_kb; ++kb) {
-              mbar_wait(empty_bar + 8 * stage, phase ^ 1);
-              const uint32_t fb = full_bar + 8 * stage;
-              const uint32_t sa = smem_base + stage * C::STAGE;
-              if (leader) mbar_expect_tx(fb, 2 * C::STAGE);
-              tma_load_2d_2sm(sa, &maps.p_hi, fb, kb * 64, n0);
-              tma_load_2d_2sm(sa + C::A_TILE, &maps.p_lo, fb, kb * 64, n0);
-              tma_load_2d_2sm(sa + 2 * C::A_TILE, &maps.q_hi[cb], fb, kb * 64, c0);
-              tma_load_2d_2sm(sa + 2 * C::A_TILE + C::B_TILE, &maps.q_lo[cb], fb, kb * 64, c0);
-              if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA of each pair) =====================
-    if (leader && lane == 0) {
-      const uint32_t idesc = make_idesc_2sm_f16_n128();
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t acc_phase[2] = {0, 0};
-      for (int64_t blk = blk0; blk < n_blocks; blk += blk_step) {
-        for (int i = 0; i <= L; ++i) {
-          for (int h = 0; h < 2; ++h) {
-            mbar_wait(tempty_bar + 8 * h, acc_phase[h] ^ 1);   // epilogue drained accumulator h
-            acc_phase[h] ^= 1;
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + (uint32_t)(h * BN);
-            for (int kb = 0; kb < n_kb; ++kb) {
-              mbar_wait(full_bar + 8 * stage, phase);
-              tc_fence_after();
-              const uint32_t sa = smem_base + stage * C::STAGE;
-              const uint64_t a_hi = make_smem_desc<32>(sa);
-              const uint64_t a_lo = make_smem_desc<32>(sa + C::A_TILE);
-              const uint64_t b_hi = make_smem_desc<32>(sa + 2 * C::A_TILE);
-              const uint64_t b_lo = make_smem_desc<32>(sa + 2 * C::A_TILE + C::B_TILE);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const uint64_t ko = (uint64_t)((k * 32) >> 4);
-                const uint32_t first = (kb | k) != 0 ? 1u : 0u;
-                if (dbg & 2) {          // timing experiment: one product instead of three
-                  umma_f16_2sm(d_tmem, a_hi + ko, b_hi + ko, idesc, first);
-                } else {
-                  umma_f16_2sm(d_tmem, a_lo + ko, b_hi + ko, idesc, first);
-                  umma_f16_2sm(d_tmem, a_hi + ko, b_lo + ko, idesc, 1u);
-                  umma_f16_2sm(d_tmem, a_hi + ko, b_hi + ko, idesc, 1u);
-                }
-              }
-              umma_commit_pair(empty_bar + 8 * stage, pair_mask);
-              if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-            }
-            umma_commit_pair(tfull_bar + 8 * h, pair_mask);
-          }
-        }
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 2..9, every CTA) =====================
-    const int quarter = warp & 3;
-    const int wsel = (warp - 2) >> 2;                       // columns [64*wsel, +64) of a half
-    const float eps = state[ZSB_ST_EPS_USED];
-    const float q_scale = scales[0];
-    const float acc_scale = scales[1];
-    const int nb = (int)(2 * pair + prank);
-    const int n = nb * BM + quarter * 32 + lane;
-    const float m_n = mass[n];
-    const float eps_over_m = fdiv(eps, m_n);
-    const float inv_m = fdiv(1.f, m_n);
-    const float b_n = bvec ? bvec[n] : 0.f;
-    const float mu_n = mu ? mu[n] : 0.f;
-    const float* qbuf[3] = {q0, qa, qb};
-    float* qwr[3] = {nullptr, qa, qb};
-    float* plw[3] = {nullptr, reinterpret_cast<float*>(planes_a),
-                     reinterpret_cast<float*>(planes_b)};
-    uint32_t tf_phase[2] = {0, 0};
-    float unused_amax = 0.f;
-    for (int64_t blk = blk0; blk < n_blocks; blk += blk_step) {
-      for (int i = 0; i <= L; ++i) {
-        const bool last = i == L;
-        const float s2 = mul(eps, (i > 0 && !last) ? 1.f : 0.5f);
-        const int cb = traj_cur(i), nx = traj_nxt(i);
-        for (int h = 0; h < 2; ++h) {
-          const int64_t c0 = blk * TBLOCK + h * TN + wsel * (TN / 2);
-          mbar_wait(tfull_bar + 8 * h, tf_phase[h]);
-          tf_phase[h] ^= 1;
-          tc_fence_after();
-          const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16) +
-                                (uint32_t)(h * BN + wsel * (TN / 2));
-          const int64_t part_row = (int64_t)(nb * 4 + quarter) * chains;
-          const EpiArgs ea{qbuf[cb], last ? nullptr : qwr[nx], last ? nullptr : plw[nx],
-                           i == 0 ? p0 : pw, pw, i == 0 ? lp0_part : lp1_part, k_part,
-                           chains, D, 1, q_scale, acc_scale};
-          if (last)
-            epilogue_half_tile<2, 0, DC, 1, TN / 2, 1>(ea, trow, n, true, true, c0, part_row, lane,
-                                                    s2, eps_over_m, inv_m, b_n, mu_n, (dbg & 1) != 0,
-                                                    unused_amax);
-          else if (i == 0)
-            epilogue_half_tile<1, 1, DC, 1, TN / 2, 1>(ea, trow, n, true, true, c0, part_row, lane,
-                                                    s2, eps_over_m, inv_m, b_n, mu_n, (dbg & 1) != 0,
-                                                    unused_amax);
-          else
-            epilogue_half_tile<0, 1, DC, 1, TN / 2, 1>(ea, trow, n, true, true, c0, part_row, lane,
-                                                    s2, eps_over_m, inv_m, b_n, mu_n, (dbg & 1) != 0,
-                                                    unused_amax);
-          tc_fence_before();
-          if (leader) mbar_arrive(tempty_bar + 8 * h);
-          else mbar_arrive_remote(tempty_bar + 8 * h, leader_rank);
-          if (!last && !(dbg & 4)) {
-            // publish q_next + planes of this warp's share of (h, i) to the whole cluster
-            __threadfence();
-            asm volatile("fence.proxy.async;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) {
-#pragma unroll
-              for (uint32_t r = 0; r < CLUSTER; ++r)
-                mbar_arrive_release_cluster(qready_bar + 8 * h, r);
-            }
-          }
-        }
-      }
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;"
-                 ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
-  }
-}
-
-}  // namespace
-
-// EXPERIMENTAL.  One launch = the L+1 passes of a trajectory for every chain (D = 1024, L >= 1).
 //   q0 / planes0: current state and its fp16 planes (zsb_hmc_dense_h16_prepare_f32);
 //   qa, qb, planes_a, planes_b: work buffers; on return the proposal is in (L-1 even ? qa : qb);
 //   p0 -> pw (final momentum); lp0_part / lp1_part / k_part as the per-pass kernel writes them.
@@ -313,39 +25,25 @@ int zsb_dense_traj_h16_launch(const float* q0, const void* planes0, float* qa, v
     zsb_set_error("dense_traj: needs D == 1024, n_leapfrogs >= 1");
     return ZSB_ERR_INVALID;
   }
-  static cudaError_t prep = cudaFuncSetAttribute(dense_traj_kernel<1024>,
-                                                 cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                 CfgT::SMEM);
-  if (prep != cudaSuccess) {
-    zsb_set_error("dense_traj: cudaFuncSetAttribute: %s", cudaGetErrorString(prep));
-    return ZSB_ERR_CUDA;
+  const float* cur = q0;
+  const void* cur_pl = planes0;
+  float* nxt = qa;
+  void* nxt_pl = planes_a;
+  const float* p_in = p0;
+  for (int i = 0; i <= L; ++i) {
+    const bool last = i == L;
+    const int rc = zsb_dense_leapfrog_h16_launch(
+        cur, cur_pl, last ? nullptr : nxt, last ? nullptr : nxt_pl, p_in, pw, P_h16, P_l16,
+        scales, bvec, mu, mass, state, (i > 0 && !last) ? 1.f : 0.5f,
+        i == 0 ? lp0_part : (last ? lp1_part : nullptr), last ? k_part : nullptr, chains, D, st);
+    if (rc != ZSB_OK) return rc;
+    p_in = pw;
+    if (!last) {
+      cur = nxt;
+      cur_pl = nxt_pl;
+      nxt = (nxt == qa) ? qb : qa;
+      nxt_pl = (nxt == qa) ? planes_a : planes_b;
+    }
   }
-  TrajMaps m;
-  int rc;
-  if ((rc = make_map(&m.p_hi, P_h16, (uint64_t)D, (uint64_t)D, BM, 32, 1))) return rc;
-  if ((rc = make_map(&m.p_lo, P_l16, (uint64_t)D, (uint64_t)D, BM, 32, 1))) return rc;
-  const __half* pl[3] = {reinterpret_cast<const __half*>(planes0),
-                         reinterpret_cast<const __half*>(planes_a),
-                         reinterpret_cast<const __half*>(planes_b)};
-  for (int b = 0; b < 3; ++b) {
-    if ((rc = make_map(&m.q_hi[b], pl[b], (uint64_t)chains, (uint64_t)D, TN / 2, 32, 1)))
-      return rc;
-    if ((rc = make_map(&m.q_lo[b], pl[b] + chains * D, (uint64_t)chains, (uint64_t)D, TN / 2, 32,
-                       1)))
-      return rc;
-  }
-  int dev = 0, sms = ZSB_NUM_SMS;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int64_t n_blocks = (chains + TBLOCK - 1) / TBLOCK;
-  int64_t clusters = 16;                                     // 2 clusters of 8 per GPC
-  static const int env_clusters = getenv("ZSB_TRAJ_CLUSTERS") ? atoi(getenv("ZSB_TRAJ_CLUSTERS")) : 0;
-  static const int env_dbg = getenv("ZSB_TRAJ_DBG") ? atoi(getenv("ZSB_TRAJ_DBG")) : 0;
-  if (env_clusters > 0) clusters = env_clusters;
-  if (clusters * CLUSTER > sms) clusters = sms / CLUSTER;
-  if (n_blocks < clusters) clusters = n_blocks;
-  dense_traj_kernel<1024><<<(unsigned)(clusters * CLUSTER), NUM_THREADS, CfgT::SMEM, st>>>(
-      m, q0, qa, qb, planes_a, planes_b, p0, pw, bvec, mu, mass, state, lp0_part, lp1_part,
-      k_part, chains, L, scales, env_dbg);
-  return zsb_check_launch("hmc_dense_trajectory");
+  return ZSB_OK;
 }

@@ -1,5 +1,5 @@
 """MultivariateNormalCholesky / UnnormalizedMultinomial / Dirichlet on the
-B200 kernels (zhusuan/distributions/multivariate.py:41-192, 339-446, 570-680)."""
+H100 kernels (zhusuan/distributions/multivariate.py:41-192, 339-446, 570-680)."""
 import torch
 
 from .. import ops

@@ -1,4 +1,4 @@
-"""Normal / Bernoulli / Categorical on the B200 kernels
+"""Normal / Bernoulli / Categorical on the H100 kernels
 (zhusuan/distributions/univariate.py:43-184, 334-406, 409-551)."""
 import torch
 

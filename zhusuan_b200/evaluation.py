@@ -1,5 +1,5 @@
 """zhusuan/evaluation.py: importance-sampling and annealed-importance-sampling
-marginal-likelihood estimators on the B200 kernels."""
+marginal-likelihood estimators on the H100 kernels."""
 import numpy as np
 import torch
 

@@ -215,7 +215,7 @@ class LNTMLogJoint(object):
 
 
 # ---------------------------------------------------------------------------
-# K8: dense layers of a VAE / BNN log-joint on tcgen05 (gemm_logjoint_tc.cu)
+# K8: dense layers of a VAE / BNN log-joint on the tensor cores (gemm_logjoint_tc.cu)
 # ---------------------------------------------------------------------------
 def _tc_split(t2d):
     """fp32 [rows, K] -> (fp16 planes [2, rows, Kp], scale float[4]) for the
@@ -337,7 +337,7 @@ _BERN_UNFUSED = os.environ.get("ZSB_BERN_FUSED", "0") != "1"
 
 def _tc_grad_weight(gpl, hpl, R):
     """dW [J, K] = g^T [J, R] @ h [R, K]: contraction over the rows, split-K over the CTA pairs.
-    Both operands are the row-major planes of g and h (MN-major tcgen05 operands,
+    Both operands are the row-major planes of g and h (MN-major wgmma operands,
     zsb_linear_tc_wgrad_f32); with ZSB_WGRAD_T=1 the transposed plane layout instead."""
     if _WGRAD_T:
         return _tc_linear(0, hpl.planes_t, hpl.scale, gpl.planes_t, gpl.scale, None, None, None,
@@ -383,7 +383,7 @@ def _tag(t, amax):
 
 
 class _Linear(torch.autograd.Function):
-    """y = relu?(h W^T + b): forward and both backward products on the tcgen05 kernel at fp32
+    """y = relu?(h W^T + b): forward and both backward products on the wgmma kernel at fp32
     accuracy (epi 0; the weight gradient reads the same row-major planes as MN-major operands, split-K).
     Memory passes around the GEMMs are fused (round 2): every GEMM leaves max|out| for its
     consumer's scale, ONE pass (zsb_split16_dual_f32) turns an activation / gradient into both
@@ -430,7 +430,7 @@ class _Linear(torch.autograd.Function):
 
 
 def linear(h, W, b=None, relu=False):
-    """``relu?(h @ W.T + b)`` (``tf.layers.dense``) on the tcgen05 kernel."""
+    """``relu?(h @ W.T + b)`` (``tf.layers.dense``) on the wgmma kernel."""
     return _Linear.apply(h, W, b, bool(relu))
 
 

@@ -1,4 +1,4 @@
-"""Parallel-chain HMC on B200 kernels -- drop-in for ``zs.HMC`` (zhusuan/hmc.py).
+"""Parallel-chain HMC on H100 kernels -- drop-in for ``zs.HMC`` (zhusuan/hmc.py).
 
 Same constructor and ``sample(meta_bn, observed, latent) -> (sample_op,
 HMCInfo)`` contract as hmc.py:252-255, 382-410.  Differences forced by the
@@ -571,14 +571,14 @@ class HMC(object):
                 (1 if D % 32 == 0 else 0)
         if int(impl) in (2, 3, 5) and D % 64 != 0:
             raise ValueError("dense_impl=2/3/5 (fp16 split) needs D % 64 == 0")
-        # impl 5: L2-resident whole-trajectory kernel (hmc_dense_res.cu).  The state of q inside
-        # a trajectory is its fp16 hi/lo plane pair; the step-size probes are trajectories with
+        # impl 5: whole-trajectory entry point (hmc_dense_res.cu).  The state of q inside a
+        # trajectory is its fp16 hi/lo plane pair; the step-size probes are trajectories with
         # L = 1; n_leapfrogs = 0 (a single half-kick pass) runs on the per-pass kernel (impl 2).
         self._res = int(impl) == 5 and self.n_leapfrogs >= 1
         if int(impl) == 5:
             impl = 2
-        # impl 4 (EXPERIMENTAL, not validated on hardware): impl 2's buffers and probe passes,
-        # but the L+1 passes of the main trajectory in ONE persistent launch (hmc_dense_traj.cu)
+        # impl 4: impl 2's buffers and probe passes, the L+1 passes of the main trajectory
+        # through one entry point (hmc_dense_traj.cu)
         self._traj = int(impl) == 4
         if self._traj:
             if D != 1024 or self.n_leapfrogs < 1:
@@ -586,10 +586,7 @@ class HMC(object):
             impl = 2
         self._impl = int(impl)
         if self._impl >= 1:            # pipeline-shape tuning knob (same results)
-            lib.call("zsb_hmc_dense_tc_config",
-                     int(os.environ.get("ZSB_TC_BK", "32"))
-                     | (int(os.environ.get("ZSB_TC_DBG", "0")) << 8)
-                     | (int(os.environ.get("ZSB_TC_PAIR", "1")) << 16))
+            lib.call("zsb_hmc_dense_tc_config", int(os.environ.get("ZSB_TC_BK", "32")))
         nt = lib.load().zsb_hmc_dense_ntiles(D, min(self._impl, 1))
         z = lambda *s: torch.zeros(*s, dtype=_F32, device=dev)
         self._pw = torch.empty_like(self._q[0])
@@ -601,13 +598,8 @@ class HMC(object):
         self._ntiles = nt
         if self._res:                  # two plane buffers + flags; no fp32 work copies of q
             shape = (2,) + tuple(self._q[0].shape)
-            # one plane buffer updated in place (8 instead of 12 B/element of L2 footprint: 40 %
-            # less HBM traffic, 2-4 % faster); ZSB_RES_INPLACE=0 selects the ping-pong pair
-            self._res_inplace = os.environ.get("ZSB_RES_INPLACE", "1") == "1"
             self._planes = [torch.empty(shape, dtype=torch.float16, device=dev)
-                            for _ in range(1 if self._res_inplace else 2)]
-            if self._res_inplace:
-                self._planes.append(self._planes[0])
+                            for _ in range(2)]
             self._res_flags = torch.zeros(
                 lib.load().zsb_hmc_dense_resident_flags(self._chains),
                 dtype=torch.int32, device=dev)
@@ -681,7 +673,7 @@ class HMC(object):
                  ctypes.byref(self._npart), ptr(self._state), s)
 
     def _resident_trajectory(self, L, s):
-        """L+1 leapfrog passes in one L2-resident launch; returns the proposal's planes."""
+        """L+1 leapfrog passes on the fp16 plane state; returns the proposal's planes."""
         f = self._fused
         lib.call("zsb_hmc_dense_resident_h16_f32", ptr(self._planes[0]),
                  ptr(self._planes[1]), ptr(self._p0[0]), ptr(self._pw),
@@ -689,7 +681,7 @@ class HMC(object):
                  ptr(f.get("mu")), ptr(self._mass[0]), ptr(self._state),
                  ptr(self._lp0_part), ptr(self._lp1_part), ptr(self._k_part),
                  ptr(self._res_flags), self._chains, f["D"], L, s)
-        return self._planes[0 if self._res_inplace else (L & 1)]
+        return self._planes[L & 1]
 
     def _iterate_dense_resident(self, noise_u, seed, it, init, s):
         q0 = self._q[0]
@@ -703,8 +695,6 @@ class HMC(object):
             def probe():               # hmc.py:314-326: one leapfrog step = a trajectory, L = 1
                 self._resident_trajectory(1, s)
                 self._dense_finish_mh(noise_u, seed, it, s, full=False)
-                if self._res_inplace:  # the probe advanced the single plane buffer: rebuild q0's
-                    prepare()
             self._search(probe, s)
         prof = None if self._dev_mode else getattr(self, "_profile_events", None)
         if prof is not None:           # bench.py: device time of the trajectory launch

@@ -1,4 +1,4 @@
-"""SG-MCMC samplers on B200 kernels -- drop-in for zhusuan/sgmcmc.py
+"""SG-MCMC samplers on H100 kernels -- drop-in for zhusuan/sgmcmc.py
 (``SGLD``, ``PSGLD``, ``SGHMC``, ``SGNHT``; same constructors and
 ``sample(meta_bn, observed, latent) -> (sample_op, SGMCMCInfo)`` contract,
 sgmcmc.py:119-161).  As in hmc.py, ``latent`` values are float32 CUDA tensors
