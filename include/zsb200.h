@@ -392,6 +392,23 @@ int zsb_lntm_logjoint_f32(const float* eta, const float* eta_mean, const float* 
                           const float* word_cnt, float* lp_out, float* grad_out, int64_t chains,
                           int64_t docs, int64_t n_topics, void* stream);
 
+/* ---- Bayesian PMF, one HMC sweep over every chunk of one factor (csrc/pmf.cu) ------------------
+ * The model of examples/probabilistic_matrix_factorization/pmf_hmc.py:19-31 with its log_joint
+ * override (136-144), Normal._log_prob of zhusuan/distributions/univariate.py:
+ *   lat [K, n_rows, D] ~ N(0, exp(logstd_lat)), fixed [K, n_cols, D] ~ N(0, exp(logstd_fixed)),
+ *   r_ij ~ N(sigmoid(lat_i . fixed_j), exp(logstd_rating)).
+ * Ratings in CSR by latent row: row_ptr [n_rows + 1], col_idx / rating [nnz].  nbr_ptr
+ * [n_chunks + 1] / nbr_idx: the distinct columns rated inside each chunk of chunk_size rows.
+ * lp_out [K, n_chunks] = prior of the chunk's latent rows + prior of the fixed factor over the
+ * chunk's neighbours + the chunk's rating terms; grad_out (like lat) = d lp / d lat.  Either may be
+ * NULL; values need work [K, n_rows].  1 <= D <= 128.  No floating-point atomics: deterministic. */
+int zsb_pmf_logjoint_f32(const float* lat, const float* fixed, const int64_t* row_ptr,
+                         const int32_t* col_idx, const float* rating, const int64_t* nbr_ptr,
+                         const int32_t* nbr_idx, float logstd_lat, float logstd_fixed,
+                         float logstd_rating, float* lp_out, float* grad_out, float* work,
+                         int64_t K, int64_t n_rows, int64_t n_cols, int64_t D, int64_t chunk_size,
+                         void* stream);
+
 /* ---- K5: SG-MCMC updates (zhusuan/sgmcmc.py) ------------------------------------------------ */
 int zsb_sgmcmc_parts(void);   /* capacity (floats) of every `part` scratch */
 int zsb_sgmcmc_sgld_f32(float* q, const float* g, const float* noise, float lr, int64_t chains,

@@ -8,7 +8,7 @@ import os
 import numpy as np
 import torch
 
-__all__ = ["GaussianLogJoint", "BNNRegressionLogJoint", "LNTMLogJoint", "linear",
+__all__ = ["GaussianLogJoint", "BNNRegressionLogJoint", "LNTMLogJoint", "PMFLogJoint", "linear",
            "linear_bernoulli_log_prob", "LinearBernoulli"]
 
 
@@ -212,6 +212,171 @@ class LNTMLogJoint(object):
         prior = (-0.5 * math.log(2 * math.pi) - self.eta_logstd
                  - 0.5 * prec * (eta - self.eta_mean) ** 2).sum(-1)
         return prior + (self.x * torch.log(doc_word)).sum(-1)
+
+
+def _as_numpy(a, dtype):
+    if isinstance(a, torch.Tensor):
+        a = a.detach().cpu().numpy()
+    return np.asarray(a).astype(dtype, copy=False)
+
+
+class PMFLogJoint(object):
+    """One HMC sweep over every chunk of one factor of Bayesian probabilistic matrix factorisation,
+    examples/probabilistic_matrix_factorization/pmf_hmc.py:19-31 with its log_joint override
+    (136-144):
+
+        u [K, n, D] ~ N(0, std), v [K, m, D] ~ N(0, fixed_std),
+        r_ij ~ N(sigmoid(u_i . v_j), rating_std)    for every observed rating (i, j).
+
+    The example runs one HMC per chunk of ``chunk_size`` users with the movie factor fixed, then
+    one per chunk of movies.  Given the other factor the chunks are independent, so one HMC
+    iteration whose latent is ``[K, n_chunks, chunk_size, D]`` (chain shape ``[K, n_chunks]``)
+    performs the example's whole sequential sweep; each chain's log-joint is the example's own
+    for its chunk: the prior of its rows, the prior of the fixed factor over the columns the chunk's
+    ratings touch (its neighbour set), and the chunk's rating terms.  ``zs.HMC.sample`` recognises
+    the object (``_zsb_fused`` kind "provider") and takes values and gradients from one
+    deterministic kernel (zsb_pmf_logjoint_f32) that never forms the [K, nnz, D] gathered
+    factors.  Called as ``lj(observed)`` it is the torch restatement of the example's graph
+    (gather, sigmoid, Normal log-probs summed per chunk), differentiable, for small shapes.
+
+    rows, cols, ratings: COO ratings (already normalised); ``rows`` index the sampled factor,
+    ``cols`` the fixed one.  fixed: the other factor, float32 ``[K, n_cols, D]`` or
+    ``[K, n_col_chunks, col_chunk, D]``, read in place on every call -- pass the other sampler's
+    latent and no copy is ever needed (``set_fixed`` rebinds it).  n_rows: rows of the sampled
+    factor, a multiple of chunk_size (pad as the example does).  1 <= D <= 128.
+
+    A Gibbs epoch of the example, and its RMSE recipe (lines 114-120) in torch::
+
+        U = torch.randn(K, N_pad, D, device="cuda") * 0.1
+        V = torch.randn(K, M_pad, D, device="cuda") * 0.1
+        u = U.view(K, N_pad // 50, 50, D)
+        v = V.view(K, M_pad // 50, 50, D)
+        lj_u = zs.fused.PMFLogJoint(user, movie, r_norm, fixed=v, n_rows=N_pad, chunk_size=50,
+                                    std=1., fixed_std=1., rating_std=0.05, name="u")
+        lj_v = zs.fused.PMFLogJoint(movie, user, r_norm, fixed=u, n_rows=M_pad, chunk_size=50,
+                                    std=1., fixed_std=1., rating_std=0.05, name="v")
+        op_u, _ = zs.HMC(step_size=1e-3, n_leapfrogs=10).sample(lj_u, {}, {"u": u})
+        op_v, _ = zs.HMC(step_size=1e-3, n_leapfrogs=10).sample(lj_v, {}, {"v": v})
+        for epoch in range(n_epochs):
+            op_u(); op_v()
+            pred = torch.sigmoid((U[:, su] * V[:, sv]).sum(-1)).mean(0)
+            rmse = torch.sqrt(((pred - (true_rating - 1.) / 4.) ** 2).mean()) * 4
+    """
+
+    def __init__(self, rows, cols, ratings, fixed, n_rows, chunk_size=50, std=1.0,
+                 fixed_std=1.0, rating_std=1.0, name="u"):
+        rows, cols = _as_numpy(rows, np.int64), _as_numpy(cols, np.int64)
+        r = _as_numpy(ratings, np.float32)
+        if rows.ndim != 1 or cols.ndim != 1 or r.ndim != 1:
+            raise ValueError("rows, cols and ratings must be 1-D")
+        if not (rows.shape[0] == cols.shape[0] == r.shape[0]):
+            raise ValueError("rows, cols and ratings have different lengths (%d, %d, %d)"
+                             % (rows.shape[0], cols.shape[0], r.shape[0]))
+        n_rows, chunk_size = int(n_rows), int(chunk_size)
+        if n_rows <= 0 or chunk_size <= 0 or n_rows % chunk_size != 0:
+            raise ValueError("n_rows (%d) must be a positive multiple of chunk_size (%d)"
+                             % (n_rows, chunk_size))
+        for nm, s in (("std", std), ("fixed_std", fixed_std), ("rating_std", rating_std)):
+            if not (float(s) > 0 and math.isfinite(float(s))):
+                raise ValueError("%s must be positive and finite" % nm)
+        if not np.all(np.isfinite(r)):
+            raise ValueError("ratings must be finite")
+        self.name = name
+        self.n_rows, self.chunk_size = n_rows, chunk_size
+        self.n_chunks = n_rows // chunk_size
+        self.std, self.fixed_std, self.rating_std = float(std), float(fixed_std), float(rating_std)
+        self.set_fixed(fixed)
+        if rows.size and (rows.min() < 0 or rows.max() >= n_rows):
+            raise ValueError("rows index outside [0, %d)" % n_rows)
+        if cols.size and (cols.min() < 0 or cols.max() >= self.n_cols):
+            raise ValueError("cols index outside [0, %d)" % self.n_cols)
+        if rows.size >= (1 << 31):
+            raise ValueError("at most 2^31 - 1 ratings")
+        # CSR by latent row; the stable sort keeps each row's ratings in input order
+        order = np.argsort(rows, kind="stable")
+        self.nnz = int(rows.size)
+        row_ptr = np.zeros(n_rows + 1, np.int64)
+        row_ptr[1:] = np.cumsum(np.bincount(rows, minlength=n_rows))
+        # per chunk: the distinct columns its ratings touch (select_from_corpus, pmf_hmc.py:34-60)
+        key = np.unique((rows // chunk_size) * self.n_cols + cols)
+        nbr_ptr = np.zeros(self.n_chunks + 1, np.int64)
+        nbr_ptr[1:] = np.cumsum(np.bincount(key // self.n_cols, minlength=self.n_chunks))
+        dev = self.fixed.device
+        pad1 = lambda a: a if a.size else np.zeros(1, a.dtype)      # noqa: E731 (no NULL pointers)
+        self.row_ptr = torch.as_tensor(row_ptr, device=dev)
+        self.row_idx = torch.as_tensor(rows[order], device=dev)
+        self.col_idx = torch.as_tensor(pad1(cols[order].astype(np.int32)), device=dev)
+        self.rating = torch.as_tensor(pad1(r[order]), device=dev)
+        self.nbr_ptr = torch.as_tensor(nbr_ptr, device=dev)
+        self.nbr_idx = torch.as_tensor(pad1((key % self.n_cols).astype(np.int32)), device=dev)
+        self.nbr_chunk = torch.as_tensor(key // self.n_cols, device=dev)
+        self._zsb_fused = {"kind": "provider", "obj": self}
+
+    def set_fixed(self, fixed):
+        """Rebind the fixed factor ([K, n_cols, D] or [K, n_col_chunks, col_chunk, D])."""
+        if not isinstance(fixed, torch.Tensor) or fixed.dtype != torch.float32 or \
+                fixed.dim() not in (3, 4) or not fixed.is_contiguous():
+            raise ValueError("fixed must be a contiguous float32 tensor [K, n_cols, D] or "
+                             "[K, n_col_chunks, col_chunk, D]")
+        K, D = int(fixed.shape[0]), int(fixed.shape[-1])
+        n_cols = int(np.prod(fixed.shape[1:-1]))
+        if K < 1 or n_cols < 1 or not 1 <= D <= 128:
+            raise ValueError("fixed has shape %s: need K >= 1, n_cols >= 1 and 1 <= D <= 128"
+                             % (tuple(fixed.shape),))
+        if getattr(self, "n_cols", n_cols) != n_cols:
+            raise ValueError("fixed has %d columns, the ratings were built for %d"
+                             % (n_cols, self.n_cols))
+        self.fixed, self.K, self.D, self.n_cols = fixed, K, D, n_cols
+
+    def _latent(self, var_list):
+        lat = var_list[0].detach()
+        want = (self.K, self.n_chunks, self.chunk_size, self.D)
+        if tuple(lat.shape) != want or lat.dtype != torch.float32:
+            raise ValueError("latent must be float32 %s, got %s %s"
+                             % (list(want), lat.dtype, list(lat.shape)))
+        return lat.contiguous()
+
+    def _launch(self, lat, want_lp, want_grad):
+        from ._lib import lib, ptr, stream
+        dev = lat.device
+        lp = torch.empty((self.K, self.n_chunks), dtype=torch.float32, device=dev) \
+            if want_lp else None
+        work = torch.empty((self.K, self.n_rows), dtype=torch.float32, device=dev) \
+            if want_lp else None
+        g = torch.empty_like(lat) if want_grad else None
+        lib.call("zsb_pmf_logjoint_f32", ptr(lat), ptr(self.fixed), ptr(self.row_ptr),
+                 ptr(self.col_idx), ptr(self.rating), ptr(self.nbr_ptr), ptr(self.nbr_idx),
+                 math.log(self.std), math.log(self.fixed_std), math.log(self.rating_std),
+                 ptr(lp), ptr(g), ptr(work), self.K, self.n_rows, self.n_cols, self.D,
+                 self.chunk_size, stream())
+        return lp, g
+
+    # provider interface used by HMC's generic path instead of autograd
+    def logp(self, var_list):
+        return self._launch(self._latent(var_list), True, False)[0]
+
+    def grad(self, var_list):
+        return [self._launch(self._latent(var_list), False, True)[1]]
+
+    def __call__(self, observed):
+        """Torch restatement of pmf_hmc.py:19-31, 136-144 per chunk: [K, n_chunks]."""
+        lat = observed[self.name]
+        K, D = int(lat.shape[0]), self.D
+        u = lat.reshape(K, self.n_rows, D)
+        v = self.fixed.reshape(self.K, self.n_cols, D).to(lat.dtype)
+        nnz = self.nnz
+        col = self.col_idx[:nnz].long()
+        c = -0.5 * math.log(2 * math.pi)
+
+        def normal(x, std):                               # Normal._log_prob, univariate.py
+            logstd = math.log(std)
+            return c - logstd - 0.5 * math.exp(-2 * logstd) * x * x
+        s = torch.sigmoid((u[:, self.row_idx] * v[:, col]).sum(-1))                # [K, nnz]
+        lp_r = normal(self.rating[:nnz].to(lat.dtype) - s, self.rating_std)
+        out = normal(u, self.std).sum(-1).reshape(K, self.n_chunks, self.chunk_size).sum(-1)
+        out = out.index_add(1, self.row_idx // self.chunk_size, lp_r)
+        lp_v = normal(v[:, self.nbr_idx[:self.nbr_chunk.numel()].long()], self.fixed_std).sum(-1)
+        return out.index_add(1, self.nbr_chunk, lp_v)
 
 
 # ---------------------------------------------------------------------------
