@@ -9,8 +9,9 @@
 // chain and pass, the algorithmic minimum.
 //
 // On H100 one pass of the benchmark shape (65 536 chains x 1024 dimensions) executes ~0.4 TFLOP of
-// fp16 products against ~1 GB of operand and state traffic, so the pass is bound by the tensor
-// cores, not by HBM: the passes run as L+1 launches of the persistent tensor-core kernel
+// fp16 products against ~1 GB of state traffic, so the pass is compute-bound, not HBM-bound (on a
+// card with a 400 W power limit it runs at the power cap, with the SM clock lowered to ~800 MHz;
+// README has the numbers): the passes run as L+1 launches of the persistent tensor-core kernel
 // (tc_pipeline_kernel) on alternating plane buffers, and the sampler state never leaves the plane
 // format between the prepare and the select.
 #include "tc_common.cuh"
@@ -166,7 +167,9 @@ __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, 
 
 template <int MODE, int NEXT, int DC>
 struct ResW {
-  static constexpr int KIND = 1, RB = 128, MNA = 0, MNB = 0, CVT = 0;
+  // 64-byte rows (32 fp16 of contraction per k-block): four 32 KB stages beside the accumulator
+  // tile, so the TMA producer runs up to three k-blocks ahead of the tensor cores
+  static constexpr int KIND = 1, RB = 64, MNA = 0, MNB = 0, CVT = 0;
   static constexpr int KE = RB / 2;
   static constexpr uint32_t TX = Cfg<RB>::STAGE;
   CUtensorMap m_phi, m_plo, m_qhi, m_qlo;
@@ -318,13 +321,14 @@ int zsb_dense_res_h16_launch(void* planes0, void* planes1, const float* p0, floa
   }
   CUtensorMap phi, plo, qhi[2], qlo[2];
   int rc;
-  if ((rc = make_map(&phi, P_h16, (uint64_t)D, (uint64_t)D, BM, 128, 1))) return rc;
-  if ((rc = make_map(&plo, P_l16, (uint64_t)D, (uint64_t)D, BM, 128, 1))) return rc;
+  constexpr int RB = ResW<0, 1, 0>::RB;
+  if ((rc = make_map(&phi, P_h16, (uint64_t)D, (uint64_t)D, BM, RB, 1))) return rc;
+  if ((rc = make_map(&plo, P_l16, (uint64_t)D, (uint64_t)D, BM, RB, 1))) return rc;
   __half* pl[2] = {reinterpret_cast<__half*>(planes0), reinterpret_cast<__half*>(planes1)};
   const int64_t plane = chains * (int64_t)D;
   for (int b = 0; b < 2; ++b) {
-    if ((rc = make_map(&qhi[b], pl[b], (uint64_t)chains, (uint64_t)D, BN, 128, 1))) return rc;
-    if ((rc = make_map(&qlo[b], pl[b] + plane, (uint64_t)chains, (uint64_t)D, BN, 128, 1)))
+    if ((rc = make_map(&qhi[b], pl[b], (uint64_t)chains, (uint64_t)D, BN, RB, 1))) return rc;
+    if ((rc = make_map(&qlo[b], pl[b] + plane, (uint64_t)chains, (uint64_t)D, BN, RB, 1)))
       return rc;
   }
   const int n_blk = (D + BM - 1) / BM;

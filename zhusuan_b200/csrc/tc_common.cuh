@@ -73,6 +73,14 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity))
     if (clock64() - t0 > WAIT_TIMEOUT_CYCLES) __trap();
 }
+// Wait without a timeout, for the MMA warpgroup's full-barrier wait inside the k-loop.  A trap
+// path there, with wgmma accumulators in flight, makes ptxas wait for every wgmma before the next
+// one issues (C7517 "warpgroup.wait is injected").  A stall of the MMA warpgroup still traps: the
+// epilogue warps wait on tfull, with a timeout, for every unit the MMA warpgroup owes them.
+__device__ __forceinline__ void mbar_spin(uint32_t bar, uint32_t parity) {
+  while (!mbar_try_wait(bar, parity)) {
+  }
+}
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar,
                                             int c0, int c1) {
   asm volatile(
@@ -235,7 +243,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
       int prev = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         const uint32_t sa = smem_base + stage * C::STAGE;
-        mbar_wait(full_bar + 8 * stage, phase);
+        mbar_spin(full_bar + 8 * stage, phase);
         if (W::CVT) {
           w.convert(u, kb, smem_raw + (sa - smem_u32(smem_raw)), tid);
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // visible to wgmma
