@@ -68,8 +68,12 @@ def test_three_product_split_matmul_is_fp32_accurate():
 
 
 def test_overflow_headroom_of_the_hmc_scale():
-    """The HMC kernels derive sq once per iteration: q may grow 8x inside a trajectory before
-    h overflows fp16 (65504 < 2^16 = 2^12 * 16 ... the first overflow is at 16x)."""
+    """sq places max|q| in [2^11, 2^12), so a scale kept fixed lets q grow at most ~16x before h
+    overflows fp16 (65504 < 2^16 = 2^12 * 16).  The HMC trajectory therefore checks an a-priori
+    bound on |q_next| every pass: where it would reach 2^16 - 2^8 at the current scale, the planes
+    also get a copy at a lower scale (impl 5: kept as a spare, used only if the planes overflowed;
+    impl 2 / 4: used directly) (hmc_dense_epilogue.cuh; emulated in
+    test_plane_scale_emulation.py)."""
     x = np.array([1.0, -3.0], np.float32)
     s = pow2_scale(x)
     for growth in (1, 4, 8, 15):

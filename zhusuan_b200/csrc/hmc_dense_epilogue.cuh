@@ -7,6 +7,87 @@
 
 namespace {
 
+// Plane scales of the fp16-split trajectory (impl 2, 4, 5).  `scales` is a device float array of
+// kScaleHdr + kScaleRec * (L + 2) words:
+//   [0] sq of q0's planes, [1] 1/(sP*sq) (copies of record 0), [2] prepare scratch (max|q0| bits),
+//   [3] sP, [4] ||P||_inf, [5] max|b| (the caller sets these three once), [6] prepare scratch
+//   (max|p0/m| bits), [7] max(1/m) (prepare);
+//   record i (pass i) at kScaleHdr + kScaleRec * i: {sq_i, sq_alt_i, max|q_i|, w}: the scale of
+//   the planes of q_i, the scale of their spare copy (impl 5; = sq_i when there is none), an upper
+//   bound of max|q_i|, and w = max|p_0/m| for record 0, else the flag "the planes of q_i
+//   overflowed: read the spare copy" (impl 5).  Maxima and flags are uint bits.  Record 0 comes
+//   from prepare, which also clears record 1; pass i writes record i + 1 and clears record i + 2.
+//   So every trajectory, step-size probes included, starts with a prepare.
+// Since g = b - P q and q_{i+1} = q_i + (eps/m) (p_i + s2 g_i),
+//   B_i = max|q_i| + drift_i + eps * s2 * max(1/m) * (max|b| + ||P||_inf * max|q_i|)
+// bounds |q_{i+1}| before any of it is computed, with drift_0 = eps * max|p_0/m| and, for i > 0,
+// drift_i = max|q_i| + max|q_{i-1}| >= max|(eps/m) p_i| = max|q_i - q_{i-1}| (so a pass only
+// reduces max|q|).  While B_i * sq_i stays below kPlaneKeep the planes of q_{i+1} cannot
+// overflow at sq_i.  Otherwise sq_alt = the power of two that puts B_i in [2^11, 2^12):
+//   impl 2 / 4 write the next planes at sq_alt;
+//   impl 5 writes them at sq_i, exactly as when the bound is not reached, plus a spare copy at
+//   sq_alt, and flags the pass if any |q_{i+1}| * sq_i reached fp16's overflow (65520); the next
+//   pass then reads the spare.  A bound is loose, so this keeps every trajectory whose planes fit
+//   bit-identical to a fixed scale, and only the ones that would overflow change.
+// B_i is a strict bound, so the only slack needed below 65520 is the rounding of B_i and q; scales
+// are powers of two, so a rescaled copy is exact up to the fp16 rounding of its lo plane.
+constexpr int kScaleHdr = 8, kScaleRec = 4;
+constexpr float kPlaneKeep = 65280.f;   // 2^16 - 2^8
+constexpr float kHalfOverflow = 65520.f;   // fp16 round-to-nearest gives inf from here on
+
+__device__ __forceinline__ const float* scale_rec(const float* scales, int pass) {
+  return scales + kScaleHdr + kScaleRec * pass;
+}
+__device__ __forceinline__ float pow2_plane_scale(float m) {
+  int e = 0;
+  if (m > 0.f) frexpf(m, &e);             // m = f * 2^e, f in [0.5, 1)  ->  m < 2^e
+  return ldexpf(1.f, 12 - e);             // m * sq in [2^11, 2^12)
+}
+// impl 5: pass `pass` reads the spare copy of its planes
+__device__ __forceinline__ bool plane_spare_in(const float* scales, int pass) {
+  return pass > 0 && __float_as_uint(scale_rec(scales, pass)[3]) != 0u;
+}
+// the scale of the planes pass `pass` reads
+__device__ __forceinline__ float plane_scale_in(const float* scales, int pass) {
+  return scale_rec(scales, pass)[plane_spare_in(scales, pass) ? 1 : 0];
+}
+// sq_alt of the planes pass `pass` writes (= sq when the bound keeps them inside fp16 at sq)
+__device__ __forceinline__ float next_plane_scale(const float* __restrict__ scales, int pass,
+                                                  float eps, float s2, float sq) {
+  const float* r = scale_rec(scales, pass);
+  const float mq = r[2];
+  const float drift = pass == 0 ? eps * r[3] : mq + r[2 - kScaleRec];
+  const float bound = mq + drift + eps * s2 * scales[7] * (scales[5] + scales[4] * mq);
+  // a non-finite bound (an infinite q or p, or step size) keeps the scale: those proposals are
+  // rejected
+  if (bound * sq < kPlaneKeep || !(bound <= 3.0e38f)) return sq;
+  return pow2_plane_scale(bound);
+}
+// max over finite |x| (NaN / inf are left to the chain that produced them)
+__device__ __forceinline__ float finite_absmax(float m, float x) {
+  const float a = fabsf(x);
+  return (a <= 3.0e38f) ? fmaxf(m, a) : m;
+}
+// end of a pass that wrote planes: the warp's bound of max|q_next| (and overflow flag) into record
+// pass + 1; block 0 publishes the scales of those planes and clears record pass + 2
+__device__ __forceinline__ void publish_plane_scale(float* __restrict__ scales, int pass,
+                                                    float sq_next, float sq_alt, float qmax,
+                                                    bool overflow, int quarter, int lane) {
+  unsigned int* r = reinterpret_cast<unsigned int*>(scales + kScaleHdr + kScaleRec * (pass + 1));
+  const float mq = warp_max(qmax);
+  const bool any_overflow = __any_sync(0xffffffffu, overflow);
+  if (lane == 0) {
+    atomicMax(r + 2, __float_as_uint(mq));
+    if (any_overflow) atomicOr(r + 3, 1u);
+  }
+  if (blockIdx.x == 0 && quarter == 0 && lane == 0) {
+    reinterpret_cast<float*>(r)[0] = sq_next;
+    reinterpret_cast<float*>(r)[1] = sq_alt;
+    r[kScaleRec + 2] = 0u;
+    r[kScaleRec + 3] = 0u;
+  }
+}
+
 // Fused leapfrog epilogue for one warp's share of a tile: this thread's dimension `n` (accumulator
 // row) against NCOL chains starting at c0 (`trow` = shared address of the row's first column).
 // MODE 0: plain pass; 1: + log-prob partials (first pass); 2: + log-prob and kinetic partials
@@ -17,7 +98,7 @@ struct EpiArgs {
   float* __restrict__ lp_part; float* __restrict__ k_part;
   int64_t chains; int D;
   // fp16-split operands (impl 2): q_next_lo is then a [2][chains][D] __half buffer (hi plane, lo
-  // plane) of q_next * q_scale, and the accumulator holds (P*sP)(q*sq): g = b - acc * acc_scale.
+  // plane) of q_next * q_scale, and the accumulator holds (P*sP)(q_cur*sq): g = b - acc * acc_scale.
   int h16; float q_scale; float acc_scale;
 };
 // residual operand(s) of q_next for the next pass's MMA
@@ -37,7 +118,9 @@ __device__ __forceinline__ void store_split(const EpiArgs& a, float* __restrict_
 // MODE: see above.  NEXT: 1 / 0 = q_next is / is not written (compile time), -1 = decided at run
 // time from a.q_next.  DC: the dimension count when known at compile time (all per-column offsets
 // j*D then fold into the load/store immediates: ~15 instead of ~40 instructions per element), 0 =
-// run-time a.D.  H16: fp16-split planes (impl 2) vs TF32 residual (impl 1).
+// run-time a.D.  H16: fp16-split planes (impl 2) vs TF32 residual (impl 1).  amax: running max of
+// |q_next| (H16 1, 2; finite values only for 2) over the elements this thread wrote (fmaxf drops
+// NaN; an inf makes the plane-scale bound infinite, which keeps the scale).
 // COHERENT: 1 when q_cur may have been written earlier in the SAME launch (trajectory kernel): the
 // non-coherent ld.global.nc path of __ldg could then return a stale L1 line.
 template <int MODE, int NEXT, int DC, int H16, int NCOL = BN, int COHERENT = 0>
@@ -84,12 +167,9 @@ __device__ __forceinline__ void epilogue_half_tile(const EpiArgs& a, uint32_t tr
       if (has_next) {
         const float qn = fmaf(eps_over_m, pn, qe[j]);
         qn_p[(uint32_t)j * D] = qn;
-        if (H16 == 2) {
-          const float aq = fabsf(qn);
-          amax = (aq <= 3.0e38f) ? fmaxf(amax, aq) : amax;      // ignores NaN / inf
-        } else {
-          store_split<H16>(a, lo_p, hp, lp, (uint32_t)j * D, qn);
-        }
+        if (H16 == 1) amax = fmaxf(amax, fabsf(qn));
+        if (H16 == 2) amax = finite_absmax(amax, qn);
+        if (H16 != 2) store_split<H16>(a, lo_p, hp, lp, (uint32_t)j * D, qn);
       }
     }
     if (MODE >= 1) {
@@ -159,12 +239,10 @@ __device__ __forceinline__ void epilogue_half_tile(const EpiArgs& a, uint32_t tr
             if (has_next) {
               const float qn = fmaf(eps_over_m, pn, qe[j]);
               qn0[cb + (uint32_t)j * D] = qn;
-              if (H16 == 2) {
-                const float aq = fabsf(qn);
-                amax = (aq <= 3.0e38f) ? fmaxf(amax, aq) : amax;
-              } else {
+              if (H16 == 1) amax = fmaxf(amax, fabsf(qn));
+              if (H16 == 2) amax = finite_absmax(amax, qn);
+              if (H16 != 2)
                 store_split<H16>(a, lo0 + cb, hi_pl0 + cb, lo_pl0 + cb, (uint32_t)j * D, qn);
-              }
             }
           }
         }

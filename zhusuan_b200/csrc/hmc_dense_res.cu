@@ -4,9 +4,12 @@
 // Replaces the L+1 iterations of the leapfrog `tf.while_loop` of zhusuan/hmc.py:347-372 (body =
 // leapfrog_integrator, hmc.py:38-43) plus the log p / kinetic terms of hamiltonian(), hmc.py:30-35.
 // Inside a trajectory the state of q is its fp16 hi/lo plane pair of q*sq (plus fp32 p): each
-// pass reads the planes it wrote in the previous pass, reconstructs q = (hi + lo)/sq (within 2^-23
-// of the fp32 value), and writes the next planes, so no fp32 copy of q travels: 16*D bytes per
-// chain and pass, the algorithmic minimum.
+// pass reads the planes it wrote in the previous pass, reconstructs q = (hi + lo)/sq_i (within
+// 2^-23 of the fp32 value), and writes the next planes at sq_{i+1}, so no fp32 copy of q travels:
+// 16*D bytes per chain and pass, the algorithmic minimum.  When an a-priori bound on |q_{i+1}|
+// (hmc_dense_epilogue.cuh) says the planes might overflow at sq_i, the pass also writes a spare
+// copy at a smaller scale, which the next pass reads if they did: a chain may move any distance
+// from where it started without losing its planes.
 //
 // On H100 one pass of the benchmark shape (65 536 chains x 1024 dimensions) executes ~0.4 TFLOP of
 // fp16 products against ~1 GB of state traffic, so the pass is compute-bound, not HBM-bound (on a
@@ -14,17 +17,20 @@
 // README has the numbers): the passes run as L+1 launches of the persistent tensor-core kernel
 // (tc_pipeline_kernel) on alternating plane buffers, and the sampler state never leaves the plane
 // format between the prepare and the select.
-#include "tc_common.cuh"
+#include "hmc_dense_epilogue.cuh"
 
 namespace {
 
 struct ResEpi {
   const __half* __restrict__ hi_cur; const __half* __restrict__ lo_cur;   // planes of q (this pass)
   __half* __restrict__ hi_nxt; __half* __restrict__ lo_nxt;               // planes of q_next
+  const __half* __restrict__ hi_cur_s; const __half* __restrict__ lo_cur_s;   // spare copies
+  __half* __restrict__ hi_nxt_s; __half* __restrict__ lo_nxt_s;
   const float* __restrict__ p_in; float* __restrict__ p_out;
   float* __restrict__ lp_part; float* __restrict__ k_part;
   int64_t chains; int D;
   float sq, inv_sq, acc_scale;
+  float rescale;                                           // sq_alt / sq (a power of two)
 };
 
 // One warp's share of a unit: dimension n (accumulator row) against NCOL chains from c0.
@@ -33,11 +39,19 @@ struct ResEpi {
 //   p  += s2 * g
 //   Qn  = Q + (eps/m * sq) * p  -> hi' = fp16(Qn), lo' = fp16(Qn - hi')
 // MODE 1 / 2 add the log-prob partial (q - mu) * g  (and the kinetic partial p^2 / m).
-template <int MODE, int NEXT, int DC>
+// SPARE: the bound says the next planes might overflow (uniform over the launch): also write the
+// spare planes of Qn * rescale, and keep the exact max|Qn| (overflow iff >= 65520).
+// qmax: running upper bound of |Qn| over the elements this thread wrote.  Without SPARE, on full
+// tiles, it is the 2-norm of the thread's 128 elements (one FMA each; a max per element made the
+// benchmark's pass ~3% slower at a 400 W power limit): >= their max, and for Gaussian-like states
+// within ~2x of the max over the whole pass.  A NaN / inf element makes it infinite, which keeps
+// the plane scale.
+template <int MODE, int NEXT, int DC, bool SPARE>
 __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, int n, bool n_ok,
                                                 bool parts_ok, int64_t c0, int64_t part_row,
                                                 int lane, float s2, float eps_over_m_sq,
-                                                float inv_m, float b_n, float mu_n, bool skip) {
+                                                float inv_m, float b_n, float mu_n, bool skip,
+                                                float& qmax) {
   constexpr int NCOL = BN;
   const uint32_t D = DC ? (uint32_t)DC : (uint32_t)a.D;
   const int64_t chains = a.chains;
@@ -52,20 +66,18 @@ __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, 
       reinterpret_cast<const unsigned short*>(a.lo_cur) + off_t;
   __half* __restrict__ hn0 = NEXT ? a.hi_nxt + off_t : nullptr;
   __half* __restrict__ ln0 = NEXT ? a.lo_nxt + off_t : nullptr;
+  __half* __restrict__ hs0 = SPARE ? a.hi_nxt_s + off_t : nullptr;
+  __half* __restrict__ ls0 = SPARE ? a.lo_nxt_s + off_t : nullptr;
 
   auto element = [&](float acc, float p, uint32_t hl, float& pn, float& lpv, float& kv,
-                     __half& hh, __half& ll) {
+                     float& Qn) {
     const float Q = __half2float(__ushort_as_half((unsigned short)(hl & 0xFFFFu))) +
                     __half2float(__ushort_as_half((unsigned short)(hl >> 16)));
     const float g = b_n - a.acc_scale * acc;
     pn = fmaf(s2, g, p);
     if (MODE >= 1) lpv = (Q * a.inv_sq - mu_n) * g;
     if (MODE >= 2) kv = pn * pn * inv_m;
-    if (NEXT) {
-      const float Qn = fmaf(eps_over_m_sq, pn, Q);
-      hh = __float2half_rn(Qn);
-      ll = __float2half_rn(Qn - __half2float(hh));
-    }
+    if (NEXT) Qn = fmaf(eps_over_m_sq, pn, Q);
   };
 
   if (fast_tile) {
@@ -79,20 +91,42 @@ __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, 
         he[j] = h | (l << 16);
       }
     };
-    auto compute = [&](const uint32_t* v, const float* pe, const uint32_t* he, int c) {
+    // one sum of squares per software-pipeline half, so the two 16-column blocks in flight stay
+    // independent
+    float ss_a = 0.f, ss_b = 0.f;
+    auto compute = [&](const uint32_t* v, const float* pe, const uint32_t* he, int c, float& ss) {
       const size_t cb = (size_t)c * D;
       float lpv[MODE >= 1 ? 16 : 1], kv[MODE >= 2 ? 16 : 1];
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        float pn, lp1 = 0.f, k1 = 0.f;
-        __half hh, ll;
-        element(__uint_as_float(v[j]), pe[j], he[j], pn, lp1, k1, hh, ll);
-        po0[cb + (uint32_t)j * D] = pn;
-        if (MODE >= 1) lpv[j] = lp1;
-        if (MODE >= 2) kv[j] = k1;
+      for (int j = 0; j < 16; j += 2) {   // element pairs: one packed conversion per plane
+        float pn[2], lp1[2] = {0.f, 0.f}, k1[2] = {0.f, 0.f}, Qn[2] = {0.f, 0.f};
+#pragma unroll
+        for (int t = 0; t < 2; ++t) {
+          element(__uint_as_float(v[j + t]), pe[j + t], he[j + t], pn[t], lp1[t], k1[t], Qn[t]);
+          po0[cb + (uint32_t)(j + t) * D] = pn[t];
+          if (MODE >= 1) lpv[j + t] = lp1[t];
+          if (MODE >= 2) kv[j + t] = k1[t];
+          if (NEXT && !SPARE) ss = fmaf(Qn[t], Qn[t], ss);
+          if (SPARE) qmax = fmaxf(qmax, fabsf(Qn[t]));
+        }
         if (NEXT) {
-          hn0[cb + (uint32_t)j * D] = hh;
-          ln0[cb + (uint32_t)j * D] = ll;
+          const __half2 h2 = __floats2half2_rn(Qn[0], Qn[1]);
+          const float2 hf = __half22float2(h2);
+          const __half2 l2 = __floats2half2_rn(Qn[0] - hf.x, Qn[1] - hf.y);
+          hn0[cb + (uint32_t)j * D] = __low2half(h2);
+          hn0[cb + (uint32_t)(j + 1) * D] = __high2half(h2);
+          ln0[cb + (uint32_t)j * D] = __low2half(l2);
+          ln0[cb + (uint32_t)(j + 1) * D] = __high2half(l2);
+        }
+        if (SPARE) {
+          const float x0 = Qn[0] * a.rescale, x1 = Qn[1] * a.rescale;
+          const __half2 h2 = __floats2half2_rn(x0, x1);
+          const float2 hf = __half22float2(h2);
+          const __half2 l2 = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
+          hs0[cb + (uint32_t)j * D] = __low2half(h2);
+          hs0[cb + (uint32_t)(j + 1) * D] = __high2half(h2);
+          ls0[cb + (uint32_t)j * D] = __low2half(l2);
+          ls0[cb + (uint32_t)(j + 1) * D] = __high2half(l2);
         }
       }
       if (MODE >= 1) {
@@ -112,10 +146,14 @@ __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, 
     for (int c = 0; c < NCOL; c += 32) {
       load(pb, hb, c + 16);
       acc_ld16(trow + 4u * (uint32_t)c, va);
-      compute(va, pa, ha, c);
+      compute(va, pa, ha, c, ss_a);
       if (c + 32 < NCOL) load(pa, ha, c + 32);
       acc_ld16(trow + 4u * (uint32_t)(c + 16), vb);
-      compute(vb, pb, hb, c + 16);
+      compute(vb, pb, hb, c + 16, ss_b);
+    }
+    if (NEXT && !SPARE) {
+      const float norm = sqrtf(ss_a + ss_b) * (1.f + 0x1p-10f);   // covers the rounding
+      qmax = fmaxf(qmax, norm == norm ? norm : INFINITY);
     }
   } else {
 #pragma unroll 1
@@ -136,9 +174,11 @@ __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, 
             hl = (uint32_t)__ldcg(hc0 + cb + (uint32_t)j * D) |
                  ((uint32_t)__ldcg(lc0 + cb + (uint32_t)j * D) << 16);
           }
-          float pn, lp1 = 0.f, k1 = 0.f;
-          __half hh, ll;
-          element(__uint_as_float(v[j]), p, hl, pn, lp1, k1, hh, ll);
+          float pn, lp1 = 0.f, k1 = 0.f, Qn = 0.f;
+          element(__uint_as_float(v[j]), p, hl, pn, lp1, k1, Qn);
+          const __half hh = __float2half_rn(Qn);
+          const __half ll = __float2half_rn(Qn - __half2float(hh));
+          if (NEXT && ok) qmax = fmaxf(qmax, fabsf(Qn));
           if (MODE >= 1) lpv[j] = ok ? lp1 : 0.f;
           if (MODE >= 2) kv[j] = ok ? k1 : 0.f;
           if (ok) {
@@ -146,6 +186,12 @@ __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, 
             if (NEXT) {
               hn0[cb + (uint32_t)j * D] = hh;
               ln0[cb + (uint32_t)j * D] = ll;
+            }
+            if (SPARE) {
+              const float x = Qn * a.rescale;
+              const __half hs = __float2half_rn(x);
+              hs0[cb + (uint32_t)j * D] = hs;
+              ls0[cb + (uint32_t)j * D] = __float2half_rn(x - __half2float(hs));
             }
           }
         }
@@ -165,6 +211,12 @@ __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, 
 }
 
 
+// the TMA producer's copy of "this pass reads the spare planes", read from global memory once
+__device__ __forceinline__ int& producer_spare_in() {
+  __shared__ int spare_in;
+  return spare_in;
+}
+
 template <int MODE, int NEXT, int DC>
 struct ResW {
   // 64-byte rows (32 fp16 of contraction per k-block): four 32 KB stages beside the accumulator
@@ -172,13 +224,13 @@ struct ResW {
   static constexpr int KIND = 1, RB = 64, MNA = 0, MNB = 0, CVT = 0;
   static constexpr int KE = RB / 2;
   static constexpr uint32_t TX = Cfg<RB>::STAGE;
-  CUtensorMap m_phi, m_plo, m_qhi, m_qlo;
+  CUtensorMap m_phi, m_plo, m_qhi, m_qlo, m_shi, m_slo;   // m_s*: spare planes of q
   ResEpi ea;
   const float* bvec; const float* mu; const float* mass; const float* state;
-  const float* scales;
+  float* scales;                                           // plane-scale records
   float p_scale;
-  int n_blk, D_rt;
-  struct EpiState {};
+  int n_blk, D_rt, pass;
+  struct EpiState { float qmax = 0.f; };
 
   __device__ __forceinline__ int D() const { return DC ? DC : D_rt; }
   __host__ __device__ __forceinline__ int64_t units() const {
@@ -191,6 +243,8 @@ struct ResW {
   __device__ __forceinline__ void prefetch() const {
     tma_prefetch_desc(&m_phi); tma_prefetch_desc(&m_plo);
     tma_prefetch_desc(&m_qhi); tma_prefetch_desc(&m_qlo);
+    tma_prefetch_desc(&m_shi); tma_prefetch_desc(&m_slo);
+    producer_spare_in() = plane_spare_in(scales, pass);   // prefetch runs on the producer thread
   }
   __device__ __forceinline__ void load(int64_t u, int kb, uint32_t sa, uint32_t fb) const {
     using C = Cfg<RB>;
@@ -198,19 +252,24 @@ struct ResW {
     const int c0 = (int)(u / n_blk) * BN;
     tma_load_2d(sa, &m_phi, fb, kb * KE, n0);
     tma_load_2d(sa + C::A_TILE, &m_plo, fb, kb * KE, n0);
-    tma_load_2d(sa + 2 * C::A_TILE, &m_qhi, fb, kb * KE, c0);
-    tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE, &m_qlo, fb, kb * KE, c0);
+    const bool s = producer_spare_in() != 0;
+    tma_load_2d(sa + 2 * C::A_TILE, s ? &m_shi : &m_qhi, fb, kb * KE, c0);
+    tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE, s ? &m_slo : &m_qlo, fb, kb * KE, c0);
   }
   __device__ __forceinline__ void convert(int64_t, int, uint8_t*, int) const {}
+  __device__ __forceinline__ float sq_alt(float eps, float sq) const {
+    return next_plane_scale(scales, pass, eps, mul(eps, p_scale), sq);
+  }
   __device__ __forceinline__ void epilogue(int64_t u, uint32_t trow, int quarter, int lane,
-                                           EpiState&) const {
+                                           EpiState& st) const {
     const int nb = (int)(u % n_blk);
     const int n = nb * BM + quarter * 32 + lane;
     const int64_t c0 = (u / n_blk) * BN;
     const bool n_ok = n < D();
     const float eps = state[ZSB_ST_EPS_USED];
     const float s2 = mul(eps, p_scale);
-    const float sq = scales[0];
+    const bool spare_in = plane_spare_in(scales, pass);
+    const float sq = plane_scale_in(scales, pass);
     const float m_n = n_ok ? mass[n] : 1.f;
     const float eps_over_m_sq = mul(fdiv(eps, m_n), sq);
     const float inv_m = fdiv(1.f, m_n);
@@ -218,42 +277,67 @@ struct ResW {
     const float mu_n = (n_ok && mu) ? mu[n] : 0.f;
     const int64_t part_row = (int64_t)(nb * 4 + quarter) * ea.chains;
     ResEpi a = ea;
+    if (spare_in) {
+      a.hi_cur = ea.hi_cur_s;
+      a.lo_cur = ea.lo_cur_s;
+    }
     a.sq = sq;
     a.inv_sq = fdiv(1.f, sq);
-    a.acc_scale = scales[1];
-    epilogue_planes<MODE, NEXT, DC>(a, trow, n, n_ok, true, c0, part_row, lane, s2,
-                                    eps_over_m_sq, inv_m, b_n, mu_n, false);
+    a.acc_scale = 1.f / (scales[3] * sq);                   // powers of two: exact
+    a.rescale = NEXT ? sq_alt(eps, sq) * a.inv_sq : 1.f;
+    if (a.rescale == 1.f)
+      epilogue_planes<MODE, NEXT, DC, false>(a, trow, n, n_ok, true, c0, part_row, lane, s2,
+                                             eps_over_m_sq, inv_m, b_n, mu_n, false, st.qmax);
+    else
+      epilogue_planes<MODE, NEXT, DC, true>(a, trow, n, n_ok, true, c0, part_row, lane, s2,
+                                            eps_over_m_sq, inv_m, b_n, mu_n, false, st.qmax);
   }
-  __device__ __forceinline__ void epi_finish(EpiState&, int, int) const {}
+  __device__ __forceinline__ void epi_finish(EpiState& st, int quarter, int lane) const {
+    if (!NEXT) return;
+    const float sq = plane_scale_in(scales, pass);
+    const float alt = sq_alt(state[ZSB_ST_EPS_USED], sq);
+    // qmax is exact when there is a spare copy: the planes at sq overflowed iff it reached 65520
+    publish_plane_scale(scales, pass, sq, alt, st.qmax * (1.f / sq),
+                        alt != sq && !(st.qmax < kHalfOverflow), quarter, lane);
+  }
 };
 
 template <int DC>
 int res_pass(const CUtensorMap& phi, const CUtensorMap& plo, const CUtensorMap& qhi,
-             const CUtensorMap& qlo, const ResEpi& ea, const float* bvec, const float* mu,
-             const float* mass, const float* state, const float* scales, float p_scale, int n_blk,
-             int D, int mode, cudaStream_t st) {
+             const CUtensorMap& qlo, const CUtensorMap& shi, const CUtensorMap& slo,
+             const ResEpi& ea, const float* bvec, const float* mu, const float* mass,
+             const float* state, float* scales, int pass, float p_scale, int n_blk, int D,
+             int mode, cudaStream_t st) {
   if (mode == 1) {
-    const ResW<1, 1, DC> w{phi, plo, qhi, qlo, ea, bvec, mu, mass, state, scales, p_scale, n_blk, D};
+    const ResW<1, 1, DC> w{phi, plo, qhi, qlo, shi, slo, ea, bvec, mu, mass, state, scales,
+                           p_scale, n_blk, D, pass};
     return tc_launch(w, st, "hmc_dense_resident");
   }
   if (mode == 0) {
-    const ResW<0, 1, DC> w{phi, plo, qhi, qlo, ea, bvec, mu, mass, state, scales, p_scale, n_blk, D};
+    const ResW<0, 1, DC> w{phi, plo, qhi, qlo, shi, slo, ea, bvec, mu, mass, state, scales,
+                           p_scale, n_blk, D, pass};
     return tc_launch(w, st, "hmc_dense_resident");
   }
-  const ResW<2, 0, DC> w{phi, plo, qhi, qlo, ea, bvec, mu, mass, state, scales, p_scale, n_blk, D};
+  const ResW<2, 0, DC> w{phi, plo, qhi, qlo, shi, slo, ea, bvec, mu, mass, state, scales, p_scale,
+                         n_blk, D, pass};
   return tc_launch(w, st, "hmc_dense_resident");
 }
 
-// q[c, :] <- (hi + lo) / sq of the proposal planes where accept[c] (hmc.py:488-497).
+// q[c, :] <- (hi + lo) / sq of the proposal planes where accept[c] (hmc.py:488-497); scales[0] is
+// the sq of `planes`.  With `spare` (impl 5), `scales` is the proposal's plane-scale record, and
+// its overflow flag selects the spare planes at scales[1].
 // One warp per chain at a time (the accept flag is warp-uniform: a rejected chain costs one 4-byte
 // load), 8 dimensions per lane and step: two 128-bit plane loads in, two 128-bit stores out, up to
 // four steps' loads issued before the first use.  D % 8 == 0 (the dense kernels need D % 64 == 0).
 __global__ void __launch_bounds__(256) select_planes_kernel(float* __restrict__ q,
                                                             const __half* __restrict__ planes,
+                                                            const __half* __restrict__ spare,
                                                             const float* __restrict__ scales,
                                                             const int32_t* __restrict__ accept,
                                                             int64_t chains, int64_t D) {
-  const float inv_sq = 1.f / scales[0];
+  const bool use_spare = spare && __float_as_uint(scales[3]) != 0u;
+  const float inv_sq = 1.f / scales[use_spare ? 1 : 0];
+  if (use_spare) planes = spare;
   const int lane = threadIdx.x & 31;
   const int n8 = (int)(D >> 3);
   const int64_t wstride = (int64_t)gridDim.x * 8;
@@ -300,13 +384,16 @@ int zsb_dense_res_group_blocks(int D) {
 }
 
 // The L+1 passes of a trajectory for every chain (D % 64 == 0, L >= 1).
-//   planes0: fp16 hi/lo planes of q * sq (zsb_hmc_dense_h16_prepare_f32), planes1: work buffer of
+//   planes0: fp16 hi/lo planes of q * sq_0 (zsb_hmc_dense_h16_prepare_f32), planes1: work buffer of
 //   the same size (must differ from planes0: a pass reads every dimension of a chain block's planes
 //   while other tiles of the same launch write the next ones); on return the proposal's planes are
-//   in buffer (L & 1); p0 -> pw (final momentum); lp0_part / lp1_part / k_part as the per-pass
-//   kernel writes them.  `flags` is not used.
-int zsb_dense_res_h16_launch(void* planes0, void* planes1, const float* p0, float* pw,
-                             const void* P_h16, const void* P_l16, const float* scales,
+//   in buffer (L & 1), or in spare buffer (L & 1) when record L flags them; spare0 / spare1: two
+//   more buffers of that size for the spare copies; p0 -> pw (final momentum); lp0_part /
+//   lp1_part / k_part as the per-pass kernel writes them; pass i writes plane-scale record i + 1.
+//   `flags` is not used.
+int zsb_dense_res_h16_launch(void* planes0, void* planes1, void* spare0, void* spare1,
+                             const float* p0, float* pw,
+                             const void* P_h16, const void* P_l16, float* scales,
                              const float* bvec, const float* mu, const float* mass,
                              const float* state, float* lp0_part, float* lp1_part, float* k_part,
                              int* flags, int64_t chains, int D, int L, cudaStream_t st) {
@@ -315,20 +402,24 @@ int zsb_dense_res_h16_launch(void* planes0, void* planes1, const float* p0, floa
     zsb_set_error("dense_res: needs D %% 64 == 0, n_leapfrogs >= 1");
     return ZSB_ERR_INVALID;
   }
-  if (planes0 == planes1) {
-    zsb_set_error("dense_res: planes1 must be a separate work buffer");
+  if (planes0 == planes1 || !spare0 || !spare1 || spare0 == spare1) {
+    zsb_set_error("dense_res: planes1, spare0 and spare1 must be separate work buffers");
     return ZSB_ERR_INVALID;
   }
-  CUtensorMap phi, plo, qhi[2], qlo[2];
+  CUtensorMap phi, plo, qhi[2], qlo[2], shi[2], slo[2];
   int rc;
   constexpr int RB = ResW<0, 1, 0>::RB;
   if ((rc = make_map(&phi, P_h16, (uint64_t)D, (uint64_t)D, BM, RB, 1))) return rc;
   if ((rc = make_map(&plo, P_l16, (uint64_t)D, (uint64_t)D, BM, RB, 1))) return rc;
   __half* pl[2] = {reinterpret_cast<__half*>(planes0), reinterpret_cast<__half*>(planes1)};
+  __half* sp[2] = {reinterpret_cast<__half*>(spare0), reinterpret_cast<__half*>(spare1)};
   const int64_t plane = chains * (int64_t)D;
   for (int b = 0; b < 2; ++b) {
     if ((rc = make_map(&qhi[b], pl[b], (uint64_t)chains, (uint64_t)D, BN, RB, 1))) return rc;
     if ((rc = make_map(&qlo[b], pl[b] + plane, (uint64_t)chains, (uint64_t)D, BN, RB, 1)))
+      return rc;
+    if ((rc = make_map(&shi[b], sp[b], (uint64_t)chains, (uint64_t)D, BN, RB, 1))) return rc;
+    if ((rc = make_map(&slo[b], sp[b] + plane, (uint64_t)chains, (uint64_t)D, BN, RB, 1)))
       return rc;
   }
   const int n_blk = (D + BM - 1) / BM;
@@ -336,27 +427,29 @@ int zsb_dense_res_h16_launch(void* planes0, void* planes1, const float* p0, floa
     const bool last = i == L;
     const int buf = i & 1;
     const ResEpi ea{pl[buf], pl[buf] + plane, pl[buf ^ 1], pl[buf ^ 1] + plane,
+                    sp[buf], sp[buf] + plane, sp[buf ^ 1], sp[buf ^ 1] + plane,
                     i == 0 ? p0 : pw, pw, i == 0 ? lp0_part : lp1_part, k_part, chains, D,
-                    1.f, 1.f, 1.f};
+                    1.f, 1.f, 1.f, 1.f};
     const int mode = last ? 2 : (i == 0 ? 1 : 0);
     const float p_scale = (i > 0 && !last) ? 1.f : 0.5f;
-    rc = (D == 1024) ? res_pass<1024>(phi, plo, qhi[buf], qlo[buf], ea, bvec, mu, mass, state,
-                                      scales, p_scale, n_blk, D, mode, st)
-                     : res_pass<0>(phi, plo, qhi[buf], qlo[buf], ea, bvec, mu, mass, state,
-                                   scales, p_scale, n_blk, D, mode, st);
+    rc = (D == 1024) ? res_pass<1024>(phi, plo, qhi[buf], qlo[buf], shi[buf], slo[buf], ea, bvec,
+                                      mu, mass, state, scales, i, p_scale, n_blk, D, mode, st)
+                     : res_pass<0>(phi, plo, qhi[buf], qlo[buf], shi[buf], slo[buf], ea, bvec, mu,
+                                   mass, state, scales, i, p_scale, n_blk, D, mode, st);
     if (rc != ZSB_OK) return rc;
   }
   return ZSB_OK;
 }
 
-int zsb_dense_select_planes_launch(float* q, const void* planes, const float* scales,
-                                   const int32_t* accept, int64_t chains, int64_t D,
-                                   cudaStream_t st) {
+int zsb_dense_select_planes_launch(float* q, const void* planes, const void* spare,
+                                   const float* scales, const int32_t* accept, int64_t chains,
+                                   int64_t D, cudaStream_t st) {
   ZSB_REQUIRE(D % 8 == 0, "zsb_dense_select_planes: D must be a multiple of 8");
   int64_t blocks = zsb_ceil_div(chains, 8);
   if (blocks > ZSB_NUM_SMS * 16) blocks = ZSB_NUM_SMS * 16;
   if (blocks < 1) blocks = 1;
   select_planes_kernel<<<(unsigned)blocks, 256, 0, st>>>(
-      q, reinterpret_cast<const __half*>(planes), scales, accept, chains, D);
+      q, reinterpret_cast<const __half*>(planes), reinterpret_cast<const __half*>(spare), scales,
+      accept, chains, D);
   return zsb_check_launch("hmc_select_planes");
 }

@@ -9,7 +9,8 @@
 //   impl 1  TF32 operands:  q = q_hi + q_lo,  P = P_hi + P_lo  (hi = top 19 bits, what the TF32
 //           datapath reads);  P q ~= P_hi q_hi + P_hi q_lo + P_lo q_hi  (dropped term ~2^-22)
 //   impl 2  fp16 operands:  hi / lo planes of P*sP and q*sq (powers of two), three fp16 products at
-//           twice the TF32 rate; the pass writes the planes of q_next for the next pass
+//           twice the TF32 rate; the pass writes the planes of q_next for the next pass, at the
+//           scale the a-priori bound on |q_next| gives (hmc_dense_epilogue.cuh)
 //   impl 3  as impl 2, but the MMA warpgroup builds the planes of q from the fp32 rows itself
 //           (no plane buffers in HBM); sq comes from the running max|q| the previous pass left
 // The GEMM is computed TRANSPOSED, G^T[n, c] = sum_k P[n, k] q[c, k]  (A = P rows, B = chain rows,
@@ -32,7 +33,7 @@ struct DenseW {
   CUtensorMap m_phi, m_plo, m_qhi, m_qlo;
   EpiArgs ea;
   const float* bvec; const float* mu; const float* mass; const float* state;
-  float* scales;                                           // OP 1: {sq, 1/(sP sq), -, sP, slots}
+  float* scales;             // H16 1: plane-scale records (hmc_dense_epilogue.cuh); 2: {-, -, -, sP, slots}
   float p_scale;
   int n_blk, D_rt, pass_index;
   struct EpiState { float amax = 0.f; };
@@ -118,12 +119,26 @@ struct DenseW {
     const float mu_n = (n_ok && mu) ? mu[n] : 0.f;
     const int64_t part_row = (int64_t)(nb * 4 + quarter) * ea.chains;
     EpiArgs a = ea;
-    if (H16 == 1) { a.q_scale = scales[0]; a.acc_scale = scales[1]; }
+    if (H16 == 1 && pass_index < 0) {   // one scale for every pass: {sq, 1/(sP sq)}
+      a.q_scale = scales[0];
+      a.acc_scale = scales[1];
+    }
+    if (H16 == 1 && pass_index >= 0) {  // planes of q_cur at sq_i, those of q_next at sq_alt
+      const float sq = scale_rec(scales, pass_index)[0];
+      a.acc_scale = 1.f / (scales[3] * sq);                  // powers of two: exact
+      a.q_scale = ea.q_next ? next_plane_scale(scales, pass_index, eps, s2, sq) : sq;
+    }
     if (H16 == 2) a.acc_scale = 1.f / (scales[3] * sq3());   // powers of two: exact
     epilogue_half_tile<MODE, -1, DC, H16>(a, trow, n, n_ok, true, c0, part_row, lane, s2,
                                           eps_over_m, inv_m, b_n, mu_n, false, st.amax);
   }
   __device__ __forceinline__ void epi_finish(EpiState& st, int quarter, int lane) const {
+    if (H16 == 1 && pass_index >= 0 && ea.q_next) {
+      const float eps = state[ZSB_ST_EPS_USED];
+      const float sq = next_plane_scale(scales, pass_index, eps, mul(eps, p_scale),
+                                        scale_rec(scales, pass_index)[0]);
+      publish_plane_scale(scales, pass_index, sq, sq, st.amax, false, quarter, lane);
+    }
     if (H16 != 2) return;
     unsigned int* slots = reinterpret_cast<unsigned int*>(scales) + 4;
     if (ea.q_next) {
@@ -149,30 +164,51 @@ __global__ void __launch_bounds__(256) split_lo_kernel(const float* __restrict__
   }
 }
 
-// fp16-split support (impl 2).  scales[0] = sq (power of two putting max|q| near 2^12: three bits of
-// head-room below fp16's 2^15 so q may grow 8x inside a trajectory), scales[1] = 1/(sP*sq),
-// scales[2] = running max|q| bits (uint), scales[3] = sP.
-__global__ void __launch_bounds__(256) absmax_kernel(const float* __restrict__ q, int64_t n,
-                                                     float* __restrict__ scales) {
-  float m = 0.f;
+// fp16-split support (impl 2, 4, 5).  sq_0 is the power of two putting max|q0| in [2^11, 2^12).
+// max|q0| and (with p) max|p0/m| go to the scratch words 2 and 6 (NaN / inf ignored).
+__global__ void __launch_bounds__(256) absmax_kernel(const float* __restrict__ q,
+                                                     const float* __restrict__ p,
+                                                     const float* __restrict__ mass, int64_t n,
+                                                     int64_t D, float* __restrict__ scales) {
+  float mq = 0.f, mv = 0.f;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (int64_t)gridDim.x * blockDim.x) {
-    const float a = fabsf(q[i]);
-    m = (a == a && a <= 3.0e38f) ? fmaxf(m, a) : m;       // ignore NaN / inf
+    mq = finite_absmax(mq, q[i]);
+    if (p) mv = finite_absmax(mv, fdiv(p[i], mass[i % D]));
   }
-  m = warp_max(m);
-  if ((threadIdx.x & 31) == 0)
-    atomicMax(reinterpret_cast<unsigned int*>(scales) + 2, __float_as_uint(m));
+  mq = warp_max(mq);
+  mv = warp_max(mv);
+  if ((threadIdx.x & 31) == 0) {
+    atomicMax(reinterpret_cast<unsigned int*>(scales) + 2, __float_as_uint(mq));
+    if (p) atomicMax(reinterpret_cast<unsigned int*>(scales) + 6, __float_as_uint(mv));
+  }
 }
-__global__ void scale_kernel(float* __restrict__ scales) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  const float m = __uint_as_float(reinterpret_cast<unsigned int*>(scales)[2]);
-  int e = 0;
-  if (m > 0.f) frexpf(m, &e);              // m = f * 2^e, f in [0.5, 1)  ->  m < 2^e
-  const float sq = ldexpf(1.f, 12 - e);    // max|q| * sq in [2^11, 2^12)
+// one warp: scales[0] = sq, scales[1] = 1/(sP*sq) from the scratch max (reset for the next call).
+// With the mass (trajectory form): also max(1/m) and record 0, and clears record 1, which pass 0
+// fills.
+__global__ void scale_kernel(float* __restrict__ scales, const float* __restrict__ mass,
+                             int64_t D) {
+  float w = 0.f;
+  if (mass)
+    for (int64_t i = threadIdx.x; i < D; i += 32) w = finite_absmax(w, fdiv(1.f, mass[i]));
+  w = warp_max(w);
+  if (threadIdx.x != 0) return;
+  unsigned int* u = reinterpret_cast<unsigned int*>(scales);
+  const float mq = __uint_as_float(u[2]), mv = __uint_as_float(u[6]);
+  const float sq = pow2_plane_scale(mq);
   scales[0] = sq;
   scales[1] = 1.f / (scales[3] * sq);
-  reinterpret_cast<unsigned int*>(scales)[2] = 0u;   // reset the running max for the next call
+  u[2] = 0u;
+  if (!mass) return;
+  float* r0 = scales + kScaleHdr;
+  r0[0] = sq;
+  r0[1] = sq;
+  r0[2] = mq;
+  r0[3] = mv;
+  u[kScaleHdr + kScaleRec + 2] = 0u;
+  u[kScaleHdr + kScaleRec + 3] = 0u;
+  scales[7] = w;
+  u[6] = 0u;
 }
 __global__ void __launch_bounds__(256) split16_kernel(const float* __restrict__ q,
                                                       __half* __restrict__ planes, int64_t n,
@@ -307,21 +343,23 @@ int zsb_dense_split_lo_launch(const float* q, float* lo, int64_t n, cudaStream_t
 // ---- impl 2: fp16-split operands ----
 int zsb_dense_leapfrog_h16_launch(const float* q_cur, const void* q_cur_planes, float* q_next,
                                   void* q_next_planes, const float* p_in, float* p_out,
-                                  const void* P_h16, const void* P_l16, const float* scales,
-                                  const float* bvec, const float* mu, const float* mass,
-                                  const float* state, float p_scale, float* lp_part, float* k_part,
-                                  int64_t chains, int D, cudaStream_t st) {
+                                  const void* P_h16, const void* P_l16, float* scales,
+                                  int pass_index, const float* bvec, const float* mu,
+                                  const float* mass, const float* state, float p_scale,
+                                  float* lp_part, float* k_part, int64_t chains, int D,
+                                  cudaStream_t st) {
   if (D % 64 != 0 || D < 64) {
     zsb_set_error("dense_h16: D must be a multiple of 64");
     return ZSB_ERR_INVALID;
   }
-  if (chains >= (1LL << 31) || (q_next && !q_next_planes) || !q_cur_planes || !scales) {
+  if (chains >= (1LL << 31) || (q_next && !q_next_planes) || !q_cur_planes || !scales ||
+      pass_index < -1) {
     zsb_set_error("dense_h16: bad arguments");
     return ZSB_ERR_INVALID;
   }
   return launch_dense<1, 128, 1>(q_cur, q_cur_planes, q_next, q_next_planes, p_in, p_out, P_h16,
                                  P_l16, bvec, mu, mass, state, p_scale, lp_part, k_part, chains, D,
-                                 const_cast<float*>(scales), 0, st, "hmc_dense_leapfrog_h16");
+                                 scales, pass_index, st, "hmc_dense_leapfrog_h16");
 }
 
 // impl 3 (in-kernel split).  scales: float[8] device scratch with scales[3] = sP.
@@ -352,14 +390,16 @@ int zsb_dense_h16i_prepare_launch(const float* q, float* scales, int64_t n, cuda
   return zsb_check_launch("hmc_dense_h16i_prepare");
 }
 
-// scales[3] must hold sP on entry; computes sq from max|q| and writes the fp16 hi/lo planes.
-int zsb_dense_h16_prepare_launch(const float* q, void* planes, float* scales, int64_t n,
-                                 cudaStream_t st) {
+// scales[3] must hold sP on entry; writes sq_0 and q's fp16 hi/lo planes at sq_0.  With p and the
+// mass (trajectory form: scales[4], [5] = ||P||_inf, max|b| on entry) also plane-scale record 0.
+int zsb_dense_h16_prepare_launch(const float* q, const float* p, const float* mass, void* planes,
+                                 float* scales, int64_t chains, int64_t D, cudaStream_t st) {
+  const int64_t n = chains * D;
   int64_t blocks = zsb_ceil_div(n, 256 * 8);
   if (blocks > ZSB_NUM_SMS * 16) blocks = ZSB_NUM_SMS * 16;
   if (blocks < 1) blocks = 1;
-  absmax_kernel<<<(unsigned)blocks, 256, 0, st>>>(q, n, scales);
-  scale_kernel<<<1, 32, 0, st>>>(scales);
+  absmax_kernel<<<(unsigned)blocks, 256, 0, st>>>(q, p, mass, n, D, scales);
+  scale_kernel<<<1, 32, 0, st>>>(scales, mass, D);
   split16_kernel<<<(unsigned)blocks, 256, 0, st>>>(q, reinterpret_cast<__half*>(planes), n, scales);
   return zsb_check_launch("hmc_dense_h16_prepare");
 }

@@ -7,17 +7,19 @@
 
 int zsb_dense_leapfrog_h16_launch(const float* q_cur, const void* q_cur_planes, float* q_next,
                                   void* q_next_planes, const float* p_in, float* p_out,
-                                  const void* P_h16, const void* P_l16, const float* scales,
-                                  const float* bvec, const float* mu, const float* mass,
-                                  const float* state, float p_scale, float* lp_part, float* k_part,
-                                  int64_t chains, int D, cudaStream_t st);
+                                  const void* P_h16, const void* P_l16, float* scales,
+                                  int pass_index, const float* bvec, const float* mu,
+                                  const float* mass, const float* state, float p_scale,
+                                  float* lp_part, float* k_part, int64_t chains, int D,
+                                  cudaStream_t st);
 
 //   q0 / planes0: current state and its fp16 planes (zsb_hmc_dense_h16_prepare_f32);
 //   qa, qb, planes_a, planes_b: work buffers; on return the proposal is in (L-1 even ? qa : qb);
-//   p0 -> pw (final momentum); lp0_part / lp1_part / k_part as the per-pass kernel writes them.
+//   p0 -> pw (final momentum); lp0_part / lp1_part / k_part and the plane-scale records as the
+//   per-pass kernel writes them (pass i = launch i).
 int zsb_dense_traj_h16_launch(const float* q0, const void* planes0, float* qa, void* planes_a,
                               float* qb, void* planes_b, const float* p0, float* pw,
-                              const void* P_h16, const void* P_l16, const float* scales,
+                              const void* P_h16, const void* P_l16, float* scales,
                               const float* bvec, const float* mu, const float* mass,
                               const float* state, float* lp0_part, float* lp1_part,
                               float* k_part, int64_t chains, int D, int L, cudaStream_t st) {
@@ -34,7 +36,7 @@ int zsb_dense_traj_h16_launch(const float* q0, const void* planes0, float* qa, v
     const bool last = i == L;
     const int rc = zsb_dense_leapfrog_h16_launch(
         cur, cur_pl, last ? nullptr : nxt, last ? nullptr : nxt_pl, p_in, pw, P_h16, P_l16,
-        scales, bvec, mu, mass, state, (i > 0 && !last) ? 1.f : 0.5f,
+        scales, i, bvec, mu, mass, state, (i > 0 && !last) ? 1.f : 0.5f,
         i == 0 ? lp0_part : (last ? lp1_part : nullptr), last ? k_part : nullptr, chains, D, st);
     if (rc != ZSB_OK) return rc;
     p_in = pw;

@@ -65,6 +65,10 @@ class GaussianLogJoint(object):
         h16 = x.astype(np.float16)
         l16 = (x - h16.astype(np.float64)).astype(np.float16)
         d["sP"] = sP
+        # bounds the fp16-split trajectory uses to keep the planes of q inside fp16's range
+        # (hmc_dense_epilogue.cuh): |g| <= max|b| + ||P||_inf max|q|
+        d["P_inf"] = float(np.abs(P32.astype(np.float64)).sum(1).max())
+        d["b_max"] = float(d["b"].abs().max()) if "b" in d else 0.0
         d["P_h16"] = torch.as_tensor(h16, device=device).contiguous()
         d["P_l16"] = torch.as_tensor(l16, device=device).contiguous()
         self._zsb_fused = d

@@ -572,7 +572,8 @@ class HMC(object):
         if int(impl) in (2, 3, 5) and D % 64 != 0:
             raise ValueError("dense_impl=2/3/5 (fp16 split) needs D % 64 == 0")
         # impl 5: whole-trajectory entry point (hmc_dense_res.cu).  The state of q inside a
-        # trajectory is its fp16 hi/lo plane pair; the step-size probes are trajectories with
+        # trajectory is its fp16 hi/lo plane pair, at a scale each pass re-derives from a bound
+        # on the q it writes (hmc_dense_epilogue.cuh); the step-size probes are trajectories with
         # L = 1; n_leapfrogs = 0 (a single half-kick pass) runs on the per-pass kernel (impl 2).
         self._res = int(impl) == 5 and self.n_leapfrogs >= 1
         if int(impl) == 5:
@@ -603,8 +604,9 @@ class HMC(object):
             self._res_flags = torch.zeros(
                 lib.load().zsb_hmc_dense_resident_flags(self._chains),
                 dtype=torch.int32, device=dev)
-            self._scales = z(4)
-            self._scales[3] = f["sP"]
+            self._spare = [torch.empty(shape, dtype=torch.float16, device=dev)
+                           for _ in range(2)]
+            self._scales = self._plane_scales(dev)
             return
         self._qa, self._qb = torch.empty_like(self._q[0]), \
             torch.empty_like(self._q[0])
@@ -615,11 +617,22 @@ class HMC(object):
             for t in (self._q[0], self._qa, self._qb):
                 self._lo[t.data_ptr()] = torch.empty(
                     (2,) + tuple(t.shape), dtype=torch.float16, device=dev)
-            self._scales = z(4)
-            self._scales[3] = f["sP"]
+            self._scales = self._plane_scales(dev)
         if self._impl == 3:            # planes are built inside the kernel
             self._scales = z(8)
             self._scales[3] = f["sP"]
+
+    def _plane_scales(self, dev):
+        """Plane-scale records of the fp16-split trajectory (hmc_dense_epilogue.cuh): a header
+        and one record per pass (the probes run L = 1)."""
+        f = self._fused
+        sc = torch.zeros(8 + 4 * (max(self.n_leapfrogs, 1) + 2), dtype=_F32, device=dev)
+        sc[3], sc[4], sc[5] = f["sP"], f["P_inf"], f["b_max"]
+        return sc
+
+    def _plane_scale_of_pass(self, i):
+        """The plane-scale record of the planes pass i reads (from its first word on)."""
+        return self._scales[8 + 4 * i:]
 
     def _dense_pass(self, q_cur, q_next, p_in, p_out, scale, lp_part, k_part,
                     s):
@@ -633,14 +646,15 @@ class HMC(object):
             self._pass_k += 1
             return
         if self._impl == 2:
-            lib.call("zsb_hmc_dense_leapfrog_h16_f32", ptr(q_cur),
+            lib.call("zsb_hmc_dense_leapfrog_h16_pass_f32", ptr(q_cur),
                      ptr(self._lo[q_cur.data_ptr()]), ptr(q_next),
                      ptr(self._lo[q_next.data_ptr()])
                      if q_next is not None else None, ptr(p_in), ptr(p_out),
                      ptr(f["P_h16"]), ptr(f["P_l16"]), ptr(self._scales),
-                     ptr(f.get("b")), ptr(f.get("mu")), ptr(self._mass[0]),
-                     ptr(self._state), scale, ptr(lp_part), ptr(k_part),
-                     self._chains, f["D"], s)
+                     self._pass_k, ptr(f.get("b")), ptr(f.get("mu")),
+                     ptr(self._mass[0]), ptr(self._state), scale, ptr(lp_part),
+                     ptr(k_part), self._chains, f["D"], s)
+            self._pass_k += 1
             return
         tc = self._impl == 1
         lo_cur = self._lo[q_cur.data_ptr()] if tc else None
@@ -673,40 +687,45 @@ class HMC(object):
                  ctypes.byref(self._npart), ptr(self._state), s)
 
     def _resident_trajectory(self, L, s):
-        """L+1 leapfrog passes on the fp16 plane state; returns the proposal's planes."""
+        """L+1 leapfrog passes on the fp16 plane state; returns the buffers that may hold the
+        proposal's planes (their plane-scale record says which)."""
         f = self._fused
         lib.call("zsb_hmc_dense_resident_h16_f32", ptr(self._planes[0]),
-                 ptr(self._planes[1]), ptr(self._p0[0]), ptr(self._pw),
+                 ptr(self._planes[1]), ptr(self._spare[0]), ptr(self._spare[1]),
+                 ptr(self._p0[0]), ptr(self._pw),
                  ptr(f["P_h16"]), ptr(f["P_l16"]), ptr(self._scales), ptr(f.get("b")),
                  ptr(f.get("mu")), ptr(self._mass[0]), ptr(self._state),
                  ptr(self._lp0_part), ptr(self._lp1_part), ptr(self._k_part),
                  ptr(self._res_flags), self._chains, f["D"], L, s)
-        return self._planes[L & 1]
+        return self._planes[L & 1], self._spare[L & 1]
 
     def _iterate_dense_resident(self, noise_u, seed, it, init, s):
         q0 = self._q[0]
 
         def prepare():
-            # planes of q * sq (sq from max|q|) into buffer 0
-            lib.call("zsb_hmc_dense_h16_prepare_f32", ptr(q0), ptr(self._planes[0]),
-                     ptr(self._scales), q0.numel(), s)
-        prepare()
+            # planes of q * sq_0 (sq_0 from max|q|) into buffer 0, plane-scale record 0
+            lib.call("zsb_hmc_dense_traj_prepare_f32", ptr(q0), ptr(self._p0[0]),
+                     ptr(self._mass[0]), ptr(self._planes[0]), ptr(self._scales),
+                     self._chains, self._row_len[0], s)
         if init:
             def probe():               # hmc.py:314-326: one leapfrog step = a trajectory, L = 1
+                prepare()              # every trajectory starts from fresh plane-scale records
                 self._resident_trajectory(1, s)
                 self._dense_finish_mh(noise_u, seed, it, s, full=False)
             self._search(probe, s)
+        prepare()
         prof = None if self._dev_mode else getattr(self, "_profile_events", None)
         if prof is not None:           # bench.py: device time of the trajectory launch
             e0, e1 = torch.cuda.Event(True), torch.cuda.Event(True)
             e0.record()
-        prop = self._resident_trajectory(self.n_leapfrogs, s)
+        prop, spare = self._resident_trajectory(self.n_leapfrogs, s)
         if prof is not None:
             e1.record()
             prof.append((e0, e1))
         self._dense_finish_mh(noise_u, seed, it, s, full=True)
-        lib.call("zsb_hmc_dense_select_planes_f32", ptr(q0), ptr(prop), ptr(self._scales),
-                 ptr(self._accept), self._chains, self._row_len[0], s)
+        lib.call("zsb_hmc_dense_select_traj_planes_f32", ptr(q0), ptr(prop), ptr(spare),
+                 ptr(self._plane_scale_of_pass(self.n_leapfrogs)), ptr(self._accept),
+                 self._chains, self._row_len[0], s)
 
     def _iterate_dense(self, noise_p, noise_u, seed, it, init, s):
         q0 = self._q[0]
@@ -716,15 +735,16 @@ class HMC(object):
         if self._impl == 1:
             lib.call("zsb_hmc_dense_split_lo_f32", ptr(q0),
                      ptr(self._lo[q0.data_ptr()]), q0.numel(), s)
-        elif self._impl == 2:
-            lib.call("zsb_hmc_dense_h16_prepare_f32", ptr(q0),
-                     ptr(self._lo[q0.data_ptr()]), ptr(self._scales),
-                     q0.numel(), s)
-        def prepare3():                # impl 3: seed the max|q| slot, restart the pass count
+
+        def prepare3():                # before every trajectory: restart the pass count; impl 2:
+            if self._impl == 2:        # planes of q0 and plane-scale record 0; impl 3: max|q|
+                lib.call("zsb_hmc_dense_traj_prepare_f32", ptr(q0), ptr(self._p0[0]),
+                         ptr(self._mass[0]), ptr(self._lo[q0.data_ptr()]),
+                         ptr(self._scales), self._chains, self._row_len[0], s)
             if self._impl == 3:
                 lib.call("zsb_hmc_dense_h16i_prepare_f32", ptr(q0),
                          ptr(self._scales), q0.numel(), s)
-                self._pass_k = 0
+            self._pass_k = 0
         if init:
             def probe():
                 prepare3()
