@@ -13,10 +13,17 @@
 //
 // On H100 one pass of the benchmark shape (65 536 chains x 1024 dimensions) executes ~0.4 TFLOP of
 // fp16 products against ~1 GB of state traffic, so the pass is compute-bound, not HBM-bound (on a
-// card with a 400 W power limit it runs at the power cap, with the SM clock lowered to ~800 MHz;
+// card with a 400 W power limit it runs at the power cap, with the SM clock lowered to ~950 MHz;
 // README has the numbers): the passes run as L+1 launches of the persistent tensor-core kernel
 // (tc_pipeline_kernel) on alternating plane buffers, and the sampler state never leaves the plane
 // format between the prepare and the select.
+//
+// Without sharing, every 128 x 128 unit pulls 1 MiB of operand planes from L2 (32 k-blocks of
+// 32 KB), 4.3 GB per pass at the benchmark shape against 1.07 GB of HBM traffic.  Where the units
+// tile by 2 x 2 (an even number of dimension blocks and of chain blocks) the pass runs on clusters
+// of four CTAs that multicast the P and q tiles they share, which halves that to 2.1 GB; the
+// products and their order do not change, so neither do the results.  At a 400 W power limit this
+// lets the power-capped SM clock rise, and the pass gets faster (README has the numbers).
 #include "hmc_dense_epilogue.cuh"
 
 namespace {
@@ -217,11 +224,16 @@ __device__ __forceinline__ int& producer_spare_in() {
   return spare_in;
 }
 
-template <int MODE, int NEXT, int DC>
+// CX x CY: a cluster takes CX dimension blocks of CY chain blocks.  Its CX CTAs on one chain block
+// share that block's q planes and its CY CTAs on one dimension block share that block's P planes:
+// each CTA loads 1/CX of the q tiles and 1/CY of the P tiles and multicasts them to the CTAs that
+// share them, with maps whose boxes are that many rows high.
+template <int MODE, int NEXT, int DC, int CX, int CY>
 struct ResW {
   // 64-byte rows (32 fp16 of contraction per k-block): four 32 KB stages beside the accumulator
   // tile, so the TMA producer runs up to three k-blocks ahead of the tensor cores
   static constexpr int KIND = 1, RB = 64, MNA = 0, MNB = 0, CVT = 0;
+  static constexpr int CLUSTER = CX * CY;
   static constexpr int KE = RB / 2;
   static constexpr uint32_t TX = Cfg<RB>::STAGE;
   CUtensorMap m_phi, m_plo, m_qhi, m_qlo, m_shi, m_slo;   // m_s*: spare planes of q
@@ -236,6 +248,15 @@ struct ResW {
   __host__ __device__ __forceinline__ int64_t units() const {
     return ((ea.chains + BN - 1) / BN) * (int64_t)n_blk;
   }
+  // unit u -> dimension block nb, chain block cb; the CTAs of a cluster take CLUSTER consecutive
+  // units (n_blk % CX == 0, chain blocks % CY == 0)
+  __device__ __forceinline__ void tile(int64_t u, int& nb, int64_t& cb) const {
+    const uint64_t cu = (uint64_t)u / CLUSTER;
+    const int r = (int)((uint64_t)u % CLUSTER);
+    const uint32_t nbx = (uint32_t)(n_blk / CX);
+    nb = (int)(cu % nbx) * CX + r % CX;
+    cb = (int64_t)(cu / nbx) * CY + r / CX;
+  }
   __device__ __forceinline__ void kb_range(int64_t, int& kb0, int& kb1) const {
     kb0 = 0;
     kb1 = D() / KE;
@@ -248,13 +269,37 @@ struct ResW {
   }
   __device__ __forceinline__ void load(int64_t u, int kb, uint32_t sa, uint32_t fb) const {
     using C = Cfg<RB>;
-    const int n0 = (int)(u % n_blk) * BM;
-    const int c0 = (int)(u / n_blk) * BN;
-    tma_load_2d(sa, &m_phi, fb, kb * KE, n0);
-    tma_load_2d(sa + C::A_TILE, &m_plo, fb, kb * KE, n0);
+    int nb;
+    int64_t cb;
+    tile(u, nb, cb);
+    const int n0 = nb * BM;
+    const int c0 = (int)cb * BN;
     const bool s = producer_spare_in() != 0;
-    tma_load_2d(sa + 2 * C::A_TILE, s ? &m_shi : &m_qhi, fb, kb * KE, c0);
-    tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE, s ? &m_slo : &m_qlo, fb, kb * KE, c0);
+    const CUtensorMap* qh = s ? &m_shi : &m_qhi;
+    const CUtensorMap* ql = s ? &m_slo : &m_qlo;
+    const int r = (int)(u % CLUSTER), rx = r % CX, ry = r / CX;   // this CTA's cluster rank
+    if constexpr (CY == 1) {
+      tma_load_2d(sa, &m_phi, fb, kb * KE, n0);
+      tma_load_2d(sa + C::A_TILE, &m_plo, fb, kb * KE, n0);
+    } else {
+      constexpr int rows = BM / CY;
+      uint16_t mask = 0;                                   // the CTAs on dimension block nb
+#pragma unroll
+      for (int y = 0; y < CY; ++y) mask |= (uint16_t)(1u << (y * CX + rx));
+      const uint32_t o = (uint32_t)(ry * rows * RB);
+      tma_load_2d_mc(sa + o, &m_phi, fb, kb * KE, n0 + ry * rows, mask);
+      tma_load_2d_mc(sa + C::A_TILE + o, &m_plo, fb, kb * KE, n0 + ry * rows, mask);
+    }
+    if constexpr (CX == 1) {
+      tma_load_2d(sa + 2 * C::A_TILE, qh, fb, kb * KE, c0);
+      tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE, ql, fb, kb * KE, c0);
+    } else {
+      constexpr int rows = BN / CX;
+      const uint16_t mask = (uint16_t)(((1u << CX) - 1u) << (ry * CX));   // on chain block cb
+      const uint32_t o = (uint32_t)(rx * rows * RB);
+      tma_load_2d_mc(sa + 2 * C::A_TILE + o, qh, fb, kb * KE, c0 + rx * rows, mask);
+      tma_load_2d_mc(sa + 2 * C::A_TILE + C::B_TILE + o, ql, fb, kb * KE, c0 + rx * rows, mask);
+    }
   }
   __device__ __forceinline__ void convert(int64_t, int, uint8_t*, int) const {}
   __device__ __forceinline__ float sq_alt(float eps, float sq) const {
@@ -262,9 +307,11 @@ struct ResW {
   }
   __device__ __forceinline__ void epilogue(int64_t u, uint32_t trow, int quarter, int lane,
                                            EpiState& st) const {
-    const int nb = (int)(u % n_blk);
+    int nb;
+    int64_t cb;
+    tile(u, nb, cb);
     const int n = nb * BM + quarter * 32 + lane;
-    const int64_t c0 = (u / n_blk) * BN;
+    const int64_t c0 = cb * BN;
     const bool n_ok = n < D();
     const float eps = state[ZSB_ST_EPS_USED];
     const float s2 = mul(eps, p_scale);
@@ -302,25 +349,41 @@ struct ResW {
   }
 };
 
-template <int DC>
+// Cluster shape of the pass (CX dimension blocks x CY chain blocks) where the unit grid tiles by
+// it; other shapes run without clusters.
+constexpr int RES_CX = 2, RES_CY = 2;
+
+template <int DC, int CX, int CY>
 int res_pass(const CUtensorMap& phi, const CUtensorMap& plo, const CUtensorMap& qhi,
              const CUtensorMap& qlo, const CUtensorMap& shi, const CUtensorMap& slo,
              const ResEpi& ea, const float* bvec, const float* mu, const float* mass,
              const float* state, float* scales, int pass, float p_scale, int n_blk, int D,
              int mode, cudaStream_t st) {
   if (mode == 1) {
-    const ResW<1, 1, DC> w{phi, plo, qhi, qlo, shi, slo, ea, bvec, mu, mass, state, scales,
-                           p_scale, n_blk, D, pass};
+    const ResW<1, 1, DC, CX, CY> w{phi, plo, qhi, qlo, shi, slo, ea, bvec, mu, mass, state,
+                                   scales, p_scale, n_blk, D, pass};
     return tc_launch(w, st, "hmc_dense_resident");
   }
   if (mode == 0) {
-    const ResW<0, 1, DC> w{phi, plo, qhi, qlo, shi, slo, ea, bvec, mu, mass, state, scales,
-                           p_scale, n_blk, D, pass};
+    const ResW<0, 1, DC, CX, CY> w{phi, plo, qhi, qlo, shi, slo, ea, bvec, mu, mass, state,
+                                   scales, p_scale, n_blk, D, pass};
     return tc_launch(w, st, "hmc_dense_resident");
   }
-  const ResW<2, 0, DC> w{phi, plo, qhi, qlo, shi, slo, ea, bvec, mu, mass, state, scales, p_scale,
-                         n_blk, D, pass};
+  const ResW<2, 0, DC, CX, CY> w{phi, plo, qhi, qlo, shi, slo, ea, bvec, mu, mass, state, scales,
+                                 p_scale, n_blk, D, pass};
   return tc_launch(w, st, "hmc_dense_resident");
+}
+
+template <int DC>
+int res_pass(bool cluster, const CUtensorMap& phi, const CUtensorMap& plo, const CUtensorMap& qhi,
+             const CUtensorMap& qlo, const CUtensorMap& shi, const CUtensorMap& slo,
+             const ResEpi& ea, const float* bvec, const float* mu, const float* mass,
+             const float* state, float* scales, int pass, float p_scale, int n_blk, int D,
+             int mode, cudaStream_t st) {
+  return cluster ? res_pass<DC, RES_CX, RES_CY>(phi, plo, qhi, qlo, shi, slo, ea, bvec, mu, mass,
+                                                state, scales, pass, p_scale, n_blk, D, mode, st)
+                 : res_pass<DC, 1, 1>(phi, plo, qhi, qlo, shi, slo, ea, bvec, mu, mass, state,
+                                      scales, pass, p_scale, n_blk, D, mode, st);
 }
 
 // q[c, :] <- (hi + lo) / sq of the proposal planes where accept[c] (hmc.py:488-497); scales[0] is
@@ -406,23 +469,26 @@ int zsb_dense_res_h16_launch(void* planes0, void* planes1, void* spare0, void* s
     zsb_set_error("dense_res: planes1, spare0 and spare1 must be separate work buffers");
     return ZSB_ERR_INVALID;
   }
+  const int n_blk = (D + BM - 1) / BM;
+  const int64_t c_blk = (chains + BN - 1) / BN;
+  const bool cluster = n_blk % RES_CX == 0 && c_blk % RES_CY == 0;
+  const uint32_t p_box = cluster ? BM / RES_CY : BM, q_box = cluster ? BN / RES_CX : BN;
   CUtensorMap phi, plo, qhi[2], qlo[2], shi[2], slo[2];
   int rc;
-  constexpr int RB = ResW<0, 1, 0>::RB;
-  if ((rc = make_map(&phi, P_h16, (uint64_t)D, (uint64_t)D, BM, RB, 1))) return rc;
-  if ((rc = make_map(&plo, P_l16, (uint64_t)D, (uint64_t)D, BM, RB, 1))) return rc;
+  constexpr int RB = ResW<0, 1, 0, 1, 1>::RB;
+  if ((rc = make_map(&phi, P_h16, (uint64_t)D, (uint64_t)D, p_box, RB, 1))) return rc;
+  if ((rc = make_map(&plo, P_l16, (uint64_t)D, (uint64_t)D, p_box, RB, 1))) return rc;
   __half* pl[2] = {reinterpret_cast<__half*>(planes0), reinterpret_cast<__half*>(planes1)};
   __half* sp[2] = {reinterpret_cast<__half*>(spare0), reinterpret_cast<__half*>(spare1)};
   const int64_t plane = chains * (int64_t)D;
   for (int b = 0; b < 2; ++b) {
-    if ((rc = make_map(&qhi[b], pl[b], (uint64_t)chains, (uint64_t)D, BN, RB, 1))) return rc;
-    if ((rc = make_map(&qlo[b], pl[b] + plane, (uint64_t)chains, (uint64_t)D, BN, RB, 1)))
+    if ((rc = make_map(&qhi[b], pl[b], (uint64_t)chains, (uint64_t)D, q_box, RB, 1))) return rc;
+    if ((rc = make_map(&qlo[b], pl[b] + plane, (uint64_t)chains, (uint64_t)D, q_box, RB, 1)))
       return rc;
-    if ((rc = make_map(&shi[b], sp[b], (uint64_t)chains, (uint64_t)D, BN, RB, 1))) return rc;
-    if ((rc = make_map(&slo[b], sp[b] + plane, (uint64_t)chains, (uint64_t)D, BN, RB, 1)))
+    if ((rc = make_map(&shi[b], sp[b], (uint64_t)chains, (uint64_t)D, q_box, RB, 1))) return rc;
+    if ((rc = make_map(&slo[b], sp[b] + plane, (uint64_t)chains, (uint64_t)D, q_box, RB, 1)))
       return rc;
   }
-  const int n_blk = (D + BM - 1) / BM;
   for (int i = 0; i <= L; ++i) {
     const bool last = i == L;
     const int buf = i & 1;
@@ -432,10 +498,11 @@ int zsb_dense_res_h16_launch(void* planes0, void* planes1, void* spare0, void* s
                     1.f, 1.f, 1.f, 1.f};
     const int mode = last ? 2 : (i == 0 ? 1 : 0);
     const float p_scale = (i > 0 && !last) ? 1.f : 0.5f;
-    rc = (D == 1024) ? res_pass<1024>(phi, plo, qhi[buf], qlo[buf], shi[buf], slo[buf], ea, bvec,
-                                      mu, mass, state, scales, i, p_scale, n_blk, D, mode, st)
-                     : res_pass<0>(phi, plo, qhi[buf], qlo[buf], shi[buf], slo[buf], ea, bvec, mu,
-                                   mass, state, scales, i, p_scale, n_blk, D, mode, st);
+    rc = (D == 1024)
+             ? res_pass<1024>(cluster, phi, plo, qhi[buf], qlo[buf], shi[buf], slo[buf], ea, bvec,
+                              mu, mass, state, scales, i, p_scale, n_blk, D, mode, st)
+             : res_pass<0>(cluster, phi, plo, qhi[buf], qlo[buf], shi[buf], slo[buf], ea, bvec, mu,
+                           mass, state, scales, i, p_scale, n_blk, D, mode, st);
     if (rc != ZSB_OK) return rc;
   }
   return ZSB_OK;

@@ -14,6 +14,14 @@
 //   warps 5-8   epilogue: warp w owns accumulator rows 32*(w-5) .. +32, all 128 columns
 // A unit is a 128 (rows of operand A) x 128 (rows of operand B) output tile; the three products of
 // the fp32-accuracy split (lo*hi, hi*lo, hi*hi) accumulate into the same registers.
+//
+// A work descriptor may declare CLUSTER > 1 (only the dense leapfrog pass, ResW, does): the CTAs
+// then run as thread-block clusters of CLUSTER consecutive blocks, which take CLUSTER consecutive
+// units per round and run the same k-block sequence.  Operand tiles two CTAs of a cluster share
+// are fetched from L2 once: each CTA loads its slice of the tile and multicasts it into every
+// CTA that uses it, so a stage of one CTA is written by several producers.  Every CTA still
+// arms its own full barrier for the whole stage; its empty barrier counts one release from each
+// CTA of the cluster, so no producer overwrites a stage that a peer has not finished reading.
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -88,6 +96,31 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       " [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
+}
+// tma_load_2d into the same shared offset of every CTA of the cluster in `mask`; each of them
+// counts the box's bytes on its own barrier at offset `bar`
+__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* map, uint32_t bar,
+                                               int c0, int c1, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
+      ".multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "h"(mask)
+      : "memory");
+}
+// arrive on the barrier at offset `bar` of cluster CTA `cta`.  Only for releasing a stage whose
+// reads have completed (wgmma.wait_group): no memory operation is ordered by it, and a
+// .release.cluster arrive would cost a MEMBAR.ALL.GPU before every call.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 rb;\n\t"
+      "mapa.shared::cluster.u32 rb, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [rb];\n\t}"
+      ::"r"(bar), "r"(cta)
+      : "memory");
+}
+// every thread of every CTA of the cluster
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
@@ -199,9 +232,21 @@ __device__ __forceinline__ void mma_kblock(float (&d)[2][64], uint32_t sa) {
 //   units(), kb_range(u, kb0, kb1)
 //   load(u, kb, stage_addr, bar)  the TMA loads of one stage (W::TX bytes)
 //   EpiState, epilogue(u, acc_row_addr, quarter, lane, st), epi_finish(st, quarter, lane)
+//   CLUSTER (optional, default 1)  CTAs per cluster; units() is then a multiple of it, and unit u
+//                                 runs on cluster CTA u % CLUSTER
+template <class W, class = void>
+struct ClusterOf {
+  static constexpr int value = 1;
+};
+template <class W>
+struct ClusterOf<W, decltype((void)W::CLUSTER)> {
+  static constexpr int value = W::CLUSTER;
+};
+
 template <class W>
 __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __grid_constant__ W w) {
   using C = Cfg<W::RB>;
+  constexpr int CS = ClusterOf<W>::value;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t acc_base = smem_base + C::STAGES * C::STAGE;
@@ -219,13 +264,27 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
   if (threadIdx.x == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(full_bar + 8 * s, 1);
-      mbar_init(empty_bar + 8 * s, 1);
+      mbar_init(empty_bar + 8 * s, CS);
     }
     mbar_init(tfull_bar, 128);
     mbar_init(tempty_bar, 32 * NUM_EPI_WARPS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncthreads();
+  // peers multicast into this CTA's stages and arrive on its empty barriers: not before they exist
+  if constexpr (CS > 1)
+    cluster_sync();
+  else
+    __syncthreads();
+  // the MMA warpgroup's release of a stage: one arrival on its empty barrier in every CTA of the
+  // cluster (each of them may write into this CTA's copy of the stage)
+  auto release = [&](int s) {
+    if constexpr (CS > 1) {
+#pragma unroll
+      for (int r = 0; r < CS; ++r) mbar_arrive_cluster(empty_bar + 8 * s, (uint32_t)r);
+    } else {
+      mbar_arrive(empty_bar + 8 * s);
+    }
+  };
 
   if (warp < 4) {
     // ===================== MMA warpgroup =====================
@@ -253,12 +312,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
         mma_kblock<W::KIND, W::RB, W::MNA, W::MNB>(d, sa);
         wgmma_commit();
         wgmma_wait<1>();                                  // the previous stage has been read
-        if (prev >= 0 && tid == 0) mbar_arrive(empty_bar + 8 * prev);
+        if (prev >= 0 && tid == 0) release(prev);
         prev = stage;
         if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
-      if (prev >= 0 && tid == 0) mbar_arrive(empty_bar + 8 * prev);
+      if (prev >= 0 && tid == 0) release(prev);
       mbar_wait(tempty_bar, acc_phase ^ 1);           // epilogue drained the previous unit
       const int row = 16 * (tid >> 5) + ((tid & 31) >> 2);
       const int col = 2 * (tid & 3);
@@ -308,25 +367,68 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
     }
     w.epi_finish(st, quarter, lane);
   }
+  // no CTA leaves while a peer may still multicast into its shared memory or arrive on its barriers
+  if constexpr (CS > 1) cluster_sync();
 }
 
 // one launch of tc_pipeline_kernel<W>: opt in to the dynamic shared memory once, one CTA per SM
+// (with clusters: as many whole clusters as fit at once, which need not cover every SM)
 template <class W>
 int tc_launch(const W& w, cudaStream_t st, const char* what) {
+  constexpr int CS = ClusterOf<W>::value;
   static const cudaError_t attr = cudaFuncSetAttribute(
       tc_pipeline_kernel<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<W::RB>::SMEM);
   if (attr != cudaSuccess) {
     zsb_set_error("%s: cudaFuncSetAttribute: %s", what, cudaGetErrorString(attr));
     return ZSB_ERR_CUDA;
   }
-  int dev = 0, sms = ZSB_NUM_SMS;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  int64_t grid = w.units();
-  if (grid > sms) grid = sms;
-  if (grid < 1) grid = 1;
-  tc_pipeline_kernel<W><<<(unsigned)grid, NUM_THREADS, Cfg<W::RB>::SMEM, st>>>(w);
-  return zsb_check_launch(what);
+  if constexpr (CS > 1) {
+    const int64_t units = w.units();
+    if (units < 1 || units % CS != 0) {
+      zsb_set_error("%s: %lld units do not tile by clusters of %d", what, (long long)units, CS);
+      return ZSB_ERR_INVALID;
+    }
+    cudaLaunchAttribute cl[1];
+    cl[0].id = cudaLaunchAttributeClusterDimension;
+    cl[0].val.clusterDim.x = CS;
+    cl[0].val.clusterDim.y = 1;
+    cl[0].val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.blockDim = dim3(NUM_THREADS);
+    cfg.dynamicSmemBytes = Cfg<W::RB>::SMEM;
+    cfg.stream = st;
+    cfg.attrs = cl;
+    cfg.numAttrs = 1;
+    static int max_clusters = 0;
+    if (max_clusters < 1) {
+      cfg.gridDim = dim3(CS);
+      const cudaError_t e =
+          cudaOccupancyMaxActiveClusters(&max_clusters, tc_pipeline_kernel<W>, &cfg);
+      if (e != cudaSuccess || max_clusters < 1) {
+        zsb_set_error("%s: no cluster of %d CTAs fits (%s)", what, CS, cudaGetErrorString(e));
+        max_clusters = 0;
+        return ZSB_ERR_CUDA;
+      }
+    }
+    int64_t grid = (int64_t)max_clusters * CS;
+    if (grid > units) grid = units;
+    cfg.gridDim = dim3((unsigned)grid);
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, tc_pipeline_kernel<W>, w);
+    if (e != cudaSuccess) {
+      zsb_set_error("%s: cudaLaunchKernelEx: %s", what, cudaGetErrorString(e));
+      return ZSB_ERR_CUDA;
+    }
+    return zsb_check_launch(what);
+  } else {
+    int dev = 0, sms = ZSB_NUM_SMS;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    int64_t grid = w.units();
+    if (grid > sms) grid = sms;
+    if (grid < 1) grid = 1;
+    tc_pipeline_kernel<W><<<(unsigned)grid, NUM_THREADS, Cfg<W::RB>::SMEM, st>>>(w);
+    return zsb_check_launch(what);
+  }
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
