@@ -78,30 +78,34 @@ class DoubleWell(object):
 class BNN(object):
     """bnn_sgmcmc.py:19-35 with layer_sizes [n_in, n_hidden, 1]; per-chain
     weights w0 [C, H, n_in+1], w1 [C, 1, H+1]; prior N(0, exp(logstd));
-    y ~ N(y_mean, exp(-0.95)); log_joint = sum log p(w) +
-    mean_batch(log p(y|x,w)) * n_train  (bnn_sgmcmc.py:74-77)."""
+    y ~ N(y_mean, exp(y_logstd)) (default -0.95); log_joint = sum log p(w) +
+    mean_batch(log p(y|x,w)) * n_train  (bnn_sgmcmc.py:74-77).  logstd0 /
+    logstd1 are scalars or arrays broadcasting against w0 / w1 (per weight,
+    per hidden unit, per chain, ...)."""
 
     Y_LOGSTD = -0.95
 
     def __init__(self, x, y, n_train, logstd0=0.0, logstd1=0.0,
-                 dtype=np.float64):
+                 dtype=np.float64, y_logstd=None):
         self.dtype = dtype
         self.x = np.asarray(x, dtype)
         self.y = np.asarray(y, dtype)
         self.n_train = dtype(n_train)
-        self.ls0, self.ls1 = dtype(logstd0), dtype(logstd1)
+        self.ls0, self.ls1 = np.asarray(logstd0, dtype), np.asarray(logstd1, dtype)
+        if y_logstd is not None:
+            self.Y_LOGSTD = y_logstd
 
     def _fwd(self, w0, w1):
         d = self.dtype
         x = self.x
         B, n_in = x.shape
         h0 = np.concatenate([x, np.ones((B, 1), d)], -1)           # [B, n_in+1]
-        a1 = np.einsum('cmk,jk->cjm', w0, h0) / np.sqrt(d(n_in + 1))
+        a1 = (h0 @ w0.transpose(0, 2, 1)) / np.sqrt(d(n_in + 1))        # [C,B,H]
         r1 = np.maximum(a1, 0)
         C = w0.shape[0]
         h1 = np.concatenate([r1, np.ones((C, B, 1), d)], -1)       # [C,B,H+1]
         H1 = h1.shape[-1]
-        out = np.einsum('cmk,cjk->cjm', w1, h1) / np.sqrt(d(H1))
+        out = (h1 @ w1.transpose(0, 2, 1)) / np.sqrt(d(H1))
         return h0, a1, h1, out[..., 0]
 
     def logp(self, qs):
@@ -123,10 +127,10 @@ class BNN(object):
         prec_y = np.exp(d(-2) * d(self.Y_LOGSTD))
         dym = prec_y * (self.y[None, :] - ym) * (self.n_train / d(B))  # [C,B]
         dout = dym / np.sqrt(d(H1))
-        gw1 = np.einsum('cj,cjk->ck', dout, h1)[:, None, :]
+        gw1 = dout[:, None, :] @ h1                                  # [C,1,H+1]
         dh1 = dout[..., None] * w1[:, 0, None, :]                  # [C,B,H+1]
         da1 = dh1[..., :-1] * (a1 > 0) / np.sqrt(d(n_in + 1))
-        gw0 = np.einsum('cjm,jk->cmk', da1, h0)
+        gw0 = da1.transpose(0, 2, 1) @ h0                            # [C,H,n_in+1]
         gw0 = gw0 - np.exp(d(-2) * self.ls0) * w0
         gw1 = gw1 - np.exp(d(-2) * self.ls1) * w1
         return [gw0.astype(d), gw1.astype(d)]

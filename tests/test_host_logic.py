@@ -487,3 +487,32 @@ def test_context_frames_are_per_thread():
         with pytest.raises(RuntimeError, match="No contexts on the stack"):
             B.get_context()
     assert seen["other"] == "No contexts on the stack."
+
+
+def test_bnn_prior_logstd_as_the_fused_kernel_reads_it():
+    """BNNRegressionLogJoint.fused_prior_logstd: the fused BNN kernel reads a prior log-stddev by
+    flat index modulo its size over one chain's weights.  Suffix shapes go through untouched,
+    shapes that only broadcast are expanded (once, until modified in place), and shapes with
+    chain axes are refused so the step takes the generic path."""
+    H, in1 = 5, 4
+    lj = lambda ls: zs.fused.BNNRegressionLogJoint(torch.zeros(2, in1 - 1), torch.zeros(2),
+                                                   [ls, torch.zeros(1, H + 1)], 10)
+    for shape in [(H, in1), (in1,), (), (1, 1), (1, H, in1)]:
+        m = lj(torch.randn(shape))
+        assert m.fused_prior_logstd(0, (H, in1)) is m.logstds[0], shape
+    for shape in [(3, H, in1), (3, H, 1), (H, 2), (H + 1, in1)]:
+        assert lj(torch.randn(shape)).fused_prior_logstd(0, (H, in1)) is None, shape
+    for shape in [(H, 1), (1, H, 1)]:
+        m = lj(torch.randn(shape))
+        e = m.fused_prior_logstd(0, (H, in1))
+        assert e.shape == (H, in1) and e.is_contiguous()
+        flat = e.reshape(-1)
+        for i in range(H * in1):              # the kernel's index: i % numel over [H, n_in+1]
+            assert flat[i % flat.numel()] == m.logstds[0].reshape(H)[i // in1]
+        assert m.fused_prior_logstd(0, (H, in1)) is e           # cached: no launch per step
+        m.logstds[0].add_(1.0)
+        e2 = m.fused_prior_logstd(0, (H, in1))
+        assert torch.equal(e2, e + 1.0)
+    m = lj(torch.randn(H, in1))
+    m.logstds[1] = torch.randn(3, 1, H + 1)
+    assert m.fused_prior_logstd(1, (1, H + 1)) is None

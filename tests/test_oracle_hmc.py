@@ -184,3 +184,22 @@ def test_oracle_reproduces_big_dense_golden(name):
     live = g["acc64"] > 1e-6
     assert np.abs(g["h1"][live] / g["h1_64"][live] - 1).max() < 2e-6
     assert (~np.isfinite(g["h1"])).any() and live.any()   # diverging and healthy trajectories
+
+
+@pytest.mark.parametrize("ls0_shape,ls1_shape", [((5, 1), ()), ((3, 5, 5), (3, 1, 6)), ((5,), (1, 6))])
+def test_bnn_oracle_gradient_with_broadcast_prior_scales(ls0_shape, ls1_shape):
+    """The BNN oracle with array prior log-stddevs (per hidden unit, per chain, ...) broadcast
+    against the weights, and a non-default y_logstd: analytic gradient vs finite differences."""
+    rng = np.random.RandomState(4)
+    x = rng.standard_normal((7, 4)); y = rng.standard_normal(7)
+    ls0 = rng.uniform(-0.7, 0.3, ls0_shape); ls1 = rng.uniform(-0.7, 0.3, ls1_shape)
+    m = OM.BNN(x, y, 100, ls0, ls1, dtype=np.float64, y_logstd=-0.3)
+    w0 = rng.standard_normal((3, 5, 5)); w1 = rng.standard_normal((3, 1, 6))
+    g0, g1 = m.grad([w0, w1])
+    h = 1e-6
+    for (arr, grad, idx) in [(w0, g0, (1, 2, 3)), (w0, g0, (2, 4, 0)), (w1, g1, (2, 0, 4)),
+                             (w1, g1, (0, 0, 5))]:
+        a2 = arr.copy(); a2[idx] += h
+        args = [a2, w1] if arr is w0 else [w0, a2]
+        fd = (m.logp(args) - m.logp([w0, w1]))[idx[0]] / h
+        np.testing.assert_allclose(grad[idx], fd, rtol=1e-4, atol=1e-4)

@@ -92,7 +92,14 @@ class BNNRegressionLogJoint(object):
     As a callable it is the generic-path log-joint (registry Normal kernels +
     torch einsum under the tape); ``zs.SGHMC.sample`` recognises it and runs
     the whole step in one fused kernel (zsb_sgmcmc_sghmc_bnn_f32).  Feed
-    minibatches with ``sample_op(observed={'x': xb, 'y': yb})``.
+    minibatches with ``sample_op(observed={'x': xb, 'y': yb})``; ``x`` is
+    [B, n_in] and ``y`` holds B values.
+
+    ``logstds[k]`` broadcasts against w_k with NumPy rules.  Shapes that
+    broadcast to one chain's weights -- for logstds[0] e.g. [H, n_in+1],
+    [H, 1] (one scale per hidden unit), [n_in+1] or [] -- run on the fused
+    kernel; shapes with chain axes, e.g. [chains, H, n_in+1] or
+    [chains, 1, H+1], run on the generic path.
     """
 
     def __init__(self, x, y, logstds, n_train, y_logstd=-0.95,
@@ -104,7 +111,33 @@ class BNNRegressionLogJoint(object):
         self.n_train = float(n_train)
         self.y_logstd = float(y_logstd)
         self.names = tuple(names)
+        self._prior_cache = {}
         self._zsb_fused = {"kind": "bnn_regression", "obj": self}
+
+    def fused_prior_logstd(self, k, shape):
+        """logstds[k] as the fused kernel reads it: flat over one chain's
+        weights of ``shape`` ([H, n_in+1] or [1, H+1]), index modulo its size.
+        A logstd whose shape, leading 1s dropped, is a suffix of ``shape``
+        already reads right and is returned as is; one that only broadcasts
+        to ``shape`` (e.g. [H, 1]) is expanded once and cached until it is
+        modified in place.  None if it does not broadcast to ``shape``
+        (it carries chain axes)."""
+        ls = self.logstds[k]
+        s = list(ls.shape)
+        while s and s[0] == 1:
+            s.pop(0)
+        shape = tuple(int(d) for d in shape)
+        if len(s) > len(shape) or any(a != 1 and a != b for a, b in
+                                      zip(s[::-1], shape[::-1])):
+            return None
+        if not s or tuple(s) == shape[len(shape) - len(s):]:
+            return ls
+        key = (k, shape, ls.data_ptr(), tuple(ls.shape), ls._version)
+        e = self._prior_cache.get(k)
+        if e is None or e[0] != key:
+            e = (key, ls.reshape(s).expand(shape).contiguous())
+            self._prior_cache[k] = e
+        return e[1]
 
     def set_batch(self, observed):
         if "x" in observed:

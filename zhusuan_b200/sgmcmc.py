@@ -223,8 +223,10 @@ class SGHMC(SGMCMC):
         self.vs = [torch.empty_like(q) for q in qs]       # sgmcmc.py:320-324
         for k, v in enumerate(self.vs):
             self._resample(k, v, {}, "v0", 0xFFFFFFFF)
-        self._mean_k = [torch.zeros(1, dtype=_F32, device=q.device)
-                        for q in qs]
+        # one buffer for every latent: the fused BNN step writes all entries at once, the generic
+        # step one per latent, so info.mean_k follows whichever path ran last
+        self._mean_k_buf = torch.zeros(len(qs), dtype=_F32, device=qs[0].device)
+        self._mean_k = [self._mean_k_buf[k:k + 1] for k in range(len(qs))]
         return {"q": dict(zip(self._latent_k, qs)),
                 "mean_k": dict(zip(self._latent_k,
                                    [m[0] for m in self._mean_k]))}
@@ -249,8 +251,20 @@ class SGHMC(SGMCMC):
             return None
         w0, w1 = self._var_list
         if w0.dim() != 3 or w1.dim() != 3 or w1.shape[1] != 1 or \
-                w1.shape[2] != w0.shape[1] + 1 or w0.shape[2] > 16 or \
-                w0.shape[1] > 64 or obj.x.shape[0] > 512:
+                w1.shape[2] != w0.shape[1] + 1:
+            return None
+        # the kernel takes n_in and B from the minibatch and walks the chain state with them
+        x, y = obj.x, obj.y
+        if x.dim() != 2 or x.shape[1] + 1 != w0.shape[2]:
+            raise ValueError("minibatch x has shape {} but w0 {} needs [B, {}]".format(
+                tuple(x.shape), tuple(w0.shape), w0.shape[2] - 1))
+        if y.numel() != x.shape[0]:
+            raise ValueError("minibatch y has {} values but x has {} rows".format(
+                y.numel(), x.shape[0]))
+        if w0.shape[2] > 16 or w0.shape[1] > 64 or x.shape[0] > 512:
+            return None
+        if obj.fused_prior_logstd(0, w0.shape[1:]) is None or \
+                obj.fused_prior_logstd(1, w1.shape[1:]) is None:
             return None
         return obj
 
@@ -258,25 +272,23 @@ class SGHMC(SGMCMC):
         """Whole step in one kernel (csrc/sgmcmc_bnn.cu)."""
         w0, w1 = self._var_list
         x, y = obj.x.contiguous(), obj.y.contiguous()
+        ls0 = obj.fused_prior_logstd(0, w0.shape[1:])
+        ls1 = obj.fused_prior_logstd(1, w1.shape[1:])
         resample = int(self.n_iter_resample_v != 0 and
                        self.t % self.n_iter_resample_v == 0)
         if not hasattr(self, "_bnn_part"):
             self._bnn_part = torch.zeros(2 * lib.load().zsb_sgmcmc_parts(),
                                          dtype=_F32, device=w0.device)
-            self._bnn_mean_k = torch.zeros(2, dtype=_F32, device=w0.device)
-            self._info.mean_k[self._latent_k[0]] = self._bnn_mean_k[0]
-            self._info.mean_k[self._latent_k[1]] = self._bnn_mean_k[1]
         lib.call("zsb_sgmcmc_sghmc_bnn_f32", ptr(w0), ptr(w1), ptr(self.vs[0]),
                  ptr(self.vs[1]), ptr(x), ptr(y), int(x.shape[0]),
-                 int(x.shape[1]), int(w0.shape[1]), ptr(obj.logstds[0]),
-                 obj.logstds[0].numel(), ptr(obj.logstds[1]),
-                 obj.logstds[1].numel(), obj.y_logstd, obj.n_train, self.lr,
+                 int(x.shape[1]), int(w0.shape[1]), ptr(ls0), ls0.numel(),
+                 ptr(ls1), ls1.numel(), obj.y_logstd, obj.n_train, self.lr,
                  self.alpha, self.beta, int(self.second_order), resample,
                  self._noise(noise, "noise", 0), self._noise(noise, "noise", 1),
                  self._noise(noise, "resample", 0),
                  self._noise(noise, "resample", 1), self._seed_now(),
                  self.t & 0xFFFFFFFF, self._row0, ptr(self._bnn_part),
-                 ptr(self._bnn_mean_k), self._chains, stream())
+                 ptr(self._mean_k_buf), self._chains, stream())
 
     def _update(self, qs, grad_func, noise):
         obj = self._fused_bnn() if self._use_fused else None
