@@ -466,7 +466,8 @@ int zsb_sgmcmc_sgnht_alpha_f32(float* out, const float* in, const float* mean_k,
  * examples/bayesian_neural_nets/bnn_sgmcmc.py:19-35, 74-91 (layer sizes [n_in, H, 1]; per-chain
  * weights w0 [chains,H,n_in+1], w1 [chains,1,H+1]): momentum resample, half step, hand-derived
  * forward/backward over the minibatch, prior gradient and the sgmcmc.py:338-358 update in ONE
- * launch.  part: 2*zsb_sgmcmc_parts() floats; mean_k: 2 floats (one per latent). */
+ * launch.  part: 2*zsb_sgmcmc_parts() floats; mean_k: 2 floats (one per latent).
+ * Same as zsb_sgmcmc_bnn_step_f32(ZSB_SGMCMC_SGHMC, ...). */
 int zsb_sgmcmc_sghmc_bnn_f32(float* w0, float* w1, float* v0, float* v1, const float* x,
                              const float* y, int B, int n_in, int H, const float* logstd0,
                              int64_t logstd0_n, const float* logstd1, int64_t logstd1_n,
@@ -475,6 +476,42 @@ int zsb_sgmcmc_sghmc_bnn_f32(float* w0, float* w1, float* v0, float* v1, const f
                              const float* noise1, const float* resample0, const float* resample1,
                              uint64_t seed, uint32_t iter, int64_t row0, float* part,
                              float* mean_k, int64_t chains, void* stream);
+
+/* Update rules of zsb_sgmcmc_bnn_step_f32. */
+enum zsb_sgmcmc_method {
+  ZSB_SGMCMC_SGHMC = 0,         /* sgmcmc.py:326-371 */
+  ZSB_SGMCMC_SGLD = 1,          /* sgmcmc.py:195-200 */
+  ZSB_SGMCMC_PSGLD = 2,         /* sgmcmc.py:225-257 */
+  ZSB_SGMCMC_SGNHT_VEC = 3,     /* sgmcmc.py:460-523, use_vector_alpha=True */
+  ZSB_SGMCMC_SGNHT_SCALAR = 4   /* sgmcmc.py:460-523, use_vector_alpha=False */
+};
+
+/* One fused SG-MCMC step of `method` for the same BNN log-joint and shape limits as
+ * zsb_sgmcmc_sghmc_bnn_f32 (n_in + 1 <= 16, H <= 64, B <= 512), replacing the generic gradient plus
+ * zsb_sgmcmc_{sgld,psgld,sghmc,sgnht_vec,sgnht_scalar}_f32 with ONE launch.  Each rule keeps the
+ * rounding and operation order of its element-wise kernel.  State (NULL where unused):
+ *   v0/v1        momenta (SGHMC, SGNHT), shaped like w0 / w1
+ *   aux0/aux1    PSGLD's RMS accumulator (sgmcmc.py:225-230) or vector SGNHT's thermostat alpha
+ *                (sgmcmc.py:454-458), shaped like w0 / w1
+ *   alpha_eff0/1 scalar SGNHT: device scalar per latent, alpha (1st order) or alpha1 (2nd)
+ *   mean_k0/1    SGHMC, scalar SGNHT: one float each, mean(v_new^2) of this call's chains;
+ *                vector SGNHT: shaped like w0 / w1, receives k = v_new^2 (sgmcmc.py:497-505)
+ *   part         2*zsb_sgmcmc_parts() floats (SGHMC, scalar SGNHT)
+ * friction/variance_estimate: SGHMC; decay/epsilon: PSGLD; variance_extra/tune_rate: SGNHT.
+ * second_order and resample apply to SGHMC and vector SGNHT; scalar SGNHT re-draws v with
+ * zsb_sgmcmc_resample_v_f32 before the step and updates alpha from mean_k after it
+ * (zsb_sgmcmc_mean_sq_f32 / zsb_sgmcmc_sgnht_alpha_f32), as the generic path does. */
+int zsb_sgmcmc_bnn_step_f32(int method, float* w0, float* w1, float* v0, float* v1, float* aux0,
+                            float* aux1, const float* alpha_eff0, const float* alpha_eff1,
+                            const float* x, const float* y, int B, int n_in, int H,
+                            const float* logstd0, int64_t logstd0_n, const float* logstd1,
+                            int64_t logstd1_n, float y_logstd, float n_train, float lr,
+                            float friction, float variance_estimate, float decay, float epsilon,
+                            float variance_extra, float tune_rate, int second_order, int resample,
+                            const float* noise0, const float* noise1, const float* resample0,
+                            const float* resample1, uint64_t seed, uint32_t iter, int64_t row0,
+                            float* part, float* mean_k0, float* mean_k1, int64_t chains,
+                            void* stream);
 
 #ifdef __cplusplus
 }

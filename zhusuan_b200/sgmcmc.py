@@ -6,7 +6,9 @@ updated in place and ``sample_op`` is a callable; minibatches that the
 reference feeds through placeholders are passed as
 ``sample_op(observed={...})`` overrides.  Gradients of the user log-joint
 come from torch autograd over the registry kernels (replaces tf.gradients,
-sgmcmc.py:96-98); the update itself is one fused kernel per latent.
+sgmcmc.py:96-98); the update itself is one fused kernel per latent.  On the
+two-layer BNN regression log-joint of ``zs.fused`` every method runs the whole
+step (gradient and update) in one launch instead (csrc/sgmcmc_bnn.cu).
 """
 from collections import namedtuple
 
@@ -20,6 +22,9 @@ from .utils import merge_dicts
 __all__ = ["SGMCMC", "SGLD", "PSGLD", "SGHMC", "SGNHT"]
 
 _F32 = torch.float32
+
+# update rules of zsb_sgmcmc_bnn_step_f32 (enum zsb_sgmcmc_method, include/zsb200.h)
+_BNN_SGHMC, _BNN_SGLD, _BNN_PSGLD, _BNN_SGNHT_VEC, _BNN_SGNHT_SCALAR = range(5)
 
 
 class _SampleOp(object):
@@ -150,18 +155,87 @@ class SGMCMC(object):
         n = noise.get(key)
         return None if n is None else ptr(n[self._latent_k[k]].contiguous())
 
+    # ------------------------------------------------ fused BNN step (every method)
+    _use_fused = True
+
+    def _fused_bnn(self):
+        """The BNN regression log-joint object when the whole step can run in one launch
+        (csrc/sgmcmc_bnn.cu), else None (generic path)."""
+        f = getattr(self._log_joint, "_zsb_fused", None)
+        if f is None or f.get("kind") != "bnn_regression":
+            return None
+        obj = f["obj"]
+        if list(self._latent_k) != list(obj.names):
+            return None
+        w0, w1 = self._var_list
+        if w0.dim() != 3 or w1.dim() != 3 or w1.shape[1] != 1 or \
+                w1.shape[2] != w0.shape[1] + 1:
+            return None
+        # the kernel takes n_in and B from the minibatch and walks the chain state with them
+        x, y = obj.x, obj.y
+        if x.dim() != 2 or x.shape[1] + 1 != w0.shape[2]:
+            raise ValueError("minibatch x has shape {} but w0 {} needs [B, {}]".format(
+                tuple(x.shape), tuple(w0.shape), w0.shape[2] - 1))
+        if y.numel() != x.shape[0]:
+            raise ValueError("minibatch y has {} values but x has {} rows".format(
+                y.numel(), x.shape[0]))
+        if w0.shape[2] > 16 or w0.shape[1] > 64 or x.shape[0] > 512:
+            return None
+        if obj.fused_prior_logstd(0, w0.shape[1:]) is None or \
+                obj.fused_prior_logstd(1, w1.shape[1:]) is None:
+            return None
+        return obj
+
+    def _bnn_part_buf(self):
+        if not hasattr(self, "_bnn_part"):
+            self._bnn_part = torch.zeros(2 * lib.load().zsb_sgmcmc_parts(),
+                                         dtype=_F32, device=self._var_list[0].device)
+        return self._bnn_part
+
+    def _bnn_step(self, obj, noise, method, v=(None, None), aux=(None, None),
+                  alpha_eff=(None, None), mean_k=(None, None), part=None, friction=0.,
+                  variance_estimate=0., decay=0., epsilon=0., variance_extra=0., tune_rate=0.,
+                  second_order=False, resample=False):
+        """One zsb_sgmcmc_bnn_step_f32 launch on (w0, w1); state pairs are (w0's, w1's)."""
+        w0, w1 = self._var_list
+        x, y = obj.x.contiguous(), obj.y.contiguous()
+        ls0 = obj.fused_prior_logstd(0, w0.shape[1:])
+        ls1 = obj.fused_prior_logstd(1, w1.shape[1:])
+        lib.call("zsb_sgmcmc_bnn_step_f32", method, ptr(w0), ptr(w1), ptr(v[0]), ptr(v[1]),
+                 ptr(aux[0]), ptr(aux[1]), ptr(alpha_eff[0]), ptr(alpha_eff[1]), ptr(x),
+                 ptr(y), int(x.shape[0]), int(x.shape[1]), int(w0.shape[1]), ptr(ls0),
+                 ls0.numel(), ptr(ls1), ls1.numel(), obj.y_logstd, obj.n_train, self.lr,
+                 friction, variance_estimate, decay, epsilon, variance_extra, tune_rate,
+                 int(second_order), int(resample), self._noise(noise, "noise", 0),
+                 self._noise(noise, "noise", 1), self._noise(noise, "resample", 0),
+                 self._noise(noise, "resample", 1), self._seed_now(), self.t & 0xFFFFFFFF,
+                 self._row0, ptr(part), ptr(mean_k[0]), ptr(mean_k[1]), self._chains,
+                 stream())
+
+    def _resample_due(self):
+        return self.n_iter_resample_v != 0 and \
+            self.t % self.n_iter_resample_v == 0           # sgmcmc.py:330-336
+
 
 class SGLD(SGMCMC):
     """sgmcmc.py:170-200."""
 
-    def __init__(self, learning_rate, **kw):
+    def __init__(self, learning_rate, use_fused=True, **kw):
+        self._use_fused = bool(use_fused)
         self.lr = float(learning_rate)
         super(SGLD, self).__init__(**kw)
 
     def _define_variables(self, qs):
         return {"q": dict(zip(self._latent_k, qs))}
 
+    def _update_fused_bnn(self, obj, noise):
+        """Whole step in one kernel (csrc/sgmcmc_bnn.cu)."""
+        self._bnn_step(obj, noise, _BNN_SGLD)
+
     def _update(self, qs, grad_func, noise):
+        obj = self._fused_bnn() if self._use_fused else None
+        if obj is not None:
+            return self._update_fused_bnn(obj, noise)
         gs = grad_func(qs)
         s = stream()
         for k, (q, g) in enumerate(zip(qs, gs)):
@@ -176,19 +250,28 @@ class PSGLD(SGLD):
     RMSHParams = namedtuple('RMSHParams', 'decay epsilon')
 
     def __init__(self, learning_rate, preconditioner='rms',
-                 preconditioner_hparams=None, **kw):
+                 preconditioner_hparams=None, use_fused=True, **kw):
         if preconditioner != 'rms':
             raise KeyError(preconditioner)
         if preconditioner_hparams is None:
             preconditioner_hparams = PSGLD.RMSHParams(decay=0.9, epsilon=1e-3)
         self.preconditioner_hparams = preconditioner_hparams
-        super(PSGLD, self).__init__(learning_rate, **kw)
+        super(PSGLD, self).__init__(learning_rate, use_fused=use_fused, **kw)
 
     def _define_variables(self, qs):
         self.vs = [torch.zeros_like(q) for q in qs]       # sgmcmc.py:225-226
         return {"q": dict(zip(self._latent_k, qs))}
 
+    def _update_fused_bnn(self, obj, noise):
+        """Whole step in one kernel (csrc/sgmcmc_bnn.cu); self.vs is the RMS accumulator."""
+        hp = self.preconditioner_hparams
+        self._bnn_step(obj, noise, _BNN_PSGLD, aux=self.vs, decay=float(hp.decay),
+                       epsilon=float(hp.epsilon))
+
     def _update(self, qs, grad_func, noise):
+        obj = self._fused_bnn() if self._use_fused else None
+        if obj is not None:
+            return self._update_fused_bnn(obj, noise)
         gs = grad_func(qs)
         s = stream()
         hp = self.preconditioner_hparams
@@ -237,58 +320,16 @@ class SGHMC(SGMCMC):
             self._resample(k, v, {"v0": noise_v0}, "v0", 0)
 
     def _maybe_resample(self, noise):
-        if self.n_iter_resample_v != 0 and \
-                self.t % self.n_iter_resample_v == 0:      # sgmcmc.py:330-336
+        if self._resample_due():                           # sgmcmc.py:330-336
             for k, v in enumerate(self.vs):
                 self._resample(k, v, noise, "resample", self.t & 0xFFFFFFFF)
 
-    def _fused_bnn(self):
-        f = getattr(self._log_joint, "_zsb_fused", None)
-        if f is None or f.get("kind") != "bnn_regression":
-            return None
-        obj = f["obj"]
-        if list(self._latent_k) != list(obj.names):
-            return None
-        w0, w1 = self._var_list
-        if w0.dim() != 3 or w1.dim() != 3 or w1.shape[1] != 1 or \
-                w1.shape[2] != w0.shape[1] + 1:
-            return None
-        # the kernel takes n_in and B from the minibatch and walks the chain state with them
-        x, y = obj.x, obj.y
-        if x.dim() != 2 or x.shape[1] + 1 != w0.shape[2]:
-            raise ValueError("minibatch x has shape {} but w0 {} needs [B, {}]".format(
-                tuple(x.shape), tuple(w0.shape), w0.shape[2] - 1))
-        if y.numel() != x.shape[0]:
-            raise ValueError("minibatch y has {} values but x has {} rows".format(
-                y.numel(), x.shape[0]))
-        if w0.shape[2] > 16 or w0.shape[1] > 64 or x.shape[0] > 512:
-            return None
-        if obj.fused_prior_logstd(0, w0.shape[1:]) is None or \
-                obj.fused_prior_logstd(1, w1.shape[1:]) is None:
-            return None
-        return obj
-
     def _update_fused_bnn(self, obj, noise):
         """Whole step in one kernel (csrc/sgmcmc_bnn.cu)."""
-        w0, w1 = self._var_list
-        x, y = obj.x.contiguous(), obj.y.contiguous()
-        ls0 = obj.fused_prior_logstd(0, w0.shape[1:])
-        ls1 = obj.fused_prior_logstd(1, w1.shape[1:])
-        resample = int(self.n_iter_resample_v != 0 and
-                       self.t % self.n_iter_resample_v == 0)
-        if not hasattr(self, "_bnn_part"):
-            self._bnn_part = torch.zeros(2 * lib.load().zsb_sgmcmc_parts(),
-                                         dtype=_F32, device=w0.device)
-        lib.call("zsb_sgmcmc_sghmc_bnn_f32", ptr(w0), ptr(w1), ptr(self.vs[0]),
-                 ptr(self.vs[1]), ptr(x), ptr(y), int(x.shape[0]),
-                 int(x.shape[1]), int(w0.shape[1]), ptr(ls0), ls0.numel(),
-                 ptr(ls1), ls1.numel(), obj.y_logstd, obj.n_train, self.lr,
-                 self.alpha, self.beta, int(self.second_order), resample,
-                 self._noise(noise, "noise", 0), self._noise(noise, "noise", 1),
-                 self._noise(noise, "resample", 0),
-                 self._noise(noise, "resample", 1), self._seed_now(),
-                 self.t & 0xFFFFFFFF, self._row0, ptr(self._bnn_part),
-                 ptr(self._mean_k_buf), self._chains, stream())
+        self._bnn_step(obj, noise, _BNN_SGHMC, v=self.vs, mean_k=self._mean_k,
+                       part=self._bnn_part_buf(), friction=self.alpha,
+                       variance_estimate=self.beta, second_order=self.second_order,
+                       resample=self._resample_due())
 
     def _update(self, qs, grad_func, noise):
         obj = self._fused_bnn() if self._use_fused else None
@@ -314,7 +355,8 @@ class SGNHT(SGMCMC):
 
     def __init__(self, learning_rate, variance_extra=0., tune_rate=1.,
                  n_iter_resample_v=None, second_order=True,
-                 use_vector_alpha=True, **kw):
+                 use_vector_alpha=True, use_fused=True, **kw):
+        self._use_fused = bool(use_fused)
         self.lr = float(learning_rate)
         self.a = float(variance_extra)
         self.tune_rate = float(tune_rate)
@@ -350,18 +392,56 @@ class SGNHT(SGMCMC):
                 "mean_k": dict(zip(self._latent_k, mk)),
                 "alpha": dict(zip(self._latent_k, al))}
 
+    def _scalar_alpha1(self):
+        """Scalar alpha, 2nd order: alpha1 from the mean of v_old^2 over all chains
+        (sgmcmc.py:494-496)."""
+        s = stream()
+        for k, v in enumerate(self.vs):
+            lib.call("zsb_sgmcmc_mean_sq_f32", ptr(v), v.numel(),
+                     ptr(self._part), ptr(self._mean_k[k]), s)
+            zdist.all_reduce_weighted_mean_(self._mean_k[k], v.numel(), self._group)
+            lib.call("zsb_sgmcmc_sgnht_alpha_f32", ptr(self._alpha1[k]),
+                     ptr(self.alphas[k]), ptr(self._mean_k[k]),
+                     0.5 * self.tune_rate, self.lr, s)
+
+    def _scalar_alpha_update(self, k, a_eff, n):
+        """Scalar alpha: alpha from mean(v_new^2) over all chains (sgmcmc.py:490, 506).  Chains
+        sharded over ranks drive the thermostat by the mean kinetic energy of ALL chains (one
+        8-byte all-reduce per latent and step; no-op on one rank)."""
+        zdist.all_reduce_weighted_mean_(self._mean_k[k], n, self._group)
+        coef = 0.5 * self.tune_rate if self.second_order else self.tune_rate
+        lib.call("zsb_sgmcmc_sgnht_alpha_f32", ptr(self.alphas[k]),
+                 ptr(a_eff), ptr(self._mean_k[k]), coef, self.lr, stream())
+
+    def _update_fused_bnn(self, obj, noise):
+        """Whole step in one kernel (csrc/sgmcmc_bnn.cu).  Scalar alpha couples every chain, so
+        the re-draw of v, alpha1 and the alpha update run around the launch, in the order of
+        the generic path."""
+        if self.use_vector_alpha:
+            self._bnn_step(obj, noise, _BNN_SGNHT_VEC, v=self.vs, aux=self.alphas,
+                           mean_k=self._mean_k, variance_extra=self.a,
+                           tune_rate=self.tune_rate, second_order=self.second_order,
+                           resample=self._resample_due())
+            return
+        self._maybe_resample(noise)
+        if self.second_order:
+            self._scalar_alpha1()
+        a_eff = self._alpha1 if self.second_order else self.alphas
+        self._bnn_step(obj, noise, _BNN_SGNHT_SCALAR, v=self.vs, alpha_eff=a_eff,
+                       mean_k=self._mean_k, part=self._bnn_part_buf(),
+                       variance_extra=self.a, second_order=self.second_order)
+        for k, q in enumerate(self._var_list):
+            self._scalar_alpha_update(k, a_eff[k], q.numel())
+
     def _update(self, qs, grad_func, noise):
+        obj = self._fused_bnn() if self._use_fused else None
+        if obj is not None:
+            return self._update_fused_bnn(obj, noise)
         s = stream()
         it = self.t & 0xFFFFFFFF
         self._maybe_resample(noise)
         if not self.use_vector_alpha and self.second_order:
-            for k, v in enumerate(self.vs):                # sgmcmc.py:494-496
-                lib.call("zsb_sgmcmc_mean_sq_f32", ptr(v), v.numel(),
-                         ptr(self._part), ptr(self._mean_k[k]), s)
-                zdist.all_reduce_weighted_mean_(self._mean_k[k], v.numel(), self._group)
-                lib.call("zsb_sgmcmc_sgnht_alpha_f32", ptr(self._alpha1[k]),
-                         ptr(self.alphas[k]), ptr(self._mean_k[k]),
-                         0.5 * self.tune_rate, self.lr, s)
+            self._scalar_alpha1()
         if self.second_order:                              # sgmcmc.py:493
             for q, v in zip(qs, self.vs):
                 lib.call("zsb_sgmcmc_half_q_f32", ptr(q), ptr(v), q.numel(), s)
@@ -382,10 +462,4 @@ class SGNHT(SGMCMC):
                          self.a, int(self.second_order), self._chains,
                          self._row_len[k], self._seed_now() + k, it,
                          self._row0, ptr(self._part), ptr(self._mean_k[k]), s)
-                # chains sharded over ranks: the thermostat is driven by the mean kinetic energy
-                # of ALL chains (one 8-byte all-reduce per latent and step; no-op on one rank)
-                zdist.all_reduce_weighted_mean_(self._mean_k[k], q.numel(), self._group)
-                coef = 0.5 * self.tune_rate if self.second_order \
-                    else self.tune_rate                    # sgmcmc.py:490, 506
-                lib.call("zsb_sgmcmc_sgnht_alpha_f32", ptr(self.alphas[k]),
-                         ptr(a_eff), ptr(self._mean_k[k]), coef, self.lr, s)
+                self._scalar_alpha_update(k, a_eff, q.numel())
