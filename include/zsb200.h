@@ -513,6 +513,24 @@ int zsb_sgmcmc_bnn_step_f32(int method, float* w0, float* w1, float* v0, float* 
                             float* part, float* mean_k0, float* mean_k1, int64_t chains,
                             void* stream);
 
+/* ---- BNN regression log-joint, value / gradient / predictions (csrc/bnn_logjoint.cu) ----------
+ * The model and log-joint of examples/bayesian_neural_nets/bnn_vi.py:18-35, 83-86 (the same as
+ * bnn_sgmcmc.py:19-35, 74-77) for K particles, replacing the einsum / concat / relu / Normal
+ * log_prob graph and its tf.gradients (bnn_vi.py:88-89) and the prediction fetches (:98-103):
+ *   lp[k] = sum log N(w0[k]; 0, exp(ls0)) + sum log N(w1[k]; 0, exp(ls1))
+ *           + n_train * mean_b log N(y_b; y_mean[k, b], exp(y_logstd))
+ * w0 [K, H, n_in+1], w1 [K, 1, H+1], x [B, n_in], y [B]; logstd0 / logstd1 are read flat over one
+ * particle's weights, index modulo logstd*_n.  y_logstd is a DEVICE scalar (learnable, no host
+ * sync).  Outputs, each written only when non-NULL: lp [K]; g0 / g1 (shaped like w0 / w1) =
+ * d lp / d w; g_ylogstd [K] = d lp[k] / d y_logstd; y_mean [K, B]; log_lik [K, B] =
+ * log N(y_b; y_mean, exp(y_logstd)), unscaled.  n_in + 1 <= 16, H <= 64, any B >= 1.  No
+ * floating-point atomics: deterministic. */
+int zsb_bnn_logjoint_f32(const float* w0, const float* w1, const float* x, const float* y,
+                         int64_t B, int n_in, int H, const float* logstd0, int64_t logstd0_n,
+                         const float* logstd1, int64_t logstd1_n, const float* y_logstd,
+                         float n_train, float* lp, float* g0, float* g1, float* g_ylogstd,
+                         float* y_mean, float* log_lik, int64_t K, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

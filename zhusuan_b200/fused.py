@@ -7,6 +7,7 @@ import os
 
 import numpy as np
 import torch
+from torch.autograd.function import once_differentiable
 
 __all__ = ["GaussianLogJoint", "BNNRegressionLogJoint", "LNTMLogJoint", "PMFLogJoint", "linear",
            "linear_bernoulli_log_prob", "LinearBernoulli"]
@@ -82,25 +83,56 @@ class GaussianLogJoint(object):
 
 class BNNRegressionLogJoint(object):
     """The log-joint of examples/bayesian_neural_nets/bnn_sgmcmc.py:19-35, 74-77
-    for layer sizes [n_in, H, 1] and per-chain weights:
+    (and bnn_vi.py:18-35, 83-86) for layer sizes [n_in, H, 1] and per-particle
+    weights:
 
-        w0 [chains, H, n_in+1] ~ N(0, exp(logstds[0])),
-        w1 [chains, 1, H+1]    ~ N(0, exp(logstds[1])),
+        w0 [K, H, n_in+1] ~ N(0, exp(logstds[0])),
+        w1 [K, 1, H+1]    ~ N(0, exp(logstds[1])),
         y ~ N(net(x; w), exp(y_logstd)),
         log_joint = sum log p(w) + mean_batch(log p(y|x,w)) * n_train.
 
     As a callable it is the generic-path log-joint (registry Normal kernels +
-    torch einsum under the tape); ``zs.SGHMC.sample`` recognises it and runs
-    the whole step in one fused kernel (zsb_sgmcmc_sghmc_bnn_f32).  Feed
-    minibatches with ``sample_op(observed={'x': xb, 'y': yb})``; ``x`` is
-    [B, n_in] and ``y`` holds B values.
+    torch einsum under the tape).  Three kinds of consumer recognise it and run
+    fused kernels instead:
+
+    * ``zs.SGHMC`` / ``SGLD`` / ``PSGLD`` / ``SGNHT`` run the whole step in one
+      launch (zsb_sgmcmc_bnn_step_f32), for minibatches of up to 512 rows and
+      a float ``y_logstd``.
+    * ``zs.variational.elbo`` / ``iw_objective`` / ``klpq`` and
+      ``zs.is_loglikelihood`` take the log-joint term from
+      ``fused_log_joint`` (zsb_bnn_logjoint_f32: value and gradient in one
+      launch, differentiable w.r.t. w0, w1 and a tensor ``y_logstd``).
+    * ``zs.HMC`` takes ``logp`` and ``grad`` from the same kernel, one launch
+      each, over any number of rows (full-batch HMC).  It decides in
+      ``sample()``; rows fed later through ``sample_op(observed=...)`` that do
+      not fit the kernel are evaluated on the generic path for that call.
+
+    ``predictive(observed)`` gives y_mean and the per-point log-likelihood of
+    every particle in one launch (test-set RMSE and log-likelihood of
+    variational, SG-MCMC or HMC samples).
+
+    Feed minibatches with ``sample_op(observed={'x': xb, 'y': yb})`` or in the
+    objective's ``observed``; ``x`` is [B, n_in] and ``y`` holds B values.
+
+    ``y_logstd`` is a float or a 0-d float32 CUDA tensor.  A tensor is read in
+    place by the kernels (no host sync) and receives a gradient, so it can be
+    learned as bnn_vi.py does; SG-MCMC then takes its generic path.
 
     ``logstds[k]`` broadcasts against w_k with NumPy rules.  Shapes that
-    broadcast to one chain's weights -- for logstds[0] e.g. [H, n_in+1],
+    broadcast to one particle's weights -- for logstds[0] e.g. [H, n_in+1],
     [H, 1] (one scale per hidden unit), [n_in+1] or [] -- run on the fused
-    kernel; shapes with chain axes, e.g. [chains, H, n_in+1] or
-    [chains, 1, H+1], run on the generic path.
+    kernels; shapes with chain axes, e.g. [chains, H, n_in+1] or
+    [chains, 1, H+1], run on the generic path.  ``fused_inputs`` is the
+    eligibility check of the objectives, HMC and ``predictive``: 3-D latents
+    [K, H, n_in+1] / [K, 1, H+1] in float32 with n_in + 1 <= 16 and H <= 64,
+    ``x`` [B, n_in] and B values of ``y``, all on one CUDA device, float32
+    prior logstds that broadcast to one particle and do not require a
+    gradient.  Under ``torch.no_grad()`` ``fused_log_joint`` launches the
+    value-only kernel; its gradient is first order (no double backward).  Anything else: the objectives and
+    HMC fall back to ``__call__`` under autograd, ``predictive`` raises.
     """
+
+    MAX_IN1, MAX_H = 16, 64      # limits of the fused kernels (n_in + 1, H)
 
     def __init__(self, x, y, logstds, n_train, y_logstd=-0.95,
                  names=("w0", "w1")):
@@ -109,9 +141,18 @@ class BNNRegressionLogJoint(object):
         self.x, self.y = x, y
         self.logstds = [l.contiguous() for l in logstds]
         self.n_train = float(n_train)
-        self.y_logstd = float(y_logstd)
+        if isinstance(y_logstd, torch.Tensor):
+            if y_logstd.dim() != 0 or y_logstd.dtype != torch.float32 or \
+                    not y_logstd.is_cuda:
+                raise ValueError("y_logstd must be a float or a 0-d float32 CUDA tensor, "
+                                 "got %s %s on %s" % (y_logstd.dtype, tuple(y_logstd.shape),
+                                                      y_logstd.device))
+            self.y_logstd = y_logstd
+        else:
+            self.y_logstd = float(y_logstd)
         self.names = tuple(names)
         self._prior_cache = {}
+        self._ys_dev = None
         self._zsb_fused = {"kind": "bnn_regression", "obj": self}
 
     def fused_prior_logstd(self, k, shape):
@@ -145,6 +186,117 @@ class BNNRegressionLogJoint(object):
         if "y" in observed:
             self.y = observed["y"]
 
+    def _y_logstd_dev(self, device):
+        """y_logstd as the one-element device array the kernel reads: the tensor itself, or a
+        copy of the float, made once per value and device."""
+        if isinstance(self.y_logstd, torch.Tensor):
+            return self.y_logstd
+        e = self._ys_dev
+        if e is None or e[0] != (self.y_logstd, device):
+            e = ((self.y_logstd, device),
+                 torch.tensor(self.y_logstd, dtype=torch.float32, device=device))
+            self._ys_dev = e
+        return e[1]
+
+    def fused_inputs(self, observed):
+        """``(w0, w1, x, y)`` when the fused log-joint kernel can evaluate ``observed``, else
+        None (the caller runs ``__call__`` under autograd).  ``x`` / ``y`` come from
+        ``observed``, else from the object; latents that are ``StochasticTensor`` samples of a
+        variational net are unwrapped."""
+        try:
+            w0, w1 = (_unwrap(observed[n]) for n in self.names)
+        except KeyError:
+            return None
+        x, y = _unwrap(observed.get("x", self.x)), _unwrap(observed.get("y", self.y))
+        ts = (w0, w1, x, y)
+        if not all(isinstance(t, torch.Tensor) and t.is_cuda for t in ts) or \
+                w0.dtype != torch.float32 or w1.dtype != torch.float32:
+            return None
+        if w0.dim() != 3 or w1.dim() != 3:
+            return None
+        K, H, in1 = (int(d) for d in w0.shape)
+        if tuple(w1.shape) != (K, 1, H + 1) or not (2 <= in1 <= self.MAX_IN1) or \
+                not (1 <= H <= self.MAX_H) or K < 1:
+            return None
+        if x.dim() != 2 or int(x.shape[1]) + 1 != in1 or x.shape[0] < 1 or \
+                y.numel() != x.shape[0]:
+            return None
+        dev = w0.device
+        if w1.device != dev or x.device != dev or y.device != dev:
+            return None
+        # the kernel reads the prior and y_logstd scales as float32 on w0's device
+        if any(ls.requires_grad or ls.dtype != torch.float32 or ls.device != dev
+               for ls in self.logstds):
+            return None
+        if isinstance(self.y_logstd, torch.Tensor) and self.y_logstd.device != dev:
+            return None
+        if self.fused_prior_logstd(0, w0.shape[1:]) is None or \
+                self.fused_prior_logstd(1, w1.shape[1:]) is None:
+            return None
+        return w0, w1, x, y
+
+    def _launch(self, w0, w1, x, y, ys, lp=False, g0=False, g1=False, gys=False,
+                ym=False, ll=False):
+        """One zsb_bnn_logjoint_f32 launch; returns the requested outputs (None elsewhere)."""
+        from ._lib import lib, ptr, stream
+        K, H, in1 = (int(d) for d in w0.shape)
+        B = int(x.shape[0])
+        dev = w0.device
+        w0, w1 = w0.detach().contiguous(), w1.detach().contiguous()
+        x = x.detach().to(torch.float32).contiguous()
+        y = y.detach().to(torch.float32).contiguous().view(-1)
+        ys = ys.detach()
+        ls0 = self.fused_prior_logstd(0, w0.shape[1:]).detach()
+        ls1 = self.fused_prior_logstd(1, w1.shape[1:]).detach()
+        e = lambda want, *s: torch.empty(s, dtype=torch.float32, device=dev) if want else None  # noqa: E731
+        out = (e(lp, K), e(g0, K, H, in1), e(g1, K, 1, H + 1), e(gys, K), e(ym, K, B),
+               e(ll, K, B))
+        lib.call("zsb_bnn_logjoint_f32", ptr(w0), ptr(w1), ptr(x), ptr(y), B, in1 - 1, H,
+                 ptr(ls0), ls0.numel(), ptr(ls1), ls1.numel(), ptr(ys), self.n_train,
+                 *[ptr(o) for o in out], K, stream())
+        return out
+
+    def fused_log_joint(self, observed):
+        """The log-joint [K] of ``observed`` on the fused kernel, differentiable w.r.t. w0, w1
+        and a tensor ``y_logstd``: the forward launch also computes the gradients of the inputs
+        that need one, and backward scales them by the upstream [K] gradient.  ValueError when
+        ``fused_inputs(observed)`` is None."""
+        got = self.fused_inputs(observed)
+        if got is None:
+            raise ValueError("BNNRegressionLogJoint.fused_log_joint: these inputs need the "
+                             "generic path (see fused_inputs)")
+        w0, w1, x, y = got
+        ys = self._y_logstd_dev(w0.device)
+        if not torch.is_grad_enabled():        # nothing is recorded: the value-only launch
+            return self._launch(w0, w1, x, y, ys, lp=True)[0]
+        return _BNNLogJoint.apply(w0.contiguous(), w1.contiguous(), ys, self, x, y)
+
+    def predictive(self, observed):
+        """``(y_mean [K, B], log_lik [K, B])`` of every particle ``observed[names]`` at the rows
+        ``observed['x']`` (else the object's x), with log_lik = log N(y_b; y_mean, exp(y_logstd))
+        unscaled -- the prediction fetches of bnn_vi.py:98-103 -- from one launch, no gradient.
+        E.g. RMSE = ((y_mean.mean(0) - y) ** 2).mean().sqrt() and test log-likelihood =
+        (log_lik.logsumexp(0) - log K).mean()."""
+        got = self.fused_inputs(observed)
+        if got is None:
+            raise ValueError("BNNRegressionLogJoint.predictive: shapes outside the fused "
+                             "kernel's limits (see fused_inputs)")
+        w0, w1, x, y = got
+        _, _, _, _, ym, ll = self._launch(w0, w1, x, y, self._y_logstd_dev(w0.device),
+                                          ym=True, ll=True)
+        return ym, ll
+
+    def hmc_provider(self, latent_names, observed, latents):
+        """The provider ``zs.HMC`` uses instead of autograd (logp / grad, one launch each) when
+        the latents are (w0, w1) and ``fused_inputs`` accepts them; else None."""
+        if list(latent_names) != list(self.names):
+            return None
+        obs = dict(observed)
+        obs.update(zip(self.names, latents))
+        if self.fused_inputs(obs) is None:
+            return None
+        return _BNNProvider(self, observed)
+
     def __call__(self, observed):
         x = observed.get("x", self.x)
         y = observed.get("y", self.y)
@@ -161,11 +313,77 @@ class BNNRegressionLogJoint(object):
             lp = lp + self._Normal(torch.zeros_like(ls), logstd=ls,
                                    group_ndims=2).log_prob(w)
         y_mean = h.squeeze(2)
-        lpy = self._Normal(y_mean, logstd=torch.full_like(y_mean,
-                                                         self.y_logstd)
-                           ).log_prob(y.unsqueeze(0))
+        if isinstance(self.y_logstd, torch.Tensor):
+            y_ls = self.y_logstd.to(y_mean.dtype).expand_as(y_mean)
+        else:
+            y_ls = torch.full_like(y_mean, self.y_logstd)
+        lpy = self._Normal(y_mean, logstd=y_ls).log_prob(y.unsqueeze(0))
         return lp + lpy.mean(1) * self.n_train
 
+
+def _unwrap(v):
+    """The tensor of a ``StochasticTensor`` (a variational net's sample), else ``v``."""
+    return v if isinstance(v, torch.Tensor) else getattr(v, "tensor", v)
+
+
+class _BNNLogJoint(torch.autograd.Function):
+    """lp [K] of BNNRegressionLogJoint over (w0, w1, y_logstd) on zsb_bnn_logjoint_f32.  The
+    forward launch writes the gradients of the inputs that need one; backward only scales
+    them by the upstream gradient (any [K] weights, e.g. iw_objective's normalised ones)."""
+
+    @staticmethod
+    def forward(ctx, w0, w1, ys, obj, x, y):
+        need = ctx.needs_input_grad
+        lp, g0, g1, gys, _, _ = obj._launch(w0, w1, x, y, ys, lp=True, g0=need[0], g1=need[1],
+                                            gys=need[2])
+        ctx.save_for_backward(g0, g1, gys)
+        return lp
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, glp):
+        g0, g1, gys = ctx.saved_tensors
+        glp = glp.to(torch.float32)
+        d0 = g0 * glp.view(-1, 1, 1) if g0 is not None else None
+        d1 = g1 * glp.view(-1, 1, 1) if g1 is not None else None
+        dys = (gys * glp).sum() if gys is not None else None
+        return d0, d1, dys, None, None, None
+
+
+class _BNNProvider(object):
+    """HMC's provider interface over BNNRegressionLogJoint: values and gradients of the latents
+    (w0, w1) at the observed rows, one zsb_bnn_logjoint_f32 launch each.  HMC picks the provider
+    once, in sample(); should later ``sample_op(observed=...)`` rows not fit the kernel, that call
+    runs the generic path (``__call__``, under autograd for the gradient) instead."""
+
+    def __init__(self, obj, observed):
+        self.obj, self.observed = obj, observed
+
+    def _obs(self, var_list):
+        obs = dict(self.observed)
+        obs.update(zip(self.obj.names, var_list))
+        return obs
+
+    def logp(self, var_list):
+        obs = self._obs(var_list)
+        got = self.obj.fused_inputs(obs)
+        if got is None:
+            return self.obj(obs)
+        w0, w1, x, y = got
+        return self.obj._launch(w0, w1, x, y, self.obj._y_logstd_dev(w0.device), lp=True)[0]
+
+    def grad(self, var_list):
+        got = self.obj.fused_inputs(self._obs(var_list))
+        if got is None:
+            xs = [v.detach().requires_grad_(True) for v in var_list]
+            with torch.enable_grad():
+                gs = torch.autograd.grad(self.obj(self._obs(xs)).sum(), xs, allow_unused=True)
+            return [g.contiguous() if g is not None else torch.zeros_like(x)
+                    for g, x in zip(gs, xs)]
+        w0, w1, x, y = got
+        out = self.obj._launch(w0, w1, x, y, self.obj._y_logstd_dev(w0.device), g0=True,
+                               g1=True)
+        return [out[1], out[2]]
 
 
 class LNTMLogJoint(object):

@@ -170,6 +170,12 @@ class HMC(object):
         if fused is not None and fused["kind"] == "provider":
             self._provider = fused["obj"]
             fused = None
+        elif fused is not None and fused["kind"] == "bnn_regression":
+            # zs.fused.BNNRegressionLogJoint: a provider when its shapes fit the fused kernel
+            prov = fused["obj"].hmc_provider(self._latent_k, self._observed, self._q)
+            if prov is not None:
+                self._provider = prov
+                fused = None
         self._fused = fused
 
         if fused is not None and fused["kind"] == "dense_gaussian":

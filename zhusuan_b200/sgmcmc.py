@@ -167,6 +167,8 @@ class SGMCMC(object):
         obj = f["obj"]
         if list(self._latent_k) != list(obj.names):
             return None
+        if isinstance(obj.y_logstd, torch.Tensor):   # the step kernel takes y_logstd by value
+            return None
         w0, w1 = self._var_list
         if w0.dim() != 3 or w1.dim() != 3 or w1.shape[1] != 1 or \
                 w1.shape[2] != w0.shape[1] + 1:

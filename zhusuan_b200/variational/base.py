@@ -102,8 +102,16 @@ class VariationalObjective(TensorArithmeticMixin):
         if self._meta_bn:
             return self.bn.log_joint()
         if "log_joint" not in self._cache:
-            self._cache["log_joint"] = self._log_joint(
-                merge_dicts(self._v_inputs, self._observed))
+            obs = merge_dicts(self._v_inputs, self._observed)
+            # zs.fused.BNNRegressionLogJoint: value and gradient from one fused launch when
+            # the shapes fit its kernel, else the callable under autograd
+            f = getattr(self._log_joint, "_zsb_fused", None)
+            obj = f.get("obj") if f is not None and \
+                f.get("kind") == "bnn_regression" else None
+            if obj is not None and obj.fused_inputs(obs) is not None:
+                self._cache["log_joint"] = obj.fused_log_joint(obs)
+            else:
+                self._cache["log_joint"] = self._log_joint(obs)
         return self._cache["log_joint"]
 
     def _entropy_term(self):
