@@ -219,6 +219,45 @@ int zsb_linear_tc_wgrad_f32(const void* h_planes, const float* scale_h, int K,
                             const void* g_planes, const float* scale_g, int J, int64_t R,
                             float* out, float* part, void* stream);
 
+/* ---- Sigmoid belief net layers: tf.layers.dense + bn.bernoulli(..., n_samples, dtype=tf.float32)
+ * of examples/sigmoid_belief_nets/sbn_vimco.py:19-44 (and sbn_adaptive_is.py), with
+ * Bernoulli._sample / _log_prob (univariate.py:386-403) in the GEMM epilogue.
+ * A "binary" activation is a 0/1 sample whose operand is ONE fp16 plane h * 2048 (its lo plane is
+ * identically zero and is neither stored nor loaded): its products issue two fp16 wgmma per k-step
+ * instead of three and give the same result bit for bit as the split planes of the same matrix.
+ *
+ * One launch per sampled layer, l = h W^T + bias never written: h_out [S R, J] = (u < sigmoid(l))
+ * (float, or int32 when h_int) with u = u_in [S R J] or the Philox draw of zsb_sample_bernoulli_i32
+ * for (seed, iter) at element (s R + r) J + j (so the result equals sampling the fp32 logits of
+ * zsb_linear_tc_f32); h_planes_out [S R][kpad(J)] = its binary operand plane; logq [S R] = the
+ * grouped log-probability of each draw; part = zsb_linear_tc_nparts(J) * S R floats of scratch.
+ * h_binary: h_planes is itself a binary plane. */
+int zsb_linear_tc_bern_sample_f32(const void* w_planes, const float* scale_w, const void* h_planes,
+                                  const float* scale_h, int h_binary, const float* bias,
+                                  const float* u_in, uint64_t seed, uint32_t iter, int S,
+                                  void* h_out, int h_int, void* h_planes_out, float* logq,
+                                  float* part, int64_t R, int J, int K, void* stream);
+/* S given rows per logit row (a [S, R, J] sample against [R, J] logits, univariate.py:398-403):
+ *   epi 1: out [S R] = sum_j Bernoulli(l[r]).log_prob(given[s R + r, j]);  part as above
+ *   epi 2: out [R, J] = sum_s gout[s R + r] * (given[s R + r, j] - sigmoid(l[r, j]))  (d/dl of the
+ *          broadcast), max |out| folded into amax_scale[2] (may be NULL) */
+int zsb_linear_tc_bern_given_f32(int epi, const void* w_planes, const float* scale_w,
+                                 const void* h_planes, const float* scale_h, int h_binary,
+                                 const float* bias, const float* given, int S, const float* gout,
+                                 float* out, float* part, int64_t R, int J, int K,
+                                 float* amax_scale, void* stream);
+/* zsb_linear_tc_amax_f32 / zsb_linear_tc_wgrad_f32 with a binary activation h (h_planes = its one
+ * plane, scale_h[0] = 2048): the forward, epi 1 / 2 and weight-gradient products of a layer fed a
+ * sample (sbn_vimco.py:25-30, 40-43). */
+int zsb_linear_tc_bin_f32(int epi, const void* w_planes, const float* scale_w,
+                          const void* h_planes, const float* scale_h, const float* bias,
+                          const float* x_obs, int64_t n_x, const float* gout, float* out,
+                          float* part, int64_t R, int J, int K, int relu, float* amax_scale,
+                          void* stream);
+int zsb_linear_tc_wgrad_bin_f32(const void* h_planes, const float* scale_h, int K,
+                                const void* g_planes, const float* scale_g, int J, int64_t R,
+                                float* out, float* part, void* stream);
+
 /* ---- diagnostics: effective sample size (zhusuan/diagnostics.py:17-64, the Stan estimator) on the
  * device; samples [M, D] row-major with burn-in already dropped -> ess [D].  M >= 2. */
 int zsb_effective_sample_size_f32(const float* samples, int64_t M, int64_t D, float* ess,

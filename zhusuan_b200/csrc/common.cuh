@@ -135,6 +135,9 @@ __device__ __forceinline__ float u32_to_uniform(uint32_t x) {        // [0, 1)
 __device__ __forceinline__ float u32_to_uniform_open(uint32_t x) {   // (0, 1]
   return ((float)(x >> 8) + 1.0f) * (1.0f / 16777216.0f);
 }
+// Logistic sigmoid with the accurate expf.  Every kernel that draws h = (u < sigmoid(l)) uses this
+// one definition, so the fused sampling epilogue and the elementwise sampler agree bit for bit.
+__device__ __forceinline__ float sigmoidf_(float l) { return 1.f / (1.f + expf(-l)); }
 __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, float& z1) {
   const float u1 = u32_to_uniform_open(a), u2 = u32_to_uniform(b);
   const float r = sqrtf(-2.0f * logf(u1));

@@ -241,7 +241,6 @@ int launch_elementwise(int64_t n, F f, cudaStream_t st, const char* what) {
 __device__ __forceinline__ float bernoulli_lp(float x, float l) {
   return -(fmaxf(l, 0.f) - l * x + __logf(1.f + __expf(-fabsf(l))));
 }
-__device__ __forceinline__ float sigmoidf_(float l) { return 1.f / (1.f + expf(-l)); }
 
 // One warp per row of C categories: returns (max, log-sum-exp) over logits[row*C .. +C).
 __device__ __forceinline__ float warp_row_lse(const float* __restrict__ l, int64_t C, int lane) {

@@ -23,11 +23,19 @@
 // warp touches 32 consecutive features of one row per instruction: coalesced x loads and out stores.
 #include "tc_common.cuh"
 
+extern "C" int zsb_linear_tc_kpad(int K);
+extern "C" int zsb_linear_tc_slices(int64_t R, int J, int K);
+
 namespace {
 
 __device__ __forceinline__ float bern_lp(float x, float l) {   // -sigmoid_cross_entropy(x, l)
   return -(fmaxf(l, 0.f) - l * x + __logf(1.f + __expf(-fabsf(l))));
 }
+
+// Scale of the fp16 operand plane of a 0/1 sample (EPI 4): the power of two zsb_split16_* picks
+// for a matrix whose max |.| is 1, so the sample's plane is the hi plane the split would make, and
+// its lo plane is exactly zero.
+constexpr float BIN_SCALE = 2048.f;
 
 // MN (bit 0: operand A, bit 1: operand B; EPI 0 only): the operand is read in a row-major plane
 // layout [contraction rows, features] -- MN-major (transposed) wgmma operand.  MN = 3: weight
@@ -36,19 +44,44 @@ __device__ __forceinline__ float bern_lp(float x, float l) {   // -sigmoid_cross
 // copy of anything.  A stage then holds, per plane, two TMA boxes of 64 contraction rows x 64
 // features (128-byte rows, SWIZZLE_128B; see gmma_desc).  `Kp` is the padded contraction length.
 // GL: the epi 2 / 3 epilogues load the upstream gradient per row instead of broadcasting it.
-template <int EPI, int MN, int GL>
+// ZLO: bit 0 / 1 = the lo plane of operand A / B is zero (a 0/1 sample, see mma_kblock): it is
+// neither loaded nor multiplied.
+//
+// Epilogues with S >= 1 rows of samples per logit row r (sample row s * R + r, k_slices = 1):
+//   EPI 4  Bernoulli sampling: h = (u < sigmoidf_(l)) with u injected or drawn from Philox keyed as
+//          zsb_sample_bernoulli_i32 keys element (s R + r) J + j; writes h (float or int32), its fp16
+//          operand plane h * BIN_SCALE [S R][kpad(J)] (pad columns zero) and the epi-1 partial rows
+//          of log Bernoulli(l).log_prob(h) ([nparts][S R])
+//   EPI 5  the epi-1 partial rows of the given samples x[s R + r] against logit row r
+//   EPI 6  out[r, j] = sum_s g[s R + r] * (x[s R + r, j] - sigmoid(l))     (d/dl of EPI 5)
+template <int EPI, int MN, int GL, int Z = 0>
 struct LinW {
-  static constexpr int KIND = 1, RB = 128, MNA = MN & 1, MNB = (MN >> 1) & 1, CVT = 0;
-  static constexpr uint32_t TX = Cfg<RB>::STAGE;
+  static constexpr int KIND = 1, RB = 128, MNA = MN & 1, MNB = (MN >> 1) & 1, CVT = 0, ZLO = Z;
+  static constexpr uint32_t TX = Cfg<RB>::STAGE - ((Z & 1) ? Cfg<RB>::A_TILE : 0) -
+                                 ((Z & 2) ? Cfg<RB>::B_TILE : 0);
   CUtensorMap map_whi, map_wlo, map_hhi, map_hlo;
   const float* bias; const float* x_obs; int64_t n_x; const float* gout;
   float* out; float* part; int64_t R; int J; int Kp; int relu;
   const float* scale_w; const float* scale_h; int k_slices; float* amax_scale;
   int n_blk; int64_t n_tiles; int n_kb_all; int kb_per;
+  // EPI 4 - 6.  EPI 4 / 5 split the S sample rows of a tile into k_slices chunks of s_per rows,
+  // each its own unit, so a layer with few logit rows and many draws still fills every SM.  The
+  // price: each chunk recomputes the tile's whole product (about 125 times for the proposal's first
+  // layer at 100 rows and K = 1000).  EPI 4 also runs one Philox-10 per element, four times the
+  // work of the elementwise sampler, which shares one draw among four elements; it keeps the
+  // sampler's keying so the samples are bit-identical.  Neither cost is measured on its own; the
+  // layer as a whole is (scripts/bench_sbn.py).
+  int S; int s_per; const float* u_in; uint64_t seed; uint32_t iter; const uint32_t* epoch;
+  int h_int; __half* pl_out;
   struct EpiState { float amax = 0.f; };
 
   __host__ __device__ __forceinline__ int64_t units() const { return n_tiles * k_slices; }
   __device__ __forceinline__ void kb_range(int64_t uu, int& kb0, int& kb1) const {
+    if (EPI >= 4) {
+      kb0 = 0;
+      kb1 = n_kb_all;
+      return;
+    }
     kb0 = (int)(uu / n_tiles) * kb_per;
     kb1 = min(kb0 + kb_per, n_kb_all);
   }
@@ -66,27 +99,116 @@ struct LinW {
       for (int b = 0; b < 2; ++b) {
         const uint32_t o = (uint32_t)b * 8192u;
         tma_load_2d(sa + o, &map_whi, fb, j0 + 64 * b, kb * 64);
-        tma_load_2d(sa + C::A_TILE + o, &map_wlo, fb, j0 + 64 * b, kb * 64);
+        if (!(Z & 1)) tma_load_2d(sa + C::A_TILE + o, &map_wlo, fb, j0 + 64 * b, kb * 64);
       }
     } else {
       tma_load_2d(sa, &map_whi, fb, kb * 64, j0);
-      tma_load_2d(sa + C::A_TILE, &map_wlo, fb, kb * 64, j0);
+      if (!(Z & 1)) tma_load_2d(sa + C::A_TILE, &map_wlo, fb, kb * 64, j0);
     }
     if (MN & 2) {
 #pragma unroll
       for (int b = 0; b < 2; ++b) {
         const uint32_t o = (uint32_t)b * 8192u;
         tma_load_2d(sa + 2 * C::A_TILE + o, &map_hhi, fb, r0 + 64 * b, kb * 64);
-        tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE + o, &map_hlo, fb, r0 + 64 * b, kb * 64);
+        if (!(Z & 2))
+          tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE + o, &map_hlo, fb, r0 + 64 * b, kb * 64);
       }
     } else {
       tma_load_2d(sa + 2 * C::A_TILE, &map_hhi, fb, kb * 64, r0);
-      tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE, &map_hlo, fb, kb * 64, r0);
+      if (!(Z & 2)) tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE, &map_hlo, fb, kb * 64, r0);
     }
   }
   __device__ __forceinline__ void convert(int64_t, int, uint8_t*, int) const {}
   __device__ __forceinline__ void epilogue(int64_t uu, uint32_t trow, int quarter, int lane,
                                            EpiState& st) const {
+    if constexpr (EPI >= 4)
+      epilogue_samples(uu, trow, quarter, lane, st);
+    else
+      epilogue_rows(uu, trow, quarter, lane, st);
+  }
+  // EPI 4 - 6: per 16-row block of this lane's feature j, the logits once, then each of the S
+  // sample rows of those logit rows
+  __device__ __forceinline__ void epilogue_samples(int64_t unit, uint32_t trow, int quarter,
+                                                   int lane, EpiState& st) const {
+    const float acc_scale = 1.f / (scale_w[0] * scale_h[0]);
+    const int s0 = (int)(unit / n_tiles) * s_per, s1 = min(S, s0 + s_per);
+    unit %= n_tiles;
+    const int nb = (int)(unit % n_blk);
+    const int j = nb * BM + quarter * 32 + lane;
+    const bool j_ok = j < J;
+    const int Jp = ((J + 63) / 64) * 64;
+    const bool col_ok = j < Jp;                    // EPI 4 plane: real and zero-padding columns
+    const float b_j = (j_ok && bias) ? bias[j] : 0.f;
+    const int64_t r0 = (unit / n_blk) * BN;
+    const int64_t part_row = (int64_t)(nb * 4 + quarter) * ((int64_t)S * R);
+    const uint32_t it = (EPI == 4) ? iter + (epoch ? *epoch : 0u) : 0u;
+#pragma unroll 1
+    for (int c = 0; c < BN; c += 16) {
+      const int64_t rbase = r0 + c;
+      uint32_t v[16];
+      acc_ld16(trow + 4u * (uint32_t)c, v);
+      float l[16], sg[16], dl[16];
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+        l[jj] = fmaf(__uint_as_float(v[jj]), acc_scale, b_j);
+        sg[jj] = sigmoidf_(l[jj]);
+        dl[jj] = 0.f;
+      }
+#pragma unroll 1
+      for (int s = s0; s < s1; ++s) {
+        float lpv[16];
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+          const int64_t r = rbase + jj;
+          const bool ok = j_ok && r < R;
+          const int64_t srow = (int64_t)s * R + r;
+          const int64_t i = srow * J + j;           // element of the flattened [S, R, J] sample
+          float x = 0.f;
+          if (EPI == 4) {
+            float uu;
+            if (u_in) {
+              uu = ok ? __ldg(u_in + i) : 1.f;
+            } else {
+              const Philox4 p = philox4x32_10((uint32_t)(i >> 2), (uint32_t)((uint64_t)i >> 34), it,
+                                              ZSB_STREAM_SAMPLE, (uint32_t)seed,
+                                              (uint32_t)(seed >> 32));
+              const uint32_t w = (i & 3) == 0 ? p.x : (i & 3) == 1 ? p.y : (i & 3) == 2 ? p.z : p.w;
+              uu = u32_to_uniform(w);
+            }
+            const int hb = (ok && uu < sg[jj]) ? 1 : 0;
+            x = (float)hb;
+            if (ok) {
+              if (h_int) reinterpret_cast<int32_t*>(out)[i] = hb;
+              else out[i] = x;
+            }
+            if (col_ok && r < R) pl_out[srow * Jp + j] = __float2half_rn(x * BIN_SCALE);
+          } else if (ok) {
+            x = __ldg(x_obs + i);
+          }
+          if (EPI == 6) {
+            const float g = r < R ? __ldg(gout + srow) : 0.f;
+            dl[jj] += g * (x - sg[jj]);
+          } else {
+            lpv[jj] = ok ? bern_lp(x, l[jj]) : 0.f;
+          }
+        }
+        if (EPI != 6) {
+          const float sum = warp_transpose_sum16(lpv, lane);
+          if (lane < 16 && rbase + lane < R) part[part_row + (int64_t)s * R + rbase + lane] = sum;
+        }
+      }
+      if (EPI == 6) {
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj)
+          if (j_ok && rbase + jj < R) {
+            out[(rbase + jj) * J + j] = dl[jj];
+            st.amax = fmaxf(st.amax, fabsf(dl[jj]));
+          }
+      }
+    }
+  }
+  __device__ __forceinline__ void epilogue_rows(int64_t uu, uint32_t trow, int quarter, int lane,
+                                                EpiState& st) const {
     float& amax = st.amax;   // max |stored output| (EPI 0 / 2): the consumer's fp16-split scale
     const float acc_scale = 1.f / (scale_w[0] * scale_h[0]);   // powers of two: exact
     // EPI 3: `out` = the fp16 plane pair [2][R][Jp_out], amax_scale[0] = their (a-priori) scale
@@ -202,7 +324,7 @@ struct LinW {
       if (EPI == 3 && part && j_ok) atomicAdd(part + j, csum);   // bias gradient (part = col_sum)
   }
   __device__ __forceinline__ void epi_finish(EpiState& st, int, int lane) const {
-    if ((EPI == 0 || EPI == 2) && amax_scale) {   // NaN / inf never win the max (fmaxf drops NaN)
+    if ((EPI == 0 || EPI == 2 || EPI == 6) && amax_scale) {   // NaN / inf never win (fmaxf drops NaN)
       const float m = warp_max(st.amax <= 3.0e38f ? st.amax : 0.f);
       if (lane == 0 && m > 0.f)
         atomicMax(reinterpret_cast<unsigned int*>(amax_scale) + 2, __float_as_uint(m));
@@ -211,20 +333,59 @@ struct LinW {
 };
 
 // one product on the tensor cores: A = w planes (J_ features), B = h planes (R rows)
-template <int EPI, int MN, int GL>
+template <int EPI, int MN, int GL, int Z = 0>
+LinW<EPI, MN, GL, Z> make_linw(const CUtensorMap& whi, const CUtensorMap& wlo,
+                               const CUtensorMap& hhi, const CUtensorMap& hlo, const float* bias,
+                               const float* x_obs, int64_t n_x, const float* gout, float* out,
+                               float* part, int64_t R, int J_, int Kp, int relu,
+                               const float* scale_w, const float* scale_h, int k_slices,
+                               float* amax_scale) {
+  const int n_blk = (J_ + BM - 1) / BM;
+  const int64_t n_tiles = ((R + BN - 1) / BN) * n_blk;
+  const int n_kb_all = Kp / 64;
+  const int kb_per = (n_kb_all + k_slices - 1) / k_slices;
+  LinW<EPI, MN, GL, Z> w{whi, wlo, hhi, hlo, bias, x_obs, n_x, gout, out, part, R, J_, Kp,
+                         relu, scale_w, scale_h, k_slices, amax_scale, n_blk, n_tiles,
+                         n_kb_all, kb_per};
+  w.S = 1;
+  w.s_per = 1;
+  return w;
+}
+template <int EPI, int MN, int GL, int Z = 0>
 int launch_linear(const CUtensorMap& whi, const CUtensorMap& wlo, const CUtensorMap& hhi,
                   const CUtensorMap& hlo, const float* bias, const float* x_obs, int64_t n_x,
                   const float* gout, float* out, float* part, int64_t R, int J_, int Kp, int relu,
                   const float* scale_w, const float* scale_h, int k_slices, float* amax_scale,
                   cudaStream_t st, const char* what) {
-  const int n_blk = (J_ + BM - 1) / BM;
-  const int64_t n_tiles = ((R + BN - 1) / BN) * n_blk;
-  const int n_kb_all = Kp / 64;
-  const int kb_per = (n_kb_all + k_slices - 1) / k_slices;
-  const LinW<EPI, MN, GL> w{whi, wlo, hhi, hlo, bias, x_obs, n_x, gout, out, part, R, J_, Kp,
-                            relu, scale_w, scale_h, k_slices, amax_scale, n_blk, n_tiles,
-                            n_kb_all, kb_per};
-  return tc_launch(w, st, what);
+  return tc_launch(make_linw<EPI, MN, GL, Z>(whi, wlo, hhi, hlo, bias, x_obs, n_x, gout, out, part,
+                                             R, J_, Kp, relu, scale_w, scale_h, k_slices,
+                                             amax_scale),
+                   st, what);
+}
+
+// EPI 4 / 5: split the S sample rows into chunks so that the launch has about two units per SM
+template <class W>
+W chunk_samples(W w) {
+  int64_t want = (2 * ZSB_NUM_SMS + w.n_tiles - 1) / w.n_tiles;
+  if (want > w.S) want = w.S;
+  if (want < 1) want = 1;
+  w.s_per = (int)((w.S + want - 1) / want);
+  w.k_slices = (w.S + w.s_per - 1) / w.s_per;
+  return w;
+}
+
+// Tensor maps of a forward-layout product: w planes [2][J][Kp] (A) and h planes [R][Kp] (B, hi
+// then lo plane).  binary_h: h has only its hi plane (a 0/1 sample); the lo map is never loaded.
+int linear_maps(const void* w_planes, const void* h_planes, int binary_h, int64_t R, int J, int Kp,
+                CUtensorMap* m) {
+  const __half* wp = reinterpret_cast<const __half*>(w_planes);
+  const __half* hp = reinterpret_cast<const __half*>(h_planes);
+  int rc;
+  if ((rc = make_map(&m[0], wp, (uint64_t)J, (uint64_t)Kp, BM, 128, 1))) return rc;
+  if ((rc = make_map(&m[1], wp + (int64_t)J * Kp, (uint64_t)J, (uint64_t)Kp, BM, 128, 1)))
+    return rc;
+  if ((rc = make_map(&m[2], hp, (uint64_t)R, (uint64_t)Kp, BN, 128, 1))) return rc;
+  return make_map(&m[3], binary_h ? hp : hp + R * Kp, (uint64_t)R, (uint64_t)Kp, BN, 128, 1);
 }
 
 // One pass over an activation / gradient matrix that produces BOTH operand layouts of the dense
@@ -478,6 +639,100 @@ int epi_gload() {
   return v;
 }
 
+// zsb_linear_tc_amax_f32 (Z = 0) and zsb_linear_tc_bin_f32 (Z = 2: h is a 0/1 sample)
+template <int Z>
+int linear_tc_amax(int epi, const void* w_planes, const float* scale_w, const void* h_planes,
+                   const float* scale_h, const float* bias, const float* x_obs, int64_t n_x,
+                   const float* gout, float* out, float* part, int64_t R, int J, int K, int relu,
+                   float* amax_scale, cudaStream_t st) {
+  ZSB_REQUIRE(epi >= 0 && epi <= 2, "zsb_linear_tc_f32: unknown epilogue");
+  ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && out && R > 0 && J > 0 && K > 0,
+              "zsb_linear_tc_f32: bad args");
+  ZSB_REQUIRE(R < (1LL << 31), "zsb_linear_tc_f32: too many rows");
+  ZSB_REQUIRE(epi == 0 || (x_obs && n_x > 0), "zsb_linear_tc_f32: observations missing");
+  ZSB_REQUIRE(epi != 1 || part, "zsb_linear_tc_f32: partial-sum scratch missing");
+  ZSB_REQUIRE(epi != 2 || gout, "zsb_linear_tc_f32: upstream gradient missing");
+  const int Kp = zsb_linear_tc_kpad(K);
+  CUtensorMap m[4];
+  int rc;
+  if ((rc = linear_maps(w_planes, h_planes, Z & 2, R, J, Kp, m))) return rc;
+  const CUtensorMap &m_whi = m[0], &m_wlo = m[1], &m_hhi = m[2], &m_hlo = m[3];
+  const int n_blk = (J + BM - 1) / BM;
+  int k_slices = 1;
+  if (epi == 0 && part) {
+    k_slices = zsb_linear_tc_slices(R, J, K);
+    if (k_slices > 1 && relu) {
+      zsb_set_error("zsb_linear_tc_f32: ReLU cannot be fused into a split-K launch");
+      return ZSB_ERR_INVALID;
+    }
+  }
+  float* out_k = (k_slices > 1) ? part : out;
+  float* amax_k = k_slices > 1 ? nullptr : amax_scale;
+  if (epi == 0)
+    rc = launch_linear<0, 0, 0, Z>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out_k, part,
+                                R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
+                                "linear_tc");
+  else if (epi == 1)
+    rc = launch_linear<1, 0, 0, Z>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, nullptr,
+                                part, R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
+                                "linear_tc");
+  else if (Z || !epi_gload())
+    rc = launch_linear<2, 0, 0, Z>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out_k, part,
+                                R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
+                                "linear_tc");
+  else if constexpr (!Z)
+    rc = launch_linear<2, 0, 1>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out_k, part,
+                                R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
+                                "linear_tc");
+
+  if (rc == ZSB_OK && k_slices > 1) {
+    const int64_t n = R * (int64_t)J;
+    int64_t blocks = zsb_ceil_div(n, 256);
+    if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
+    slice_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, k_slices, n, out);
+    return zsb_check_launch("linear_tc_slice_sum");
+  }
+  if (rc != ZSB_OK || epi != 1) return rc;
+  int64_t blocks = zsb_ceil_div(R, 256);
+  if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
+  part_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, 4 * n_blk, R, out);
+  return zsb_check_launch("linear_tc_part_sum");
+}
+
+// zsb_linear_tc_wgrad_f32 (Z = 0) and zsb_linear_tc_wgrad_bin_f32 (Z = 1: h is a 0/1 sample)
+template <int Z>
+int linear_tc_wgrad(const void* h_planes, const float* scale_h, int K, const void* g_planes,
+                    const float* scale_g, int J, int64_t R, float* out, float* part,
+                    cudaStream_t st) {
+  ZSB_REQUIRE(h_planes && g_planes && scale_h && scale_g && out && R > 0 && J > 0 && K > 0,
+              "zsb_linear_tc_wgrad_f32: bad args");
+  ZSB_REQUIRE(R < (1LL << 31) - 64, "zsb_linear_tc_wgrad_f32: too many rows");
+  const int Kp_h = zsb_linear_tc_kpad(K), Jp_g = zsb_linear_tc_kpad(J);
+  const int Rp = zsb_linear_tc_kpad((int)R);                 // padded contraction length
+  const __half* hp = reinterpret_cast<const __half*>(h_planes);
+  const __half* gp = reinterpret_cast<const __half*>(g_planes);
+  CUtensorMap m_whi, m_wlo, m_hhi, m_hlo;                    // "w" = h (rows = k), "h" = g
+  int rc;
+  if ((rc = make_map(&m_whi, hp, (uint64_t)R, (uint64_t)Kp_h, 64, 128, 1))) return rc;
+  if ((rc = make_map(&m_wlo, (Z & 1) ? hp : hp + R * Kp_h, (uint64_t)R, (uint64_t)Kp_h, 64, 128, 1))) return rc;
+  if ((rc = make_map(&m_hhi, gp, (uint64_t)R, (uint64_t)Jp_g, 64, 128, 1))) return rc;
+  if ((rc = make_map(&m_hlo, gp + R * Jp_g, (uint64_t)R, (uint64_t)Jp_g, 64, 128, 1))) return rc;
+  const int k_slices = part ? zsb_linear_tc_slices(J, K, (int)R) : 1;
+  rc = launch_linear<0, 3, 0, Z>(m_whi, m_wlo, m_hhi, m_hlo, nullptr, nullptr, 0, nullptr,
+                              k_slices > 1 ? part : out, part, (int64_t)J, K, Rp, 0, scale_h,
+                              scale_g, k_slices, nullptr, st, "linear_tc_wgrad");
+
+  if (rc == ZSB_OK && k_slices > 1) {
+    const int64_t n = (int64_t)J * K;
+    int64_t blocks = zsb_ceil_div(n, 256);
+    if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
+    slice_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, k_slices, n, out);
+    return zsb_check_launch("linear_tc_wgrad_slice_sum");
+  }
+  return rc;
+}
+
+
 }  // namespace
 
 extern "C" {
@@ -590,64 +845,19 @@ int zsb_linear_tc_amax_f32(int epi, const void* w_planes, const float* scale_w,
                            const float* x_obs, int64_t n_x, const float* gout, float* out,
                            float* part, int64_t R, int J, int K, int relu, float* amax_scale,
                            void* stream) {
-  ZSB_REQUIRE(epi >= 0 && epi <= 2, "zsb_linear_tc_f32: unknown epilogue");
-  ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && out && R > 0 && J > 0 && K > 0,
-              "zsb_linear_tc_f32: bad args");
-  ZSB_REQUIRE(R < (1LL << 31), "zsb_linear_tc_f32: too many rows");
-  ZSB_REQUIRE(epi == 0 || (x_obs && n_x > 0), "zsb_linear_tc_f32: observations missing");
-  ZSB_REQUIRE(epi != 1 || part, "zsb_linear_tc_f32: partial-sum scratch missing");
-  ZSB_REQUIRE(epi != 2 || gout, "zsb_linear_tc_f32: upstream gradient missing");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int Kp = zsb_linear_tc_kpad(K);
-  const __half* wp = reinterpret_cast<const __half*>(w_planes);
-  const __half* hp = reinterpret_cast<const __half*>(h_planes);
-  CUtensorMap m_whi, m_wlo, m_hhi, m_hlo;
-  int rc;
-  if ((rc = make_map(&m_whi, wp, (uint64_t)J, (uint64_t)Kp, BM, 128, 1))) return rc;
-  if ((rc = make_map(&m_wlo, wp + (int64_t)J * Kp, (uint64_t)J, (uint64_t)Kp, BM, 128, 1)))
-    return rc;
-  if ((rc = make_map(&m_hhi, hp, (uint64_t)R, (uint64_t)Kp, BN, 128, 1))) return rc;
-  if ((rc = make_map(&m_hlo, hp + R * Kp, (uint64_t)R, (uint64_t)Kp, BN, 128, 1))) return rc;
-  const int n_blk = (J + BM - 1) / BM;
-  int k_slices = 1;
-  if (epi == 0 && part) {
-    k_slices = zsb_linear_tc_slices(R, J, K);
-    if (k_slices > 1 && relu) {
-      zsb_set_error("zsb_linear_tc_f32: ReLU cannot be fused into a split-K launch");
-      return ZSB_ERR_INVALID;
-    }
-  }
-  float* out_k = (k_slices > 1) ? part : out;
-  float* amax_k = k_slices > 1 ? nullptr : amax_scale;
-  if (epi == 0)
-    rc = launch_linear<0, 0, 0>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out_k, part,
-                                R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
-                                "linear_tc");
-  else if (epi == 1)
-    rc = launch_linear<1, 0, 0>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, nullptr,
-                                part, R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
-                                "linear_tc");
-  else if (!epi_gload())
-    rc = launch_linear<2, 0, 0>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out_k, part,
-                                R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
-                                "linear_tc");
-  else
-    rc = launch_linear<2, 0, 1>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out_k, part,
-                                R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
-                                "linear_tc");
-
-  if (rc == ZSB_OK && k_slices > 1) {
-    const int64_t n = R * (int64_t)J;
-    int64_t blocks = zsb_ceil_div(n, 256);
-    if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
-    slice_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, k_slices, n, out);
-    return zsb_check_launch("linear_tc_slice_sum");
-  }
-  if (rc != ZSB_OK || epi != 1) return rc;
-  int64_t blocks = zsb_ceil_div(R, 256);
-  if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
-  part_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, 4 * n_blk, R, out);
-  return zsb_check_launch("linear_tc_part_sum");
+  return linear_tc_amax<0>(epi, w_planes, scale_w, h_planes, scale_h, bias, x_obs, n_x, gout, out,
+                           part, R, J, K, relu, amax_scale, (cudaStream_t)stream);
+}
+// As zsb_linear_tc_amax_f32 for a 0/1 activation h whose planes are its hi plane only, at scale
+// 2048 (zsb_linear_tc_bern_sample_f32): two fp16 products per k-step instead of three, the same
+// result bit for bit.
+int zsb_linear_tc_bin_f32(int epi, const void* w_planes, const float* scale_w,
+                          const void* h_planes, const float* scale_h, const float* bias,
+                          const float* x_obs, int64_t n_x, const float* gout, float* out,
+                          float* part, int64_t R, int J, int K, int relu, float* amax_scale,
+                          void* stream) {
+  return linear_tc_amax<2>(epi, w_planes, scale_w, h_planes, scale_h, bias, x_obs, n_x, gout, out,
+                           part, R, J, K, relu, amax_scale, (cudaStream_t)stream);
 }
 
 // Backward of the Bernoulli likelihood layer with the operand split fused into the GEMM epilogue:
@@ -733,33 +943,98 @@ int zsb_linear_tc_dgrad_f32(const void* w_planes, const float* scale_w, const vo
 int zsb_linear_tc_wgrad_f32(const void* h_planes, const float* scale_h, int K,
                             const void* g_planes, const float* scale_g, int J, int64_t R,
                             float* out, float* part, void* stream) {
-  ZSB_REQUIRE(h_planes && g_planes && scale_h && scale_g && out && R > 0 && J > 0 && K > 0,
-              "zsb_linear_tc_wgrad_f32: bad args");
-  ZSB_REQUIRE(R < (1LL << 31) - 64, "zsb_linear_tc_wgrad_f32: too many rows");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int Kp_h = zsb_linear_tc_kpad(K), Jp_g = zsb_linear_tc_kpad(J);
-  const int Rp = zsb_linear_tc_kpad((int)R);                 // padded contraction length
-  const __half* hp = reinterpret_cast<const __half*>(h_planes);
-  const __half* gp = reinterpret_cast<const __half*>(g_planes);
-  CUtensorMap m_whi, m_wlo, m_hhi, m_hlo;                    // "w" = h (rows = k), "h" = g
-  int rc;
-  if ((rc = make_map(&m_whi, hp, (uint64_t)R, (uint64_t)Kp_h, 64, 128, 1))) return rc;
-  if ((rc = make_map(&m_wlo, hp + R * Kp_h, (uint64_t)R, (uint64_t)Kp_h, 64, 128, 1))) return rc;
-  if ((rc = make_map(&m_hhi, gp, (uint64_t)R, (uint64_t)Jp_g, 64, 128, 1))) return rc;
-  if ((rc = make_map(&m_hlo, gp + R * Jp_g, (uint64_t)R, (uint64_t)Jp_g, 64, 128, 1))) return rc;
-  const int k_slices = part ? zsb_linear_tc_slices(J, K, (int)R) : 1;
-  rc = launch_linear<0, 3, 0>(m_whi, m_wlo, m_hhi, m_hlo, nullptr, nullptr, 0, nullptr,
-                              k_slices > 1 ? part : out, part, (int64_t)J, K, Rp, 0, scale_h,
-                              scale_g, k_slices, nullptr, st, "linear_tc_wgrad");
+  return linear_tc_wgrad<0>(h_planes, scale_h, K, g_planes, scale_g, J, R, out, part,
+                            (cudaStream_t)stream);
+}
+// As zsb_linear_tc_wgrad_f32 for a 0/1 activation h whose planes are its hi plane only
+// (zsb_linear_tc_bern_sample_f32): two products per k-step, the same result bit for bit.
+int zsb_linear_tc_wgrad_bin_f32(const void* h_planes, const float* scale_h, int K,
+                                const void* g_planes, const float* scale_g, int J, int64_t R,
+                                float* out, float* part, void* stream) {
+  return linear_tc_wgrad<1>(h_planes, scale_h, K, g_planes, scale_g, J, R, out, part,
+                            (cudaStream_t)stream);
+}
 
-  if (rc == ZSB_OK && k_slices > 1) {
-    const int64_t n = (int64_t)J * K;
-    int64_t blocks = zsb_ceil_div(n, 256);
-    if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
-    slice_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, k_slices, n, out);
-    return zsb_check_launch("linear_tc_wgrad_slice_sum");
-  }
-  return rc;
+// Bernoulli layer with S draws per logit row, l = h W^T + bias never leaving the epilogue (EPI 4):
+//   h_out [S R, J] = (u < sigmoid(l[r])), float (h_int = 0) or int32; u = u_in [S R J] or the
+//                    Philox draw of zsb_sample_bernoulli_i32 for (seed, iter) at element (s R + r) J + j
+//   h_planes_out [S R][kpad(J)] fp16 = h * 2048, zero padding: the operand of the next layer
+//   logq [S R] = sum_j Bernoulli(l[r]).log_prob(h[s R + r]);  part = nparts(J) * S R floats
+// h_binary: h_planes is itself such a sample plane (one plane, lo plane zero).
+int zsb_linear_tc_bern_sample_f32(const void* w_planes, const float* scale_w, const void* h_planes,
+                                  const float* scale_h, int h_binary, const float* bias,
+                                  const float* u_in, uint64_t seed, uint32_t iter, int S,
+                                  void* h_out, int h_int, void* h_planes_out, float* logq,
+                                  float* part, int64_t R, int J, int K, void* stream) {
+  ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && h_out && h_planes_out && logq &&
+                  part && R > 0 && J > 0 && K > 0 && S >= 1,
+              "zsb_linear_tc_bern_sample_f32: bad args");
+  ZSB_REQUIRE((int64_t)S * R < (1LL << 31), "zsb_linear_tc_bern_sample_f32: too many rows");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Kp = zsb_linear_tc_kpad(K);
+  CUtensorMap m[4];
+  int rc;
+  if ((rc = linear_maps(w_planes, h_planes, h_binary, R, J, Kp, m))) return rc;
+  auto fill = [&](auto w) {
+    w.S = S; w.u_in = u_in; w.seed = seed; w.iter = iter; w.epoch = zsb_epoch_ptr();
+    w.h_int = h_int; w.pl_out = reinterpret_cast<__half*>(h_planes_out);
+    return tc_launch(chunk_samples(w), st, "linear_tc_bern_sample");
+  };
+  float* ho = reinterpret_cast<float*>(h_out);
+  if (h_binary)
+    rc = fill(make_linw<4, 0, 0, 2>(m[0], m[1], m[2], m[3], bias, nullptr, 0, nullptr, ho, part, R,
+                                    J, Kp, 0, scale_w, scale_h, 1, nullptr));
+  else
+    rc = fill(make_linw<4, 0, 0, 0>(m[0], m[1], m[2], m[3], bias, nullptr, 0, nullptr, ho, part, R,
+                                    J, Kp, 0, scale_w, scale_h, 1, nullptr));
+  if (rc != ZSB_OK) return rc;
+  const int64_t SR = (int64_t)S * R;
+  int64_t blocks = zsb_ceil_div(SR, 256);
+  if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
+  part_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, 4 * ((J + BM - 1) / BM), SR, logq);
+  return zsb_check_launch("linear_tc_bern_sample_part_sum");
+}
+
+// Bernoulli layer against S given rows per logit row, l[r] = (h W^T + bias)[r]:
+//   epi 1: out [S R] = sum_j Bernoulli(l[r]).log_prob(given[s R + r, j]); part = nparts(J) * S R
+//   epi 2: out [R, J] = sum_s gout[s R + r] * (given[s R + r, j] - sigmoid(l[r, j])), the gradient
+//          of sum gout * (epi 1) wrt the logits; max |out| folded into amax_scale[2] (may be NULL)
+// h_binary as in zsb_linear_tc_bern_sample_f32.
+int zsb_linear_tc_bern_given_f32(int epi, const void* w_planes, const float* scale_w,
+                                 const void* h_planes, const float* scale_h, int h_binary,
+                                 const float* bias, const float* given, int S, const float* gout,
+                                 float* out, float* part, int64_t R, int J, int K,
+                                 float* amax_scale, void* stream) {
+  ZSB_REQUIRE(epi == 1 || epi == 2, "zsb_linear_tc_bern_given_f32: epi must be 1 or 2");
+  ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && given && out && R > 0 && J > 0 &&
+                  K > 0 && S >= 1 && (epi != 1 || part) && (epi != 2 || gout),
+              "zsb_linear_tc_bern_given_f32: bad args");
+  ZSB_REQUIRE((int64_t)S * R < (1LL << 31), "zsb_linear_tc_bern_given_f32: too many rows");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Kp = zsb_linear_tc_kpad(K);
+  CUtensorMap m[4];
+  int rc;
+  if ((rc = linear_maps(w_planes, h_planes, h_binary, R, J, Kp, m))) return rc;
+  auto fill = [&](auto w) {
+    w.S = S;
+    w.s_per = S;                          // EPI 6 sums over the draws: one chunk
+    return tc_launch(epi == 1 ? chunk_samples(w) : w, st, "linear_tc_bern_given");
+  };
+#define ZSB_GIVEN(E, Z)                                                                       \
+  fill(make_linw<E, 0, 0, Z>(m[0], m[1], m[2], m[3], bias, given, (int64_t)S * R, gout,       \
+                             epi == 2 ? out : nullptr, part, R, J, Kp, 0, scale_w, scale_h, 1, \
+                             epi == 2 ? amax_scale : nullptr))
+  if (epi == 1)
+    rc = h_binary ? ZSB_GIVEN(5, 2) : ZSB_GIVEN(5, 0);
+  else
+    rc = h_binary ? ZSB_GIVEN(6, 2) : ZSB_GIVEN(6, 0);
+#undef ZSB_GIVEN
+  if (rc != ZSB_OK || epi != 1) return rc;
+  const int64_t SR = (int64_t)S * R;
+  int64_t blocks = zsb_ceil_div(SR, 256);
+  if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
+  part_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, 4 * ((J + BM - 1) / BM), SR, out);
+  return zsb_check_launch("linear_tc_bern_given_part_sum");
 }
 
 }  // extern "C"

@@ -198,7 +198,10 @@ __device__ __forceinline__ float warp_transpose_sum16(float v[16], int lane) {
 
 // One k-block (RB bytes of contraction per operand row) of the three split products for both
 // 64-row halves of the tile.  KIND 0: TF32 operands, 1: fp16.  MNA / MNB: operand read MN-major.
-template <int KIND, int RB, int MNA, int MNB>
+// ZLO (fp16 only): bit 0 / bit 1 = the lo plane of operand A / B is identically zero (a 0/1
+// sample at an exact scale), so its product is skipped: two wgmma per half instead of three.  The
+// skipped product adds exact zeros, so the result is bit-identical to the three-product order.
+template <int KIND, int RB, int MNA, int MNB, int ZLO = 0>
 __device__ __forceinline__ void mma_kblock(float (&d)[2][64], uint32_t sa) {
   using C = Cfg<RB>;
 #pragma unroll
@@ -218,8 +221,8 @@ __device__ __forceinline__ void mma_kblock(float (&d)[2][64], uint32_t sa) {
         wgmma_tf32(d[mh], a_hi, b_lo);
         wgmma_tf32(d[mh], a_hi, b_hi);
       } else {
-        wgmma_f16<MNA, MNB>(d[mh], a_lo, b_hi);
-        wgmma_f16<MNA, MNB>(d[mh], a_hi, b_lo);
+        if (!(ZLO & 1)) wgmma_f16<MNA, MNB>(d[mh], a_lo, b_hi);
+        if (!(ZLO & 2)) wgmma_f16<MNA, MNB>(d[mh], a_hi, b_lo);
         wgmma_f16<MNA, MNB>(d[mh], a_hi, b_hi);
       }
     }
@@ -241,6 +244,17 @@ struct ClusterOf {
 template <class W>
 struct ClusterOf<W, decltype((void)W::CLUSTER)> {
   static constexpr int value = W::CLUSTER;
+};
+
+// ZLO (optional, default 0)      operands whose lo plane is zero (mma_kblock); W::load then
+//                                 skips those planes and W::TX counts only what it loads
+template <class W, class = void>
+struct ZloOf {
+  static constexpr int value = 0;
+};
+template <class W>
+struct ZloOf<W, decltype((void)W::ZLO)> {
+  static constexpr int value = W::ZLO;
 };
 
 template <class W>
@@ -309,7 +323,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
           asm volatile("bar.sync 1, 128;" ::: "memory");
         }
         wgmma_fence();
-        mma_kblock<W::KIND, W::RB, W::MNA, W::MNB>(d, sa);
+        mma_kblock<W::KIND, W::RB, W::MNA, W::MNB, ZloOf<W>::value>(d, sa);
         wgmma_commit();
         wgmma_wait<1>();                                  // the previous stage has been read
         if (prev >= 0 && tid == 0) release(prev);

@@ -89,7 +89,6 @@ int launch_uni(float* out, int64_t n_out, int64_t group, Ops3 ops, F f, cudaStre
 __device__ __forceinline__ float softplusf_(float t) {       // tf.nn.softplus
   return fmaxf(t, 0.f) + log1pf(expf(-fabsf(t)));
 }
-__device__ __forceinline__ float sigmoidf_(float t) { return 1.f / (1.f + expf(-t)); }
 // psi(x) for x > 0: recurrence up to x >= 6, then the asymptotic series
 __device__ __forceinline__ float digammaf_(float x) {
   float r = 0.f;

@@ -667,11 +667,15 @@ def _tc_split_t(t2d):
 class _Planes(object):
     """fp16 hi/lo operand planes of one [rows, K] matrix times a power-of-two scale: row-major
     ``planes`` [2, rows, Kp] (all three products of a layer) and, only with ZSB_WGRAD_T=1, transposed ``planes_t``
-    [2, K, Rp] (weight-gradient product, contraction over the rows); ``scale`` = device float[4]."""
-    __slots__ = ("planes", "planes_t", "scale", "rows", "K")
+    [2, K, Rp] (weight-gradient product, contraction over the rows); ``scale`` = device float[4].
+    ``binary``: a 0/1 sample of LinearBernoulli.sample -- ``planes`` [1, rows, Kp] is the hi plane
+    only (the lo plane is identically zero), read by the two-product kernels; valid while the
+    sample's ``_version`` is ``version``."""
+    __slots__ = ("planes", "planes_t", "scale", "rows", "K", "binary", "version")
 
-    def __init__(self, planes, planes_t, scale, rows, K):
+    def __init__(self, planes, planes_t, scale, rows, K, binary=False, version=None):
         self.planes, self.planes_t, self.scale, self.rows, self.K = planes, planes_t, scale, rows, K
+        self.binary, self.version = binary, version
 
 
 def _tc_split_dual(t2d, mask=None, want=(True, True), amax=None, col_sum=None):
@@ -708,7 +712,8 @@ def _planes_of(h2, src, need_t):
     R, K = int(h2.shape[0]), int(h2.shape[1])
     pl = getattr(src, "_zsb_pl", None)
     if (pl is not None and pl.rows == R and pl.K == K and pl.planes is not None
-            and (not need_t or pl.planes_t is not None)):
+            and (not need_t or pl.planes_t is not None)
+            and (not pl.binary or (pl.version is not None and pl.version == _version(src)))):
         return pl
     amax = getattr(src, "_zsb_amax", None)
     pl = _tc_split_dual(h2, want=(True, need_t), amax=None if K % 2 else amax)
@@ -768,13 +773,15 @@ def _tc_grad_weight(gpl, hpl, R):
     slices = lib.load().zsb_linear_tc_slices(J, K, R)
     part = torch.empty(slices * J * K, dtype=torch.float32, device=dev) if slices > 1 else None
     out = torch.empty((J, K), dtype=torch.float32, device=dev)
-    lib.call("zsb_linear_tc_wgrad_f32", ptr(hpl.planes), ptr(hpl.scale), K, ptr(gpl.planes),
-             ptr(gpl.scale), J, R, ptr(out), ptr(part), stream())
+    lib.call("zsb_linear_tc_wgrad_bin_f32" if hpl.binary else "zsb_linear_tc_wgrad_f32",
+             ptr(hpl.planes), ptr(hpl.scale), K, ptr(gpl.planes), ptr(gpl.scale), J, R, ptr(out),
+             ptr(part), stream())
     return out
 
 
 def _tc_linear(epi, wp, ws, hp, hs, bias, x, gout, R, J, K, relu=False,
-               split_k=False, amax=None):
+               split_k=False, amax=None, binary=False):
+    """One product on the wgmma kernel; ``binary``: ``hp`` is the one plane of a 0/1 sample."""
     from ._lib import lib, ptr, stream
     dev = hp.device
     part = None
@@ -788,7 +795,8 @@ def _tc_linear(epi, wp, ws, hp, hs, bias, x, gout, R, J, K, relu=False,
                            dtype=torch.float32, device=dev)
     else:
         out = torch.empty((R, J), dtype=torch.float32, device=dev)
-    lib.call("zsb_linear_tc_amax_f32", epi, ptr(wp), ptr(ws), ptr(hp), ptr(hs),
+    lib.call("zsb_linear_tc_bin_f32" if binary else "zsb_linear_tc_amax_f32", epi, ptr(wp),
+             ptr(ws), ptr(hp), ptr(hs),
              ptr(bias), ptr(x), int(x.shape[0]) if x is not None else 0,
              ptr(gout), ptr(out), ptr(part), R, J, K, int(bool(relu)), ptr(amax), stream())
     return out
@@ -820,7 +828,7 @@ class _Linear(torch.autograd.Function):
         bias = b.detach().to(torch.float32).contiguous() if b is not None else None
         amax = torch.zeros(4, dtype=torch.float32, device=h2.device)
         y = _tc_linear(0, wp, ws, hpl.planes, hpl.scale, bias, None, None, R, J, K, relu,
-                       amax=amax)
+                       amax=amax, binary=hpl.binary)
         ctx.save_for_backward(W, y if relu else None)
         ctx.hpl = hpl
         ctx.wpl = (wp, ws)
@@ -872,7 +880,8 @@ class _LinearBernoulliLogProb(torch.autograd.Function):
         wp, ws = _tc_split(W)
         hpl = _planes_of(h2, h, bool(ctx.needs_input_grad[1]) and _WGRAD_T)
         bias = b.detach().to(torch.float32).contiguous() if b is not None else None
-        lp = _tc_linear(1, wp, ws, hpl.planes, hpl.scale, bias, x2, None, R, J, K)
+        lp = _tc_linear(1, wp, ws, hpl.planes, hpl.scale, bias, x2, None, R, J, K,
+                        binary=hpl.binary)
         ctx.save_for_backward(W, bias, x2, wp, ws)
         ctx.hpl = hpl
         ctx.meta = (lead, R, J, K, b is not None)
@@ -887,9 +896,10 @@ class _LinearBernoulliLogProb(torch.autograd.Function):
         g = glp.reshape(-1).to(torch.float32).contiguous()
         db = torch.zeros(J, dtype=torch.float32, device=g.device) \
             if (has_b and need[2]) else None
-        if _WGRAD_T or _BERN_UNFUSED:        # round-2 scheme: fp32 dl, then one split pass
+        if _WGRAD_T or _BERN_UNFUSED or hpl.binary:   # fp32 dl, then one split pass
             amax = torch.zeros(4, dtype=torch.float32, device=g.device)
-            dl = _tc_linear(2, wp, ws, hpl.planes, hpl.scale, bias, x2, g, R, J, K, amax=amax)
+            dl = _tc_linear(2, wp, ws, hpl.planes, hpl.scale, bias, x2, g, R, J, K, amax=amax,
+                            binary=hpl.binary)
             dlpl = _tc_split_dual(dl, want=(bool(need[0]) or (bool(need[1]) and not _WGRAD_T),
                                             bool(need[1]) and _WGRAD_T), amax=amax, col_sum=db)
         else:                                # dl leaves the GEMM epilogue as operand planes
@@ -918,11 +928,101 @@ def linear_bernoulli_log_prob(h, W, b, x):
     return _LinearBernoulliLogProb.apply(h, W, b, x)
 
 
+_BIN_SCALES = {}
+
+
+def _bin_scale(device):
+    """The scale slot of a sample's binary plane: 2048, the power of two the split of a 0/1
+    matrix picks (zsb_linear_tc_bern_sample_f32).  One read-only tensor per device."""
+    t = _BIN_SCALES.get(device)
+    if t is None:
+        t = torch.tensor([2048.0, 0.0, 0.0, 0.0], dtype=torch.float32, device=device)
+        _BIN_SCALES[device] = t
+    return t
+
+
+class _LinearBernoulliGiven(torch.autograd.Function):
+    """log Bernoulli(logits = h W^T + b).log_prob(x[s]) summed over the features, [S, *lead], for
+    S given rows per logit row (x2 = [S * rows, J]), differentiable w.r.t. h, W and b.  Forward:
+    the epi-1 launch with S given rows, or -- for the layer's own sample -- the log q its sampling
+    launch already wrote (``lq``).  Backward: d/dlogits summed over the S draws, so the input and
+    weight gradients stay products over the rows of h (nothing is expanded S-fold)."""
+
+    @staticmethod
+    def forward(ctx, h, W, b, x2, S, lq, wp, ws, hpl):
+        from ._lib import lib, ptr, stream
+        lead = h.shape[:-1]
+        R, K, J = hpl.rows, hpl.K, int(W.shape[0])
+        if _WGRAD_T and ctx.needs_input_grad[1] and hpl.planes_t is None:
+            hpl = _planes_of(h.reshape(R, K), h, True)
+        bias = b.detach().to(torch.float32).contiguous() if b is not None else None
+        if lq is None:
+            lq = torch.empty(S * R, dtype=torch.float32, device=x2.device)
+            part = torch.empty(lib.load().zsb_linear_tc_nparts(J) * S * R, dtype=torch.float32,
+                               device=x2.device)
+            lib.call("zsb_linear_tc_bern_given_f32", 1, ptr(wp), ptr(ws), ptr(hpl.planes),
+                     ptr(hpl.scale), int(hpl.binary), ptr(bias), ptr(x2), S, None, ptr(lq),
+                     ptr(part), R, J, K, None, stream())
+        else:
+            lq = lq.clone()
+        ctx.save_for_backward(W, bias, x2, wp, ws)
+        ctx.hpl = hpl
+        ctx.meta = (lead, S, R, J, K, b is not None)
+        return lq.reshape((S,) + tuple(lead))
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, glq):
+        from ._lib import lib, ptr, stream
+        W, bias, x2, wp, ws = ctx.saved_tensors
+        lead, S, R, J, K, has_b = ctx.meta
+        hpl = ctx.hpl
+        need = ctx.needs_input_grad
+        g = glq.reshape(-1).to(torch.float32).contiguous()
+        db = torch.zeros(J, dtype=torch.float32, device=g.device) if (has_b and need[2]) else None
+        amax = torch.zeros(4, dtype=torch.float32, device=g.device)
+        dl = torch.empty((R, J), dtype=torch.float32, device=g.device)
+        lib.call("zsb_linear_tc_bern_given_f32", 2, ptr(wp), ptr(ws), ptr(hpl.planes),
+                 ptr(hpl.scale), int(hpl.binary), ptr(bias), ptr(x2), S, ptr(g), ptr(dl), None,
+                 R, J, K, ptr(amax), stream())
+        dlpl = _tc_split_dual(dl, want=(bool(need[0]) or (bool(need[1]) and not _WGRAD_T),
+                                        bool(need[1]) and _WGRAD_T), amax=amax, col_sum=db)
+        dh = None
+        if need[0]:
+            dh2, a2 = _tc_grad_input(dlpl, W, R, wp, ws)
+            dh = _tag(dh2.reshape(tuple(lead) + (K,)), a2)
+        dW = _tc_grad_weight(dlpl, hpl, R) if need[1] else None
+        ctx.hpl = None
+        return dh, dW, db, None, None, None, None, None, None
+
+
+def _version(t):
+    """The in-place version counter of ``t``; None for an inference tensor, which has none (it is
+    then never trusted as an unchanged cache key)."""
+    try:
+        return t._version
+    except RuntimeError:
+        return None
+
+
+def _versions(*ts):
+    return tuple(None if t is None else _version(t) for t in ts)
+
+
 class LinearBernoulli(object):
     """Drop-in for ``Bernoulli(logits=dense(h), group_ndims=1)`` as a
     distribution plugin (duck-typed contract of bn.py:96-115): ``log_prob`` runs
-    the fused GEMM + Bernoulli epilogue; the logits are only materialised when
-    the node is *sampled* rather than observed."""
+    the fused GEMM + Bernoulli epilogue; the logits never reach memory.
+
+    ``sample(n_samples)`` is one launch (zsb_linear_tc_bern_sample_f32) that draws the sample --
+    element for element what ``Bernoulli(linear(h, W, b)).sample(n_samples)`` draws from the same
+    ``zs.random`` state -- together with its log-probability and its operand plane for the next
+    layer.  ``log_prob`` of that very sample returns the stored log-probability (no second GEMM),
+    differentiable w.r.t. h, W and b.  A sample fed to ``linear`` or to another ``LinearBernoulli``
+    (the sigmoid belief nets of examples/sigmoid_belief_nets, where every activation is a 0/1
+    sample) is multiplied on the two-product mainloop: same result bit for bit, a third fewer
+    tensor-core products and operand bytes.  ``given`` with leading sample axes beyond the rows of
+    ``h`` ([S, *h.shape[:-1], J]) is scored against the shared logits without expanding them."""
 
     def __init__(self, h, W, b=None, dtype=torch.int32, group_ndims=1):
         if group_ndims != 1:
@@ -948,13 +1048,73 @@ class LinearBernoulli(object):
     batch_shape = property(lambda self: self.get_batch_shape())
     value_shape = property(lambda self: self.get_value_shape())
 
-    def sample(self, n_samples=None):
-        from .distributions import Bernoulli
-        return Bernoulli(self.logits, dtype=self.dtype).sample(n_samples)
+    def sample(self, n_samples=None, u=None):
+        """``n_samples`` as in ``Bernoulli.sample``; ``u``: injected uniforms that broadcast to the
+        sample's shape (``Bernoulli._sample(n, u=...)``), else the Philox stream of
+        ``zs.random``."""
+        from . import random as zrandom
+        from ._lib import lib, ptr, stream
+        if isinstance(n_samples, torch.Tensor):
+            n_samples = int(n_samples.item())
+        S = 1 if n_samples is None else int(n_samples)
+        h, W, b = self._h, self._W, self._b
+        lead = tuple(h.shape[:-1])
+        J, K = int(W.shape[0]), int(h.shape[-1])
+        h2 = h.reshape(-1, K)
+        R = int(h2.shape[0])
+        dev = W.device
+        hpl = _planes_of(h2, h, False)
+        wp, ws = _tc_split(W)
+        bias = b.detach().to(torch.float32).contiguous() if b is not None else None
+        seed, it = zrandom.get_seed(), zrandom.next_counter()
+        full = (S,) + lead + (J,)
+        h_int = self.dtype == torch.int32
+        hs = torch.empty(full, dtype=torch.int32 if h_int else torch.float32, device=dev)
+        planes = torch.empty((1, S * R, lib.load().zsb_linear_tc_kpad(J)), dtype=torch.float16,
+                             device=dev)
+        lq = torch.empty(S * R, dtype=torch.float32, device=dev)
+        part = torch.empty(lib.load().zsb_linear_tc_nparts(J) * S * R, dtype=torch.float32,
+                           device=dev)
+        uu = None if u is None else u.to(torch.float32).expand(full).contiguous()
+        lib.call("zsb_linear_tc_bern_sample_f32", ptr(wp), ptr(ws), ptr(hpl.planes),
+                 ptr(hpl.scale), int(hpl.binary), ptr(bias), ptr(uu), int(seed), int(it), S,
+                 ptr(hs), int(h_int), ptr(planes), ptr(lq), ptr(part), R, J, K, stream())
+        if self.dtype not in (torch.int32, torch.float32):
+            hs = hs.to(self.dtype)
+        if n_samples is None:
+            hs = hs.squeeze(0)
+        vs = _versions(hs, h, W, b)
+        if all(v is not None for t, v in zip((hs, h, W, b), vs) if t is not None):
+            # (inference tensors of torch.inference_mode() have no version: nothing is cached)
+            hs._zsb_pl = _Planes(planes, None, _bin_scale(dev), S * R, J, binary=True,
+                                 version=vs[0])
+            self._own = (hs, lq, S, wp, ws, hpl, vs)
+        else:
+            self._own = None
+        return hs
 
     def log_prob(self, given):
         J = int(self._W.shape[0])
         lead = tuple(self._h.shape[:-1])
+        own = getattr(self, "_own", None)
+        if own is not None and given is own[0] and \
+                own[6] == _versions(given, self._h, self._W, self._b):
+            hs, lq, S, wp, ws, hpl, _ = own
+            x2 = hs.reshape(-1, J).to(torch.float32).contiguous()
+            return _LinearBernoulliGiven.apply(self._h, self._W, self._b, x2, S, lq, wp, ws, hpl)\
+                .reshape(tuple(given.shape[:-1]))
+        nd = len(lead) + 1
+        if given.dim() > nd and tuple(given.shape[-nd:]) == lead + (J,):
+            # leading sample axes beyond the rows of h: [S, *lead, J] against the [*lead, J] logits
+            S = 1
+            for d in given.shape[:-nd]:
+                S *= int(d)
+            h2 = self._h.reshape(-1, int(self._h.shape[-1]))
+            hpl = _planes_of(h2, self._h, False)
+            wp, ws = _tc_split(self._W)
+            x2 = given.reshape(-1, J).to(torch.float32).contiguous()
+            return _LinearBernoulliGiven.apply(self._h, self._W, self._b, x2, S, None, wp, ws,
+                                               hpl).reshape(tuple(given.shape[:-1]))
         g = given.reshape(-1, J)
         n_x = int(g.shape[0])
         rows = 1
