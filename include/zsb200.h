@@ -336,23 +336,12 @@ int zsb_hmc_dense_leapfrog_f32(const float* q_cur, const float* q_cur_lo, float*
                                const float* mu, const float* mass, const float* state,
                                float p_scale, float* lp_part, float* k_part, int64_t chains,
                                int64_t D, int impl, void* stream);
-int zsb_hmc_dense_tc_config(int bk);   /* impl-1 pipeline shape: 32 (2x64 KB) or 16 (4x32 KB) */
 int zsb_hmc_dense_split_lo_f32(const float* q, float* lo, int64_t n, void* stream);
 /* impl 2: fp16-split tensor-core path (3 fp16 wgmma products per k-step at twice the TF32 rate).
- * P_h16/P_l16: [D,D] __half hi/lo of P*sP; q_*_planes: [2][chains][D] __half hi/lo of q*sq;
- * scales: device float[4] = {sq, 1/(sP*sq), scratch, sP}: one sq for every pass, so the planes
- * overflow once |q| grows ~16x past the max|q| prepare saw.  D % 64 == 0. */
-int zsb_hmc_dense_h16_prepare_f32(const float* q, void* planes, float* scales, int64_t n,
-                                  void* stream);
-int zsb_hmc_dense_leapfrog_h16_f32(const float* q_cur, const void* q_cur_planes, float* q_next,
-                                   void* q_next_planes, const float* p_in, float* p_out,
-                                   const void* P_h16, const void* P_l16, const float* scales,
-                                   const float* bvec, const float* mu, const float* mass,
-                                   const float* state, float p_scale, float* lp_part,
-                                   float* k_part, int64_t chains, int64_t D, void* stream);
-/* Trajectory form of impl 2 (what the sampler runs), whose plane scale follows the chains.
- * scales: device float[8 + 4*(L+2)] for trajectories of up to L+1 passes; the caller sets
- * [3] = sP, [4] = ||P||_inf (max row sum of |P|), [5] = max|b| once.  Record i at [8 + 4*i] =
+ * P_h16/P_l16: [D,D] __half hi/lo of P*sP; q_*_planes: [2][chains][D] __half hi/lo of q*sq_i,
+ * where the plane scale sq_i follows the chains through the trajectory.  scales: device
+ * float[8 + 4*(L+2)] for trajectories of up to L+1 passes; the caller sets [3] = sP,
+ * [4] = ||P||_inf (max row sum of |P|), [5] = max|b| once.  Record i at [8 + 4*i] =
  * {sq_i, sq_alt_i, max|q_i| bound, flag} describes the planes pass i reads.  traj_prepare (after
  * the momentum is drawn, p = p0; before every trajectory) writes record 0 and q's planes at sq_0
  * (max|q| * sq_0 in [2^11, 2^12)); pass `pass_index` (from 0) writes q_next's planes at sq_i, or
@@ -367,27 +356,6 @@ int zsb_hmc_dense_leapfrog_h16_pass_f32(const float* q_cur, const void* q_cur_pl
                                         const float* mu, const float* mass, const float* state,
                                         float p_scale, float* lp_part, float* k_part,
                                         int64_t chains, int64_t D, void* stream);
-/* impl 3: impl 2 with the fp16 planes of q produced inside the kernel (by the MMA warpgroup from
- * the fp32 rows): HBM traffic per pass = the algorithmic 16*D bytes per chain.  scales: device
- * float[8], [3] = sP, [4..6] rotating max|q| slots; prepare before pass 0 of each trajectory. */
-int zsb_hmc_dense_h16i_prepare_f32(const float* q, float* scales, int64_t n, void* stream);
-int zsb_hmc_dense_leapfrog_h16i_f32(const float* q_cur, float* q_next, const float* p_in,
-                                    float* p_out, const void* P_h16, const void* P_l16,
-                                    float* scales, int pass_index, const float* bvec,
-                                    const float* mu, const float* mass, const float* state,
-                                    float p_scale, float* lp_part, float* k_part, int64_t chains,
-                                    int64_t D, void* stream);
-/* impl 4: the whole leapfrog `while_loop` of hmc.py:347-372 (L+1 passes) through one entry point
- * with impl 2's buffers and ping-pong schedule.  D == 1024, L >= 1.
- * Buffers and scales as impl 2's trajectory form (planes0 from zsb_hmc_dense_traj_prepare_f32);
- * the proposal ends in qa when L - 1 is even, else in qb; pw holds the final momentum. */
-int zsb_hmc_dense_trajectory_h16_f32(const float* q0, const void* planes0, float* qa,
-                                     void* planes_a, float* qb, void* planes_b, const float* p0,
-                                     float* pw, const void* P_h16, const void* P_l16,
-                                     float* scales, const float* bvec, const float* mu,
-                                     const float* mass, const float* state, float* lp0_part,
-                                     float* lp1_part, float* k_part, int64_t chains, int64_t D,
-                                     int n_leapfrogs, void* stream);
 /* impl 5: the whole leapfrog `while_loop` of hmc.py:347-372 (L+1 passes, body = leapfrog_integrator
  * hmc.py:38-43, plus the log p / kinetic terms of hamiltonian() hmc.py:30-35) with the fp16 hi/lo
  * plane pair of q*sq_i as the state of q inside the trajectory (planes0 from
@@ -397,20 +365,13 @@ int zsb_hmc_dense_trajectory_h16_f32(const float* q0, const void* planes0, float
  * did overflow; trajectories whose planes fit are unchanged by the bound.  The proposal's planes
  * end in buffer (n_leapfrogs & 1) or its spare, and zsb_hmc_dense_select_traj_planes_f32, given
  * both and &scales[8 + 4*n_leapfrogs], assigns them to the accepted chains (the `tf.where` +
- * assign of hmc.py:488-497).  `flags` (zsb_hmc_dense_resident_flags(chains) int32 words) is
- * reserved scratch.  D % 64 == 0, n_leapfrogs >= 1. */
-int zsb_hmc_dense_resident_flags(int64_t chains);
-int zsb_hmc_dense_resident_group(int64_t D);
+ * assign of hmc.py:488-497).  D % 64 == 0, n_leapfrogs >= 1. */
 int zsb_hmc_dense_resident_h16_f32(void* planes0, void* planes1, void* spare0, void* spare1,
                                    const float* p0, float* pw, const void* P_h16,
                                    const void* P_l16, float* scales, const float* bvec,
                                    const float* mu, const float* mass, const float* state,
                                    float* lp0_part, float* lp1_part, float* k_part,
-                                   int32_t* flags, int64_t chains, int64_t D, int n_leapfrogs,
-                                   void* stream);
-int zsb_hmc_dense_select_planes_f32(float* q, const void* planes, const float* scales,
-                                    const int32_t* accept, int64_t chains, int64_t D,
-                                    void* stream);
+                                   int64_t chains, int64_t D, int n_leapfrogs, void* stream);
 int zsb_hmc_dense_select_traj_planes_f32(float* q, const void* planes, const void* spare,
                                          const float* record, const int32_t* accept,
                                          int64_t chains, int64_t D, void* stream);

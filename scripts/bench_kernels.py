@@ -66,11 +66,12 @@ def main():
     part = torch.empty(lib.load().zsb_hmc_mass_parts() * 2 * D, device=dev); st2 = torch.empty(2 * D, device=dev); mean = torch.zeros(D, device=dev)
     ms = timeit(lambda: lib.call("zsb_hmc_mass_stats_f32", ptr(q), ptr(mean), C, D, ptr(part), ptr(st2), s))
     report("hmc_mass_stats", 4 * n, ms)
-    lo = torch.empty(2, C, D, dtype=torch.float16, device=dev); sc = torch.zeros(4, device=dev); sc[3] = 1.0
-    ms = timeit(lambda: lib.call("zsb_hmc_dense_h16_prepare_f32", ptr(q), ptr(lo), ptr(sc), n, s))
-    report("dense_h16_prepare (absmax+split)", 12 * n, ms, "read q twice, write 2 fp16 planes")
-    ms = timeit(lambda: lib.call("zsb_hmc_dense_select_planes_f32", ptr(q), ptr(lo), ptr(sc), ptr(acc), C, D, s))
-    report("dense_select_planes", 8 * n, ms, "all accepted: read 2 fp16 planes, write q")
+    lo = torch.empty(2, C, D, dtype=torch.float16, device=dev); sc = torch.zeros(8 + 4 * 3, device=dev); sc[3] = 1.0
+    ms = timeit(lambda: lib.call("zsb_hmc_dense_traj_prepare_f32", ptr(q), ptr(p_), ptr(mass), ptr(lo), ptr(sc), C, D, s))
+    report("dense_traj_prepare (absmax+split)", 16 * n, ms, "read q twice and p, write 2 fp16 planes")
+    # record 0 has no overflow flag: the planes are read, never the spare
+    ms = timeit(lambda: lib.call("zsb_hmc_dense_select_traj_planes_f32", ptr(q), ptr(lo), ptr(lo), ptr(sc[8:]), ptr(acc), C, D, s))
+    report("dense_select_traj_planes", 8 * n, ms, "all accepted: read 2 fp16 planes, write q")
     # sgmcmc
     ms = timeit(lambda: lib.call("zsb_sgmcmc_sgld_f32", ptr(q), ptr(g), None, 1e-6, C, D, 1, 1, 0, s))
     report("sgmcmc_sgld (Philox)", 12 * n, ms)

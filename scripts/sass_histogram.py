@@ -47,7 +47,7 @@ for f, name in zip(hist, demangle):
 print()
 print("Full-opcode detail of the flagship kernel (the 49 middle passes of a dense_impl 5 trajectory):")
 for f, name in zip(hist, demangle):
-    if "tc_pipeline_kernel<(anonymous namespace)::ResW<0, 1, 1024> >" in name:
+    if "tc_pipeline_kernel<(anonymous namespace)::ResW<0, 1, 1024, 2, 2> >" in name:
         c = hist[f]
         print("\n`%s`" % short(name))
         print(", ".join("%s x%d" % kv for kv in sorted(c.items(), key=lambda kv: -kv[1])

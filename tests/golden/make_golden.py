@@ -147,7 +147,7 @@ def make_sgmcmc():
 
 # ---------------------------------------------------------------------------
 # Large dense-Gaussian replays for the tensor-core kernels (impl 2 = fp16-split per-pass kernel,
-# impl 4 / 5 = trajectory-fused kernels): D = 64 and the benchmark's D = 1024, L = 50, step-size +
+# impl 5 = whole-trajectory entry point): D = 64 and the benchmark's D = 1024, L = 50, step-size +
 # mass adaptation, mass != 1 after `mass_collect_iters`, both step-size searches, iterations whose
 # trajectories diverge (non-finite -> acceptance 0, hmc.py:56-59) and healthy ones.
 #

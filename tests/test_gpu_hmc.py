@@ -294,7 +294,7 @@ def _dense_pass_reference(q, p, P, b, mu, mass, eps, scale):
     return pn, qn, lp, k
 
 
-@pytest.mark.parametrize("impl", [0, 1, 2, 3])
+@pytest.mark.parametrize("impl", [0, 1, 2])
 @pytest.mark.parametrize("C,D", [(300, 512), (24, 32), (129, 288), (1000, 1024),
                                  (130, 64), (515, 192)])
 def test_dense_single_pass_vs_float64(zs, impl, C, D):
@@ -323,23 +323,17 @@ def test_dense_single_pass_vs_float64(zs, impl, C, D):
     lpp = torch.zeros(nt * C, device="cuda"); kp = torch.zeros(nt * C, device="cuda")
     lp = torch.empty(C, device="cuda"); k = torch.empty(C, device="cuda")
     s = stream()
-    if impl == 3:   # planes built inside the kernel; scale from the max|q| slot
-        lj = zs.fused.GaussianLogJoint(P64, device="cuda")._zsb_fused
-        scales = torch.zeros(8, device="cuda"); scales[3] = lj["sP"]
-        lib.call("zsb_hmc_dense_h16i_prepare_f32", ptr(qt), ptr(scales), qt.numel(), s)
-        lib.call("zsb_hmc_dense_leapfrog_h16i_f32", ptr(qt), ptr(qn), ptr(pt), ptr(pn),
-                 ptr(lj["P_h16"]), ptr(lj["P_l16"]), ptr(scales), 0, ptr(bt), ptr(mut),
-                 ptr(mt), ptr(state), scale, ptr(lpp), ptr(kp), C, D, s)
-    elif impl == 2:
+    if impl == 2:   # pass 0 of a trajectory, plane-scale records laid out as HMC._plane_scales
         lj = zs.fused.GaussianLogJoint(P64, device="cuda")._zsb_fused
         planes = torch.empty(2, C, D, dtype=torch.float16, device="cuda")
         nplanes = torch.empty_like(planes)
-        scales = torch.zeros(4, device="cuda"); scales[3] = lj["sP"]
-        lib.call("zsb_hmc_dense_h16_prepare_f32", ptr(qt), ptr(planes),
-                 ptr(scales), qt.numel(), s)
-        lib.call("zsb_hmc_dense_leapfrog_h16_f32", ptr(qt), ptr(planes), ptr(qn),
+        scales = torch.zeros(8 + 4 * 3, device="cuda")
+        scales[3], scales[4], scales[5] = lj["sP"], lj["P_inf"], float(np.abs(b).max())
+        lib.call("zsb_hmc_dense_traj_prepare_f32", ptr(qt), ptr(pt), ptr(mt), ptr(planes),
+                 ptr(scales), C, D, s)
+        lib.call("zsb_hmc_dense_leapfrog_h16_pass_f32", ptr(qt), ptr(planes), ptr(qn),
                  ptr(nplanes), ptr(pt), ptr(pn), ptr(lj["P_h16"]),
-                 ptr(lj["P_l16"]), ptr(scales), ptr(bt), ptr(mut), ptr(mt),
+                 ptr(lj["P_l16"]), ptr(scales), 0, ptr(bt), ptr(mut), ptr(mt),
                  ptr(state), scale, ptr(lpp), ptr(kp), C, D, s)
     else:
         if impl == 1:
@@ -367,15 +361,13 @@ def test_dense_single_pass_vs_float64(zs, impl, C, D):
         qn32 = N(qn)
         res = qn32 - (qn32.view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
         np.testing.assert_array_equal(N(qnlo), res)
-    if impl == 3:   # slot 1 now holds max|q_next| for the next pass, slot 2 is clear
-        slots = scales.view(torch.int32)[4:7].cpu().numpy().view(np.float32)
-        assert slots[1] == np.abs(N(qn)).max() and slots[2] == 0
-    if impl == 2:   # the planes reconstruct q_next * sq to ~2^-22 relative
-        sq = float(scales[0])
+    if impl == 2:   # the planes reconstruct q_next * sq_1 to ~2^-22 relative
+        sq = float(scales[8 + 4])     # record 1: the scale of q_next's planes
         rec = (N(nplanes[0]).astype(np.float64) + N(nplanes[1]).astype(np.float64)) / sq
         np.testing.assert_allclose(rec, N(qn).astype(np.float64), rtol=1e-6,
                                    atol=1e-6 * np.abs(N(qn)).max())
-        assert 2 ** 11 <= np.abs(q).max() * sq < 2 ** 12
+        sq0 = float(scales[8])        # record 0: the scale of q's planes
+        assert 2 ** 11 <= np.abs(q).max() * sq0 < 2 ** 12
 
 
 def test_golden_dense_fused_tc(zs):
@@ -478,11 +470,12 @@ def test_golden_dense64_l50_adaptive(zs, impl):
     _replay_big(zs, "hmc_dense64", impl)
 
 
-@pytest.mark.parametrize("impl", [2, 4, 5])
+@pytest.mark.parametrize("impl", [2, 5])
 def test_golden_dense1024_l50_adaptive(zs, impl):
     """The benchmark configuration's shape (D = 1024, L = 50, step + mass adaptation) at 320
-    chains on the benchmarked kernels: impl 2 (fp16-split, one launch per pass) and impl 4 (the
-    trajectory-fused launch) vs the oracle -- accept decisions, Hamiltonians, step sizes, mass."""
+    chains on the benchmarked kernels: impl 2 (fp16-split, one launch per pass) and impl 5 (the
+    whole trajectory on the plane state) vs the oracle -- accept decisions, Hamiltonians, step
+    sizes, mass."""
     _replay_big(zs, "hmc_dense1024", impl)
 
 
@@ -553,7 +546,7 @@ def test_leapfrog_count_edges_all_paths(zs, L):
     u = rng.random_sample(C).astype(np.float32)
     om = OM.DenseGaussian(P.astype(np.float32), None, const)
     oq, oi = OH.HMC(step_size=0.15, n_leapfrogs=L).step([q0], om.logp, om.grad, [npz], u)
-    for impl in (0, 1, 2, 3, 5):
+    for impl in (0, 1, 2, 5):
         x = T(q0)
         h = zs.HMC(step_size=0.15, n_leapfrogs=L, dense_impl=impl)
         op, info = h.sample(zs.fused.GaussianLogJoint(P), {}, {"x": x})
@@ -637,13 +630,13 @@ def test_cuda_graph_replay_is_bitwise_eager(zs, path):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("impl", [4, 5])
+@pytest.mark.parametrize("impl", [5])
 @pytest.mark.parametrize("C,L", [(300, 3), (2048, 5), (8192, 2), (9472 + 256 + 40, 4)])
 def test_trajectory_kernels_match_per_pass_kernel(zs, impl, C, L):
-    """dense_impl=4 (clusters of 8, one launch per trajectory) and dense_impl=5 (L2-resident
-    groups, planes-only state, flag-synchronised passes; the last shape spans two groups and a
-    ragged block) against dense_impl=2 (one launch per pass): same operands and products, so the
-    chains must agree to fp32 rounding."""
+    """dense_impl=5 (the whole trajectory on the fp16 plane state, clusters of 2 x 2 CTAs where
+    the units tile by them; the last shape ends in a ragged chain block) against dense_impl=2
+    (fp32 q between passes): same operands and products, so the chains must agree to fp32
+    rounding."""
     D = 1024
     P, _ = OM.make_dense_gaussian_problem(D, seed=2)
     res = []

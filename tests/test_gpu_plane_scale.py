@@ -2,7 +2,7 @@
 started: chains initialised at zero or at a small scale, chains of very different magnitudes in
 one batch, and a step size beyond the leapfrog's stability limit.
 
-The fp16-split paths (dense_impl 2, 4, 5) hold q inside a trajectory as fp16 hi/lo planes of
+The fp16-split paths (dense_impl 2, 5) hold q inside a trajectory as fp16 hi/lo planes of
 q * sq with one power-of-two sq per pass for all chains.  These tests pin that the plane scale
 follows the trajectory: every path must give the decisions, Hamiltonians and positions of the
 float64 oracle, with the injected momentum and uniforms of test_gpu_hmc.py."""
@@ -72,8 +72,6 @@ def _run(zs, impl, P, const, q0, npz, u, eps, L):
     op.synchronize()
     if impl == 5 and L >= 1:
         assert h._res
-    if impl == 4:
-        assert h._traj
     return N(x), {k: N(getattr(info, k)) for k in
                   ("acceptance_rate", "orig_hamiltonian", "hamiltonian", "orig_log_prob",
                    "log_prob")}
@@ -133,7 +131,7 @@ def _case(D, init, wide, L, eps):
     return _ORACLE[key]
 
 
-_IMPL_D = [(i, 64) for i in (0, 1, 2, 3, 5)] + [(i, 1024) for i in (0, 1, 2, 3, 4, 5)]
+_IMPL_D = [(i, 64) for i in (0, 1, 2, 5)] + [(i, 1024) for i in (0, 1, 2, 5)]
 
 
 @pytest.mark.parametrize("L", [1, 10, 50])

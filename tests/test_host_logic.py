@@ -32,12 +32,21 @@ def test_library_exports_every_declared_symbol():
     defined = set(re.findall(r"^int (zsb_\w+)\(", src, flags=re.M))
     internal = {"zsb_check_launch", "zsb_dense_leapfrog_tc_launch",
                 "zsb_dense_tc_ntiles", "zsb_dense_split_lo_launch",
-                "zsb_dense_tc_set_bk", "zsb_dense_leapfrog_h16_launch",
-                "zsb_dense_h16_prepare_launch", "zsb_dense_leapfrog_h16i_launch",
-                "zsb_dense_h16i_prepare_launch", "zsb_dense_traj_h16_launch",
-                    "zsb_dense_res_group_blocks", "zsb_dense_res_h16_launch",
-                    "zsb_dense_select_planes_launch"}
+                "zsb_dense_leapfrog_h16_launch", "zsb_dense_h16_prepare_launch",
+                "zsb_dense_res_h16_launch", "zsb_dense_select_planes_launch"}
     assert defined - internal <= set(protos), defined - internal - set(protos)
+
+
+@pytest.mark.parametrize("impl", [3, 4, 6, -1])
+def test_dense_impl_outside_the_four_paths_is_rejected(impl):
+    """dense_impl / GaussianLogJoint(impl=) take None, 0, 1, 2 or 5; anything else raises before
+    any launch, so this runs on host tensors."""
+    P = np.eye(64)
+    x = torch.zeros(4, 64)
+    with pytest.raises(ValueError, match="dense_impl must be"):
+        zs.HMC(dense_impl=impl).sample(zs.fused.GaussianLogJoint(P, device="cpu"), {}, {"x": x})
+    with pytest.raises(ValueError, match="dense_impl must be"):
+        zs.HMC().sample(zs.fused.GaussianLogJoint(P, device="cpu", impl=impl), {}, {"x": x})
 
 
 def test_header_cites_reference_lines():

@@ -1,5 +1,5 @@
 """NumPy emulation (CPU) of the fp16 plane state of the dense-Gaussian trajectory (dense_impl 5,
-hmc_dense_res.cu; impl 2 / 4 write their planes the same way): inside a trajectory q exists only
+hmc_dense_res.cu; impl 2 writes its planes the same way): inside a trajectory q exists only
 as fp16 hi / lo planes of q * sq.  Each pass rebuilds Q = hi + lo, kicks p with g = b - P q,
 drifts Q by (eps / m) * sq * p and rounds the result into the next planes.
 
@@ -10,7 +10,7 @@ Two plane-scale rules:
               B_i = max|q_i| + drift_i + eps s2 max(1/m) (max|b| + ||P||_inf max|q_i|),
               drift_0 = eps max|p_0/m|,  drift_i = max|q_i| + max|q_{i-1}|  (i > 0),
             on |q_{i+1}| keeps B_i * sq_i below 2^16 - 2^8, else at the power of two placing B_i
-            in [2^11, 2^12) (hmc_dense_epilogue.cuh; dense_impl 2 / 4);
+            in [2^11, 2^12) (hmc_dense_epilogue.cuh; dense_impl 2);
   spare  -- (dense_impl 5) the planes are always written at sq_i; where the bound is reached a
             spare copy at the lowered scale is written too, and the next pass reads it only if
             some |q_{i+1}| * sq_i reached fp16's overflow."""

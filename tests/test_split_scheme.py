@@ -72,7 +72,7 @@ def test_overflow_headroom_of_the_hmc_scale():
     overflows fp16 (65504 < 2^16 = 2^12 * 16).  The HMC trajectory therefore checks an a-priori
     bound on |q_next| every pass: where it would reach 2^16 - 2^8 at the current scale, the planes
     also get a copy at a lower scale (impl 5: kept as a spare, used only if the planes overflowed;
-    impl 2 / 4: used directly) (hmc_dense_epilogue.cuh; emulated in
+    impl 2: used directly) (hmc_dense_epilogue.cuh; emulated in
     test_plane_scale_emulation.py)."""
     x = np.array([1.0, -3.0], np.float32)
     s = pow2_scale(x)
@@ -83,9 +83,10 @@ def test_overflow_headroom_of_the_hmc_scale():
 
 
 def test_trajectory_kernel_buffer_schedule_matches_the_per_pass_host_loop():
-    """hmc_dense_traj.cu (experimental impl 4) hard-codes the ping-pong of the per-pass host loop
-    (zhusuan_b200/hmc.py::_iterate_dense): pass i reads traj_cur(i) and writes traj_nxt(i) with
-    0 = q0, 1 = qa, 2 = qb; the proposal ends in qa when L - 1 is even, else in qb."""
+    """Closed form of the buffer ping-pong of the per-pass host loop
+    (zhusuan_b200/hmc.py::_iterate_dense, dense_impl 0 / 1 / 2): pass i reads traj_cur(i) and
+    writes traj_nxt(i) with 0 = q0, 1 = qa, 2 = qb; the proposal ends in qa when L - 1 is even,
+    else in qb."""
     traj_cur = lambda i: 0 if i == 0 else (1 if i & 1 else 2)
     traj_nxt = lambda i: 2 if i & 1 else 1
     for L in range(1, 12):

@@ -56,7 +56,7 @@ constexpr float BIN_SCALE = 2048.f;
 //   EPI 6  out[r, j] = sum_s g[s R + r] * (x[s R + r, j] - sigmoid(l))     (d/dl of EPI 5)
 template <int EPI, int MN, int GL, int Z = 0>
 struct LinW {
-  static constexpr int KIND = 1, RB = 128, MNA = MN & 1, MNB = (MN >> 1) & 1, CVT = 0, ZLO = Z;
+  static constexpr int KIND = 1, RB = 128, MNA = MN & 1, MNB = (MN >> 1) & 1, ZLO = Z;
   static constexpr uint32_t TX = Cfg<RB>::STAGE - ((Z & 1) ? Cfg<RB>::A_TILE : 0) -
                                  ((Z & 2) ? Cfg<RB>::B_TILE : 0);
   CUtensorMap map_whi, map_wlo, map_hhi, map_hlo;
@@ -118,7 +118,6 @@ struct LinW {
       if (!(Z & 2)) tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE, &map_hlo, fb, kb * 64, r0);
     }
   }
-  __device__ __forceinline__ void convert(int64_t, int, uint8_t*, int) const {}
   __device__ __forceinline__ void epilogue(int64_t uu, uint32_t trow, int quarter, int lane,
                                            EpiState& st) const {
     if constexpr (EPI >= 4)

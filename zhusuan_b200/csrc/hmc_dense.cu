@@ -182,7 +182,6 @@ int zsb_dense_leapfrog_tc_launch(const float* q_cur, const float* q_cur_lo, floa
                                  int D, cudaStream_t st);
 int zsb_dense_split_lo_launch(const float* q, float* lo, int64_t n, cudaStream_t st);
 int zsb_dense_tc_ntiles(int D);
-int zsb_dense_tc_set_bk(int bk);
 int zsb_dense_leapfrog_h16_launch(const float* q_cur, const void* q_cur_planes, float* q_next,
                                   void* q_next_planes, const float* p_in, float* p_out,
                                   const void* P_h16, const void* P_l16, float* scales,
@@ -192,29 +191,15 @@ int zsb_dense_leapfrog_h16_launch(const float* q_cur, const void* q_cur_planes, 
                                   cudaStream_t st);
 int zsb_dense_h16_prepare_launch(const float* q, const float* p, const float* mass, void* planes,
                                  float* scales, int64_t chains, int64_t D, cudaStream_t st);
-int zsb_dense_leapfrog_h16i_launch(const float* q_cur, float* q_next, const float* p_in,
-                                   float* p_out, const void* P_h16, const void* P_l16,
-                                   float* scales, int pass_index, const float* bvec,
-                                   const float* mu, const float* mass, const float* state,
-                                   float p_scale, float* lp_part, float* k_part, int64_t chains,
-                                   int D, cudaStream_t st);
-int zsb_dense_h16i_prepare_launch(const float* q, float* scales, int64_t n, cudaStream_t st);
-int zsb_dense_traj_h16_launch(const float* q0, const void* planes0, float* qa, void* planes_a,
-                              float* qb, void* planes_b, const float* p0, float* pw,
-                              const void* P_h16, const void* P_l16, float* scales,
-                              const float* bvec, const float* mu, const float* mass,
-                              const float* state, float* lp0_part, float* lp1_part,
-                              float* k_part, int64_t chains, int D, int L, cudaStream_t st);
 // implemented in hmc_dense_res.cu
 int zsb_dense_res_h16_launch(void* planes0, void* planes1, void* spare0, void* spare1,
                              const float* p0, float* pw, const void* P_h16, const void* P_l16,
                              float* scales, const float* bvec, const float* mu, const float* mass,
                              const float* state, float* lp0_part, float* lp1_part, float* k_part,
-                             int* flags, int64_t chains, int D, int L, cudaStream_t st);
+                             int64_t chains, int D, int L, cudaStream_t st);
 int zsb_dense_select_planes_launch(float* q, const void* planes, const void* spare,
-                                   const float* scales, const int32_t* accept, int64_t chains,
+                                   const float* record, const int32_t* accept, int64_t chains,
                                    int64_t D, cudaStream_t st);
-int zsb_dense_res_group_blocks(int D);
 
 extern "C" {
 
@@ -251,13 +236,6 @@ int zsb_hmc_dense_leapfrog_f32(const float* q_cur, const float* q_cur_lo, float*
   return zsb_check_launch("hmc_dense_leapfrog_simt");
 }
 
-// Pipeline shape of the tensor-core kernel: bk = 32 -> 2 stages x 96 KB (128B swizzle),
-// bk = 16 -> 4 stages x 48 KB (64B swizzle).  Tuning knob; results are identical.
-int zsb_hmc_dense_tc_config(int bk) {
-  ZSB_REQUIRE(zsb_dense_tc_set_bk(bk) == ZSB_OK, "zsb_hmc_dense_tc_config: bk must be 16 or 32");
-  return ZSB_OK;
-}
-
 // lo[i] = q[i] - tf32_trunc(q[i])  (the residual operand of the 3xTF32 split), n % 4 == 0
 int zsb_hmc_dense_split_lo_f32(const float* q, float* lo, int64_t n, void* stream) {
   ZSB_REQUIRE(q && lo && n >= 0, "zsb_hmc_dense_split_lo_f32: bad args");
@@ -265,38 +243,15 @@ int zsb_hmc_dense_split_lo_f32(const float* q, float* lo, int64_t n, void* strea
   return zsb_dense_split_lo_launch(q, lo, n, (cudaStream_t)stream);
 }
 
-// impl 2 (fp16-split tensor-core path).  Operands are fp16 hi/lo planes of P*sP and q*sq:
-//   P_h16, P_l16: [D, D] __half;  q_*_planes: [2][chains][D] __half (hi plane, lo plane);
-//   scales (device float[4]): [0] sq, [1] 1/(sP*sq), [2] scratch, [3] sP (set by the caller once).
-// zsb_hmc_dense_h16_prepare_f32 derives sq from max|q| (power of two, max|q| * sq in
-// [2^11, 2^12)) and writes q's planes; the leapfrog pass writes q_next's planes with the same sq,
-// which overflow fp16 once |q_next| grows ~16x past max|q|.  D % 64 == 0.
-int zsb_hmc_dense_h16_prepare_f32(const float* q, void* planes, float* scales, int64_t n,
-                                  void* stream) {
-  ZSB_REQUIRE(q && planes && scales && n > 0, "zsb_hmc_dense_h16_prepare_f32: bad args");
-  return zsb_dense_h16_prepare_launch(q, nullptr, nullptr, planes, scales, n, 1,
-                                      (cudaStream_t)stream);
-}
-int zsb_hmc_dense_leapfrog_h16_f32(const float* q_cur, const void* q_cur_planes, float* q_next,
-                                   void* q_next_planes, const float* p_in, float* p_out,
-                                   const void* P_h16, const void* P_l16, const float* scales,
-                                   const float* bvec, const float* mu, const float* mass,
-                                   const float* state, float p_scale, float* lp_part,
-                                   float* k_part, int64_t chains, int64_t D, void* stream) {
-  ZSB_REQUIRE(q_cur && p_in && p_out && P_h16 && P_l16 && mass && state,
-              "zsb_hmc_dense_leapfrog_h16_f32: null arg");
-  ZSB_REQUIRE(q_next != q_cur, "zsb_hmc_dense_leapfrog_h16_f32: q_next must not alias q_cur");
-  return zsb_dense_leapfrog_h16_launch(q_cur, q_cur_planes, q_next, q_next_planes, p_in, p_out,
-                                       P_h16, P_l16, const_cast<float*>(scales), -1, bvec, mu,
-                                       mass, state, p_scale, lp_part, k_part, chains, (int)D,
-                                       (cudaStream_t)stream);
-}
-// Trajectory form of impl 2, whose plane scale follows the chains: scales is a device
-// float[8 + 4 * (L + 2)] of plane-scale records (hmc_dense_epilogue.cuh) with [3] sP,
-// [4] ||P||_inf, [5] max|b| set by the caller once.  zsb_hmc_dense_traj_prepare_f32 (before every
+// impl 2 (fp16-split tensor-core path, one launch per leapfrog pass).  Operands are fp16 hi/lo
+// planes of P*sP and q*sq: P_h16, P_l16: [D, D] __half; q_*_planes: [2][chains][D] __half (hi
+// plane, lo plane).  The plane scale follows the chains: scales is a device float[8 + 4 * (L + 2)]
+// of plane-scale records (hmc_dense_epilogue.cuh) with [3] sP, [4] ||P||_inf, [5] max|b| set by
+// the caller once.  zsb_hmc_dense_traj_prepare_f32 (before every
 // trajectory, after the momentum p is drawn) writes record 0 and q's planes; pass `pass_index`
 // (from 0) reads planes at the scale of record pass_index and writes q_next's planes, and record
 // pass_index + 1, at a scale lowered whenever a bound on |q_next| could overflow fp16.
+// D % 64 == 0.
 int zsb_hmc_dense_traj_prepare_f32(const float* q, const float* p, const float* mass, void* planes,
                                    float* scales, int64_t chains, int64_t D, void* stream) {
   ZSB_REQUIRE(q && p && mass && planes && scales && chains > 0 && D > 0,
@@ -321,85 +276,33 @@ int zsb_hmc_dense_leapfrog_h16_pass_f32(const float* q_cur, const void* q_cur_pl
                                        (cudaStream_t)stream);
 }
 
-// impl 3: as impl 2, but the fp16 planes of q are built inside the kernel from the fp32 tile, so
-// a pass moves only the algorithmic 16*D bytes per chain through HBM.  scales: device float[8],
-// [3] = sP (caller), [4..6] = rotating max|q| slots.  Call the prepare entry point before pass 0
-// of every trajectory; pass_index counts the passes of that trajectory from 0.
-int zsb_hmc_dense_h16i_prepare_f32(const float* q, float* scales, int64_t n, void* stream) {
-  ZSB_REQUIRE(q && scales && n > 0, "zsb_hmc_dense_h16i_prepare_f32: bad args");
-  return zsb_dense_h16i_prepare_launch(q, scales, n, (cudaStream_t)stream);
-}
-int zsb_hmc_dense_leapfrog_h16i_f32(const float* q_cur, float* q_next, const float* p_in,
-                                    float* p_out, const void* P_h16, const void* P_l16,
-                                    float* scales, int pass_index, const float* bvec,
-                                    const float* mu, const float* mass, const float* state,
-                                    float p_scale, float* lp_part, float* k_part, int64_t chains,
-                                    int64_t D, void* stream) {
-  ZSB_REQUIRE(q_cur && p_in && p_out && P_h16 && P_l16 && mass && state && scales,
-              "zsb_hmc_dense_leapfrog_h16i_f32: null arg");
-  ZSB_REQUIRE(q_next != q_cur, "zsb_hmc_dense_leapfrog_h16i_f32: q_next must not alias q_cur");
-  return zsb_dense_leapfrog_h16i_launch(q_cur, q_next, p_in, p_out, P_h16, P_l16, scales,
-                                        pass_index, bvec, mu, mass, state, p_scale, lp_part,
-                                        k_part, chains, (int)D, (cudaStream_t)stream);
-}
-
-// EXPERIMENTAL (impl 4, not yet validated on hardware): the L+1 passes of a trajectory in one
-// persistent launch with L2-resident chain blocks (hmc_dense_traj.cu).  D == 1024, n_leapfrogs >= 1.
-// scales and planes0 as zsb_hmc_dense_leapfrog_h16_pass_f32 (zsb_hmc_dense_traj_prepare_f32).
-int zsb_hmc_dense_trajectory_h16_f32(const float* q0, const void* planes0, float* qa,
-                                     void* planes_a, float* qb, void* planes_b, const float* p0,
-                                     float* pw, const void* P_h16, const void* P_l16,
-                                     float* scales, const float* bvec, const float* mu,
-                                     const float* mass, const float* state, float* lp0_part,
-                                     float* lp1_part, float* k_part, int64_t chains, int64_t D,
-                                     int n_leapfrogs, void* stream) {
-  ZSB_REQUIRE(q0 && planes0 && qa && planes_a && qb && planes_b && p0 && pw && P_h16 && P_l16 &&
-                  scales && mass && state && lp0_part && lp1_part && k_part,
-              "zsb_hmc_dense_trajectory_h16_f32: null arg");
-  return zsb_dense_traj_h16_launch(q0, planes0, qa, planes_a, qb, planes_b, p0, pw, P_h16, P_l16,
-                                   scales, bvec, mu, mass, state, lp0_part, lp1_part, k_part,
-                                   chains, (int)D, n_leapfrogs, (cudaStream_t)stream);
-}
-
 // impl 5: the whole leapfrog `while_loop` of hmc.py:347-372 (L+1 passes, one launch each,
 // hmc_dense_res.cu).  The sampler state inside the trajectory is the fp16 hi/lo plane pair of
 // q*sq_i (+ fp32 p), with the plane-scale records of impl 2's trajectory form; planes0 comes from
 // zsb_hmc_dense_traj_prepare_f32, planes1, spare0 and spare1 are work buffers of the same size
-// (spare copies of the planes when a pass's bound could overflow them), flags an int32 scratch of
-// zsb_hmc_dense_resident_flags(chains) words.  On return the proposal's planes are in buffer
-// (n_leapfrogs & 1) or its spare -- zsb_hmc_dense_select_traj_planes_f32, given both and record
-// n_leapfrogs, assigns them to the accepted chains -- and pw holds the final momentum.
+// (spare copies of the planes when a pass's bound could overflow them).  On return the proposal's
+// planes are in buffer (n_leapfrogs & 1) or its spare -- zsb_hmc_dense_select_traj_planes_f32,
+// given both and record n_leapfrogs, assigns them to the accepted chains -- and pw holds the final
+// momentum.
 // D % 64 == 0, n_leapfrogs >= 1.
-int zsb_hmc_dense_resident_flags(int64_t chains) { return 2 * (int)zsb_ceil_div(chains, 256); }
-int zsb_hmc_dense_resident_group(int64_t D) { return zsb_dense_res_group_blocks((int)D); }
 int zsb_hmc_dense_resident_h16_f32(void* planes0, void* planes1, void* spare0, void* spare1,
                                    const float* p0, float* pw, const void* P_h16,
                                    const void* P_l16, float* scales, const float* bvec,
                                    const float* mu, const float* mass, const float* state,
                                    float* lp0_part, float* lp1_part, float* k_part,
-                                   int32_t* flags, int64_t chains, int64_t D, int n_leapfrogs,
-                                   void* stream) {
+                                   int64_t chains, int64_t D, int n_leapfrogs, void* stream) {
   ZSB_REQUIRE(planes0 && planes1 && spare0 && spare1 && p0 && pw && P_h16 && P_l16 && scales &&
-                  mass && state && lp0_part && lp1_part && k_part && flags,
+                  mass && state && lp0_part && lp1_part && k_part,
               "zsb_hmc_dense_resident_h16_f32: null arg");
   ZSB_REQUIRE(p0 != pw, "zsb_hmc_dense_resident_h16_f32: aliased buffers");
   return zsb_dense_res_h16_launch(planes0, planes1, spare0, spare1, p0, pw, P_h16, P_l16, scales,
-                                  bvec, mu, mass, state, lp0_part, lp1_part, k_part, flags, chains,
-                                  (int)D, n_leapfrogs, (cudaStream_t)stream);
+                                  bvec, mu, mass, state, lp0_part, lp1_part, k_part, chains, (int)D,
+                                  n_leapfrogs, (cudaStream_t)stream);
 }
-// q[c, :] <- (hi + lo) / sq of `planes` for the chains with accept[c] != 0 (hmc.py:488-497);
-// scales[0] = sq of those planes
-int zsb_hmc_dense_select_planes_f32(float* q, const void* planes, const float* scales,
-                                    const int32_t* accept, int64_t chains, int64_t D,
-                                    void* stream) {
-  ZSB_REQUIRE(q && planes && scales && accept && chains > 0 && D > 0 && D % 2 == 0,
-              "zsb_hmc_dense_select_planes_f32: bad args");
-  return zsb_dense_select_planes_launch(q, planes, nullptr, scales, accept, chains, D,
-                                        (cudaStream_t)stream);
-}
-// As zsb_hmc_dense_select_planes_f32 for the proposal of an impl-5 trajectory: `record` is its
-// plane-scale record (&scales[8 + 4 * n_leapfrogs]), which says whether `planes` or `spare` holds
-// the proposal, and at which scale.
+// q[c, :] <- (hi + lo) / sq of the proposal of an impl-5 trajectory for the chains with
+// accept[c] != 0 (hmc.py:488-497): `record` is its plane-scale record
+// (&scales[8 + 4 * n_leapfrogs]), which says whether `planes` or `spare` holds the proposal, and
+// at which scale.
 int zsb_hmc_dense_select_traj_planes_f32(float* q, const void* planes, const void* spare,
                                          const float* record, const int32_t* accept,
                                          int64_t chains, int64_t D, void* stream) {

@@ -1,13 +1,13 @@
-// Fused leapfrog epilogue shared by the dense-Gaussian tensor-core kernels (hmc_dense_tc.cu: one
-// pass per launch; hmc_dense_traj.cu: a whole trajectory per launch).  Velocity-Verlet update of
-// zhusuan/hmc.py:38-43 on the accumulator tile: p += s2 * g, q_next = q + (eps / m) * p, plus the
-// log p / kinetic partials of hamiltonian() (hmc.py:30-35) on the first / last pass.
+// Fused leapfrog epilogue of the per-pass dense-Gaussian tensor-core kernel (hmc_dense_tc.cu), and
+// the plane-scale records it shares with the trajectory kernel (hmc_dense_res.cu).  Velocity-Verlet
+// update of zhusuan/hmc.py:38-43 on the accumulator tile: p += s2 * g, q_next = q + (eps / m) * p,
+// plus the log p / kinetic partials of hamiltonian() (hmc.py:30-35) on the first / last pass.
 #pragma once
 #include "tc_common.cuh"
 
 namespace {
 
-// Plane scales of the fp16-split trajectory (impl 2, 4, 5).  `scales` is a device float array of
+// Plane scales of the fp16-split trajectory (impl 2, 5).  `scales` is a device float array of
 // kScaleHdr + kScaleRec * (L + 2) words:
 //   [0] sq of q0's planes, [1] 1/(sP*sq) (copies of record 0), [2] prepare scratch (max|q0| bits),
 //   [3] sP, [4] ||P||_inf, [5] max|b| (the caller sets these three once), [6] prepare scratch
@@ -24,7 +24,7 @@ namespace {
 // drift_i = max|q_i| + max|q_{i-1}| >= max|(eps/m) p_i| = max|q_i - q_{i-1}| (so a pass only
 // reduces max|q|).  While B_i * sq_i stays below kPlaneKeep the planes of q_{i+1} cannot
 // overflow at sq_i.  Otherwise sq_alt = the power of two that puts B_i in [2^11, 2^12):
-//   impl 2 / 4 write the next planes at sq_alt;
+//   impl 2 writes the next planes at sq_alt;
 //   impl 5 writes them at sq_i, exactly as when the bound is not reached, plus a spare copy at
 //   sq_alt, and flags the pass if any |q_{i+1}| * sq_i reached fp16's overflow (65520); the next
 //   pass then reads the spare.  A bound is loose, so this keeps every trajectory whose planes fit
@@ -89,7 +89,7 @@ __device__ __forceinline__ void publish_plane_scale(float* __restrict__ scales, 
 }
 
 // Fused leapfrog epilogue for one warp's share of a tile: this thread's dimension `n` (accumulator
-// row) against NCOL chains starting at c0 (`trow` = shared address of the row's first column).
+// row) against BN chains starting at c0 (`trow` = shared address of the row's first column).
 // MODE 0: plain pass; 1: + log-prob partials (first pass); 2: + log-prob and kinetic partials
 // (last pass).
 struct EpiArgs {
@@ -99,7 +99,7 @@ struct EpiArgs {
   int64_t chains; int D;
   // fp16-split operands (impl 2): q_next_lo is then a [2][chains][D] __half buffer (hi plane, lo
   // plane) of q_next * q_scale, and the accumulator holds (P*sP)(q_cur*sq): g = b - acc * acc_scale.
-  int h16; float q_scale; float acc_scale;
+  float acc_scale; float q_scale;
 };
 // residual operand(s) of q_next for the next pass's MMA
 template <int H16>   // 0: TF32 residual, 1: fp16 hi/lo planes
@@ -115,25 +115,23 @@ __device__ __forceinline__ void store_split(const EpiArgs& a, float* __restrict_
     lo_f32[off] = qn - __uint_as_float(__float_as_uint(qn) & 0xFFFFE000u);
   }
 }
-// MODE: see above.  NEXT: 1 / 0 = q_next is / is not written (compile time), -1 = decided at run
-// time from a.q_next.  DC: the dimension count when known at compile time (all per-column offsets
-// j*D then fold into the load/store immediates: ~15 instead of ~40 instructions per element), 0 =
-// run-time a.D.  H16: fp16-split planes (impl 2) vs TF32 residual (impl 1).  amax: running max of
-// |q_next| (H16 1, 2; finite values only for 2) over the elements this thread wrote (fmaxf drops
-// NaN; an inf makes the plane-scale bound infinite, which keeps the scale).
-// COHERENT: 1 when q_cur may have been written earlier in the SAME launch (trajectory kernel): the
-// non-coherent ld.global.nc path of __ldg could then return a stale L1 line.
-template <int MODE, int NEXT, int DC, int H16, int NCOL = BN, int COHERENT = 0>
+// MODE: see above.  q_next is written when a.q_next is set.  DC: the dimension count when known
+// at compile time (all per-column offsets j*D then fold into the load/store immediates: ~15
+// instead of ~40 instructions per element), 0 = run-time a.D.  H16: fp16-split planes (impl 2) vs
+// TF32 residual (impl 1).  amax: running max of |q_next| (H16 1) over the elements this thread
+// wrote (fmaxf drops NaN; an inf makes the plane-scale bound infinite, which keeps the scale).
+template <int MODE, int DC, int H16>
 __device__ __forceinline__ void epilogue_half_tile(const EpiArgs& a, uint32_t trow, int n,
-                                                   bool n_ok, bool parts_ok, int64_t c0,
-                                                   int64_t part_row, int lane, float s2,
-                                                   float eps_over_m, float inv_m, float b_n,
-                                                   float mu_n, bool skip, float& amax) {
+                                                   bool n_ok, int64_t c0, int64_t part_row,
+                                                   int lane, float s2, float eps_over_m,
+                                                   float inv_m, float b_n, float mu_n,
+                                                   float& amax) {
+  constexpr int NCOL = BN;
   const uint32_t D = DC ? (uint32_t)DC : (uint32_t)a.D;
   const int64_t chains = a.chains;
-  const bool has_next = NEXT < 0 ? (a.q_next != nullptr) : (NEXT != 0);
+  const bool has_next = a.q_next != nullptr;
   const bool warp_n_ok = __all_sync(0xffffffffu, n_ok);
-  const bool fast_tile = warp_n_ok && (c0 + NCOL <= chains) && !skip;
+  const bool fast_tile = warp_n_ok && (c0 + NCOL <= chains);
 
   // this thread's element of chain c0 in every array (the same element offset everywhere)
   const int64_t off_t = c0 * (int64_t)D + n;
@@ -141,8 +139,6 @@ __device__ __forceinline__ void epilogue_half_tile(const EpiArgs& a, uint32_t tr
   const float* __restrict__ qc0 = a.q_cur + off_t;
   float* __restrict__ po0 = a.p_out + off_t;
   float* __restrict__ qn0 = has_next ? a.q_next + off_t : nullptr;
-  // H16 == 2: the next pass splits q_next itself (in-kernel conversion); only max|q_next| is
-  // tracked here for its scale
   float* __restrict__ lo0 = (has_next && H16 == 0) ? a.q_next_lo + off_t : nullptr;
   __half* __restrict__ hi_pl0 =
       (has_next && H16 == 1) ? reinterpret_cast<__half*>(a.q_next_lo) + off_t : nullptr;
@@ -168,8 +164,7 @@ __device__ __forceinline__ void epilogue_half_tile(const EpiArgs& a, uint32_t tr
         const float qn = fmaf(eps_over_m, pn, qe[j]);
         qn_p[(uint32_t)j * D] = qn;
         if (H16 == 1) amax = fmaxf(amax, fabsf(qn));
-        if (H16 == 2) amax = finite_absmax(amax, qn);
-        if (H16 != 2) store_split<H16>(a, lo_p, hp, lp, (uint32_t)j * D, qn);
+        store_split<H16>(a, lo_p, hp, lp, (uint32_t)j * D, qn);
       }
     }
     if (MODE >= 1) {
@@ -187,7 +182,7 @@ __device__ __forceinline__ void epilogue_half_tile(const EpiArgs& a, uint32_t tr
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       pe[j] = __ldcs(pin + (uint32_t)j * D);       // p is streamed: evict-first
-      qe[j] = COHERENT ? __ldcg(qc + (uint32_t)j * D) : __ldg(qc + (uint32_t)j * D);
+      qe[j] = __ldg(qc + (uint32_t)j * D);
     }
   };
 
@@ -212,20 +207,15 @@ __device__ __forceinline__ void epilogue_half_tile(const EpiArgs& a, uint32_t tr
       uint32_t v[16];
       acc_ld16(trow + 4u * (uint32_t)c, v);
       const int64_t cbase = c0 + c;
-      if (cbase < chains && !skip) {
+      if (cbase < chains) {
         const size_t cb = (size_t)c * D;
         float pe[16], qe[16];
         float lpv[MODE >= 1 ? 16 : 1], kv[MODE >= 2 ? 16 : 1];
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const bool ok = n_ok && cbase + j < chains;
-          if (COHERENT) {     // written earlier in this launch: no ld.global.nc
-            pe[j] = ok ? __ldcg(pin0 + cb + (uint32_t)j * D) : 0.f;
-            qe[j] = ok ? __ldcg(qc0 + cb + (uint32_t)j * D) : 0.f;
-          } else {
-            pe[j] = ok ? pin0[cb + (uint32_t)j * D] : 0.f;
-            qe[j] = ok ? qc0[cb + (uint32_t)j * D] : 0.f;
-          }
+          pe[j] = ok ? pin0[cb + (uint32_t)j * D] : 0.f;
+          qe[j] = ok ? qc0[cb + (uint32_t)j * D] : 0.f;
         }
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
@@ -240,21 +230,17 @@ __device__ __forceinline__ void epilogue_half_tile(const EpiArgs& a, uint32_t tr
               const float qn = fmaf(eps_over_m, pn, qe[j]);
               qn0[cb + (uint32_t)j * D] = qn;
               if (H16 == 1) amax = fmaxf(amax, fabsf(qn));
-              if (H16 == 2) amax = finite_absmax(amax, qn);
-              if (H16 != 2)
-                store_split<H16>(a, lo0 + cb, hi_pl0 + cb, lo_pl0 + cb, (uint32_t)j * D, qn);
+              store_split<H16>(a, lo0 + cb, hi_pl0 + cb, lo_pl0 + cb, (uint32_t)j * D, qn);
             }
           }
         }
         if (MODE >= 1) {
           const float sum = warp_transpose_sum16(lpv, lane);
-          if (parts_ok && lane < 16 && cbase + lane < chains)
-            a.lp_part[part_row + cbase + lane] = sum;
+          if (lane < 16 && cbase + lane < chains) a.lp_part[part_row + cbase + lane] = sum;
         }
         if (MODE >= 2) {
           const float sum = warp_transpose_sum16(kv, lane);
-          if (parts_ok && lane < 16 && cbase + lane < chains)
-            a.k_part[part_row + cbase + lane] = sum;
+          if (lane < 16 && cbase + lane < chains) a.k_part[part_row + cbase + lane] = sum;
         }
       }
     }

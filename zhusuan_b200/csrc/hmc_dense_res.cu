@@ -55,15 +55,14 @@ struct ResEpi {
 // the plane scale.
 template <int MODE, int NEXT, int DC, bool SPARE>
 __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, int n, bool n_ok,
-                                                bool parts_ok, int64_t c0, int64_t part_row,
-                                                int lane, float s2, float eps_over_m_sq,
-                                                float inv_m, float b_n, float mu_n, bool skip,
-                                                float& qmax) {
+                                                int64_t c0, int64_t part_row, int lane, float s2,
+                                                float eps_over_m_sq, float inv_m, float b_n,
+                                                float mu_n, float& qmax) {
   constexpr int NCOL = BN;
   const uint32_t D = DC ? (uint32_t)DC : (uint32_t)a.D;
   const int64_t chains = a.chains;
   const bool warp_n_ok = __all_sync(0xffffffffu, n_ok);
-  const bool fast_tile = warp_n_ok && (c0 + NCOL <= chains) && !skip;
+  const bool fast_tile = warp_n_ok && (c0 + NCOL <= chains);
   const int64_t off_t = c0 * (int64_t)D + n;
   const float* __restrict__ pin0 = a.p_in + off_t;
   float* __restrict__ po0 = a.p_out + off_t;
@@ -168,7 +167,7 @@ __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, 
       uint32_t v[16];
       acc_ld16(trow + 4u * (uint32_t)c, v);
       const int64_t cbase = c0 + c;
-      if (cbase < chains && !skip) {
+      if (cbase < chains) {
         const size_t cb = (size_t)c * D;
         float lpv[MODE >= 1 ? 16 : 1], kv[MODE >= 2 ? 16 : 1];
 #pragma unroll
@@ -204,13 +203,11 @@ __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, 
         }
         if (MODE >= 1) {
           const float sum = warp_transpose_sum16(lpv, lane);
-          if (parts_ok && lane < 16 && cbase + lane < chains)
-            a.lp_part[part_row + cbase + lane] = sum;
+          if (lane < 16 && cbase + lane < chains) a.lp_part[part_row + cbase + lane] = sum;
         }
         if (MODE >= 2) {
           const float sum = warp_transpose_sum16(kv, lane);
-          if (parts_ok && lane < 16 && cbase + lane < chains)
-            a.k_part[part_row + cbase + lane] = sum;
+          if (lane < 16 && cbase + lane < chains) a.k_part[part_row + cbase + lane] = sum;
         }
       }
     }
@@ -232,7 +229,7 @@ template <int MODE, int NEXT, int DC, int CX, int CY>
 struct ResW {
   // 64-byte rows (32 fp16 of contraction per k-block): four 32 KB stages beside the accumulator
   // tile, so the TMA producer runs up to three k-blocks ahead of the tensor cores
-  static constexpr int KIND = 1, RB = 64, MNA = 0, MNB = 0, CVT = 0;
+  static constexpr int KIND = 1, RB = 64, MNA = 0, MNB = 0;
   static constexpr int CLUSTER = CX * CY;
   static constexpr int KE = RB / 2;
   static constexpr uint32_t TX = Cfg<RB>::STAGE;
@@ -301,7 +298,6 @@ struct ResW {
       tma_load_2d_mc(sa + 2 * C::A_TILE + C::B_TILE + o, ql, fb, kb * KE, c0 + rx * rows, mask);
     }
   }
-  __device__ __forceinline__ void convert(int64_t, int, uint8_t*, int) const {}
   __device__ __forceinline__ float sq_alt(float eps, float sq) const {
     return next_plane_scale(scales, pass, eps, mul(eps, p_scale), sq);
   }
@@ -333,11 +329,11 @@ struct ResW {
     a.acc_scale = 1.f / (scales[3] * sq);                   // powers of two: exact
     a.rescale = NEXT ? sq_alt(eps, sq) * a.inv_sq : 1.f;
     if (a.rescale == 1.f)
-      epilogue_planes<MODE, NEXT, DC, false>(a, trow, n, n_ok, true, c0, part_row, lane, s2,
-                                             eps_over_m_sq, inv_m, b_n, mu_n, false, st.qmax);
+      epilogue_planes<MODE, NEXT, DC, false>(a, trow, n, n_ok, c0, part_row, lane, s2,
+                                             eps_over_m_sq, inv_m, b_n, mu_n, st.qmax);
     else
-      epilogue_planes<MODE, NEXT, DC, true>(a, trow, n, n_ok, true, c0, part_row, lane, s2,
-                                            eps_over_m_sq, inv_m, b_n, mu_n, false, st.qmax);
+      epilogue_planes<MODE, NEXT, DC, true>(a, trow, n, n_ok, c0, part_row, lane, s2,
+                                            eps_over_m_sq, inv_m, b_n, mu_n, st.qmax);
   }
   __device__ __forceinline__ void epi_finish(EpiState& st, int quarter, int lane) const {
     if (!NEXT) return;
@@ -386,20 +382,20 @@ int res_pass(bool cluster, const CUtensorMap& phi, const CUtensorMap& plo, const
                                       scales, pass, p_scale, n_blk, D, mode, st);
 }
 
-// q[c, :] <- (hi + lo) / sq of the proposal planes where accept[c] (hmc.py:488-497); scales[0] is
-// the sq of `planes`.  With `spare` (impl 5), `scales` is the proposal's plane-scale record, and
-// its overflow flag selects the spare planes at scales[1].
+// q[c, :] <- (hi + lo) / sq of the proposal planes where accept[c] (hmc.py:488-497).  `record` is
+// the proposal's plane-scale record: the planes are in `planes` at record[0], or, when its
+// overflow flag is set, in `spare` at record[1].
 // One warp per chain at a time (the accept flag is warp-uniform: a rejected chain costs one 4-byte
 // load), 8 dimensions per lane and step: two 128-bit plane loads in, two 128-bit stores out, up to
 // four steps' loads issued before the first use.  D % 8 == 0 (the dense kernels need D % 64 == 0).
 __global__ void __launch_bounds__(256) select_planes_kernel(float* __restrict__ q,
                                                             const __half* __restrict__ planes,
                                                             const __half* __restrict__ spare,
-                                                            const float* __restrict__ scales,
+                                                            const float* __restrict__ record,
                                                             const int32_t* __restrict__ accept,
                                                             int64_t chains, int64_t D) {
-  const bool use_spare = spare && __float_as_uint(scales[3]) != 0u;
-  const float inv_sq = 1.f / scales[use_spare ? 1 : 0];
+  const bool use_spare = __float_as_uint(record[3]) != 0u;
+  const float inv_sq = 1.f / record[use_spare ? 1 : 0];
   if (use_spare) planes = spare;
   const int lane = threadIdx.x & 31;
   const int n8 = (int)(D >> 3);
@@ -440,27 +436,19 @@ __global__ void __launch_bounds__(256) select_planes_kernel(float* __restrict__ 
 
 }  // namespace
 
-// Chain blocks per scheduling group (one group = every chain: the passes run as separate launches)
-int zsb_dense_res_group_blocks(int D) {
-  (void)D;
-  return 1 << 30;
-}
-
 // The L+1 passes of a trajectory for every chain (D % 64 == 0, L >= 1).
-//   planes0: fp16 hi/lo planes of q * sq_0 (zsb_hmc_dense_h16_prepare_f32), planes1: work buffer of
-//   the same size (must differ from planes0: a pass reads every dimension of a chain block's planes
-//   while other tiles of the same launch write the next ones); on return the proposal's planes are
-//   in buffer (L & 1), or in spare buffer (L & 1) when record L flags them; spare0 / spare1: two
+//   planes0: fp16 hi/lo planes of q * sq_0 (zsb_hmc_dense_traj_prepare_f32), planes1: work buffer
+//   of the same size (must differ from planes0: a pass reads every dimension of a chain block's
+//   planes while other tiles of the same launch write the next ones); on return the proposal's
+//   planes are in buffer (L & 1), or in spare buffer (L & 1) when record L flags them; spare0 / spare1: two
 //   more buffers of that size for the spare copies; p0 -> pw (final momentum); lp0_part /
 //   lp1_part / k_part as the per-pass kernel writes them; pass i writes plane-scale record i + 1.
-//   `flags` is not used.
 int zsb_dense_res_h16_launch(void* planes0, void* planes1, void* spare0, void* spare1,
                              const float* p0, float* pw,
                              const void* P_h16, const void* P_l16, float* scales,
                              const float* bvec, const float* mu, const float* mass,
                              const float* state, float* lp0_part, float* lp1_part, float* k_part,
-                             int* flags, int64_t chains, int D, int L, cudaStream_t st) {
-  (void)flags;
+                             int64_t chains, int D, int L, cudaStream_t st) {
   if (D % 64 != 0 || D < 64 || L < 1 || chains <= 0 || chains >= (1LL << 31)) {
     zsb_set_error("dense_res: needs D %% 64 == 0, n_leapfrogs >= 1");
     return ZSB_ERR_INVALID;
@@ -509,14 +497,14 @@ int zsb_dense_res_h16_launch(void* planes0, void* planes1, void* spare0, void* s
 }
 
 int zsb_dense_select_planes_launch(float* q, const void* planes, const void* spare,
-                                   const float* scales, const int32_t* accept, int64_t chains,
+                                   const float* record, const int32_t* accept, int64_t chains,
                                    int64_t D, cudaStream_t st) {
   ZSB_REQUIRE(D % 8 == 0, "zsb_dense_select_planes: D must be a multiple of 8");
   int64_t blocks = zsb_ceil_div(chains, 8);
   if (blocks > ZSB_NUM_SMS * 16) blocks = ZSB_NUM_SMS * 16;
   if (blocks < 1) blocks = 1;
   select_planes_kernel<<<(unsigned)blocks, 256, 0, st>>>(
-      q, reinterpret_cast<const __half*>(planes), reinterpret_cast<const __half*>(spare), scales,
+      q, reinterpret_cast<const __half*>(planes), reinterpret_cast<const __half*>(spare), record,
       accept, chains, D);
   return zsb_check_launch("hmc_select_planes");
 }

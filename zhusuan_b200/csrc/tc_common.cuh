@@ -1,5 +1,5 @@
 // Shared Hopper (sm_90a) building blocks of the tensor-core kernels (hmc_dense_tc.cu,
-// hmc_dense_res.cu, hmc_dense_traj.cu, gemm_logjoint_tc.cu): tile constants, mbarrier pipeline,
+// hmc_dense_res.cu, gemm_logjoint_tc.cu): tile constants, mbarrier pipeline,
 // TMA loads, wgmma descriptors and instructions, the shared-memory accumulator tile the epilogue
 // warps read, the warp-transpose reduction of the epilogues, the host-side tensor-map encoder and
 // one warp-specialised persistent kernel that every tensor-core product runs on.
@@ -230,8 +230,7 @@ __device__ __forceinline__ void mma_kblock(float (&d)[2][64], uint32_t sa) {
 }
 
 // The persistent warp-specialised kernel.  W describes one product:
-//   KIND, RB, MNA, MNB, CVT       compile-time shape (CVT: the MMA warpgroup writes the B planes
-//                                 itself through W::convert; the producer then loads A only)
+//   KIND, RB, MNA, MNB            compile-time shape
 //   units(), kb_range(u, kb0, kb1)
 //   load(u, kb, stage_addr, bar)  the TMA loads of one stage (W::TX bytes)
 //   EpiState, epilogue(u, acc_row_addr, quarter, lane, st), epi_finish(st, quarter, lane)
@@ -317,11 +316,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
       for (int kb = kb0; kb < kb1; ++kb) {
         const uint32_t sa = smem_base + stage * C::STAGE;
         mbar_spin(full_bar + 8 * stage, phase);
-        if (W::CVT) {
-          w.convert(u, kb, smem_raw + (sa - smem_u32(smem_raw)), tid);
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // visible to wgmma
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-        }
         wgmma_fence();
         mma_kblock<W::KIND, W::RB, W::MNA, W::MNB, ZloOf<W>::value>(d, sa);
         wgmma_commit();

@@ -24,7 +24,6 @@ Three execution paths, all ending in the same MH / adaptation kernels:
                  per gradient evaluation (BASELINE config 2).
 """
 import ctypes
-import os
 
 import torch
 
@@ -568,15 +567,17 @@ class HMC(object):
     # ---- fused dense gaussian -----------------------------------------------
     def _setup_dense(self, dev):
         f = self._fused
-        D = f["D"]
         impl = self._dense_impl
         if impl is None:
             impl = f.get("impl")
+        if impl is not None and impl not in (0, 1, 2, 5):
+            raise ValueError("dense_impl must be None, 0, 1, 2 or 5, got {!r}".format(impl))
+        D = f["D"]
         if impl is None:               # default: fastest legal tensor-core path
             impl = (5 if self.n_leapfrogs >= 1 else 2) if D % 64 == 0 else \
                 (1 if D % 32 == 0 else 0)
-        if int(impl) in (2, 3, 5) and D % 64 != 0:
-            raise ValueError("dense_impl=2/3/5 (fp16 split) needs D % 64 == 0")
+        if int(impl) in (2, 5) and D % 64 != 0:
+            raise ValueError("dense_impl=2/5 (fp16 split) needs D % 64 == 0")
         # impl 5: whole-trajectory entry point (hmc_dense_res.cu).  The state of q inside a
         # trajectory is its fp16 hi/lo plane pair, at a scale each pass re-derives from a bound
         # on the q it writes (hmc_dense_epilogue.cuh); the step-size probes are trajectories with
@@ -584,16 +585,7 @@ class HMC(object):
         self._res = int(impl) == 5 and self.n_leapfrogs >= 1
         if int(impl) == 5:
             impl = 2
-        # impl 4: impl 2's buffers and probe passes, the L+1 passes of the main trajectory
-        # through one entry point (hmc_dense_traj.cu)
-        self._traj = int(impl) == 4
-        if self._traj:
-            if D != 1024 or self.n_leapfrogs < 1:
-                raise ValueError("dense_impl=4 needs D == 1024 and n_leapfrogs >= 1")
-            impl = 2
         self._impl = int(impl)
-        if self._impl >= 1:            # pipeline-shape tuning knob (same results)
-            lib.call("zsb_hmc_dense_tc_config", int(os.environ.get("ZSB_TC_BK", "32")))
         nt = lib.load().zsb_hmc_dense_ntiles(D, min(self._impl, 1))
         z = lambda *s: torch.zeros(*s, dtype=_F32, device=dev)
         self._pw = torch.empty_like(self._q[0])
@@ -603,13 +595,10 @@ class HMC(object):
             z(nt * self._chains)
         self._k_part = z(nt * self._chains)
         self._ntiles = nt
-        if self._res:                  # two plane buffers + flags; no fp32 work copies of q
+        if self._res:                  # two plane buffers and their spares; no fp32 copies of q
             shape = (2,) + tuple(self._q[0].shape)
             self._planes = [torch.empty(shape, dtype=torch.float16, device=dev)
                             for _ in range(2)]
-            self._res_flags = torch.zeros(
-                lib.load().zsb_hmc_dense_resident_flags(self._chains),
-                dtype=torch.int32, device=dev)
             self._spare = [torch.empty(shape, dtype=torch.float16, device=dev)
                            for _ in range(2)]
             self._scales = self._plane_scales(dev)
@@ -624,9 +613,6 @@ class HMC(object):
                 self._lo[t.data_ptr()] = torch.empty(
                     (2,) + tuple(t.shape), dtype=torch.float16, device=dev)
             self._scales = self._plane_scales(dev)
-        if self._impl == 3:            # planes are built inside the kernel
-            self._scales = z(8)
-            self._scales[3] = f["sP"]
 
     def _plane_scales(self, dev):
         """Plane-scale records of the fp16-split trajectory (hmc_dense_epilogue.cuh): a header
@@ -643,14 +629,6 @@ class HMC(object):
     def _dense_pass(self, q_cur, q_next, p_in, p_out, scale, lp_part, k_part,
                     s):
         f = self._fused
-        if self._impl == 3:
-            lib.call("zsb_hmc_dense_leapfrog_h16i_f32", ptr(q_cur), ptr(q_next),
-                     ptr(p_in), ptr(p_out), ptr(f["P_h16"]), ptr(f["P_l16"]),
-                     ptr(self._scales), self._pass_k, ptr(f.get("b")),
-                     ptr(f.get("mu")), ptr(self._mass[0]), ptr(self._state),
-                     scale, ptr(lp_part), ptr(k_part), self._chains, f["D"], s)
-            self._pass_k += 1
-            return
         if self._impl == 2:
             lib.call("zsb_hmc_dense_leapfrog_h16_pass_f32", ptr(q_cur),
                      ptr(self._lo[q_cur.data_ptr()]), ptr(q_next),
@@ -702,7 +680,7 @@ class HMC(object):
                  ptr(f["P_h16"]), ptr(f["P_l16"]), ptr(self._scales), ptr(f.get("b")),
                  ptr(f.get("mu")), ptr(self._mass[0]), ptr(self._state),
                  ptr(self._lp0_part), ptr(self._lp1_part), ptr(self._k_part),
-                 ptr(self._res_flags), self._chains, f["D"], L, s)
+                 self._chains, f["D"], L, s)
         return self._planes[L & 1], self._spare[L & 1]
 
     def _iterate_dense_resident(self, noise_u, seed, it, init, s):
@@ -720,14 +698,7 @@ class HMC(object):
                 self._dense_finish_mh(noise_u, seed, it, s, full=False)
             self._search(probe, s)
         prepare()
-        prof = None if self._dev_mode else getattr(self, "_profile_events", None)
-        if prof is not None:           # bench.py: device time of the trajectory launch
-            e0, e1 = torch.cuda.Event(True), torch.cuda.Event(True)
-            e0.record()
-        prop, spare = self._resident_trajectory(self.n_leapfrogs, s)
-        if prof is not None:
-            e1.record()
-            prof.append((e0, e1))
+        prop, spare = self._profiled(lambda: self._resident_trajectory(self.n_leapfrogs, s))
         self._dense_finish_mh(noise_u, seed, it, s, full=True)
         lib.call("zsb_hmc_dense_select_traj_planes_f32", ptr(q0), ptr(prop), ptr(spare),
                  ptr(self._plane_scale_of_pass(self.n_leapfrogs)), ptr(self._accept),
@@ -742,18 +713,15 @@ class HMC(object):
             lib.call("zsb_hmc_dense_split_lo_f32", ptr(q0),
                      ptr(self._lo[q0.data_ptr()]), q0.numel(), s)
 
-        def prepare3():                # before every trajectory: restart the pass count; impl 2:
-            if self._impl == 2:        # planes of q0 and plane-scale record 0; impl 3: max|q|
+        def prepare():                 # before every trajectory: restart the pass count; impl 2:
+            if self._impl == 2:        # planes of q0 and plane-scale record 0
                 lib.call("zsb_hmc_dense_traj_prepare_f32", ptr(q0), ptr(self._p0[0]),
                          ptr(self._mass[0]), ptr(self._lo[q0.data_ptr()]),
                          ptr(self._scales), self._chains, self._row_len[0], s)
-            if self._impl == 3:
-                lib.call("zsb_hmc_dense_h16i_prepare_f32", ptr(q0),
-                         ptr(self._scales), q0.numel(), s)
             self._pass_k = 0
         if init:
             def probe():
-                prepare3()
+                prepare()
                 self._dense_pass(q0, self._qa, self._p0[0], self._pw, 0.5,
                                  self._lp0_part, None, s)
                 self._dense_pass(self._qa, None, self._pw, self._pw, 0.5,
@@ -761,57 +729,42 @@ class HMC(object):
                 self._dense_finish_mh(noise_u, seed, it, s, full=False)
             self._search(probe, s)
         L = self.n_leapfrogs
-        cur, nxt = q0, self._qa
-        p_in = self._p0[0]
-        prepare3()
-        if self._traj:
-            f = self._fused
-            prof = None if self._dev_mode else getattr(self, "_profile_events", None)
-            if prof is not None:
-                e0, e1 = torch.cuda.Event(True), torch.cuda.Event(True)
-                e0.record()
-            lib.call("zsb_hmc_dense_trajectory_h16_f32", ptr(q0),
-                     ptr(self._lo[q0.data_ptr()]), ptr(self._qa),
-                     ptr(self._lo[self._qa.data_ptr()]), ptr(self._qb),
-                     ptr(self._lo[self._qb.data_ptr()]), ptr(self._p0[0]),
-                     ptr(self._pw), ptr(f["P_h16"]), ptr(f["P_l16"]),
-                     ptr(self._scales), ptr(f.get("b")), ptr(f.get("mu")),
-                     ptr(self._mass[0]), ptr(self._state), ptr(self._lp0_part),
-                     ptr(self._lp1_part), ptr(self._k_part), self._chains, f["D"],
-                     L, s)
-            if prof is not None:
-                e1.record()
-                prof.append((e0, e1))
-            cur = self._qa if (L - 1) % 2 == 0 else self._qb
-            self._dense_finish_mh(noise_u, seed, it, s, full=True)
-            lib.call("zsb_hmc_select_f32", ptr(q0), ptr(cur), ptr(self._accept),
-                     self._chains, self._row_len[0], s)
-            return
-        prof = getattr(self, "_profile_events", None)
-        if self._dev_mode:
-            prof = None
-        if prof is not None:           # bench.py: device time of the L+1 passes
-            e0, e1 = torch.cuda.Event(True), torch.cuda.Event(True)
-            e0.record()
-        for i in range(L + 1):
-            last = i == L
-            self._dense_pass(
-                cur, None if last else nxt, p_in, self._pw,
-                1.0 if 0 < i < L else 0.5,
-                self._lp0_part if i == 0 else
-                (self._lp1_part if last else None),
-                self._k_part if last else None, s)
-            p_in = self._pw
-            if not last:
-                cur, nxt = nxt, (self._qb if nxt is self._qa else self._qa)
-        if prof is not None:
-            e1.record()
-            prof.append((e0, e1))
+        prepare()
+
+        def passes():                  # the L+1 passes; returns the buffer holding the proposal
+            cur, nxt = q0, self._qa
+            p_in = self._p0[0]
+            for i in range(L + 1):
+                last = i == L
+                self._dense_pass(
+                    cur, None if last else nxt, p_in, self._pw,
+                    1.0 if 0 < i < L else 0.5,
+                    self._lp0_part if i == 0 else
+                    (self._lp1_part if last else None),
+                    self._k_part if last else None, s)
+                p_in = self._pw
+                if not last:
+                    cur, nxt = nxt, (self._qb if nxt is self._qa else self._qa)
+            return cur
+        cur = self._profiled(passes)
         if L == 0:
             self._lp1_part.copy_(self._lp0_part)
         self._dense_finish_mh(noise_u, seed, it, s, full=True)
         lib.call("zsb_hmc_select_f32", ptr(q0), ptr(cur), ptr(self._accept),
                  self._chains, self._row_len[0], s)
+
+    def _profiled(self, launch):
+        """launch(); when `_profile_events` is a list (bench.py sets it) and no CUDA graph is
+        being captured, also appends a pair of CUDA events around it: its device time."""
+        prof = None if self._dev_mode else getattr(self, "_profile_events", None)
+        if prof is None:
+            return launch()
+        e0, e1 = torch.cuda.Event(True), torch.cuda.Event(True)
+        e0.record()
+        out = launch()
+        e1.record()
+        prof.append((e0, e1))
+        return out
 
     # ----------------------------------------------------------- checkpointing
     def state_dict(self):
