@@ -19,11 +19,13 @@
 // format between the prepare and the select.
 //
 // Without sharing, every 128 x 128 unit pulls 1 MiB of operand planes from L2 (32 k-blocks of
-// 32 KB), 4.3 GB per pass at the benchmark shape against 1.07 GB of HBM traffic.  Where the units
-// tile by 2 x 2 (an even number of dimension blocks and of chain blocks) the pass runs on clusters
-// of four CTAs that multicast the P and q tiles they share, which halves that to 2.1 GB; the
-// products and their order do not change, so neither do the results.  At a 400 W power limit this
-// lets the power-capped SM clock rise, and the pass gets faster (README has the numbers).
+// 32 KB), 4.3 GB per pass at the benchmark shape against 1.07 GB of HBM traffic.  Where the
+// dimension blocks pair up (an even number of them) the pass runs on clusters of two CTAs on
+// neighbouring dimension blocks of one chain block, which multicast that block's q planes: each
+// CTA fetches half of its q tile, 3.2 GB per pass; the products and their order do not change, so
+// neither do the results.  Clusters of two tile every GPC of an H100, so the pass runs on all 132
+// SMs (clusters of four or eight leave 12 idle), and the benchmark card, at its power cap, does
+// more work per joule on more SMs at a lower clock (README has the numbers).
 #include "hmc_dense_epilogue.cuh"
 
 namespace {
@@ -227,8 +229,8 @@ __device__ __forceinline__ int& producer_spare_in() {
 // share them, with maps whose boxes are that many rows high.
 template <int MODE, int NEXT, int DC, int CX, int CY>
 struct ResW {
-  // 64-byte rows (32 fp16 of contraction per k-block): four 32 KB stages beside the accumulator
-  // tile, so the TMA producer runs up to three k-blocks ahead of the tensor cores
+  // 64-byte rows (32 fp16 of contraction per k-block): five 32 KB stages beside the accumulator
+  // tile, so the TMA producer runs up to four k-blocks ahead of the tensor cores
   static constexpr int KIND = 1, RB = 64, MNA = 0, MNB = 0;
   static constexpr int CLUSTER = CX * CY;
   static constexpr int KE = RB / 2;
@@ -346,8 +348,9 @@ struct ResW {
 };
 
 // Cluster shape of the pass (CX dimension blocks x CY chain blocks) where the unit grid tiles by
-// it; other shapes run without clusters.
-constexpr int RES_CX = 2, RES_CY = 2;
+// it; other shapes run without clusters.  On a 700 W H100 2 x 1 (or 1 x 2) ran the benchmark's
+// pass faster than 1 x 1, 2 x 2, 2 x 4 and 4 x 2 (README).
+constexpr int RES_CX = 2, RES_CY = 1;
 
 template <int DC, int CX, int CY>
 int res_pass(const CUtensorMap& phi, const CUtensorMap& plo, const CUtensorMap& qhi,
@@ -495,6 +498,19 @@ int zsb_dense_res_h16_launch(void* planes0, void* planes1, void* spare0, void* s
   }
   return ZSB_OK;
 }
+
+#ifdef ZSB_PASS_PROFILE
+// Stall accounting build only (tc_common.cuh): copy the per-CTA counters of the dense pass
+// kernels, PASS_PROF_SLOTS per CTA for the first `ctas` CTAs, to `host` and clear them.
+extern "C" int zsb_pass_profile_read(unsigned long long* host, int ctas) {
+  if (ctas < 0 || ctas > PASS_PROF_CTAS) return ZSB_ERR_INVALID;
+  const size_t bytes = sizeof(unsigned long long) * PASS_PROF_SLOTS * (size_t)ctas;
+  if (cudaMemcpyFromSymbol(host, g_pass_prof, bytes) != cudaSuccess) return ZSB_ERR_CUDA;
+  static unsigned long long zeros[PASS_PROF_CTAS * PASS_PROF_SLOTS];
+  if (cudaMemcpyToSymbol(g_pass_prof, zeros, sizeof(zeros)) != cudaSuccess) return ZSB_ERR_CUDA;
+  return ZSB_OK;
+}
+#endif
 
 int zsb_dense_select_planes_launch(float* q, const void* planes, const void* spare,
                                    const float* record, const int32_t* accept, int64_t chains,

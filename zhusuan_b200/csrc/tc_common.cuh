@@ -37,17 +37,55 @@ constexpr int EPI_WARP0 = 5;
 constexpr int NUM_THREADS = 32 * (EPI_WARP0 + NUM_EPI_WARPS);   // 288
 constexpr int ACC_LD = BN + 4;                            // padded row: conflict-free float4 reads
 constexpr int ACC_BYTES = BM * ACC_LD * 4;                // 66 KB
-constexpr int STAGE_BUDGET = 128 * 1024;                  // operand ring
-constexpr long long WAIT_TIMEOUT_CYCLES = 4000000000LL;   // ~2 s: trap instead of hanging the box
+constexpr unsigned long long WAIT_TIMEOUT_NS = 2000000000ULL;   // 2 s: trap instead of hanging
 
-// operand ring of a product whose smem rows are RB bytes (128: SWIZZLE_128B, 64: SWIZZLE_64B)
+// Stall accounting of tc_pipeline_kernel (scripts/pass_stalls.py builds it; off in the shipped
+// library, whose tensor-core kernels read no cycle counter).  Each CTA adds the clock64() cycles
+// of its roles' waits into PASS_PROF_SLOTS counters of g_pass_prof[blockIdx.x], over every launch
+// until zsb_pass_profile_read (hmc_dense_res.cu) copies them out and clears them.
+enum PassProfSlot {
+  PROF_MMA_TOTAL,        // MMA warpgroup: first unit to the last accumulator store
+  PROF_MMA_FULL,         //   in mbar_spin(full) of the k-loop
+  PROF_MMA_TEMPTY,       //   in mbar_wait(tempty): the epilogue has not drained the tile yet
+  PROF_MMA_STORE,        //   storing the accumulator tile
+  PROF_PROD_EMPTY,       // producer: in mbar_wait(empty)
+  PROF_EPI_TFULL,        // epilogue warp 0: in mbar_wait(tfull)
+  PROF_EPI_UNIT,         //   in the epilogue of its units
+  PROF_UNITS,            // units of this CTA
+  PASS_PROF_SLOTS
+};
+constexpr int PASS_PROF_CTAS = 1024;
+#ifdef ZSB_PASS_PROFILE
+constexpr bool kPassProfile = true;
+__device__ unsigned long long g_pass_prof[PASS_PROF_CTAS * PASS_PROF_SLOTS];
+#else
+constexpr bool kPassProfile = false;
+#endif
+__device__ __forceinline__ long long prof_clock() {
+  if constexpr (kPassProfile) return clock64();
+  return 0;
+}
+__device__ __forceinline__ void prof_add(int slot, long long v) {
+#ifdef ZSB_PASS_PROFILE
+  if (blockIdx.x < PASS_PROF_CTAS)
+    atomicAdd(&g_pass_prof[blockIdx.x * PASS_PROF_SLOTS + slot], (unsigned long long)v);
+#endif
+}
+
+// operand ring of a product whose smem rows are RB bytes (128: SWIZZLE_128B, 64: SWIZZLE_64B).
+// With 64-byte rows the ring takes five 32 KB stages: 160 KB beside the accumulator tile, the
+// barriers and the 512 B that aligning a SWIZZLE_64B ring may cost, within the 227 KB of shared
+// memory a CTA may have.  The stall accounting of the dense pass (scripts/pass_stalls.py) showed
+// its MMA warpgroup waiting on full stages for over a third of its cycles with four.
 template <int RB>
 struct Cfg {
   static constexpr int A_TILE = BM * RB;
   static constexpr int B_TILE = BN * RB;
   static constexpr int STAGE = 2 * A_TILE + 2 * B_TILE;      // hi + lo planes of A and B
-  static constexpr int STAGES = STAGE_BUDGET / STAGE;        // 2 (RB 128) / 4 (RB 64)
-  static constexpr int SMEM = STAGES * STAGE + ACC_BYTES + 128 + 1024;
+  static constexpr int STAGES = RB == 128 ? 2 : 5;
+  static constexpr int ALIGN = RB == 128 ? 1024 : 512;       // the swizzle pattern's period
+  static constexpr int SMEM = STAGES * STAGE + ACC_BYTES + 128 + ALIGN;
+  static_assert(SMEM <= 227 * 1024, "operand ring exceeds shared memory");
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -74,12 +112,18 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// no printf on timeout: a call anywhere in the kernel would serialise the wgmma pipeline
+__device__ __forceinline__ unsigned long long global_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+// no printf on timeout: a call anywhere in the kernel would serialise the wgmma pipeline.  The
+// timeout runs on the global timer, so that the cycle counter is read only by the stall accounting
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
+  const unsigned long long t0 = global_ns();
   while (!mbar_try_wait(bar, parity))
-    if (clock64() - t0 > WAIT_TIMEOUT_CYCLES) __trap();
+    if (global_ns() - t0 > WAIT_TIMEOUT_NS) __trap();
 }
 // Wait without a timeout, for the MMA warpgroup's full-barrier wait inside the k-loop.  A trap
 // path there, with wgmma accumulators in flight, makes ptxas wait for every wgmma before the next
@@ -261,7 +305,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
   using C = Cfg<W::RB>;
   constexpr int CS = ClusterOf<W>::value;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t smem_base = (smem_u32(smem_raw) + (C::ALIGN - 1)) & ~(uint32_t)(C::ALIGN - 1);
   const uint32_t acc_base = smem_base + C::STAGES * C::STAGE;
   const uint32_t bars = acc_base + ACC_BYTES;
   const uint32_t full_bar = bars;                          // [STAGES]
@@ -305,6 +349,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
     float d[2][64];
     int stage = 0;
     uint32_t phase = 0, acc_phase = 0;
+    const long long t_begin = prof_clock();
+    long long t_full = 0, t_tempty = 0, t_store = 0, units = 0;
     for (int64_t u = blockIdx.x; u < n_units; u += gridDim.x) {
       int kb0, kb1;
       w.kb_range(u, kb0, kb1);
@@ -315,7 +361,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
       int prev = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         const uint32_t sa = smem_base + stage * C::STAGE;
+        const long long t0 = prof_clock();
         mbar_spin(full_bar + 8 * stage, phase);
+        t_full += prof_clock() - t0;
         wgmma_fence();
         mma_kblock<W::KIND, W::RB, W::MNA, W::MNB, ZloOf<W>::value>(d, sa);
         wgmma_commit();
@@ -326,7 +374,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
       }
       wgmma_wait<0>();
       if (prev >= 0 && tid == 0) release(prev);
+      const long long t1 = prof_clock();
       mbar_wait(tempty_bar, acc_phase ^ 1);           // epilogue drained the previous unit
+      const long long t2 = prof_clock();
+      t_tempty += t2 - t1;
       const int row = 16 * (tid >> 5) + ((tid & 31) >> 2);
       const int col = 2 * (tid & 3);
 #pragma unroll
@@ -341,6 +392,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
         }
       mbar_arrive(tfull_bar);
       acc_phase ^= 1;
+      t_store += prof_clock() - t2;
+      ++units;
+    }
+    if (kPassProfile && tid == 0) {
+      prof_add(PROF_MMA_TOTAL, prof_clock() - t_begin);
+      prof_add(PROF_MMA_FULL, t_full);
+      prof_add(PROF_MMA_TEMPTY, t_tempty);
+      prof_add(PROF_MMA_STORE, t_store);
+      prof_add(PROF_UNITS, units);
     }
   } else if (warp == PRODUCER_WARP) {
     // ===================== TMA producer =====================
@@ -348,17 +408,21 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
       w.prefetch();
       int stage = 0;
       uint32_t phase = 0;
+      long long t_empty = 0;
       for (int64_t u = blockIdx.x; u < n_units; u += gridDim.x) {
         int kb0, kb1;
         w.kb_range(u, kb0, kb1);
         for (int kb = kb0; kb < kb1; ++kb) {
+          const long long t0 = prof_clock();
           mbar_wait(empty_bar + 8 * stage, phase ^ 1);
+          t_empty += prof_clock() - t0;
           const uint32_t fb = full_bar + 8 * stage;
           mbar_expect_tx(fb, W::TX);
           w.load(u, kb, smem_base + stage * C::STAGE, fb);
           if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
         }
       }
+      if (kPassProfile) prof_add(PROF_PROD_EMPTY, t_empty);
     }
   } else {
     // ===================== epilogue =====================
@@ -366,12 +430,21 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
     const uint32_t trow = acc_base + (uint32_t)((quarter * 32 + lane) * ACC_LD * 4);
     typename W::EpiState st;
     uint32_t acc_phase = 0;
+    long long t_tfull = 0, t_unit = 0;
     for (int64_t u = blockIdx.x; u < n_units; u += gridDim.x) {
+      const long long t0 = prof_clock();
       mbar_wait(tfull_bar, acc_phase);
+      const long long t1 = prof_clock();
       w.epilogue(u, trow, quarter, lane, st);
       __syncwarp();
       mbar_arrive(tempty_bar);
       acc_phase ^= 1;
+      t_tfull += t1 - t0;
+      t_unit += prof_clock() - t1;
+    }
+    if (kPassProfile && quarter == 0 && lane == 0) {
+      prof_add(PROF_EPI_TFULL, t_tfull);
+      prof_add(PROF_EPI_UNIT, t_unit);
     }
     w.epi_finish(st, quarter, lane);
   }
