@@ -167,11 +167,10 @@ int zsb_linear_tc_kpad(int K);
 int zsb_linear_tc_nparts(int J);
 int zsb_split16_pad_f32(const float* src, int64_t rows, int K, void* planes, float* scale,
                         void* stream);
-/* src [R, C] -> planes [2][C][kpad(R)] of src^T (operands of the weight-gradient product) */
-int zsb_split16_pad_t_f32(const float* src, int64_t R, int C, void* planes, float* scale,
-                          void* stream);
-/* split-K slices an epi-0 launch uses when `part` (slices * R * J floats) is supplied */
+/* split-K slices of the weight-gradient product zsb_linear_tc_wgrad_f32 with R output rows, J
+ * features and contraction length K (its `part` holds slices * R * J floats) */
 int zsb_linear_tc_slices(int64_t R, int J, int K);
+/* `part` is read by epi 1 only */
 int zsb_linear_tc_f32(int epi, const void* w_planes, const float* scale_w, const void* h_planes,
                       const float* scale_h, const float* bias, const float* x_obs, int64_t n_x,
                       const float* gout, float* out, float* part, int64_t R, int J, int K,
@@ -183,25 +182,13 @@ int zsb_linear_tc_amax_f32(int epi, const void* w_planes, const float* scale_w,
                            const float* x_obs, int64_t n_x, const float* gout, float* out,
                            float* part, int64_t R, int J, int K, int relu, float* amax_scale,
                            void* stream);
-/* Both operand layouts of an activation / gradient matrix in one pass: planes [2][R][Kp] and
- * planes_t [2][K][Rp] (either may be NULL) of src * scale, optionally times the ReLU mask
- * (mask_src > 0) -- the `g * (y > 0)` of the dense layer's backward (tf.layers.dense + relu,
- * iwae.py:23-44) -- and the column sums of the masked matrix (bias gradient) into col_sum. */
+/* The operand planes of an activation / gradient matrix in one pass: planes [2][R][Kp] of
+ * src * scale, optionally times the ReLU mask (mask_src > 0) -- the `g * (y > 0)` of the dense
+ * layer's backward (tf.layers.dense + relu, iwae.py:23-44) -- and the column sums of the masked
+ * matrix (bias gradient) into col_sum (may be NULL).  K must be even. */
 int zsb_split16_dual_f32(const float* src, const float* mask_src, int64_t R, int K, void* planes,
-                         void* planes_t, float* col_sum, float* scale, int have_amax,
-                         void* stream);
+                         float* col_sum, float* scale, int have_amax, void* stream);
 
-/* Backward of the fused Bernoulli likelihood layer (gradient of epi 1 wrt the logits, epi 2)
- * emitted directly as the operand planes of the two backward products: dl_planes [2][R][kpad(J)]
- * = fp16 hi/lo of gout[r] * (x - sigmoid(logits)) * scale_out[0], col_sum [J] += its column sums
- * (bias gradient, may be NULL).  scale_out = device float[4], zeroed once by the caller; the power
- * of two follows from max|gout| * (1 + max|x_obs|) >= max|dl| BEFORE the GEMM, so the fp32
- * dl matrix (822 MB at config 3: univariate.py:398-403 differentiated) never exists. */
-int zsb_linear_tc_bern_grad_planes_f32(const void* w_planes, const float* scale_w,
-                                       const void* h_planes, const float* scale_h,
-                                       const float* bias, const float* x_obs, int64_t n_x,
-                                       const float* gout, void* dl_planes, float* col_sum,
-                                       float* scale_out, int64_t R, int J, int K, void* stream);
 /* Input gradient of the dense layer, dh [R, K] = g W = sum_j g[r, j] * W[j, k] (tf.gradients of
  * tf.layers.dense w.r.t. its input), with operand A = the FORWARD planes of W [J, K]
  * (w_planes [2][J][kpad(K)], read MN-major) and B = g_planes [2][R][kpad(J)]: no W^T copy.

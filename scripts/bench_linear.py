@@ -41,9 +41,7 @@ def main():
         flops = 2.0 * R * K * J
         t = {}
         t["split_h"] = timeit(lambda: Fz._tc_split(h))
-        t["split_t_h"] = timeit(lambda: Fz._tc_split_t(h))
         t["split_gy"] = timeit(lambda: Fz._tc_split(gy))
-        t["split_t_gy"] = timeit(lambda: Fz._tc_split_t(gy))
         t["gemm_epi0_store"] = timeit(lambda: Fz._tc_linear(0, wp, ws, hp, hs, b, None, None, R, J, K, True))
         t["gemm_epi1_bernoulli"] = timeit(lambda: Fz._tc_linear(1, wp, ws, hp, hs, b, x, None, R, J, K))
         t["gemm_epi2_dlogits"] = timeit(lambda: Fz._tc_linear(2, wp, ws, hp, hs, b, x, g, R, J, K))

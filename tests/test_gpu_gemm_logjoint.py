@@ -51,8 +51,8 @@ def test_linear_forward_fp32_accuracy(zs, R, K, J, relu):
 @pytest.mark.parametrize("R,K,J,relu", [(5000, 500, 784, True), (300, 40, 500, False),
                                         (70000, 64, 50, True)])
 def test_linear_backward_on_tensor_cores(zs, R, K, J, relu):
-    """dh = g W and dW = g^T h (transposed operand planes, split-K over the CTA pairs, ragged
-    contraction length) and db against float64."""
+    """dh = g W and dW = g^T h (row-major operand planes read MN-major, split-K over the CTA pairs,
+    ragged contraction length) and db against float64."""
     rng = np.random.RandomState(R + J)
     h = rng.standard_normal((R, K)).astype(np.float32)
     W = (rng.standard_normal((J, K)) / np.sqrt(K)).astype(np.float32)
@@ -72,13 +72,36 @@ def test_linear_backward_on_tensor_cores(zs, R, K, J, relu):
         assert np.quantile(err, 0.999) < 3e-6 and got.shape == want.shape
 
 
+def test_bias_gradient_alone(zs):
+    """Only the bias asks for a gradient: the split pass of the backward still runs, and its column
+    sums are db, for the ReLU dense layer and for the Bernoulli likelihood layer."""
+    rng = np.random.RandomState(11)
+    R, K, J = 300, 40, 64
+    h = rng.standard_normal((R, K)).astype(np.float32)
+    W = (rng.standard_normal((J, K)) / np.sqrt(K)).astype(np.float32)
+    b = (0.1 * rng.standard_normal(J)).astype(np.float32)
+    gy = rng.standard_normal((R, J)).astype(np.float32)
+    x = (rng.random_sample((R, J)) < 0.3).astype(np.float32)
+    w = rng.standard_normal(R).astype(np.float32)
+    pre = h.astype(np.float64) @ W.astype(np.float64).T + b
+    tb = T(b).requires_grad_(True)
+    db, = torch.autograd.grad((zs.fused.linear(T(h), T(W), tb, relu=True) * T(gy)).sum(), [tb])
+    g = gy * (pre > 0)
+    np.testing.assert_allclose(N(db), g.sum(0), rtol=0, atol=3e-6 * np.abs(g).sum(0).max())
+    lp = zs.fused.linear_bernoulli_log_prob(T(h), T(W), tb, T(x))
+    db, = torch.autograd.grad((lp * T(w)).sum(), [tb])
+    g = w[:, None] * (x - 1 / (1 + np.exp(-pre)))
+    np.testing.assert_allclose(N(db), g.sum(0), rtol=0, atol=3e-6 * np.abs(g).sum(0).max())
+
+
 @pytest.mark.parametrize("R,K,J", [(1000, 500, 784), (63, 1, 5), (4097, 130, 257), (64, 64, 128),
                                    (20000, 40, 500)])
-def test_weight_gradient_from_row_major_planes(zs, R, K, J):
+def test_weight_gradient_from_row_major_planes_vs_forward_product(zs, R, K, J):
     """zsb_linear_tc_wgrad_f32: dW = g^T h with both operands read as MN-major wgmma operands
-    from the ROW-MAJOR planes (no transposed copy) against float64 and against the transposed-plane
-    product of zsb_linear_tc_f32; ragged contraction length (TMA zero fill of the last 64-row box),
-    odd / tiny widths, feature counts that are not multiples of the 64-column box."""
+    from the ROW-MAJOR planes (no transposed copy) against float64 and against the K-major forward
+    product of zsb_linear_tc_f32 on the planes of explicit transposes; ragged contraction length
+    (TMA zero fill of the last 64-row box), odd / tiny widths, feature counts that are not
+    multiples of the 64-column box."""
     from zhusuan_b200 import fused
     from zhusuan_b200._lib import lib, ptr, stream
     rng = np.random.RandomState(R + K + J)
@@ -94,11 +117,10 @@ def test_weight_gradient_from_row_major_planes(zs, R, K, J):
     want = g.astype(np.float64).T @ h.astype(np.float64)
     scale = np.abs(g).astype(np.float64).T @ np.abs(h).astype(np.float64)
     assert np.max(np.abs(N(out) - want) / (scale + 1e-30)) < 3e-6
-    # the transposed-plane scheme (round 2) computes the same products
-    hpt, hst = fused._tc_split_t(T(h))
-    gpt, gst = fused._tc_split_t(T(g))
-    old = fused._tc_linear(0, hpt, hst, gpt, gst, None, None, None, J, K, R, split_k=True)
-    np.testing.assert_allclose(N(out), N(old), rtol=0, atol=3e-6 * float(scale.max()))
+    # the forward product on the planes of g^T [J, R] and h^T [K, R] is dW^T [K, J]
+    fwd = fused._tc_linear(0, *fused._tc_split(T(g).t()), *fused._tc_split(T(h).t()), None, None,
+                           None, K, J, R)
+    np.testing.assert_allclose(N(out), N(fwd).T, rtol=0, atol=3e-6 * float(scale.max()))
 
 
 @pytest.mark.parametrize("P,Nb,K,J", [(3, 100, 500, 784), (1, 64, 40, 20), (2, 257, 96, 130)])
@@ -156,46 +178,6 @@ def test_input_gradient_from_the_forward_weight_planes(zs, R, K, J):
     wtp, wts = fused._tc_split(tW.t())
     old = fused._tc_linear(0, wtp, wts, gp, gs, None, None, None, R, K, J)
     np.testing.assert_allclose(N(out), N(old), rtol=0, atol=3e-6 * float(scale.max()))
-
-
-@pytest.mark.parametrize("R,Nb,K,J,xmax", [(700, 100, 500, 784, 1.0), (64, 64, 40, 21, 1.0),
-                                            (515, 103, 96, 130, 3.5), (256, 256, 64, 64, 0.0)])
-def test_bernoulli_gradient_planes_from_the_epilogue(zs, R, Nb, K, J, xmax):
-    """zsb_linear_tc_bern_grad_planes_f32 (epi 3): the d/dlogits of the Bernoulli layer leaves
-    the GEMM as fp16 hi/lo operand planes with the a-priori scale max|g| * (1 + max|x|):
-    (hi + lo) / scale reproduces the fp32 epi-2 matrix to 2^-22 of the bound, pad columns are
-    zero, the column sums are the bias gradient, nothing overflows for x outside [0, 1]."""
-    from zhusuan_b200 import fused
-    from zhusuan_b200._lib import lib, ptr, stream
-    rng = np.random.RandomState(R + J)
-    h = np.maximum(rng.standard_normal((R, K)), 0).astype(np.float32)
-    W = (rng.standard_normal((J, K)) * 2 / np.sqrt(K)).astype(np.float32)
-    b = (0.3 * rng.standard_normal(J)).astype(np.float32)
-    x = ((rng.random_sample((Nb, J)) < 0.3) * xmax).astype(np.float32)
-    g = (rng.standard_normal(R) * 1e-4).astype(np.float32)
-    wp, ws = fused._tc_split(T(W))
-    hp, hs = fused._tc_split(T(h))
-    tb, tx, tg = T(b), T(x), T(g)          # kept alive: the ABI takes raw device pointers
-    dl = fused._tc_linear(2, wp, ws, hp, hs, tb, tx, tg, R, J, K)             # fp32 epi 2
-    Jp = lib.load().zsb_linear_tc_kpad(J)
-    planes = torch.full((2, R, Jp), float("nan"), dtype=torch.float16, device="cuda")
-    scale = torch.zeros(4, device="cuda")
-    db = torch.zeros(J, device="cuda")
-    lib.call("zsb_linear_tc_bern_grad_planes_f32", ptr(wp), ptr(ws), ptr(hp), ptr(hs), ptr(tb),
-             ptr(tx), Nb, ptr(tg), ptr(planes), ptr(db), ptr(scale), R, J, K, stream())
-    s = float(scale[0])
-    bound = float(np.abs(g).max()) * (1.0 + float(np.abs(x).max()))
-    assert 2.0 ** 11 <= bound * s < 2.0 ** 12 and np.log2(s) == np.round(np.log2(s))
-    pl = N(planes.float())
-    assert np.isfinite(pl).all()
-    np.testing.assert_array_equal(pl[:, :, J:], 0.0)
-    rec = (pl[0].astype(np.float64) + pl[1]) / s
-    np.testing.assert_allclose(rec[:, :J], N(dl), rtol=0, atol=2.0 ** -21 * bound)
-    logits = h.astype(np.float64) @ W.astype(np.float64).T + b
-    want = g[:, None] * (np.tile(x, (R // Nb, 1)) - 1 / (1 + np.exp(-logits)))
-    np.testing.assert_allclose(rec[:, :J], want, rtol=0, atol=3e-6 * bound)
-    np.testing.assert_allclose(N(db), want.sum(0), rtol=0,
-                               atol=3e-6 * np.abs(want).sum(0).max() + 1e-12)
 
 
 def test_linear_bernoulli_as_distribution_plugin(zs):

@@ -74,6 +74,20 @@ def test_no_cpu_fallback_and_error_string():
                       None, 0, 0, None)
 
 
+def test_no_environment_switches():
+    """What runs is chosen by arguments, never by the environment: no kernel source calls getenv
+    and no module of the package reads os.environ."""
+    csrc = os.path.join(ROOT, "zhusuan_b200", "csrc")
+    for f in sorted(os.listdir(csrc)):
+        if f.endswith((".cu", ".cuh")):
+            assert "getenv" not in open(os.path.join(csrc, f)).read(), f
+    for dirpath, _, files in os.walk(os.path.join(ROOT, "zhusuan_b200")):
+        for f in files:
+            if f.endswith(".py"):
+                s = open(os.path.join(dirpath, f)).read()
+                assert not re.search(r"\benviron\b|\bgetenv\b", s), os.path.join(dirpath, f)
+
+
 def test_product_does_not_import_oracle():
     for dirpath, _, files in os.walk(os.path.join(ROOT, "zhusuan_b200")):
         for f in files:

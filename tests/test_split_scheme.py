@@ -98,36 +98,3 @@ def test_trajectory_kernel_buffer_schedule_matches_the_per_pass_host_loop():
                 assert traj_nxt(i) == nxt
                 cur, nxt = nxt, (2 if nxt == 1 else 1)
         assert cur == (1 if (L - 1) % 2 == 0 else 2)
-
-
-def test_a_priori_scale_from_a_bound_is_equivalent_to_the_exact_scale():
-    """gemm_logjoint_tc.cu epi 3 takes the power-of-two scale of the d/dlogits planes from the
-    bound max|g| (1 + max|x|) >= max|g (x - sigmoid(l))| BEFORE the values exist.  A scale that is
-    too small by up to 2^8 leaves the split matmul at fp32-GEMM accuracy: the hi plane keeps its 11
-    bits, the lo plane only loses bits below an ABSOLUTE floor of 2^-25 in scaled units, i.e.
-    2^-25 / 2^(12 - 8) = 2^-29 of the maximum -- far below the 2^-22 of the dropped lo*lo term."""
-    rng = np.random.RandomState(5)
-    m, n, k = 48, 40, 784
-    g = (rng.standard_normal((m, 1)) * 1e-5).astype(np.float32)
-    x = (rng.random_sample((m, k)) < 0.3).astype(np.float32)
-    sig = 1 / (1 + np.exp(-rng.standard_normal((m, k)) * 4))
-    a = (g * (x - sig)).astype(np.float32)                      # the d/dlogits matrix
-    b = (rng.standard_normal((n, k)) / np.sqrt(k)).astype(np.float32)
-    exact = a.astype(np.float64) @ b.astype(np.float64).T
-    scale = np.abs(a).astype(np.float64) @ np.abs(b).astype(np.float64).T
-    bh, bl, sb = split(b)
-    f = lambda t: t.astype(np.float32)
-    errs = {}
-    for loose in (0, 1, 4, 8):                                  # bound / max|a| = 2^loose
-        sa = pow2_scale(a) / np.float32(2.0 ** loose)
-        xs = a * sa
-        ah = xs.astype(np.float16)
-        al = (xs - f(ah)).astype(np.float16)
-        assert np.isfinite(f(ah)).all()
-        acc = (f(al) @ f(bh).T + f(ah) @ f(bl).T + f(ah) @ f(bh).T) / (sa * sb)
-        errs[loose] = float(np.max(np.abs(acc - exact) / scale))
-    assert max(errs.values()) < 2e-6, errs
-    assert errs[8] < 2 * max(errs[0], 2.0 ** -22), errs
-    # the bound itself: never exceeded, at most 2x loose for binary observations
-    bound = float(np.abs(g).max()) * (1.0 + float(np.abs(x).max()))
-    assert np.abs(a).max() <= bound <= 2.0 ** 8 * np.abs(a).max()

@@ -197,8 +197,7 @@ int launch_row_reduce4(float* out, int64_t n_out, int64_t group, Ops3 ops, F f, 
   bool vec = side_ok && group % 4 == 0;
   for (int o = 0; o < NOPS && vec; ++o)
     vec = ops.n[o] == 1 || (ops.n[o] % group == 0 && aligned16(ops.p[o]));
-  static const bool off = getenv("ZSB_NO_VEC4") != nullptr;
-  if (!vec || off) return launch_row_reduce<NOPS>(out, n_out, group, ops, f, st, what);
+  if (!vec) return launch_row_reduce<NOPS>(out, n_out, group, ops, f, st, what);
   int lanes = 1;
   while (lanes < 32 && lanes * 8 <= group) lanes <<= 1;      // >= 4 elements per lane
   const int rows_per_block = 256 / lanes;

@@ -9,10 +9,6 @@
 //          = Bernoulli(logits = l).log_prob(x) summed over the feature axis (univariate.py:398-403
 //            + group_ndims = 1, base.py:303-304) once the partial rows are added up
 //   EPI 2  out[r, j] = g[r] * (x - sigmoid(l))                   d(sum_r g[r] * log_prob[r]) / dl
-//   EPI 3  the EPI 2 values, emitted directly as the fp16 hi/lo operand planes [2][R][Jp] of the
-//          two backward products (dh = dl W, dW = dl^T h) plus their column sums (bias gradient):
-//          the fp32 dl matrix (822 MB at config 3) is never written or re-read.  The planes' scale
-//          is known BEFORE the GEMM: |dl| <= max|g| * (1 + max|x|)  (sigmoid in (0, 1)).
 //
 // fp32 accuracy on fp16 tensor cores: both operands are pre-split into scaled fp16 hi + lo planes
 // (zsb_split16_pad_f32), three fp16 wgmma products per k-step accumulate hi*hi + hi*lo + lo*hi
@@ -43,7 +39,6 @@ constexpr float BIN_SCALE = 2048.f;
 // A = the FORWARD planes of W [J, K] (no W^T copy): no product of a dense layer needs a transposed
 // copy of anything.  A stage then holds, per plane, two TMA boxes of 64 contraction rows x 64
 // features (128-byte rows, SWIZZLE_128B; see gmma_desc).  `Kp` is the padded contraction length.
-// GL: the epi 2 / 3 epilogues load the upstream gradient per row instead of broadcasting it.
 // ZLO: bit 0 / 1 = the lo plane of operand A / B is zero (a 0/1 sample, see mma_kblock): it is
 // neither loaded nor multiplied.
 //
@@ -54,7 +49,7 @@ constexpr float BIN_SCALE = 2048.f;
 //          of log Bernoulli(l).log_prob(h) ([nparts][S R])
 //   EPI 5  the epi-1 partial rows of the given samples x[s R + r] against logit row r
 //   EPI 6  out[r, j] = sum_s g[s R + r] * (x[s R + r, j] - sigmoid(l))     (d/dl of EPI 5)
-template <int EPI, int MN, int GL, int Z = 0>
+template <int EPI, int MN, int Z = 0>
 struct LinW {
   static constexpr int KIND = 1, RB = 128, MNA = MN & 1, MNB = (MN >> 1) & 1, ZLO = Z;
   static constexpr uint32_t TX = Cfg<RB>::STAGE - ((Z & 1) ? Cfg<RB>::A_TILE : 0) -
@@ -210,10 +205,6 @@ struct LinW {
                                                 EpiState& st) const {
     float& amax = st.amax;   // max |stored output| (EPI 0 / 2): the consumer's fp16-split scale
     const float acc_scale = 1.f / (scale_w[0] * scale_h[0]);   // powers of two: exact
-    // EPI 3: `out` = the fp16 plane pair [2][R][Jp_out], amax_scale[0] = their (a-priori) scale
-    __half* __restrict__ pl_out = reinterpret_cast<__half*>(out);
-    const int Jp_out = ((J + 63) / 64) * 64;
-    const float s_out = (EPI == 3) ? amax_scale[0] : 1.f;
     const int64_t u = uu % n_tiles;
     const int slice = (int)(uu / n_tiles);
     const bool empty_slice = slice * kb_per >= n_kb_all;   // accumulator never written
@@ -225,102 +216,72 @@ struct LinW {
     const int64_t r0 = (u / n_blk) * BN;
     const int64_t part_row = (int64_t)(nb * 4 + quarter) * R;
     const float b_use = (slice == 0) ? b_j : 0.f;           // bias once across the slices
-      const bool warp_j_ok = __all_sync(0xffffffffu, j_ok);
-      float csum = 0.f;                                       // EPI 3: column sum of this lane's j
-      // observations of one 16-column block (rows rbase .. rbase+15, this lane's feature j); all
-      // 16 loads are issued back to back, one block AHEAD of their use (L2 latency ~1 us)
-      auto load_x = [&](float* xe, float& ge, int c) {
-        if (EPI == 0) return;
-        const int64_t rbase = r0 + c;
-        if (rbase >= R) return;                     // warp-uniform
-        int64_t xr = rbase % n_x;
-        const float* __restrict__ xp = x_obs + xr * J + j;
-        const bool full = warp_j_ok && rbase + 16 <= R;
-        if (full && xr + 16 <= n_x) {               // common case: no wrap, no predicates
+    const bool warp_j_ok = __all_sync(0xffffffffu, j_ok);
+    // observations of one 16-column block (rows rbase .. rbase+15, this lane's feature j); all
+    // 16 loads are issued back to back, one block AHEAD of their use (L2 latency ~1 us)
+    auto load_x = [&](float* xe, float& ge, int c) {
+      if (EPI == 0) return;
+      const int64_t rbase = r0 + c;
+      if (rbase >= R) return;                     // warp-uniform
+      int64_t xr = rbase % n_x;
+      const float* __restrict__ xp = x_obs + xr * J + j;
+      const bool full = warp_j_ok && rbase + 16 <= R;
+      if (full && xr + 16 <= n_x) {               // common case: no wrap, no predicates
 #pragma unroll
-          for (int jj = 0; jj < 16; ++jj) xe[jj] = __ldg(xp + (uint32_t)jj * (uint32_t)J);
-        } else {
-#pragma unroll
-          for (int jj = 0; jj < 16; ++jj) {
-            xe[jj] = (j_ok && rbase + jj < R) ? __ldg(xp) : 0.f;
-            if (++xr == n_x) { xr = 0; xp = x_obs + j; } else xp += J;
-          }
-        }
-        // upstream gradient of the 16 rows: lane jj holds gout[rbase + jj] (GL = 0: broadcast by
-        // shuffle in process(); GL = 1: process() loads it itself, warp-uniform addresses)
-        if (EPI >= 2 && !GL) ge = (lane < 16 && rbase + lane < R) ? __ldg(gout + rbase + lane) : 0.f;
-      };
-      auto process = [&](const uint32_t* v, const float* xe, float ge, int c) {
-        // NO early return for rbase >= R: every access below is predicated on the row anyway, and
-        // a return here (uniform, but not provably so) makes the compiler wrap each warp shuffle of
-        // the row sums in a WARPSYNC.COLLECTIVE sequence (125 SHFL + 70 WARPSYNC -> 63 SHFL)
-        const int64_t rbase = r0 + c;
-        float lpv[16];
-        float* __restrict__ po = (EPI == 0 || EPI == 2) ? out_s + rbase * J + j : nullptr;
-        const bool full = warp_j_ok && rbase + 16 <= R;   // no per-element predicates
+        for (int jj = 0; jj < 16; ++jj) xe[jj] = __ldg(xp + (uint32_t)jj * (uint32_t)J);
+      } else {
 #pragma unroll
         for (int jj = 0; jj < 16; ++jj) {
-          const bool ok = full || (j_ok && rbase + jj < R);
-          const float l = empty_slice ? b_use : fmaf(__uint_as_float(v[jj]), acc_scale, b_use);
-          if (EPI == 0) {
-            const float y = relu ? fmaxf(l, 0.f) : l;
-            if (ok) { *po = y; amax = fmaxf(amax, fabsf(y)); }
-          } else if (EPI == 1) {
-            lpv[jj] = ok ? bern_lp(xe[jj], l) : 0.f;
-          } else if (EPI == 2) {
-            const float g = GL ? ((full || rbase + jj < R) ? __ldg(gout + rbase + jj) : 0.f)
-                               : __shfl_sync(0xffffffffu, ge, jj);
-            const float y = g * (xe[jj] - __fdividef(1.f, 1.f + __expf(-l)));
-            if (ok) { *po = y; amax = fmaxf(amax, fabsf(y)); }
-          } else {
-            const float g = GL ? ((full || rbase + jj < R) ? __ldg(gout + rbase + jj) : 0.f)
-                               : __shfl_sync(0xffffffffu, ge, jj);
-            const float y = ok ? g * (xe[jj] - __fdividef(1.f, 1.f + __expf(-l))) : 0.f;
-            csum += y;
-            lpv[jj] = y * s_out;
-          }
-          if (EPI == 0 || EPI == 2) po += J;
+          xe[jj] = (j_ok && rbase + jj < R) ? __ldg(xp) : 0.f;
+          if (++xr == n_x) { xr = 0; xp = x_obs + j; } else xp += J;
         }
-        if (EPI == 3) {
-          // fp16 hi/lo planes of this lane's feature column, two rows per packed conversion;
-          // a warp instruction stores 64 contiguous bytes of one plane row
-          __half* __restrict__ ph = pl_out + rbase * Jp_out + j;
-          __half* __restrict__ pq = ph + R * (int64_t)Jp_out;
-          const bool col_ok = j < Jp_out;
-#pragma unroll
-          for (int jj = 0; jj < 16; jj += 2) {
-            const __half2 h2 = __floats2half2_rn(lpv[jj], lpv[jj + 1]);
-            const float2 hf = __half22float2(h2);
-            const __half2 l2 = __floats2half2_rn(lpv[jj] - hf.x, lpv[jj + 1] - hf.y);
-            if (col_ok && (full || rbase + jj < R)) {
-              ph[(size_t)jj * (size_t)Jp_out] = __low2half(h2);
-              pq[(size_t)jj * (size_t)Jp_out] = __low2half(l2);
-            }
-            if (col_ok && (full || rbase + jj + 1 < R)) {
-              ph[(size_t)(jj + 1) * (size_t)Jp_out] = __high2half(h2);
-              pq[(size_t)(jj + 1) * (size_t)Jp_out] = __high2half(l2);
-            }
-          }
-        }
-        if (EPI == 1) {
-          const float sum = warp_transpose_sum16(lpv, lane);
-          if (lane < 16 && rbase + lane < R) part[part_row + rbase + lane] = sum;
-        }
-      };
-      // the observation loads of block i+1 are in flight while block i is processed
-      uint32_t va[16], vb[16];
-      float xa[EPI ? 16 : 1], xb[EPI ? 16 : 1], ga = 0.f, gb = 0.f;
-      load_x(xa, ga, 0);
-#pragma unroll 1
-      for (int c = 0; c < BN; c += 32) {
-        load_x(xb, gb, c + 16);
-        acc_ld16(trow + 4u * (uint32_t)c, va);
-        process(va, xa, ga, c);
-        if (c + 32 < BN) load_x(xa, ga, c + 32);
-        acc_ld16(trow + 4u * (uint32_t)(c + 16), vb);
-        process(vb, xb, gb, c + 16);
       }
-      if (EPI == 3 && part && j_ok) atomicAdd(part + j, csum);   // bias gradient (part = col_sum)
+      // upstream gradient of the 16 rows: lane jj holds gout[rbase + jj], broadcast by shuffle
+      // in process()
+      if (EPI == 2) ge = (lane < 16 && rbase + lane < R) ? __ldg(gout + rbase + lane) : 0.f;
+    };
+    auto process = [&](const uint32_t* v, const float* xe, float ge, int c) {
+      // NO early return for rbase >= R: every access below is predicated on the row anyway, and
+      // a return here (uniform, but not provably so) makes the compiler wrap each warp shuffle of
+      // the row sums in a WARPSYNC.COLLECTIVE sequence (125 SHFL + 70 WARPSYNC -> 63 SHFL)
+      const int64_t rbase = r0 + c;
+      float lpv[16];
+      float* __restrict__ po = (EPI == 0 || EPI == 2) ? out_s + rbase * J + j : nullptr;
+      const bool full = warp_j_ok && rbase + 16 <= R;   // no per-element predicates
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+        const bool ok = full || (j_ok && rbase + jj < R);
+        const float l = empty_slice ? b_use : fmaf(__uint_as_float(v[jj]), acc_scale, b_use);
+        if (EPI == 0) {
+          const float y = relu ? fmaxf(l, 0.f) : l;
+          if (ok) { *po = y; amax = fmaxf(amax, fabsf(y)); }
+        } else if (EPI == 1) {
+          lpv[jj] = ok ? bern_lp(xe[jj], l) : 0.f;
+        } else {
+          const float g = __shfl_sync(0xffffffffu, ge, jj);
+          const float y = g * (xe[jj] - __fdividef(1.f, 1.f + __expf(-l)));
+          if (ok) { *po = y; amax = fmaxf(amax, fabsf(y)); }
+        }
+        if (EPI == 0 || EPI == 2) po += J;
+      }
+      if (EPI == 1) {
+        const float sum = warp_transpose_sum16(lpv, lane);
+        if (lane < 16 && rbase + lane < R) part[part_row + rbase + lane] = sum;
+      }
+    };
+    // the observation loads of block i+1 are in flight while block i is processed
+    uint32_t va[16], vb[16];
+    float xa[EPI ? 16 : 1], xb[EPI ? 16 : 1], ga = 0.f, gb = 0.f;
+    load_x(xa, ga, 0);
+#pragma unroll 1
+    for (int c = 0; c < BN; c += 32) {
+      load_x(xb, gb, c + 16);
+      acc_ld16(trow + 4u * (uint32_t)c, va);
+      process(va, xa, ga, c);
+      if (c + 32 < BN) load_x(xa, ga, c + 32);
+      acc_ld16(trow + 4u * (uint32_t)(c + 16), vb);
+      process(vb, xb, gb, c + 16);
+    }
   }
   __device__ __forceinline__ void epi_finish(EpiState& st, int, int lane) const {
     if ((EPI == 0 || EPI == 2 || EPI == 6) && amax_scale) {   // NaN / inf never win (fmaxf drops NaN)
@@ -332,33 +293,32 @@ struct LinW {
 };
 
 // one product on the tensor cores: A = w planes (J_ features), B = h planes (R rows)
-template <int EPI, int MN, int GL, int Z = 0>
-LinW<EPI, MN, GL, Z> make_linw(const CUtensorMap& whi, const CUtensorMap& wlo,
-                               const CUtensorMap& hhi, const CUtensorMap& hlo, const float* bias,
-                               const float* x_obs, int64_t n_x, const float* gout, float* out,
-                               float* part, int64_t R, int J_, int Kp, int relu,
-                               const float* scale_w, const float* scale_h, int k_slices,
-                               float* amax_scale) {
+template <int EPI, int MN, int Z = 0>
+LinW<EPI, MN, Z> make_linw(const CUtensorMap& whi, const CUtensorMap& wlo,
+                           const CUtensorMap& hhi, const CUtensorMap& hlo, const float* bias,
+                           const float* x_obs, int64_t n_x, const float* gout, float* out,
+                           float* part, int64_t R, int J_, int Kp, int relu,
+                           const float* scale_w, const float* scale_h, int k_slices,
+                           float* amax_scale) {
   const int n_blk = (J_ + BM - 1) / BM;
   const int64_t n_tiles = ((R + BN - 1) / BN) * n_blk;
   const int n_kb_all = Kp / 64;
   const int kb_per = (n_kb_all + k_slices - 1) / k_slices;
-  LinW<EPI, MN, GL, Z> w{whi, wlo, hhi, hlo, bias, x_obs, n_x, gout, out, part, R, J_, Kp,
-                         relu, scale_w, scale_h, k_slices, amax_scale, n_blk, n_tiles,
-                         n_kb_all, kb_per};
+  LinW<EPI, MN, Z> w{whi, wlo, hhi, hlo, bias, x_obs, n_x, gout, out, part, R, J_, Kp,
+                     relu, scale_w, scale_h, k_slices, amax_scale, n_blk, n_tiles,
+                     n_kb_all, kb_per};
   w.S = 1;
   w.s_per = 1;
   return w;
 }
-template <int EPI, int MN, int GL, int Z = 0>
+template <int EPI, int MN, int Z = 0>
 int launch_linear(const CUtensorMap& whi, const CUtensorMap& wlo, const CUtensorMap& hhi,
                   const CUtensorMap& hlo, const float* bias, const float* x_obs, int64_t n_x,
                   const float* gout, float* out, float* part, int64_t R, int J_, int Kp, int relu,
                   const float* scale_w, const float* scale_h, int k_slices, float* amax_scale,
                   cudaStream_t st, const char* what) {
-  return tc_launch(make_linw<EPI, MN, GL, Z>(whi, wlo, hhi, hlo, bias, x_obs, n_x, gout, out, part,
-                                             R, J_, Kp, relu, scale_w, scale_h, k_slices,
-                                             amax_scale),
+  return tc_launch(make_linw<EPI, MN, Z>(whi, wlo, hhi, hlo, bias, x_obs, n_x, gout, out, part,
+                                         R, J_, Kp, relu, scale_w, scale_h, k_slices, amax_scale),
                    st, what);
 }
 
@@ -387,23 +347,22 @@ int linear_maps(const void* w_planes, const void* h_planes, int binary_h, int64_
   return make_map(&m[3], binary_h ? hp : hp + R * Kp, (uint64_t)R, (uint64_t)Kp, BN, 128, 1);
 }
 
-// One pass over an activation / gradient matrix that produces BOTH operand layouts of the dense
-// layers: src [R, K] fp32 (optionally times the ReLU mask (mask_src > 0)) ->
-//   planes   [2][R][Kp]  fp16 hi/lo of src * scale   (forward / input-gradient products)
-//   planes_t [2][K][Rp]  fp16 hi/lo of (src * scale)^T (weight-gradient product, contraction over R)
+// One pass over an activation / gradient matrix that produces its operand planes:
+// src [R, K] fp32 (optionally times the ReLU mask (mask_src > 0)) ->
+//   planes   [2][R][Kp]  fp16 hi/lo of src * scale   (the operand of all three products of a layer)
 //   col_sum  [K] += sum_r src[r, k] * mask           (the bias gradient; float atomics)
-// 64 x 64 tiles through shared memory; float2 loads, half2 stores in both layouts.
-__global__ void __launch_bounds__(256) split16_dual_kernel(
+// 64 x 64 tiles, float2 loads, half2 stores; the column sums of a tile meet in shared memory.
+// At most 32 registers, so that 8 blocks fill an SM: left free, ptxas takes 44 to hoist loads,
+// 5 blocks fit, and this memory-bound pass ran 7-16% slower (H100 SXM, 700 W).
+__global__ void __launch_bounds__(256, 8) split16_dual_kernel(
     const float* __restrict__ src, const float* __restrict__ mask_src, int64_t R, int K, int Kp,
-    int64_t Rp, __half* __restrict__ planes, __half* __restrict__ planes_t,
-    float* __restrict__ col_sum, const float* __restrict__ scale) {
-  __shared__ float tile[64][65];
+    __half* __restrict__ planes, float* __restrict__ col_sum, const float* __restrict__ scale) {
   __shared__ float csum[8][64];
   const float s = scale[0];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;        // 32 x 8
-  const int64_t r_tiles = (Rp + 63) / 64;
+  const int64_t r_tiles = (R + 63) / 64;
   const int c_tiles = (Kp + 63) / 64;
-  const int64_t n_pl = R * (int64_t)Kp, n_plt = (int64_t)K * Rp;
+  const int64_t n_pl = R * (int64_t)Kp;
   for (int64_t t = blockIdx.x; t < r_tiles * c_tiles; t += gridDim.x) {
     const int64_t r0 = (t / c_tiles) * 64;
     const int c0 = (int)(t % c_tiles) * 64;
@@ -411,8 +370,7 @@ __global__ void __launch_bounds__(256) split16_dual_kernel(
     float cs0 = 0.f, cs1 = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      const int rl = ty + 8 * i;
-      const int64_t r = r0 + rl;
+      const int64_t r = r0 + ty + 8 * i;
       float2 v = make_float2(0.f, 0.f);
       if (r < R && c < K) {                      // K is even: c + 1 < K as well
         v = *reinterpret_cast<const float2*>(src + r * K + c);
@@ -424,9 +382,7 @@ __global__ void __launch_bounds__(256) split16_dual_kernel(
       }
       cs0 += v.x; cs1 += v.y;
       v.x *= s; v.y *= s;
-      tile[rl][2 * tx] = v.x;
-      tile[rl][2 * tx + 1] = v.y;
-      if (planes && r < R && c < Kp) {
+      if (r < R && c < Kp) {
         const __half2 h = __floats2half2_rn(v.x, v.y);
         const float2 hf = __half22float2(h);
         *reinterpret_cast<__half2*>(planes + r * Kp + c) = h;
@@ -442,27 +398,11 @@ __global__ void __launch_bounds__(256) split16_dual_kernel(
       for (int i = 0; i < 8; ++i) a += csum[i][threadIdx.x];
       atomicAdd(col_sum + c0 + threadIdx.x, a);
     }
-    if (planes_t) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int kl = ty + 8 * i;
-        const int k = c0 + kl;
-        const int64_t r = r0 + 2 * tx;
-        if (k < K && r < Rp) {                   // Rp is a multiple of 64: r + 1 < Rp as well
-          const float x0 = tile[2 * tx][kl], x1 = tile[2 * tx + 1][kl];
-          const __half2 h = __floats2half2_rn(x0, x1);
-          const float2 hf = __half22float2(h);
-          *reinterpret_cast<__half2*>(planes_t + (int64_t)k * Rp + r) = h;
-          *reinterpret_cast<__half2*>(planes_t + n_plt + (int64_t)k * Rp + r) =
-              __floats2half2_rn(x0 - hf.x, x1 - hf.y);
-        }
-      }
-    }
     __syncthreads();
   }
 }
 
-// scale[0] = power of two s with max|src| * s in [2^11, 2^12); scale[2] = running max bits
+// scale[2] = running max |src| bits (atomicMax over the blocks; NaN and inf are skipped)
 __global__ void __launch_bounds__(256) absmax2_kernel(const float* __restrict__ src, int64_t n,
                                                       float* __restrict__ scale) {
   float m = 0.f;
@@ -475,64 +415,8 @@ __global__ void __launch_bounds__(256) absmax2_kernel(const float* __restrict__ 
   if ((threadIdx.x & 31) == 0)
     atomicMax(reinterpret_cast<unsigned int*>(scale) + 2, __float_as_uint(m));
 }
-// Ticketed variant (ZSB_ABSMAX_TICKET=1):
-// scale[0] = power of two s with max|src| * s in [2^11, 2^12); scale[2] = running max bits;
-// scale[1] = block ticket.  The LAST block to finish turns the maximum into scale[0] and clears
-// slots 1 and 2 again (no separate single-thread kernel; the slot must start zeroed).
-__global__ void __launch_bounds__(256) absmax2_ticket_kernel(const float* __restrict__ src, int64_t n,
-                                                      float* __restrict__ scale) {
-  __shared__ float wm[8];
-  float m = 0.f;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    const float a = fabsf(src[i]);
-    m = (a == a && a <= 3.0e38f) ? fmaxf(m, a) : m;
-  }
-  m = warp_max(m);
-  if ((threadIdx.x & 31) == 0) wm[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float bm = wm[0];
-#pragma unroll
-    for (int w = 1; w < 8; ++w) bm = fmaxf(bm, wm[w]);
-    unsigned int* u = reinterpret_cast<unsigned int*>(scale);
-    atomicMax(u + 2, __float_as_uint(bm));
-    __threadfence();
-    if (atomicAdd(u + 1, 1u) == gridDim.x - 1) {
-      const float mx = __uint_as_float(atomicAdd(u + 2, 0u));
-      int e = 0;
-      if (mx > 0.f) frexpf(mx, &e);
-      scale[0] = ldexpf(1.f, 12 - e);
-      u[2] = 0u;
-      u[1] = 0u;
-    }
-  }
-}
-// EPI 3 scale, known before the GEMM runs: |g (x - sigmoid(l))| <= max|g| * (1 + max|x|).
-// absmax_slot_kernel folds max|src| into scale[slot] (uint bits); bern_grad_scale_kernel turns
-// slots 2 (g) and 3 (x) into scale[0] = power of two s with bound * s in [2^11, 2^12).
-__global__ void __launch_bounds__(256) absmax_slot_kernel(const float* __restrict__ src, int64_t n,
-                                                          float* __restrict__ scale, int slot) {
-  float m = 0.f;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    const float a = fabsf(src[i]);
-    m = (a == a && a <= 3.0e38f) ? fmaxf(m, a) : m;
-  }
-  m = warp_max(m);
-  if ((threadIdx.x & 31) == 0)
-    atomicMax(reinterpret_cast<unsigned int*>(scale) + slot, __float_as_uint(m));
-}
-__global__ void bern_grad_scale_kernel(float* __restrict__ scale) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  unsigned int* u = reinterpret_cast<unsigned int*>(scale);
-  const float m = __uint_as_float(u[2]) * (1.f + __uint_as_float(u[3]));
-  int e = 0;
-  if (m > 0.f && m <= 3.0e38f) frexpf(m, &e);
-  scale[0] = ldexpf(1.f, 12 - e);
-  u[2] = 0u;
-  u[3] = 0u;
-}
+// scale[0] = power of two s with max|src| * s in [2^11, 2^12), from the max in scale[2], which
+// it clears again for the next split
 __global__ void pow2_scale_kernel(float* __restrict__ scale) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   const float m = __uint_as_float(reinterpret_cast<unsigned int*>(scale)[2]);
@@ -541,20 +425,11 @@ __global__ void pow2_scale_kernel(float* __restrict__ scale) {
   scale[0] = ldexpf(1.f, 12 - e);
   reinterpret_cast<unsigned int*>(scale)[2] = 0u;
 }
-// max pass of an operand split: leaves scale[0].  Default: max kernel + single-thread power-of-two
-// kernel; ZSB_ABSMAX_TICKET=1: one kernel whose last block converts the maximum.
-inline bool absmax_ticket() {
-  static const bool v = getenv("ZSB_ABSMAX_TICKET") && atoi(getenv("ZSB_ABSMAX_TICKET")) != 0;
-  return v;
-}
+// max pass of an operand split: leaves scale[0]
 inline void launch_absmax_scale(const float* src, int64_t n, float* scale, unsigned blocks,
                                 cudaStream_t st) {
-  if (absmax_ticket()) {
-    absmax2_ticket_kernel<<<blocks, 256, 0, st>>>(src, n, scale);
-  } else {
-    absmax2_kernel<<<blocks, 256, 0, st>>>(src, n, scale);
-    pow2_scale_kernel<<<1, 32, 0, st>>>(scale);
-  }
+  absmax2_kernel<<<blocks, 256, 0, st>>>(src, n, scale);
+  pow2_scale_kernel<<<1, 32, 0, st>>>(scale);
 }
 // src [rows, K] fp32 -> planes [2][rows][Kp] fp16 (hi, lo) of src * scale, zero padded to Kp
 __global__ void __launch_bounds__(256) split16_pad_kernel(const float* __restrict__ src,
@@ -571,42 +446,6 @@ __global__ void __launch_bounds__(256) split16_pad_kernel(const float* __restric
     const __half h = __float2half_rn(x);
     planes[i] = h;
     planes[n + i] = __float2half_rn(x - __half2float(h));
-  }
-}
-// src [R, C] fp32 -> planes [2][C][Rp] fp16 of (src * scale)^T, zero padded along R: the operand
-// layout of the weight-gradient product dW = dl^T h, whose contraction runs over the rows.
-__global__ void __launch_bounds__(256) split16_pad_t_kernel(const float* __restrict__ src,
-                                                            int64_t R, int C, int64_t Rp,
-                                                            __half* __restrict__ planes,
-                                                            const float* __restrict__ scale) {
-  __shared__ float tile[32][33];
-  const float s = scale[0];
-  const int64_t n = (int64_t)C * Rp;
-  const int64_t r_tiles = (Rp + 31) / 32;
-  const int c_tiles = (C + 31) / 32;
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;      // 32 x 8
-  for (int64_t t = blockIdx.x; t < r_tiles * c_tiles; t += gridDim.x) {
-    const int64_t r0 = (t / c_tiles) * 32;
-    const int c0 = (int)(t % c_tiles) * 32;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int64_t r = r0 + ty + 8 * i;
-      const int c = c0 + tx;
-      tile[ty + 8 * i][tx] = (r < R && c < C) ? src[r * C + c] * s : 0.f;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int c = c0 + ty + 8 * i;
-      const int64_t r = r0 + tx;
-      if (c < C && r < Rp) {
-        const float x = tile[tx][ty + 8 * i];
-        const __half h = __float2half_rn(x);
-        planes[(int64_t)c * Rp + r] = h;
-        planes[n + (int64_t)c * Rp + r] = __float2half_rn(x - __half2float(h));
-      }
-    }
-    __syncthreads();
   }
 }
 // out[i] = sum_s scratch[s][i]
@@ -631,13 +470,6 @@ __global__ void __launch_bounds__(256) part_sum_kernel(const float* __restrict__
   }
 }
 
-// ZSB_EPI_GLOAD=1: the epi 2 / 3 epilogues load the upstream gradient per row (warp-uniform loads)
-// instead of broadcasting it by shuffle (A/B switch of an experiment; default = shuffle)
-int epi_gload() {
-  static const int v = getenv("ZSB_EPI_GLOAD") ? atoi(getenv("ZSB_EPI_GLOAD")) : 0;
-  return v;
-}
-
 // zsb_linear_tc_amax_f32 (Z = 0) and zsb_linear_tc_bin_f32 (Z = 2: h is a 0/1 sample)
 template <int Z>
 int linear_tc_amax(int epi, const void* w_planes, const float* scale_w, const void* h_planes,
@@ -657,40 +489,15 @@ int linear_tc_amax(int epi, const void* w_planes, const float* scale_w, const vo
   if ((rc = linear_maps(w_planes, h_planes, Z & 2, R, J, Kp, m))) return rc;
   const CUtensorMap &m_whi = m[0], &m_wlo = m[1], &m_hhi = m[2], &m_hlo = m[3];
   const int n_blk = (J + BM - 1) / BM;
-  int k_slices = 1;
-  if (epi == 0 && part) {
-    k_slices = zsb_linear_tc_slices(R, J, K);
-    if (k_slices > 1 && relu) {
-      zsb_set_error("zsb_linear_tc_f32: ReLU cannot be fused into a split-K launch");
-      return ZSB_ERR_INVALID;
-    }
-  }
-  float* out_k = (k_slices > 1) ? part : out;
-  float* amax_k = k_slices > 1 ? nullptr : amax_scale;
   if (epi == 0)
-    rc = launch_linear<0, 0, 0, Z>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out_k, part,
-                                R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
-                                "linear_tc");
+    rc = launch_linear<0, 0, Z>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out, part, R,
+                                J, Kp, relu, scale_w, scale_h, 1, amax_scale, st, "linear_tc");
   else if (epi == 1)
-    rc = launch_linear<1, 0, 0, Z>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, nullptr,
-                                part, R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
-                                "linear_tc");
-  else if (Z || !epi_gload())
-    rc = launch_linear<2, 0, 0, Z>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out_k, part,
-                                R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
-                                "linear_tc");
-  else if constexpr (!Z)
-    rc = launch_linear<2, 0, 1>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out_k, part,
-                                R, J, Kp, relu, scale_w, scale_h, k_slices, amax_k, st,
-                                "linear_tc");
-
-  if (rc == ZSB_OK && k_slices > 1) {
-    const int64_t n = R * (int64_t)J;
-    int64_t blocks = zsb_ceil_div(n, 256);
-    if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
-    slice_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, k_slices, n, out);
-    return zsb_check_launch("linear_tc_slice_sum");
-  }
+    rc = launch_linear<1, 0, Z>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, nullptr, part,
+                                R, J, Kp, relu, scale_w, scale_h, 1, amax_scale, st, "linear_tc");
+  else
+    rc = launch_linear<2, 0, Z>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out, part, R,
+                                J, Kp, relu, scale_w, scale_h, 1, amax_scale, st, "linear_tc");
   if (rc != ZSB_OK || epi != 1) return rc;
   int64_t blocks = zsb_ceil_div(R, 256);
   if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
@@ -717,9 +524,9 @@ int linear_tc_wgrad(const void* h_planes, const float* scale_h, int K, const voi
   if ((rc = make_map(&m_hhi, gp, (uint64_t)R, (uint64_t)Jp_g, 64, 128, 1))) return rc;
   if ((rc = make_map(&m_hlo, gp + R * Jp_g, (uint64_t)R, (uint64_t)Jp_g, 64, 128, 1))) return rc;
   const int k_slices = part ? zsb_linear_tc_slices(J, K, (int)R) : 1;
-  rc = launch_linear<0, 3, 0, Z>(m_whi, m_wlo, m_hhi, m_hlo, nullptr, nullptr, 0, nullptr,
-                              k_slices > 1 ? part : out, part, (int64_t)J, K, Rp, 0, scale_h,
-                              scale_g, k_slices, nullptr, st, "linear_tc_wgrad");
+  rc = launch_linear<0, 3, Z>(m_whi, m_wlo, m_hhi, m_hlo, nullptr, nullptr, 0, nullptr,
+                           k_slices > 1 ? part : out, part, (int64_t)J, K, Rp, 0, scale_h,
+                           scale_g, k_slices, nullptr, st, "linear_tc_wgrad");
 
   if (rc == ZSB_OK && k_slices > 1) {
     const int64_t n = (int64_t)J * K;
@@ -759,35 +566,16 @@ int zsb_split16_pad_f32(const float* src, int64_t rows, int K, void* planes, flo
   return zsb_check_launch("split16_pad");
 }
 
-// Transposed variant: src [R, C] -> planes [2][C][Rp] (Rp = zsb_linear_tc_kpad(R)) of src^T.
-int zsb_split16_pad_t_f32(const float* src, int64_t R, int C, void* planes, float* scale,
-                          void* stream) {
-  ZSB_REQUIRE(src && planes && scale && R > 0 && C > 0, "zsb_split16_pad_t_f32: bad args");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t Rp = ((R + 63) / 64) * 64;
-  const int64_t n = R * (int64_t)C;
-  int64_t blocks = zsb_ceil_div(n, 256 * 8);
-  if (blocks > ZSB_NUM_SMS * 16) blocks = ZSB_NUM_SMS * 16;
-  launch_absmax_scale(src, n, scale, (unsigned)blocks, st);
-  int64_t tiles = ((Rp + 31) / 32) * ((C + 31) / 32);
-  if (tiles > ZSB_NUM_SMS * 32) tiles = ZSB_NUM_SMS * 32;
-  split16_pad_t_kernel<<<(unsigned)tiles, 256, 0, st>>>(src, R, C, Rp,
-                                                        reinterpret_cast<__half*>(planes), scale);
-  return zsb_check_launch("split16_pad_t");
-}
-
-// Both operand layouts of one matrix in ONE pass (see split16_dual_kernel): planes [2][R][Kp]
-// and / or planes_t [2][K][Rp] (either may be NULL), optional ReLU mask source, optional column
-// sums (bias gradient; col_sum must be zeroed by the caller).  have_amax = 1: scale[2] already
-// holds max |src| (written by zsb_linear_tc_amax_f32), so no max pass is run.  K must be even.
+// The operand planes of one matrix in ONE pass (see split16_dual_kernel): planes [2][R][Kp],
+// optional ReLU mask source, optional column sums (bias gradient; col_sum must be zeroed by the
+// caller).  have_amax = 1: scale[2] already holds max |src| (written by zsb_linear_tc_amax_f32),
+// so no max pass is run.  K must be even.
 int zsb_split16_dual_f32(const float* src, const float* mask_src, int64_t R, int K, void* planes,
-                         void* planes_t, float* col_sum, float* scale, int have_amax,
-                         void* stream) {
-  ZSB_REQUIRE(src && scale && R > 0 && K > 0 && K % 2 == 0 && (planes || planes_t),
+                         float* col_sum, float* scale, int have_amax, void* stream) {
+  ZSB_REQUIRE(src && planes && scale && R > 0 && K > 0 && K % 2 == 0,
               "zsb_split16_dual_f32: bad args (K must be even)");
   cudaStream_t st = (cudaStream_t)stream;
   const int Kp = zsb_linear_tc_kpad(K);
-  const int64_t Rp = ((R + 63) / 64) * 64;
   if (!have_amax) {
     const int64_t n = R * (int64_t)K;
     int64_t blocks = zsb_ceil_div(n, 256 * 8);
@@ -796,11 +584,10 @@ int zsb_split16_dual_f32(const float* src, const float* mask_src, int64_t R, int
   } else {
     pow2_scale_kernel<<<1, 32, 0, st>>>(scale);    // max|src| left in scale[2] by a GEMM epilogue
   }
-  int64_t tiles = ((Rp + 63) / 64) * ((Kp + 63) / 64);
+  int64_t tiles = ((R + 63) / 64) * ((Kp + 63) / 64);
   if (tiles > ZSB_NUM_SMS * 16) tiles = ZSB_NUM_SMS * 16;
   split16_dual_kernel<<<(unsigned)tiles, 256, 0, st>>>(
-      src, mask_src, R, K, Kp, Rp, reinterpret_cast<__half*>(planes),
-      reinterpret_cast<__half*>(planes_t), col_sum, scale);
+      src, mask_src, R, K, Kp, reinterpret_cast<__half*>(planes), col_sum, scale);
   return zsb_check_launch("split16_dual");
 }
 
@@ -810,9 +597,11 @@ int zsb_split16_dual_f32(const float* src, const float* mask_src, int64_t R, int
 //   epi 1: out [R] = sum_j Bernoulli(logits = h W^T + bias).log_prob(x[r % n_x, j]);
 //          part = scratch of zsb_linear_tc_nparts(J) * R floats
 //   epi 2: out [R, J] = gout[r] * (x - sigmoid(logits))
-// Split-K (epi 0 only): when the output has fewer than one 128 x 128 tile per SM and `part` is
-// given (zsb_linear_tc_slices(R, J, K) * R * J floats), the contraction is cut into slices that
-// run on different SMs and are summed afterwards (the weight-gradient shape dW = dl^T h).
+// `part` is read by epi 1 only.
+//
+// Split-K slices of the weight-gradient product zsb_linear_tc_wgrad_f32 (R output rows, J
+// features, contraction length K): when the output has fewer than one 128 x 128 tile per SM, the
+// contraction is cut into slices that run on different SMs and are summed afterwards.
 int zsb_linear_tc_slices(int64_t R, int J, int K) {
   const int n_blk = (J + BM - 1) / BM;
   const int64_t tiles = ((R + BN - 1) / BN) * n_blk;
@@ -836,7 +625,7 @@ int zsb_linear_tc_f32(int epi, const void* w_planes, const float* scale_w, const
   return zsb_linear_tc_amax_f32(epi, w_planes, scale_w, h_planes, scale_h, bias, x_obs, n_x, gout,
                                 out, part, R, J, K, relu, nullptr, stream);
 }
-// As zsb_linear_tc_f32; additionally the running max |out| (epi 0 / 2, not with split-K) is
+// As zsb_linear_tc_f32; additionally the running max |out| (epi 0 / 2) is
 // folded into amax_scale[2] (uint bits, atomicMax): the scale slot zsb_split16_dual_f32 consumes
 // with have_amax = 1, so the consumer's operand split needs no separate max pass over `out`.
 int zsb_linear_tc_amax_f32(int epi, const void* w_planes, const float* scale_w,
@@ -857,51 +646,6 @@ int zsb_linear_tc_bin_f32(int epi, const void* w_planes, const float* scale_w,
                           void* stream) {
   return linear_tc_amax<2>(epi, w_planes, scale_w, h_planes, scale_h, bias, x_obs, n_x, gout, out,
                            part, R, J, K, relu, amax_scale, (cudaStream_t)stream);
-}
-
-// Backward of the Bernoulli likelihood layer with the operand split fused into the GEMM epilogue:
-//   dl[r, j] = gout[r] * (x[r % n_x, j] - sigmoid(h W^T + bias))        (the epi-2 values)
-// is written ONLY as its fp16 hi/lo planes dl_planes [2][R][kpad(J)] times scale_out[0] (the
-// operands of dh = dl W and dW = dl^T h) and summed over the rows into col_sum [J] (+=, the bias
-// gradient; may be NULL).  scale_out: device float[4], zeroed once by the caller; its power of two
-// comes from the bound max|gout| * (1 + max|x_obs|) >= max|dl|, so no pass over dl is needed.
-int zsb_linear_tc_bern_grad_planes_f32(const void* w_planes, const float* scale_w,
-                                       const void* h_planes, const float* scale_h,
-                                       const float* bias, const float* x_obs, int64_t n_x,
-                                       const float* gout, void* dl_planes, float* col_sum,
-                                       float* scale_out, int64_t R, int J, int K, void* stream) {
-  ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && x_obs && n_x > 0 && gout &&
-                  dl_planes && scale_out && R > 0 && J > 0 && K > 0,
-              "zsb_linear_tc_bern_grad_planes_f32: bad args");
-  ZSB_REQUIRE(R < (1LL << 31), "zsb_linear_tc_bern_grad_planes_f32: too many rows");
-  cudaStream_t st = (cudaStream_t)stream;
-  {
-    int64_t bg = zsb_ceil_div(R, 256 * 8), bx = zsb_ceil_div(n_x * (int64_t)J, 256 * 8);
-    if (bg > ZSB_NUM_SMS * 16) bg = ZSB_NUM_SMS * 16;
-    if (bx > ZSB_NUM_SMS * 16) bx = ZSB_NUM_SMS * 16;
-    absmax_slot_kernel<<<(unsigned)bg, 256, 0, st>>>(gout, R, scale_out, 2);
-    absmax_slot_kernel<<<(unsigned)bx, 256, 0, st>>>(x_obs, n_x * (int64_t)J, scale_out, 3);
-    bern_grad_scale_kernel<<<1, 32, 0, st>>>(scale_out);
-  }
-  const int Kp = zsb_linear_tc_kpad(K);
-  const __half* wp = reinterpret_cast<const __half*>(w_planes);
-  const __half* hp = reinterpret_cast<const __half*>(h_planes);
-  CUtensorMap m_whi, m_wlo, m_hhi, m_hlo;
-  int rc;
-  if ((rc = make_map(&m_whi, wp, (uint64_t)J, (uint64_t)Kp, BM, 128, 1))) return rc;
-  if ((rc = make_map(&m_wlo, wp + (int64_t)J * Kp, (uint64_t)J, (uint64_t)Kp, BM, 128, 1)))
-    return rc;
-  if ((rc = make_map(&m_hhi, hp, (uint64_t)R, (uint64_t)Kp, BN, 128, 1))) return rc;
-  if ((rc = make_map(&m_hlo, hp + R * Kp, (uint64_t)R, (uint64_t)Kp, BN, 128, 1))) return rc;
-  if (epi_gload())
-    return launch_linear<3, 0, 1>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout,
-                                  reinterpret_cast<float*>(dl_planes), col_sum, R, J, Kp, 0,
-                                  scale_w, scale_h, 1, scale_out, st,
-                                  "linear_tc_bern_grad_planes");
-  return launch_linear<3, 0, 0>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout,
-                                reinterpret_cast<float*>(dl_planes), col_sum, R, J, Kp, 0,
-                                scale_w, scale_h, 1, scale_out, st, "linear_tc_bern_grad_planes");
-
 }
 
 // Input gradient of a dense layer from the FORWARD weight planes:
@@ -926,10 +670,9 @@ int zsb_linear_tc_dgrad_f32(const void* w_planes, const float* scale_w, const vo
     return rc;
   if ((rc = make_map(&m_hhi, gp, (uint64_t)R, (uint64_t)Jp, BN, 128, 1))) return rc;
   if ((rc = make_map(&m_hlo, gp + R * Jp, (uint64_t)R, (uint64_t)Jp, BN, 128, 1))) return rc;
-  return launch_linear<0, 1, 0>(m_whi, m_wlo, m_hhi, m_hlo, nullptr, nullptr, 0, nullptr, out,
-                                nullptr, R, K, Jp, 0, scale_w, scale_g, 1, amax_scale, st,
-                                "linear_tc_dgrad");
-
+  return launch_linear<0, 1>(m_whi, m_wlo, m_hhi, m_hlo, nullptr, nullptr, 0, nullptr, out,
+                             nullptr, R, K, Jp, 0, scale_w, scale_g, 1, amax_scale, st,
+                             "linear_tc_dgrad");
 }
 
 // Weight gradient of a dense layer WITHOUT transposed operands:
@@ -937,8 +680,8 @@ int zsb_linear_tc_dgrad_f32(const void* w_planes, const float* scale_w, const vo
 // h_planes [2][R][Kp(K)], g_planes [2][R][Kp(J)]: the row-major fp16 hi/lo planes the forward /
 // input-gradient products already use (zsb_split16_pad_f32 / zsb_split16_dual_f32).  The contraction
 // runs over the rows, so both operands are MN-major wgmma operands (LinW<0, 3>);
-// split-K over the SMs as in zsb_linear_tc_f32 (part = zsb_linear_tc_slices(J, K, R) * J * K
-// floats, or NULL for a single slice).
+// split-K over the SMs (part = zsb_linear_tc_slices(J, K, R) * J * K floats, or NULL for a single
+// slice).
 int zsb_linear_tc_wgrad_f32(const void* h_planes, const float* scale_h, int K,
                             const void* g_planes, const float* scale_g, int J, int64_t R,
                             float* out, float* part, void* stream) {
@@ -981,11 +724,11 @@ int zsb_linear_tc_bern_sample_f32(const void* w_planes, const float* scale_w, co
   };
   float* ho = reinterpret_cast<float*>(h_out);
   if (h_binary)
-    rc = fill(make_linw<4, 0, 0, 2>(m[0], m[1], m[2], m[3], bias, nullptr, 0, nullptr, ho, part, R,
-                                    J, Kp, 0, scale_w, scale_h, 1, nullptr));
+    rc = fill(make_linw<4, 0, 2>(m[0], m[1], m[2], m[3], bias, nullptr, 0, nullptr, ho, part, R,
+                                 J, Kp, 0, scale_w, scale_h, 1, nullptr));
   else
-    rc = fill(make_linw<4, 0, 0, 0>(m[0], m[1], m[2], m[3], bias, nullptr, 0, nullptr, ho, part, R,
-                                    J, Kp, 0, scale_w, scale_h, 1, nullptr));
+    rc = fill(make_linw<4, 0, 0>(m[0], m[1], m[2], m[3], bias, nullptr, 0, nullptr, ho, part, R,
+                                 J, Kp, 0, scale_w, scale_h, 1, nullptr));
   if (rc != ZSB_OK) return rc;
   const int64_t SR = (int64_t)S * R;
   int64_t blocks = zsb_ceil_div(SR, 256);
@@ -1020,9 +763,9 @@ int zsb_linear_tc_bern_given_f32(int epi, const void* w_planes, const float* sca
     return tc_launch(epi == 1 ? chunk_samples(w) : w, st, "linear_tc_bern_given");
   };
 #define ZSB_GIVEN(E, Z)                                                                       \
-  fill(make_linw<E, 0, 0, Z>(m[0], m[1], m[2], m[3], bias, given, (int64_t)S * R, gout,       \
-                             epi == 2 ? out : nullptr, part, R, J, Kp, 0, scale_w, scale_h, 1, \
-                             epi == 2 ? amax_scale : nullptr))
+  fill(make_linw<E, 0, Z>(m[0], m[1], m[2], m[3], bias, given, (int64_t)S * R, gout,          \
+                          epi == 2 ? out : nullptr, part, R, J, Kp, 0, scale_w, scale_h, 1,    \
+                          epi == 2 ? amax_scale : nullptr))
   if (epi == 1)
     rc = h_binary ? ZSB_GIVEN(5, 2) : ZSB_GIVEN(5, 0);
   else

@@ -3,7 +3,6 @@ kernels.  Each is also a plain ``log_joint(observed_dict)`` callable built
 from torch ops, so it works on the generic path and as its own cross-check.
 """
 import math
-import os
 
 import numpy as np
 import torch
@@ -651,72 +650,53 @@ def _tc_split(t2d):
     return planes, scale
 
 
-def _tc_split_t(t2d):
-    """fp32 [R, C] -> (fp16 planes [2, C, Rp] of the transpose, scale)."""
-    from ._lib import lib, ptr, stream
-    t2d = t2d.detach().to(torch.float32).contiguous()
-    R, C = int(t2d.shape[0]), int(t2d.shape[1])
-    Rp = lib.load().zsb_linear_tc_kpad(R)
-    planes = torch.empty((2, C, Rp), dtype=torch.float16, device=t2d.device)
-    scale = torch.zeros(4, dtype=torch.float32, device=t2d.device)
-    lib.call("zsb_split16_pad_t_f32", ptr(t2d), R, C, ptr(planes), ptr(scale),
-             stream())
-    return planes, scale
-
-
 class _Planes(object):
-    """fp16 hi/lo operand planes of one [rows, K] matrix times a power-of-two scale: row-major
-    ``planes`` [2, rows, Kp] (all three products of a layer) and, only with ZSB_WGRAD_T=1, transposed ``planes_t``
-    [2, K, Rp] (weight-gradient product, contraction over the rows); ``scale`` = device float[4].
+    """fp16 hi/lo operand planes ``planes`` [2, rows, Kp] of one [rows, K] matrix times a
+    power-of-two scale, read by all three products of a layer; ``scale`` = device float[4].
     ``binary``: a 0/1 sample of LinearBernoulli.sample -- ``planes`` [1, rows, Kp] is the hi plane
     only (the lo plane is identically zero), read by the two-product kernels; valid while the
     sample's ``_version`` is ``version``."""
-    __slots__ = ("planes", "planes_t", "scale", "rows", "K", "binary", "version")
+    __slots__ = ("planes", "scale", "rows", "K", "binary", "version")
 
-    def __init__(self, planes, planes_t, scale, rows, K, binary=False, version=None):
-        self.planes, self.planes_t, self.scale, self.rows, self.K = planes, planes_t, scale, rows, K
+    def __init__(self, planes, scale, rows, K, binary=False, version=None):
+        self.planes, self.scale, self.rows, self.K = planes, scale, rows, K
         self.binary, self.version = binary, version
 
 
-def _tc_split_dual(t2d, mask=None, want=(True, True), amax=None, col_sum=None):
-    """One pass over fp32 ``t2d`` [R, K] (times the ReLU mask ``mask > 0``) -> _Planes with the
-    layouts asked for in ``want`` = (row-major, transposed); ``amax`` = scale slot whose max-|.|
-    word a producing GEMM already filled (no max pass then); ``col_sum`` [K] += column sums."""
+def _tc_split_dual(t2d, mask=None, amax=None, col_sum=None):
+    """One pass over fp32 ``t2d`` [R, K] (times the ReLU mask ``mask > 0``) -> its _Planes;
+    ``amax`` = scale slot whose max-|.| word a producing GEMM already filled (no max pass then);
+    ``col_sum`` [K] += column sums."""
     from ._lib import lib, ptr, stream
     t2d = t2d.detach().to(torch.float32).contiguous()
     R, K = int(t2d.shape[0]), int(t2d.shape[1])
     dev = t2d.device
-    if K % 2:                      # odd widths: the two single-layout kernels (same max|.| in
-        if mask is not None:       # both -> the same power-of-two scale)
+    if K % 2:                      # odd widths: mask and column sums in torch, then the plain split
+        if mask is not None:
             t2d = t2d * (mask > 0)
         if col_sum is not None:
             col_sum += t2d.sum(0)
-        pl, sc = _tc_split(t2d) if want[0] else (None, None)
-        plt, sct = _tc_split_t(t2d) if want[1] else (None, None)
-        return _Planes(pl, plt, sc if sc is not None else sct, R, K)
+        return _Planes(*_tc_split(t2d), R, K)
     Kp = lib.load().zsb_linear_tc_kpad(K)
-    Rp = lib.load().zsb_linear_tc_kpad(R)
-    planes = torch.empty((2, R, Kp), dtype=torch.float16, device=dev) if want[0] else None
-    planes_t = torch.empty((2, K, Rp), dtype=torch.float16, device=dev) if want[1] else None
+    planes = torch.empty((2, R, Kp), dtype=torch.float16, device=dev)
     scale = amax if amax is not None else torch.zeros(4, dtype=torch.float32, device=dev)
     m = None if mask is None else mask.detach().to(torch.float32).contiguous()
-    lib.call("zsb_split16_dual_f32", ptr(t2d), ptr(m), R, K, ptr(planes), ptr(planes_t),
-             ptr(col_sum), ptr(scale), int(amax is not None), stream())
-    return _Planes(planes, planes_t, scale, R, K)
+    lib.call("zsb_split16_dual_f32", ptr(t2d), ptr(m), R, K, ptr(planes), ptr(col_sum),
+             ptr(scale), int(amax is not None), stream())
+    return _Planes(planes, scale, R, K)
 
 
-def _planes_of(h2, src, need_t):
+def _planes_of(h2, src):
     """Operand planes of activation ``h2`` (= ``src`` flattened to 2-D), cached on ``src``: the
     producing GEMM left the max |.| in ``src._zsb_amax`` (no max pass), and every consumer of the
     same activation (e.g. the two heads of the encoder) shares one split."""
     R, K = int(h2.shape[0]), int(h2.shape[1])
     pl = getattr(src, "_zsb_pl", None)
-    if (pl is not None and pl.rows == R and pl.K == K and pl.planes is not None
-            and (not need_t or pl.planes_t is not None)
+    if (pl is not None and pl.rows == R and pl.K == K
             and (not pl.binary or (pl.version is not None and pl.version == _version(src)))):
         return pl
     amax = getattr(src, "_zsb_amax", None)
-    pl = _tc_split_dual(h2, want=(True, need_t), amax=None if K % 2 else amax)
+    pl = _tc_split_dual(h2, amax=None if K % 2 else amax)
     try:
         src._zsb_pl = pl
         if amax is not None:
@@ -728,16 +708,11 @@ def _planes_of(h2, src, need_t):
 
 def _tc_grad_input(gpl, W, R, wp=None, ws=None):
     """dh [R, K] = g [R, J] @ W [J, K] on the tensor cores (+ the scale slot holding max|dh|).
-    ``wp, ws``: the forward planes of W when the caller still has them -- the product reads them
-    as an MN-major operand (zsb_linear_tc_dgrad_f32), so W^T is never formed; ZSB_DGRAD_MN=0 (or
-    ZSB_WGRAD_T=1): split of W^T, K-major operands."""
-    amax = torch.zeros(4, dtype=torch.float32, device=W.device)
-    if _WGRAD_T or not _DGRAD_MN:
-        wtp, wts = _tc_split(W.detach().t())
-        dh = _tc_linear(0, wtp, wts, gpl.planes, gpl.scale, None, None, None, R,
-                        int(W.shape[1]), int(W.shape[0]), amax=amax)
-        return dh, amax
+    ``wp, ws``: the forward planes of W when the caller still has them (else W is split again) --
+    the product reads them as an MN-major operand (zsb_linear_tc_dgrad_f32), so W^T is never
+    formed."""
     from ._lib import lib, ptr, stream
+    amax = torch.zeros(4, dtype=torch.float32, device=W.device)
     if wp is None:
         wp, ws = _tc_split(W)
     J, K = int(W.shape[0]), int(W.shape[1])
@@ -747,26 +722,10 @@ def _tc_grad_input(gpl, W, R, wp=None, ws=None):
     return dh, amax
 
 
-# ZSB_WGRAD_T=1: the weight gradient reads TRANSPOSED operand planes (the round-2 scheme, kept as a
-# cross-check); default: MN-major operands straight from the row-major planes.
-_WGRAD_T = os.environ.get("ZSB_WGRAD_T", "0") == "1"
-# The input gradient reads the forward weight planes as an MN-major operand
-# (zsb_linear_tc_dgrad_f32) instead of splitting W^T; ZSB_DGRAD_MN=0 restores the W^T split.
-_DGRAD_MN = os.environ.get("ZSB_DGRAD_MN", "1") == "1"
-# ZSB_BERN_FUSED=1: the Bernoulli layer's backward emits d/dlogits directly as operand planes from
-# the GEMM epilogue (zsb_linear_tc_bern_grad_planes_f32, epi 3).  Correct (tests) but MEASURED SLOWER
-# than fp32 dlogits + one split pass (1.47 vs 0.75 + 0.5 ms at config 3: the longer epilogue is no
-# longer hidden behind the next unit's MMAs), so it is opt-in.
-_BERN_UNFUSED = os.environ.get("ZSB_BERN_FUSED", "0") != "1"
-
-
 def _tc_grad_weight(gpl, hpl, R):
     """dW [J, K] = g^T [J, R] @ h [R, K]: contraction over the rows, split-K over the CTA pairs.
     Both operands are the row-major planes of g and h (MN-major wgmma operands,
-    zsb_linear_tc_wgrad_f32); with ZSB_WGRAD_T=1 the transposed plane layout instead."""
-    if _WGRAD_T:
-        return _tc_linear(0, hpl.planes_t, hpl.scale, gpl.planes_t, gpl.scale, None, None, None,
-                          gpl.K, hpl.K, R, split_k=True)
+    zsb_linear_tc_wgrad_f32)."""
     from ._lib import lib, ptr, stream
     J, K = gpl.K, hpl.K
     dev = gpl.planes.device
@@ -779,16 +738,12 @@ def _tc_grad_weight(gpl, hpl, R):
     return out
 
 
-def _tc_linear(epi, wp, ws, hp, hs, bias, x, gout, R, J, K, relu=False,
-               split_k=False, amax=None, binary=False):
+def _tc_linear(epi, wp, ws, hp, hs, bias, x, gout, R, J, K, relu=False, amax=None,
+               binary=False):
     """One product on the wgmma kernel; ``binary``: ``hp`` is the one plane of a 0/1 sample."""
     from ._lib import lib, ptr, stream
     dev = hp.device
     part = None
-    if epi == 0 and split_k:
-        slices = lib.load().zsb_linear_tc_slices(R, J, K)
-        if slices > 1:
-            part = torch.empty(slices * R * J, dtype=torch.float32, device=dev)
     if epi == 1:
         out = torch.empty(R, dtype=torch.float32, device=dev)
         part = torch.empty(lib.load().zsb_linear_tc_nparts(J) * R,
@@ -813,17 +768,16 @@ def _tag(t, amax):
 class _Linear(torch.autograd.Function):
     """y = relu?(h W^T + b): forward and both backward products on the wgmma kernel at fp32
     accuracy (epi 0; the weight gradient reads the same row-major planes as MN-major operands, split-K).
-    Memory passes around the GEMMs are fused (round 2): every GEMM leaves max|out| for its
-    consumer's scale, ONE pass (zsb_split16_dual_f32) turns an activation / gradient into both
-    operand layouts, applies the ReLU mask and accumulates the bias gradient."""
+    Memory passes around the GEMMs are fused: every GEMM leaves max|out| for its consumer's
+    scale, ONE pass (zsb_split16_dual_f32) turns an activation / gradient into its operand planes,
+    applies the ReLU mask and accumulates the bias gradient."""
 
     @staticmethod
     def forward(ctx, h, W, b, relu):
         lead = h.shape[:-1]
         h2 = h if h.dim() == 2 else h.reshape(-1, h.shape[-1])
         R, K, J = int(h2.shape[0]), int(h2.shape[1]), int(W.shape[0])
-        need_dw = bool(ctx.needs_input_grad[1])
-        hpl = _planes_of(h2, h, need_dw and _WGRAD_T)
+        hpl = _planes_of(h2, h)
         wp, ws = _tc_split(W)
         bias = b.detach().to(torch.float32).contiguous() if b is not None else None
         amax = torch.zeros(4, dtype=torch.float32, device=h2.device)
@@ -843,10 +797,8 @@ class _Linear(torch.autograd.Function):
         g = gy.reshape(-1, J)
         db = torch.zeros(J, dtype=torch.float32, device=g.device) \
             if (has_b and need[2]) else None
-        gpl = _tc_split_dual(g, mask=y if relu else None,
-                             want=(bool(need[0]) or (bool(need[1]) and not _WGRAD_T),
-                                   bool(need[1]) and _WGRAD_T),
-                             amax=getattr(gy, "_zsb_amax", None), col_sum=db)
+        gpl = _tc_split_dual(g, mask=y if relu else None, amax=getattr(gy, "_zsb_amax", None),
+                             col_sum=db)
         dh = None
         if need[0]:
             dh2, amax = _tc_grad_input(gpl, W, R, *(ctx.wpl or (None, None)))
@@ -878,7 +830,7 @@ class _LinearBernoulliLogProb(torch.autograd.Function):
             raise ValueError("rows of the observation (%d) must divide the rows "
                              "of the activations (%d)" % (x2.shape[0], R))
         wp, ws = _tc_split(W)
-        hpl = _planes_of(h2, h, bool(ctx.needs_input_grad[1]) and _WGRAD_T)
+        hpl = _planes_of(h2, h)
         bias = b.detach().to(torch.float32).contiguous() if b is not None else None
         lp = _tc_linear(1, wp, ws, hpl.planes, hpl.scale, bias, x2, None, R, J, K,
                         binary=hpl.binary)
@@ -896,21 +848,10 @@ class _LinearBernoulliLogProb(torch.autograd.Function):
         g = glp.reshape(-1).to(torch.float32).contiguous()
         db = torch.zeros(J, dtype=torch.float32, device=g.device) \
             if (has_b and need[2]) else None
-        if _WGRAD_T or _BERN_UNFUSED or hpl.binary:   # fp32 dl, then one split pass
-            amax = torch.zeros(4, dtype=torch.float32, device=g.device)
-            dl = _tc_linear(2, wp, ws, hpl.planes, hpl.scale, bias, x2, g, R, J, K, amax=amax,
-                            binary=hpl.binary)
-            dlpl = _tc_split_dual(dl, want=(bool(need[0]) or (bool(need[1]) and not _WGRAD_T),
-                                            bool(need[1]) and _WGRAD_T), amax=amax, col_sum=db)
-        else:                                # dl leaves the GEMM epilogue as operand planes
-            from ._lib import lib, ptr, stream
-            Jp = lib.load().zsb_linear_tc_kpad(J)
-            planes = torch.empty((2, R, Jp), dtype=torch.float16, device=g.device)
-            scale = torch.zeros(4, dtype=torch.float32, device=g.device)
-            lib.call("zsb_linear_tc_bern_grad_planes_f32", ptr(wp), ptr(ws), ptr(hpl.planes),
-                     ptr(hpl.scale), ptr(bias), ptr(x2), int(x2.shape[0]), ptr(g), ptr(planes),
-                     ptr(db), ptr(scale), R, J, K, stream())
-            dlpl = _Planes(planes, None, scale, R, J)
+        amax = torch.zeros(4, dtype=torch.float32, device=g.device)
+        dl = _tc_linear(2, wp, ws, hpl.planes, hpl.scale, bias, x2, g, R, J, K, amax=amax,
+                        binary=hpl.binary)
+        dlpl = _tc_split_dual(dl, amax=amax, col_sum=db)
         dh = None
         if need[0]:
             dh2, a2 = _tc_grad_input(dlpl, W, R, wp, ws)
@@ -953,8 +894,6 @@ class _LinearBernoulliGiven(torch.autograd.Function):
         from ._lib import lib, ptr, stream
         lead = h.shape[:-1]
         R, K, J = hpl.rows, hpl.K, int(W.shape[0])
-        if _WGRAD_T and ctx.needs_input_grad[1] and hpl.planes_t is None:
-            hpl = _planes_of(h.reshape(R, K), h, True)
         bias = b.detach().to(torch.float32).contiguous() if b is not None else None
         if lq is None:
             lq = torch.empty(S * R, dtype=torch.float32, device=x2.device)
@@ -985,8 +924,7 @@ class _LinearBernoulliGiven(torch.autograd.Function):
         lib.call("zsb_linear_tc_bern_given_f32", 2, ptr(wp), ptr(ws), ptr(hpl.planes),
                  ptr(hpl.scale), int(hpl.binary), ptr(bias), ptr(x2), S, ptr(g), ptr(dl), None,
                  R, J, K, ptr(amax), stream())
-        dlpl = _tc_split_dual(dl, want=(bool(need[0]) or (bool(need[1]) and not _WGRAD_T),
-                                        bool(need[1]) and _WGRAD_T), amax=amax, col_sum=db)
+        dlpl = _tc_split_dual(dl, amax=amax, col_sum=db)
         dh = None
         if need[0]:
             dh2, a2 = _tc_grad_input(dlpl, W, R, wp, ws)
@@ -1063,7 +1001,7 @@ class LinearBernoulli(object):
         h2 = h.reshape(-1, K)
         R = int(h2.shape[0])
         dev = W.device
-        hpl = _planes_of(h2, h, False)
+        hpl = _planes_of(h2, h)
         wp, ws = _tc_split(W)
         bias = b.detach().to(torch.float32).contiguous() if b is not None else None
         seed, it = zrandom.get_seed(), zrandom.next_counter()
@@ -1086,8 +1024,7 @@ class LinearBernoulli(object):
         vs = _versions(hs, h, W, b)
         if all(v is not None for t, v in zip((hs, h, W, b), vs) if t is not None):
             # (inference tensors of torch.inference_mode() have no version: nothing is cached)
-            hs._zsb_pl = _Planes(planes, None, _bin_scale(dev), S * R, J, binary=True,
-                                 version=vs[0])
+            hs._zsb_pl = _Planes(planes, _bin_scale(dev), S * R, J, binary=True, version=vs[0])
             self._own = (hs, lq, S, wp, ws, hpl, vs)
         else:
             self._own = None
@@ -1110,7 +1047,7 @@ class LinearBernoulli(object):
             for d in given.shape[:-nd]:
                 S *= int(d)
             h2 = self._h.reshape(-1, int(self._h.shape[-1]))
-            hpl = _planes_of(h2, self._h, False)
+            hpl = _planes_of(h2, self._h)
             wp, ws = _tc_split(self._W)
             x2 = given.reshape(-1, J).to(torch.float32).contiguous()
             return _LinearBernoulliGiven.apply(self._h, self._W, self._b, x2, S, None, wp, ws,
