@@ -245,6 +245,35 @@ int zsb_linear_tc_wgrad_bin_f32(const void* h_planes, const float* scale_h, int 
                                 const void* g_planes, const float* scale_g, int J, int64_t R,
                                 float* out, float* part, void* stream);
 
+/* ---- Class-conditioned dense layer: tf.layers.dense of a one-hot class y beside an activation h,
+ * examples/semi_supervised_vae/vae_ssl.py:24-28 (relu(dense(z) + dense(onehot(y)))) and :38
+ * (dense(concat([x, y]))).  onehot(y) W_y^T is row y of the class table ctab [C, J] = W_y^T, added
+ * in the epilogue of the product h W^T instead of multiplied:
+ *   cls != NULL: out [R, J] = act(h W^T + bias + ctab[cls[r % n_cls]]); a row whose class is
+ *                outside [0, C) is written as NaN (ctab is not read for it)
+ *   cls == NULL: out [C R, J], row c R + r = act(h W^T + bias + ctab[c])[r] for every class c
+ *                (class-major), from ONE product over the R rows -- the unlabeled bound's class
+ *                enumeration, vae_ssl.py:108-124, without tiling h C times.  Bit-identical to the
+ *                cls form on h tiled C times with cls = c for the rows of block c.
+ * act = ReLU if relu.  max |out| is folded into amax_scale[2] (may be NULL) as in
+ * zsb_linear_tc_amax_f32; h_binary: h_planes is a binary plane (zsb_linear_tc_bern_sample_f32). */
+int zsb_linear_tc_class_f32(const void* w_planes, const float* scale_w, const void* h_planes,
+                            const float* scale_h, int h_binary, const float* bias,
+                            const float* ctab, int C, const int32_t* cls, int64_t n_cls,
+                            float* out, int64_t R, int J, int K, int relu, float* amax_scale,
+                            void* stream);
+/* Its backward pass over the upstream gradient src (times the ReLU mask mask_src > 0 when not
+ * NULL) in one pass: planes [2][R][kpad(K)] of G for zsb_linear_tc_dgrad_f32 /
+ * zsb_linear_tc_wgrad_f32, with G = src [R, K] (cls != NULL) or G[r] = sum_c src[c R + r]
+ * (cls == NULL, src [C R, K] class-major: the products then run over R rows, not C R);
+ * col_sum [K] += column sums of G (bias gradient) and dtab [C, K] += the column sums of src over
+ * the rows of each class (class-table gradient); both may be NULL and are zeroed by the caller.
+ * have_amax: scale[2] holds max |src| from the producing GEMM.  The planes' scale bounds
+ * C max|src| in the cls == NULL form. */
+int zsb_split16_class_f32(const float* src, const float* mask_src, int64_t R, int K,
+                          const int32_t* cls, int64_t n_cls, int C, void* planes, float* col_sum,
+                          float* dtab, float* scale, int have_amax, void* stream);
+
 /* ---- diagnostics: effective sample size (zhusuan/diagnostics.py:17-64, the Stan estimator) on the
  * device; samples [M, D] row-major with burn-in already dropped -> ess [D].  M >= 2. */
 int zsb_effective_sample_size_f32(const float* samples, int64_t M, int64_t D, float* ess,

@@ -49,6 +49,14 @@ constexpr float BIN_SCALE = 2048.f;
 //          of log Bernoulli(l).log_prob(h) ([nparts][S R])
 //   EPI 5  the epi-1 partial rows of the given samples x[s R + r] against logit row r
 //   EPI 6  out[r, j] = sum_s g[s R + r] * (x[s R + r, j] - sigmoid(l))     (d/dl of EPI 5)
+//
+// Class-conditioned epilogues (a dense layer of [h, onehot(y)]: the one-hot block of the product is
+// column y of the class weights, gathered from the class table ctab [C, J] instead of multiplied):
+//   EPI 7  out[r, j] = act(l + ctab[y, j]) with y = cls[r % n_cls]; a row whose y is outside
+//          [0, C) is written as NaN and ctab is not read for it
+//   EPI 8  out[c R + r, j] = act(l + ctab[c, j]) for every class c (class-major), from one product
+//          over the R rows.  The same additions in the same order as EPI 7, so the result equals
+//          EPI 7 on the input tiled C times bit for bit.
 template <int EPI, int MN, int Z = 0>
 struct LinW {
   static constexpr int KIND = 1, RB = 128, MNA = MN & 1, MNB = (MN >> 1) & 1, ZLO = Z;
@@ -68,6 +76,7 @@ struct LinW {
   // layer as a whole is (scripts/bench_sbn.py).
   int S; int s_per; const float* u_in; uint64_t seed; uint32_t iter; const uint32_t* epoch;
   int h_int; __half* pl_out;
+  const float* ctab; int C; const int32_t* cls; int64_t n_cls;   // EPI 7 / 8
   struct EpiState { float amax = 0.f; };
 
   __host__ __device__ __forceinline__ int64_t units() const { return n_tiles * k_slices; }
@@ -115,10 +124,71 @@ struct LinW {
   }
   __device__ __forceinline__ void epilogue(int64_t uu, uint32_t trow, int quarter, int lane,
                                            EpiState& st) const {
-    if constexpr (EPI >= 4)
+    if constexpr (EPI >= 7)
+      epilogue_class(uu, trow, quarter, lane, st);
+    else if constexpr (EPI >= 4)
       epilogue_samples(uu, trow, quarter, lane, st);
     else
       epilogue_rows(uu, trow, quarter, lane, st);
+  }
+  // EPI 7 / 8, per 16-row block of this lane's feature j
+  __device__ __forceinline__ void epilogue_class(int64_t u, uint32_t trow, int quarter, int lane,
+                                                 EpiState& st) const {
+    const float acc_scale = 1.f / (scale_w[0] * scale_h[0]);
+    const int nb = (int)(u % n_blk);
+    const int j = nb * BM + quarter * 32 + lane;
+    const bool j_ok = j < J;
+    const float b_j = (j_ok && bias) ? bias[j] : 0.f;
+    const int64_t r0 = (u / n_blk) * BN;
+    const float* __restrict__ tj = ctab + j;                 // ctab[c, j] = tj[c * J]
+    // the one rounding order of both forms: (acc * scale + bias) + table entry, then ReLU
+    auto act = [&](float l, float t) {
+      const float y = l + t;
+      return relu ? fmaxf(y, 0.f) : y;
+    };
+#pragma unroll 1
+    for (int c = 0; c < BN; c += 16) {
+      const int64_t rbase = r0 + c;
+      if (rbase >= R) break;                                 // warp-uniform
+      uint32_t v[16];
+      acc_ld16(trow + 4u * (uint32_t)c, v);
+      float l[16];
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) l[jj] = fmaf(__uint_as_float(v[jj]), acc_scale, b_j);
+      if (EPI == 7) {
+        int64_t yr = rbase % n_cls;
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+          const int64_t r = rbase + jj;
+          if (j_ok && r < R) {
+            const int k = __ldg(cls + yr);
+            float y;
+            if (k >= 0 && k < C) {
+              y = act(l[jj], __ldg(tj + (int64_t)k * J));
+              st.amax = fmaxf(st.amax, fabsf(y));
+            } else {
+              y = __int_as_float(0x7fffffff);               // NaN: the class is not in the table
+            }
+            out[r * J + j] = y;
+          }
+          if (++yr == n_cls) yr = 0;
+        }
+      } else {
+#pragma unroll 1
+        for (int k = 0; k < C; ++k) {
+          if (!j_ok) break;
+          const float t = __ldg(tj + (int64_t)k * J);
+          float* __restrict__ po = out + ((int64_t)k * R + rbase) * J + j;
+#pragma unroll
+          for (int jj = 0; jj < 16; ++jj)
+            if (rbase + jj < R) {
+              const float y = act(l[jj], t);
+              po[(int64_t)jj * J] = y;
+              st.amax = fmaxf(st.amax, fabsf(y));
+            }
+        }
+      }
+    }
   }
   // EPI 4 - 6: per 16-row block of this lane's feature j, the logits once, then each of the S
   // sample rows of those logit rows
@@ -284,7 +354,7 @@ struct LinW {
     }
   }
   __device__ __forceinline__ void epi_finish(EpiState& st, int, int lane) const {
-    if ((EPI == 0 || EPI == 2 || EPI == 6) && amax_scale) {   // NaN / inf never win (fmaxf drops NaN)
+    if ((EPI == 0 || EPI == 2 || EPI >= 6) && amax_scale) {   // NaN / inf never win (fmaxf drops NaN)
       const float m = warp_max(st.amax <= 3.0e38f ? st.amax : 0.f);
       if (lane == 0 && m > 0.f)
         atomicMax(reinterpret_cast<unsigned int*>(amax_scale) + 2, __float_as_uint(m));
@@ -402,6 +472,117 @@ __global__ void __launch_bounds__(256, 8) split16_dual_kernel(
   }
 }
 
+// Backward pass of the class-conditioned layer (EPI 7 / 8) in one pass over the upstream gradient
+// src (optionally times the ReLU mask (mask_src > 0)):
+//   planes  [2][R][Kp]  fp16 hi/lo of G * scale, where G = src [R, K] (per-row classes cls) or,
+//                       with cls == NULL, G[r] = sum_c src[c R + r] (src [C R, K], class-major):
+//                       the operand of the input- and weight-gradient products, over R rows
+//   col_sum [K]    += sum_r G[r, k]                              (bias gradient)
+//   dtab    [C, K] += sum of src over the rows of class c        (class-table gradient)
+// A thread holds 8 consecutive rows of a 64 x 64 tile and the two columns tx and tx + 32.  The
+// class-table sums of a tile whose rows all have one class are its column sums (met in shared
+// memory); in any other tile each thread adds every run of equal classes with a float atomic.
+// Rows whose class is outside [0, C) add nothing to dtab.
+__global__ void __launch_bounds__(256) split16_class_kernel(
+    const float* __restrict__ src, const float* __restrict__ mask_src, int64_t R, int K, int Kp,
+    const int32_t* __restrict__ cls, int64_t n_cls, int C, __half* __restrict__ planes,
+    float* __restrict__ col_sum, float* __restrict__ dtab, const float* __restrict__ scale) {
+  __shared__ float csum[8][64];
+  const float s = scale[0];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;        // 32 x 8
+  const int64_t r_tiles = (R + 63) / 64;
+  const int c_tiles = (Kp + 63) / 64;
+  const int64_t n_pl = R * (int64_t)Kp;
+  const int n_pass = cls ? 1 : C;
+  for (int64_t t = blockIdx.x; t < r_tiles * c_tiles; t += gridDim.x) {
+    const int64_t r0 = (t / c_tiles) * 64;
+    const int c0 = (int)(t % c_tiles) * 64;
+    const int64_t rt = r0 + 8 * ty;                              // this thread's first row
+    const int col[2] = {c0 + tx, c0 + tx + 32};
+    int k8[8];                                                   // class of each row (per-row form)
+    int k0 = 0;
+    bool uniform = true;
+    if (cls) {
+      k0 = __ldg(cls + r0 % n_cls);
+      int64_t yr = rt % n_cls;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        k8[i] = rt + i < R ? __ldg(cls + yr) : k0;
+        uniform = uniform && k8[i] == k0;
+        if (++yr == n_cls) yr = 0;
+      }
+      uniform = __syncthreads_and(uniform && k0 >= 0 && k0 < C);
+    }
+    float g[8][2];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) g[i][0] = g[i][1] = 0.f;
+    float tsum = 0.f;                              // threads < 64: the tile's column sums of G
+    for (int p = 0; p < n_pass; ++p) {
+      float cs[2] = {0.f, 0.f}, run[2] = {0.f, 0.f};
+      int run_k = -1;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int64_t r = rt + i;
+        float v[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          v[h] = 0.f;
+          if (r < R && col[h] < K) {
+            const int64_t idx = ((int64_t)p * R + r) * K + col[h];
+            v[h] = src[idx];
+            if (mask_src && !(mask_src[idx] > 0.f)) v[h] = 0.f;
+          }
+          g[i][h] += v[h];
+          cs[h] += v[h];
+        }
+        if (cls && !uniform && dtab) {
+          if (k8[i] != run_k) {
+            if (run_k >= 0 && run_k < C) {
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                if (col[h] < K) atomicAdd(dtab + (int64_t)run_k * K + col[h], run[h]);
+            }
+            run_k = k8[i];
+            run[0] = run[1] = 0.f;
+          }
+          run[0] += v[0];
+          run[1] += v[1];
+        }
+      }
+      if (cls && !uniform && dtab && run_k >= 0 && run_k < C) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (col[h] < K) atomicAdd(dtab + (int64_t)run_k * K + col[h], run[h]);
+      }
+      csum[ty][tx] = cs[0];
+      csum[ty][tx + 32] = cs[1];
+      __syncthreads();
+      if (threadIdx.x < 64 && c0 + (int)threadIdx.x < K) {
+        float a = 0.f;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) a += csum[i][threadIdx.x];
+        tsum += a;
+        if (dtab && uniform) atomicAdd(dtab + (int64_t)(cls ? k0 : p) * K + c0 + threadIdx.x, a);
+      }
+      __syncthreads();
+    }
+    if (col_sum && threadIdx.x < 64 && c0 + (int)threadIdx.x < K)
+      atomicAdd(col_sum + c0 + threadIdx.x, tsum);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int64_t r = rt + i;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (r < R && col[h] < Kp) {
+          const float x = g[i][h] * s;
+          const __half hi = __float2half_rn(x);
+          planes[r * Kp + col[h]] = hi;
+          planes[n_pl + r * Kp + col[h]] = __float2half_rn(x - __half2float(hi));
+        }
+    }
+  }
+}
+
 // scale[2] = running max |src| bits (atomicMax over the blocks; NaN and inf are skipped)
 __global__ void __launch_bounds__(256) absmax2_kernel(const float* __restrict__ src, int64_t n,
                                                       float* __restrict__ scale) {
@@ -420,6 +601,16 @@ __global__ void __launch_bounds__(256) absmax2_kernel(const float* __restrict__ 
 __global__ void pow2_scale_kernel(float* __restrict__ scale) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   const float m = __uint_as_float(reinterpret_cast<unsigned int*>(scale)[2]);
+  int e = 0;
+  if (m > 0.f) frexpf(m, &e);
+  scale[0] = ldexpf(1.f, 12 - e);
+  reinterpret_cast<unsigned int*>(scale)[2] = 0u;
+}
+// As pow2_scale_kernel for the bound mult * max|src| (the class fold of split16_class_kernel adds
+// up to `mult` rows of src)
+__global__ void pow2_scale_mult_kernel(float* __restrict__ scale, float mult) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  const float m = __uint_as_float(reinterpret_cast<unsigned int*>(scale)[2]) * mult;
   int e = 0;
   if (m > 0.f) frexpf(m, &e);
   scale[0] = ldexpf(1.f, 12 - e);
@@ -777,6 +968,71 @@ int zsb_linear_tc_bern_given_f32(int epi, const void* w_planes, const float* sca
   if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
   part_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, 4 * ((J + BM - 1) / BM), SR, out);
   return zsb_check_launch("linear_tc_bern_given_part_sum");
+}
+
+// Class-conditioned dense layer (EPI 7 / 8): l = h W^T + bias plus row y of the class table
+// ctab [C, J] (the class weights transposed), ReLU if relu.
+//   cls != NULL: out [R, J], y = cls[r % n_cls]; a row with y outside [0, C) is all NaN
+//   cls == NULL: out [C R, J], row c R + r for class c (every class, one product over R rows)
+// max |out| (NaN rows excluded) is folded into amax_scale[2] (may be NULL).  h_binary as in
+// zsb_linear_tc_bern_sample_f32.
+int zsb_linear_tc_class_f32(const void* w_planes, const float* scale_w, const void* h_planes,
+                            const float* scale_h, int h_binary, const float* bias,
+                            const float* ctab, int C, const int32_t* cls, int64_t n_cls,
+                            float* out, int64_t R, int J, int K, int relu, float* amax_scale,
+                            void* stream) {
+  ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && ctab && out && R > 0 && J > 0 &&
+                  K > 0 && C > 0 && (!cls || n_cls > 0),
+              "zsb_linear_tc_class_f32: bad args");
+  ZSB_REQUIRE(R < (1LL << 31), "zsb_linear_tc_class_f32: too many rows");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Kp = zsb_linear_tc_kpad(K);
+  CUtensorMap m[4];
+  int rc;
+  if ((rc = linear_maps(w_planes, h_planes, h_binary, R, J, Kp, m))) return rc;
+  auto fill = [&](auto w) {
+    w.ctab = ctab; w.C = C; w.cls = cls; w.n_cls = n_cls;
+    return tc_launch(w, st, "linear_tc_class");
+  };
+#define ZSB_CLASS(E, Z)                                                                        \
+  fill(make_linw<E, 0, Z>(m[0], m[1], m[2], m[3], bias, nullptr, 0, nullptr, out, nullptr, R, J, \
+                          Kp, relu, scale_w, scale_h, 1, amax_scale))
+  if (cls)
+    rc = h_binary ? ZSB_CLASS(7, 2) : ZSB_CLASS(7, 0);
+  else
+    rc = h_binary ? ZSB_CLASS(8, 2) : ZSB_CLASS(8, 0);
+#undef ZSB_CLASS
+  return rc;
+}
+
+// The backward pass of zsb_linear_tc_class_f32 in one pass (split16_class_kernel) over the upstream
+// gradient src (times the ReLU mask mask_src > 0, the layer's output, when not NULL):
+//   cls != NULL: src [R, K], planes [2][R][kpad(K)] of src
+//   cls == NULL: src [C R, K] class-major, planes of G[r] = sum_c src[c R + r]
+//   col_sum [K] += column sums of G, dtab [C, K] += per-class column sums (both may be NULL and
+//   must be zeroed by the caller).
+// have_amax = 1: scale[2] already holds max |src| (written by the producing GEMM).  The planes'
+// scale is that of C * max|src| in the enumerated form (a bound of max|G|), else of max|src|.
+int zsb_split16_class_f32(const float* src, const float* mask_src, int64_t R, int K,
+                          const int32_t* cls, int64_t n_cls, int C, void* planes, float* col_sum,
+                          float* dtab, float* scale, int have_amax, void* stream) {
+  ZSB_REQUIRE(src && planes && scale && R > 0 && K > 0 && C > 0 && (!cls || n_cls > 0),
+              "zsb_split16_class_f32: bad args");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Kp = zsb_linear_tc_kpad(K);
+  const int64_t n = (cls ? 1 : C) * R * (int64_t)K;
+  if (!have_amax) {
+    int64_t blocks = zsb_ceil_div(n, 256 * 8);
+    if (blocks > ZSB_NUM_SMS * 16) blocks = ZSB_NUM_SMS * 16;
+    absmax2_kernel<<<(unsigned)blocks, 256, 0, st>>>(src, n, scale);
+  }
+  pow2_scale_mult_kernel<<<1, 32, 0, st>>>(scale, cls ? 1.f : (float)C);
+  int64_t tiles = ((R + 63) / 64) * ((Kp + 63) / 64);
+  if (tiles > ZSB_NUM_SMS * 16) tiles = ZSB_NUM_SMS * 16;
+  split16_class_kernel<<<(unsigned)tiles, 256, 0, st>>>(src, mask_src, R, K, Kp, cls, n_cls, C,
+                                                        reinterpret_cast<__half*>(planes), col_sum,
+                                                        dtab, scale);
+  return zsb_check_launch("split16_class");
 }
 
 }  // extern "C"

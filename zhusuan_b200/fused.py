@@ -9,7 +9,7 @@ import torch
 from torch.autograd.function import once_differentiable
 
 __all__ = ["GaussianLogJoint", "BNNRegressionLogJoint", "LNTMLogJoint", "PMFLogJoint", "linear",
-           "linear_bernoulli_log_prob", "LinearBernoulli"]
+           "class_linear", "linear_bernoulli_log_prob", "LinearBernoulli"]
 
 
 class GaussianLogJoint(object):
@@ -859,6 +859,124 @@ class _LinearBernoulliLogProb(torch.autograd.Function):
         dW = _tc_grad_weight(dlpl, hpl, R) if need[1] else None
         ctx.hpl = None
         return dh, dW, db, None
+
+
+def _class_indices(y, lead, C):
+    """``y`` as the int32 class indices [n_y] the class kernel reads (row r of the flattened
+    ``lead`` takes index r % n_y): int indices whose shape is a suffix of ``lead``, or a one-hot
+    ``[..., C]`` whose leading shape is (turned into indices on the device, no host sync).  A
+    shape that fits both is read as indices."""
+    lead = tuple(int(d) for d in lead)
+    ys = tuple(int(d) for d in y.shape)
+
+    def suffix(s):
+        return len(s) <= len(lead) and s == lead[len(lead) - len(s):]
+    if not y.is_floating_point() and suffix(ys):
+        idx = y
+    elif ys and ys[-1] == C and suffix(ys[:-1]):
+        idx = y.detach().argmax(-1)
+    else:
+        raise ValueError("y %s is neither class indices whose shape is a suffix of %s nor a "
+                         "one-hot [..., %d] over such a shape" % (ys, lead, C))
+    return idx.detach().reshape(-1).to(torch.int32).contiguous()
+
+
+def _tc_split_class(g2, R, cls, C, mask=None, amax=None, col_sum=None, dtab=None):
+    """The backward pass of the class-conditioned layer (zsb_split16_class_f32): _Planes [2, R, Jp]
+    of the upstream gradient ``g2`` (times the ReLU mask ``mask > 0``) -- of its class fold
+    ``sum_c g2[c R + r]`` when ``cls`` is None -- with ``col_sum`` [J] and ``dtab`` [C, J]
+    accumulating the bias and class-table gradients."""
+    from ._lib import lib, ptr, stream
+    g2 = g2.detach().to(torch.float32).contiguous()
+    J = int(g2.shape[1])
+    dev = g2.device
+    planes = torch.empty((2, R, lib.load().zsb_linear_tc_kpad(J)), dtype=torch.float16,
+                         device=dev)
+    scale = amax if amax is not None else torch.zeros(4, dtype=torch.float32, device=dev)
+    m = None if mask is None else mask.detach().to(torch.float32).contiguous()
+    lib.call("zsb_split16_class_f32", ptr(g2), ptr(m), R, J, ptr(cls),
+             0 if cls is None else int(cls.numel()), C, ptr(planes), ptr(col_sum), ptr(dtab),
+             ptr(scale), int(amax is not None), stream())
+    return _Planes(planes, scale, R, J)
+
+
+class _ClassLinear(torch.autograd.Function):
+    """relu?(h W^T + b + W_class[:, y]) on the class epilogue of the wgmma kernel, per row (``cls``)
+    or for every class (``cls`` None, class-major).  Backward: one pass over the upstream gradient
+    gives the class-table and bias gradients and the operand planes of the input- and
+    weight-gradient products -- over the rows of h also in the enumerated form, whose gradient is
+    first folded over the classes."""
+
+    @staticmethod
+    def forward(ctx, h, W, W_class, b, cls, relu):
+        from ._lib import lib, ptr, stream
+        lead = h.shape[:-1]
+        h2 = h if h.dim() == 2 else h.reshape(-1, h.shape[-1])
+        R, K, J, C = int(h2.shape[0]), int(h2.shape[1]), int(W.shape[0]), int(W_class.shape[1])
+        hpl = _planes_of(h2, h)
+        wp, ws = _tc_split(W)
+        tab = W_class.detach().to(torch.float32).t().contiguous()          # [C, J]
+        bias = b.detach().to(torch.float32).contiguous() if b is not None else None
+        amax = torch.zeros(4, dtype=torch.float32, device=h2.device)
+        y = torch.empty(((C if cls is None else 1) * R, J), dtype=torch.float32, device=h2.device)
+        lib.call("zsb_linear_tc_class_f32", ptr(wp), ptr(ws), ptr(hpl.planes), ptr(hpl.scale),
+                 int(hpl.binary), ptr(bias), ptr(tab), C, ptr(cls),
+                 0 if cls is None else int(cls.numel()), ptr(y), R, J, K, int(bool(relu)),
+                 ptr(amax), stream())
+        ctx.save_for_backward(W, y if relu else None)
+        ctx.cls = cls
+        ctx.hpl = hpl
+        ctx.wpl = (wp, ws)
+        ctx.meta = (lead, relu, b is not None, R, K, J, C)
+        shape = tuple(lead) + (J,) if cls is not None else (C,) + tuple(lead) + (J,)
+        return _tag(y.reshape(shape), amax)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        W, y = ctx.saved_tensors
+        lead, relu, has_b, R, K, J, C = ctx.meta
+        need = ctx.needs_input_grad
+        dev = gy.device
+        db = torch.zeros(J, dtype=torch.float32, device=dev) if (has_b and need[3]) else None
+        dtab = torch.zeros((C, J), dtype=torch.float32, device=dev) if need[2] else None
+        gpl = _tc_split_class(gy.reshape(-1, J), R, ctx.cls, C, mask=y if relu else None,
+                              amax=getattr(gy, "_zsb_amax", None), col_sum=db, dtab=dtab)
+        dh = None
+        if need[0]:
+            dh2, amax = _tc_grad_input(gpl, W, R, *ctx.wpl)
+            dh = _tag(dh2.reshape(tuple(lead) + (K,)), amax)
+        dW = _tc_grad_weight(gpl, ctx.hpl, R) if need[1] else None
+        ctx.hpl = None
+        ctx.wpl = None
+        return dh, dW, None if dtab is None else dtab.t(), db, None, None
+
+
+def class_linear(h, W, W_class, y=None, b=None, relu=False):
+    """``relu?(h @ W.T + onehot(y) @ W_class.T + b)`` -- ``tf.layers.dense`` of ``[h, onehot(y)]``
+    (vae_ssl.py:38), or the sum of two dense layers of ``h`` and ``onehot(y)`` (vae_ssl.py:24-28)
+    with their biases added into one ``b`` -- on the wgmma kernel, where the one-hot block of the
+    product is the gather ``W_class[:, y]`` in the epilogue (exact, no C-wide product).
+
+    ``W`` [J, K] and ``W_class`` [J, C] are ``tf.layers.dense`` kernels transposed, as in
+    ``linear``.  ``y``: int class indices whose shape is a suffix of ``h.shape[:-1]`` (broadcast
+    over the leading axes), or a one-hot ``[..., C]`` over such a shape; the result is
+    ``h.shape[:-1] + (J,)``.  A class index outside ``[0, C)`` gives a NaN row.
+
+    ``y=None`` enumerates every class from one product over the rows of h: the result is
+    ``[C, *h.shape[:-1], J]``, class-major, bit for bit the per-row layer on h tiled C times.
+    This differs from the reference's unlabeled bound (vae_ssl.py:108-124), which tiles each row
+    of x C times (row ``n C + c``): here class c of row n sits at ``[c, n]``, so per-datum bounds
+    built on it come out ``[C, N]`` where the reference reshapes to ``[N, C]``.
+
+    Differentiable w.r.t. h, W, W_class and b.  The output carries the max |.| that the next
+    ``linear`` / ``LinearBernoulli`` uses for its operand split."""
+    C = int(W_class.shape[1])
+    if int(W_class.shape[0]) != int(W.shape[0]):
+        raise ValueError("W %s and W_class %s have different output widths"
+                         % (tuple(W.shape), tuple(W_class.shape)))
+    cls = None if y is None else _class_indices(y, h.shape[:-1], C)
+    return _ClassLinear.apply(h, W, W_class, b, cls, bool(relu))
 
 
 def linear_bernoulli_log_prob(h, W, b, x):
