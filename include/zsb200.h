@@ -274,6 +274,43 @@ int zsb_split16_class_f32(const float* src, const float* mask_src, int64_t R, in
                           const int32_t* cls, int64_t n_cls, int C, void* planes, float* col_sum,
                           float* dtab, float* scale, int have_amax, void* stream);
 
+/* ---- Noisy, batch-normalised dense layer of examples/bayesian_neural_nets/variational_dropout.py:26-37:
+ * relu(batch_norm(fully_connected(h * eps))), with tf.contrib.layers defaults (no bias, beta but no
+ * gamma, population variance over all rows in training, moving averages updated in place with
+ * m -= (m - batch) * (1 - decay), the moving statistics in evaluation).
+ * Operand planes [2][R][kpad(K)] of x = h[r % n_h] * noise[r] (h [n_h, K] broadcast over the
+ * particle rows of noise [R, K]; n_h divides R), scale[0] from a max pass over x; x is never
+ * written in fp32.  scale = device float[4], zero-initialised. */
+int zsb_split16_noisy_f32(const float* h, int64_t n_h, const float* noise, int64_t R, int K,
+                          void* planes, float* scale, void* stream);
+/* a = x W^T from those planes and the planes of W; out [R, J] = act((a - mean) rstd + beta) (act =
+ * ReLU if relu), stats [2][J] = (mean, rstd).
+ *   training: mean and population variance of a over its R rows, rstd = rsqrt(var + eps); a [R, J]
+ *     is written, part = ceil(R / 128) * 2 J floats of moment partials (per 128-row tile: mean and
+ *     sum of squared deviations), merged in a fixed order (Chan); moving_mean / moving_var -=
+ *     (moving - batch) * rate, rate = 1 - decay.
+ *   else: mean / rstd of the moving statistics (unchanged), applied in the product's epilogue;
+ *     a and part are not used.
+ * max |out| is folded into amax_scale[2] (may be NULL) as in zsb_linear_tc_amax_f32. */
+int zsb_linear_tc_bn_f32(int training, const void* w_planes, const float* scale_w,
+                         const void* h_planes, const float* scale_h, const float* beta,
+                         float* moving_mean, float* moving_var, float rate, float eps,
+                         float* stats, float* a, float* part, float* out, int64_t R, int J, int K,
+                         int relu, float* amax_scale, void* stream);
+/* Its backward pass from the upstream gradient g [R, J], the output y (read when relu), a
+ * (training) and stats: g' = g [y > 0] (relu) or g, dbeta [J] = sum_r g' (may be NULL), and the
+ * planes [2][R][kpad(J)] of da = rstd (g' - mean_r g' - xhat mean_r(g' xhat)), xhat = (a - mean)
+ * rstd, in training, or of da = rstd g' otherwise -- the operand of zsb_linear_tc_dgrad_f32 /
+ * zsb_linear_tc_wgrad_f32.  Column sums are deterministic.  part = (ceil(R / 128) + 1) * 2 J floats;
+ * scale = device float[4] with scale[2] zero. */
+int zsb_bn_grad_f32(int training, const float* g, const float* y, const float* a,
+                    const float* stats, int relu, int64_t R, int J, float* part, float* dbeta,
+                    void* planes, float* scale, void* stream);
+/* From d = d(h * noise) [R, K]: dnoise [R, K] = d * h[r % n_h], dh [n_h, K] = sum over the R / n_h
+ * particle rows of d * noise (either may be NULL). */
+int zsb_noisy_grad_f32(const float* d, const float* h, int64_t n_h, const float* noise, int64_t R,
+                       int K, float* dnoise, float* dh, void* stream);
+
 /* ---- diagnostics: effective sample size (zhusuan/diagnostics.py:17-64, the Stan estimator) on the
  * device; samples [M, D] row-major with burn-in already dropped -> ess [D].  M >= 2. */
 int zsb_effective_sample_size_f32(const float* samples, int64_t M, int64_t D, float* ess,

@@ -57,6 +57,13 @@ constexpr float BIN_SCALE = 2048.f;
 //   EPI 8  out[c R + r, j] = act(l + ctab[c, j]) for every class c (class-major), from one product
 //          over the R rows.  The same additions in the same order as EPI 7, so the result equals
 //          EPI 7 on the input tiled C times bit for bit.
+//
+// Batch-normalised epilogues (no bias; variational_dropout.py:26-37, tf.contrib.layers.batch_norm):
+//   EPI 9  out[r, j] = a = l (the pre-activation), and per 128-row tile t the moment partials of
+//          column j over the tile's rows, part[2 t J + j] = mean and part[(2 t + 1) J + j] = M2
+//          (sum of squared deviations from the tile mean); the tile's count is min(128, R - 128 t)
+//   EPI 10 out[r, j] = act((l - bn_stats[j]) * bn_stats[J + j] + bn_beta[j]), bn_stats = (mean,
+//          rsqrt(var + eps)) of the moving statistics (evaluation mode)
 template <int EPI, int MN, int Z = 0>
 struct LinW {
   static constexpr int KIND = 1, RB = 128, MNA = MN & 1, MNB = (MN >> 1) & 1, ZLO = Z;
@@ -77,6 +84,7 @@ struct LinW {
   int S; int s_per; const float* u_in; uint64_t seed; uint32_t iter; const uint32_t* epoch;
   int h_int; __half* pl_out;
   const float* ctab; int C; const int32_t* cls; int64_t n_cls;   // EPI 7 / 8
+  const float* bn_stats; const float* bn_beta;                   // EPI 10
   struct EpiState { float amax = 0.f; };
 
   __host__ __device__ __forceinline__ int64_t units() const { return n_tiles * k_slices; }
@@ -124,12 +132,78 @@ struct LinW {
   }
   __device__ __forceinline__ void epilogue(int64_t uu, uint32_t trow, int quarter, int lane,
                                            EpiState& st) const {
-    if constexpr (EPI >= 7)
+    if constexpr (EPI >= 9)
+      epilogue_bn(uu, trow, quarter, lane, st);
+    else if constexpr (EPI >= 7)
       epilogue_class(uu, trow, quarter, lane, st);
     else if constexpr (EPI >= 4)
       epilogue_samples(uu, trow, quarter, lane, st);
     else
       epilogue_rows(uu, trow, quarter, lane, st);
+  }
+  // EPI 9 / 10: this lane's feature j over the tile's rows.  EPI 9 reads the accumulator twice:
+  // once for the tile mean, once for M2 about it (never a sum of squares, which cancels).
+  __device__ __forceinline__ void epilogue_bn(int64_t u, uint32_t trow, int quarter, int lane,
+                                              EpiState& st) const {
+    const float acc_scale = 1.f / (scale_w[0] * scale_h[0]);
+    const int j = (int)(u % n_blk) * BM + quarter * 32 + lane;
+    const bool j_ok = j < J;
+    const int64_t tile = u / n_blk;
+    const int64_t r0 = tile * BN;
+    if (EPI == 9) {
+      float sum = 0.f;
+#pragma unroll 1
+      for (int c = 0; c < BN; c += 16) {
+        const int64_t rbase = r0 + c;
+        if (rbase >= R) break;                                 // warp-uniform
+        uint32_t v[16];
+        acc_ld16(trow + 4u * (uint32_t)c, v);
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj)
+          if (j_ok && rbase + jj < R) {
+            const float l = __uint_as_float(v[jj]) * acc_scale;
+            out[(rbase + jj) * J + j] = l;
+            sum += l;
+          }
+      }
+      const float mean = sum / (float)min((int64_t)BN, R - r0);
+      float m2 = 0.f;
+#pragma unroll 1
+      for (int c = 0; c < BN; c += 16) {
+        const int64_t rbase = r0 + c;
+        if (rbase >= R) break;
+        uint32_t v[16];
+        acc_ld16(trow + 4u * (uint32_t)c, v);
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj)
+          if (rbase + jj < R) {
+            const float d = __uint_as_float(v[jj]) * acc_scale - mean;
+            m2 = fmaf(d, d, m2);
+          }
+      }
+      if (j_ok) {
+        part[2 * tile * J + j] = mean;
+        part[(2 * tile + 1) * J + j] = m2;
+      }
+    } else {
+      const float mu = j_ok ? bn_stats[j] : 0.f, rs = j_ok ? bn_stats[J + j] : 0.f;
+      const float bt = j_ok ? bn_beta[j] : 0.f;
+#pragma unroll 1
+      for (int c = 0; c < BN; c += 16) {
+        const int64_t rbase = r0 + c;
+        if (rbase >= R) break;
+        uint32_t v[16];
+        acc_ld16(trow + 4u * (uint32_t)c, v);
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj)
+          if (j_ok && rbase + jj < R) {
+            float y = (__uint_as_float(v[jj]) * acc_scale - mu) * rs + bt;
+            if (relu) y = fmaxf(y, 0.f);
+            out[(rbase + jj) * J + j] = y;
+            st.amax = fmaxf(st.amax, fabsf(y));
+          }
+      }
+    }
   }
   // EPI 7 / 8, per 16-row block of this lane's feature j
   __device__ __forceinline__ void epilogue_class(int64_t u, uint32_t trow, int quarter, int lane,
@@ -583,6 +657,252 @@ __global__ void __launch_bounds__(256) split16_class_kernel(
   }
 }
 
+// ---- The noisy, batch-normalised dense layer of variational_dropout.py:26-37 --------------------
+// Elementwise passes over [rows, cols] matrices run on 32 x 8 thread blocks: a warp takes 32
+// consecutive columns of one row (coalesced for any width, odd ones included), the 8 warps take
+// 8 rows, and the blocks stride over the rows.
+constexpr int BN_TILE = 128;     // rows per moment partial: the product's row tile (BN)
+
+// x = h[r % n_h, k] * noise[r, k] for r < R, k < K: the layer's input, never stored in fp32.
+// PLANES = false: its max |x| into scale[2] (atomicMax; NaN and inf skipped).  PLANES = true:
+// planes [2][R][Kp] = fp16 hi/lo of x * scale[0], pad columns zero.
+template <bool PLANES>
+__global__ void __launch_bounds__(256) noisy_split_kernel(
+    const float* __restrict__ h, int64_t n_h, const float* __restrict__ noise, int64_t R, int K,
+    int Kp, __half* __restrict__ planes, float* __restrict__ scale) {
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const float s = PLANES ? scale[0] : 0.f;
+  const int64_t n_pl = R * (int64_t)Kp;
+  float m = 0.f;
+  for (int64_t r = (int64_t)blockIdx.x * 8 + ty; r < R; r += (int64_t)gridDim.x * 8) {
+    const float* __restrict__ hr = h + (r % n_h) * K;
+    const float* __restrict__ nr = noise + r * K;
+    for (int k = tx; k < (PLANES ? Kp : K); k += 32) {
+      const float x = k < K ? __ldg(hr + k) * nr[k] : 0.f;
+      if (PLANES) {
+        const float xs = x * s;
+        const __half hi = __float2half_rn(xs);
+        planes[r * Kp + k] = hi;
+        planes[n_pl + r * Kp + k] = __float2half_rn(xs - __half2float(hi));
+      } else {
+        const float a = fabsf(x);
+        m = (a <= 3.0e38f) ? fmaxf(m, a) : m;
+      }
+    }
+  }
+  if (!PLANES) {
+    m = warp_max(m);
+    if (tx == 0) atomicMax(reinterpret_cast<unsigned int*>(scale) + 2, __float_as_uint(m));
+  }
+}
+
+// Chan's update of (count n, mean, M2) with a second set (nb, mb, qb)
+__device__ __forceinline__ void chan_merge(double& n, double& mean, double& m2, double nb,
+                                           double mb, double qb) {
+  if (nb == 0.0) return;
+  const double nn = n + nb, d = mb - mean;
+  mean += d * (nb / nn);
+  m2 += qb + d * d * (n * nb / nn);
+  n = nn;
+}
+
+// One warp per column j.  training: the batch moments from the EPI 9 partials, merged in a fixed
+// order (lane l folds tiles l, l + 32, ... in turn, then a fixed shuffle tree), so two identical
+// calls give identical bits; stats = (mean, rsqrt(var + eps)) with the population variance, and
+// the moving statistics move towards the batch's: m -= (m - batch) * rate (rate = 1 - decay).
+// Evaluation: stats from the moving statistics, which stay as they are.
+__global__ void __launch_bounds__(256) bn_stats_kernel(const float* __restrict__ part, int64_t R,
+                                                       int J, float* __restrict__ mmean,
+                                                       float* __restrict__ mvar, float rate,
+                                                       float eps, int training,
+                                                       float* __restrict__ stats) {
+  const int lane = threadIdx.x & 31;
+  const int j = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (j >= J) return;                                            // warp-uniform
+  if (!training) {
+    if (lane == 0) {
+      stats[j] = mmean[j];
+      stats[J + j] = rsqrtf(mvar[j] + eps);
+    }
+    return;
+  }
+  const int64_t n_t = (R + BN_TILE - 1) / BN_TILE;
+  double n = 0.0, mean = 0.0, m2 = 0.0;
+  for (int64_t t = lane; t < n_t; t += 32)
+    chan_merge(n, mean, m2, (double)min((int64_t)BN_TILE, R - t * BN_TILE),
+               part[2 * t * J + j], part[(2 * t + 1) * J + j]);
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    const double nb = __shfl_down_sync(0xffffffffu, n, off);
+    const double mb = __shfl_down_sync(0xffffffffu, mean, off);
+    const double qb = __shfl_down_sync(0xffffffffu, m2, off);
+    chan_merge(n, mean, m2, nb, mb, qb);
+  }
+  if (lane == 0) {
+    const float mu = (float)mean, var = (float)(m2 / n);
+    stats[j] = mu;
+    stats[J + j] = rsqrtf(var + eps);
+    mmean[j] -= (mmean[j] - mu) * rate;
+    mvar[j] -= (mvar[j] - var) * rate;
+  }
+}
+
+// Training forward after EPI 9: out = act((a - mean) * rstd + beta), max |out| into scale[2]
+__global__ void __launch_bounds__(256) bn_apply_kernel(const float* __restrict__ a, int64_t R,
+                                                       int J, const float* __restrict__ stats,
+                                                       const float* __restrict__ beta, int relu,
+                                                       float* __restrict__ out,
+                                                       float* __restrict__ amax_scale) {
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  float m = 0.f;
+  for (int64_t r = (int64_t)blockIdx.x * 8 + ty; r < R; r += (int64_t)gridDim.x * 8)
+    for (int j = tx; j < J; j += 32) {
+      float y = (a[r * J + j] - __ldg(stats + j)) * __ldg(stats + J + j) + __ldg(beta + j);
+      if (relu) y = fmaxf(y, 0.f);
+      out[r * J + j] = y;
+      m = fmaxf(m, fabsf(y));
+    }
+  if (amax_scale) {
+    m = warp_max(m <= 3.0e38f ? m : 0.f);
+    if (tx == 0 && m > 0.f)
+      atomicMax(reinterpret_cast<unsigned int*>(amax_scale) + 2, __float_as_uint(m));
+  }
+}
+
+// Backward, per 128-row tile t and column j (block: 32 columns x 8 warps, 16 rows per warp, then
+// the 8 warps meet in shared memory in a fixed order):
+//   part[2 t J + j] = sum_r g',  part[(2 t + 1) J + j] = sum_r g' xhat   (training only)
+// with g' = g [y > 0] (relu) or g, xhat = (a - mean) * rstd.
+__global__ void __launch_bounds__(256) bn_grad_sums_kernel(
+    const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ a,
+    const float* __restrict__ stats, int relu, int64_t R, int J, float* __restrict__ part) {
+  __shared__ float sh[2][8][32];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int64_t t = blockIdx.x;
+  const int j = blockIdx.y * 32 + tx;
+  float s1 = 0.f, s2 = 0.f;
+  if (j < J) {
+    const float mu = a ? stats[j] : 0.f, rs = a ? stats[J + j] : 0.f;
+#pragma unroll 4
+    for (int i = 0; i < BN_TILE / 8; ++i) {
+      const int64_t r = t * BN_TILE + ty + 8 * i;
+      if (r >= R) break;
+      float gg = g[r * J + j];
+      if (relu && !(y[r * J + j] > 0.f)) gg = 0.f;
+      s1 += gg;
+      if (a) s2 = fmaf(gg, (a[r * J + j] - mu) * rs, s2);
+    }
+  }
+  sh[0][ty][tx] = s1;
+  sh[1][ty][tx] = s2;
+  __syncthreads();
+  if (ty < 2 && j < J) {
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) s += sh[ty][i][tx];
+    part[(2 * t + ty) * J + j] = s;
+  }
+}
+
+// One warp per column: the tile sums of bn_grad_sums_kernel in a fixed order (lane-strided runs,
+// then a fixed shuffle tree) -> dbeta[j] = sum g' (may be NULL), coef = (sum g' / R,
+// sum g' xhat / R)
+__global__ void __launch_bounds__(256) bn_grad_combine_kernel(const float* __restrict__ part,
+                                                              int64_t R, int J,
+                                                              float* __restrict__ dbeta,
+                                                              float* __restrict__ coef) {
+  const int lane = threadIdx.x & 31;
+  const int j = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (j >= J) return;
+  const int64_t n_t = (R + BN_TILE - 1) / BN_TILE;
+  float s1 = 0.f, s2 = 0.f;
+  for (int64_t t = lane; t < n_t; t += 32) {
+    s1 += part[2 * t * J + j];
+    s2 += part[(2 * t + 1) * J + j];
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    s1 += __shfl_down_sync(0xffffffffu, s1, off);
+    s2 += __shfl_down_sync(0xffffffffu, s2, off);
+  }
+  if (lane == 0) {
+    if (dbeta) dbeta[j] = s1;
+    coef[j] = s1 / (float)R;
+    coef[J + j] = s2 / (float)R;
+  }
+}
+
+// da = rstd (g' - coef[0] - xhat coef[1]) in training (a != NULL), rstd g' in evaluation.
+// PLANES = false: max |da| into scale[2]; PLANES = true: planes [2][R][Jp] = fp16 hi/lo of
+// da * scale[0], pad columns zero -- the operand zsb_linear_tc_dgrad_f32 / _wgrad_f32 read.
+template <bool PLANES>
+__global__ void __launch_bounds__(256) bn_grad_apply_kernel(
+    const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ a,
+    const float* __restrict__ stats, const float* __restrict__ coef, int relu, int64_t R, int J,
+    int Jp, __half* __restrict__ planes, float* __restrict__ scale) {
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const float s = PLANES ? scale[0] : 0.f;
+  const int64_t n_pl = R * (int64_t)Jp;
+  float m = 0.f;
+  for (int64_t r = (int64_t)blockIdx.x * 8 + ty; r < R; r += (int64_t)gridDim.x * 8)
+    for (int j = tx; j < (PLANES ? Jp : J); j += 32) {
+      float d = 0.f;
+      if (j < J) {
+        float gg = g[r * J + j];
+        if (relu && !(y[r * J + j] > 0.f)) gg = 0.f;
+        const float rs = __ldg(stats + J + j);
+        if (a) {
+          const float xh = (a[r * J + j] - __ldg(stats + j)) * rs;
+          gg = gg - __ldg(coef + j) - xh * __ldg(coef + J + j);
+        }
+        d = rs * gg;
+      }
+      if (PLANES) {
+        const float ds = d * s;
+        const __half hi = __float2half_rn(ds);
+        planes[r * Jp + j] = hi;
+        planes[n_pl + r * Jp + j] = __float2half_rn(ds - __half2float(hi));
+      } else {
+        const float ad = fabsf(d);
+        m = (ad <= 3.0e38f) ? fmaxf(m, ad) : m;
+      }
+    }
+  if (!PLANES) {
+    m = warp_max(m);
+    if (tx == 0) atomicMax(reinterpret_cast<unsigned int*>(scale) + 2, __float_as_uint(m));
+  }
+}
+
+// From d = d(h * noise) [R, K]: dnoise[r] = d[r] * h[r % n_h] and dh[i] = sum_s d[s n_h + i] *
+// noise[s n_h + i] over the R / n_h particle rows that share row i of h, in order (either output
+// may be NULL).
+__global__ void __launch_bounds__(256) noisy_grad_kernel(
+    const float* __restrict__ d, const float* __restrict__ h, int64_t n_h,
+    const float* __restrict__ noise, int64_t R, int K, float* __restrict__ dnoise,
+    float* __restrict__ dh) {
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int64_t S = R / n_h;
+  for (int64_t i = (int64_t)blockIdx.x * 8 + ty; i < n_h; i += (int64_t)gridDim.x * 8)
+    for (int k = tx; k < K; k += 32) {
+      const float hv = h[i * K + k];
+      float acc = 0.f;
+      for (int64_t s = 0; s < S; ++s) {
+        const int64_t e = (s * n_h + i) * K + k;
+        const float dv = d[e];
+        if (dnoise) dnoise[e] = dv * hv;
+        if (dh) acc = fmaf(dv, noise[e], acc);
+      }
+      if (dh) dh[i * K + k] = acc;
+    }
+}
+
+// blocks of an elementwise 32 x 8 pass over `rows` rows
+inline unsigned row_blocks(int64_t rows) {
+  int64_t b = (rows + 7) / 8;
+  if (b > ZSB_NUM_SMS * 16) b = ZSB_NUM_SMS * 16;
+  return (unsigned)(b < 1 ? 1 : b);
+}
+
 // scale[2] = running max |src| bits (atomicMax over the blocks; NaN and inf are skipped)
 __global__ void __launch_bounds__(256) absmax2_kernel(const float* __restrict__ src, int64_t n,
                                                       float* __restrict__ scale) {
@@ -1033,6 +1353,109 @@ int zsb_split16_class_f32(const float* src, const float* mask_src, int64_t R, in
                                                         reinterpret_cast<__half*>(planes), col_sum,
                                                         dtab, scale);
   return zsb_check_launch("split16_class");
+}
+
+// Operand planes [2][R][kpad(K)] of x = h[r % n_h] * noise[r] (h [n_h, K], noise [R, K], n_h
+// dividing R) with scale[0] chosen from max |x| as zsb_split16_dual_f32 chooses it: a max pass
+// and a split pass, both reading h and noise; x is never stored in fp32.
+int zsb_split16_noisy_f32(const float* h, int64_t n_h, const float* noise, int64_t R, int K,
+                          void* planes, float* scale, void* stream) {
+  ZSB_REQUIRE(h && noise && planes && scale && R > 0 && K > 0 && n_h > 0 && R % n_h == 0,
+              "zsb_split16_noisy_f32: bad args");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Kp = zsb_linear_tc_kpad(K);
+  __half* pl = reinterpret_cast<__half*>(planes);
+  noisy_split_kernel<false><<<row_blocks(R), 256, 0, st>>>(h, n_h, noise, R, K, Kp, pl, scale);
+  pow2_scale_kernel<<<1, 32, 0, st>>>(scale);
+  noisy_split_kernel<true><<<row_blocks(R), 256, 0, st>>>(h, n_h, noise, R, K, Kp, pl, scale);
+  return zsb_check_launch("split16_noisy");
+}
+
+// Batch-normalised dense layer, no bias: a = h W^T from the planes of zsb_split16_noisy_f32, then
+// out [R, J] = act((a - mean) rstd + beta) (act = ReLU if relu), stats [2][J] = (mean, rstd).
+//   training != 0: mean and the population variance over the R rows (EPI 9 writes a [R, J] and
+//     the moment partials part [ceil(R / 128) * 2 J], merged in a fixed order), rstd =
+//     rsqrt(var + eps); moving_mean / moving_var -= (moving - batch) * rate; a pass applies the
+//     affine step and ReLU.
+//   training == 0: mean / rstd of the moving statistics, which are not changed; the product's
+//     epilogue writes out (EPI 10): a and part are not used.
+// max |out| is folded into amax_scale[2] (may be NULL).
+int zsb_linear_tc_bn_f32(int training, const void* w_planes, const float* scale_w,
+                         const void* h_planes, const float* scale_h, const float* beta,
+                         float* moving_mean, float* moving_var, float rate, float eps,
+                         float* stats, float* a, float* part, float* out, int64_t R, int J, int K,
+                         int relu, float* amax_scale, void* stream) {
+  ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && beta && moving_mean && moving_var &&
+                  stats && out && R > 0 && J > 0 && K > 0 && (!training || (a && part)),
+              "zsb_linear_tc_bn_f32: bad args");
+  ZSB_REQUIRE(R < (1LL << 31), "zsb_linear_tc_bn_f32: too many rows");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Kp = zsb_linear_tc_kpad(K);
+  CUtensorMap m[4];
+  int rc;
+  if ((rc = linear_maps(w_planes, h_planes, 0, R, J, Kp, m))) return rc;
+  const unsigned col_blocks = (unsigned)((J + 7) / 8);
+  if (!training) {
+    bn_stats_kernel<<<col_blocks, 256, 0, st>>>(nullptr, R, J, moving_mean, moving_var, rate, eps,
+                                                0, stats);
+    if ((rc = zsb_check_launch("linear_tc_bn_stats")) != ZSB_OK) return rc;
+    auto w = make_linw<10, 0>(m[0], m[1], m[2], m[3], nullptr, nullptr, 0, nullptr, out, nullptr,
+                              R, J, Kp, relu, scale_w, scale_h, 1, amax_scale);
+    w.bn_stats = stats;
+    w.bn_beta = beta;
+    return tc_launch(w, st, "linear_tc_bn_eval");
+  }
+  rc = launch_linear<9, 0>(m[0], m[1], m[2], m[3], nullptr, nullptr, 0, nullptr, a, part, R, J,
+                           Kp, relu, scale_w, scale_h, 1, nullptr, st, "linear_tc_bn_train");
+  if (rc != ZSB_OK) return rc;
+  bn_stats_kernel<<<col_blocks, 256, 0, st>>>(part, R, J, moving_mean, moving_var, rate, eps, 1,
+                                              stats);
+  bn_apply_kernel<<<row_blocks(R), 256, 0, st>>>(a, R, J, stats, beta, relu, out, amax_scale);
+  return zsb_check_launch("linear_tc_bn_apply");
+}
+
+// Backward of zsb_linear_tc_bn_f32 from the upstream gradient g [R, J], its output y (the ReLU
+// mask, read when relu), a (training) and stats:
+//   g' = g [y > 0] (relu) or g;  dbeta [J] = sum_r g' (may be NULL)
+//   training: da = rstd (g' - mean_r g' - xhat mean_r(g' xhat)), xhat = (a - mean) rstd
+//   else:     da = rstd g'
+// The column sums run per 128-row tile and are merged in a fixed order (deterministic).
+// planes [2][R][kpad(J)] = fp16 hi/lo of da times scale[0], a power of two picked from max |da|:
+// the operand of zsb_linear_tc_dgrad_f32 / zsb_linear_tc_wgrad_f32.  part = (ceil(R / 128) + 1)
+// * 2 J floats of scratch; scale = device float[4] with scale[2] zero.
+int zsb_bn_grad_f32(int training, const float* g, const float* y, const float* a,
+                    const float* stats, int relu, int64_t R, int J, float* part, float* dbeta,
+                    void* planes, float* scale, void* stream) {
+  ZSB_REQUIRE(g && stats && part && planes && scale && R > 0 && J > 0 && (!relu || y) &&
+                  (!training || a),
+              "zsb_bn_grad_f32: bad args");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Jp = zsb_linear_tc_kpad(J);
+  const int64_t n_t = (R + BN_TILE - 1) / BN_TILE;
+  const float* at = training ? a : nullptr;
+  float* coef = part + 2 * n_t * J;
+  bn_grad_sums_kernel<<<dim3((unsigned)n_t, (unsigned)((J + 31) / 32)), 256, 0, st>>>(
+      g, y, at, stats, relu, R, J, part);
+  bn_grad_combine_kernel<<<(unsigned)((J + 7) / 8), 256, 0, st>>>(part, R, J, dbeta, coef);
+  __half* pl = reinterpret_cast<__half*>(planes);
+  bn_grad_apply_kernel<false><<<row_blocks(R), 256, 0, st>>>(g, y, at, stats, coef, relu, R, J, Jp,
+                                                             pl, scale);
+  pow2_scale_kernel<<<1, 32, 0, st>>>(scale);
+  bn_grad_apply_kernel<true><<<row_blocks(R), 256, 0, st>>>(g, y, at, stats, coef, relu, R, J, Jp,
+                                                            pl, scale);
+  return zsb_check_launch("bn_grad");
+}
+
+// Gradients of x = h[r % n_h] * noise[r] from d = dL/dx [R, K]: dnoise [R, K] = d * h[r % n_h] and
+// dh [n_h, K] = the sum of d * noise over the R / n_h rows that share each row of h, added in row
+// order.  Either output may be NULL.
+int zsb_noisy_grad_f32(const float* d, const float* h, int64_t n_h, const float* noise, int64_t R,
+                       int K, float* dnoise, float* dh, void* stream) {
+  ZSB_REQUIRE(d && h && noise && R > 0 && K > 0 && n_h > 0 && R % n_h == 0,
+              "zsb_noisy_grad_f32: bad args");
+  noisy_grad_kernel<<<row_blocks(n_h), 256, 0, (cudaStream_t)stream>>>(d, h, n_h, noise, R, K,
+                                                                       dnoise, dh);
+  return zsb_check_launch("noisy_grad");
 }
 
 }  // extern "C"

@@ -9,7 +9,7 @@ import torch
 from torch.autograd.function import once_differentiable
 
 __all__ = ["GaussianLogJoint", "BNNRegressionLogJoint", "LNTMLogJoint", "PMFLogJoint", "linear",
-           "class_linear", "linear_bernoulli_log_prob", "LinearBernoulli"]
+           "class_linear", "noisy_bn_linear", "linear_bernoulli_log_prob", "LinearBernoulli"]
 
 
 class GaussianLogJoint(object):
@@ -977,6 +977,128 @@ def class_linear(h, W, W_class, y=None, b=None, relu=False):
                          % (tuple(W.shape), tuple(W_class.shape)))
     cls = None if y is None else _class_indices(y, h.shape[:-1], C)
     return _ClassLinear.apply(h, W, W_class, b, cls, bool(relu))
+
+
+class _NoisyBNLinear(torch.autograd.Function):
+    """relu?(BN((h * noise) W^T)) on the batch-norm epilogues of the wgmma kernel.  Forward: one
+    split pass turns h * noise into operand planes (zsb_split16_noisy_f32), then the product and the
+    batch-norm step (zsb_linear_tc_bn_f32).  Backward: one pass gives d beta and the planes of the
+    pre-activation gradient (zsb_bn_grad_f32), the unchanged input- and weight-gradient products
+    read them, and one pass turns d(h * noise) into d noise and d h (zsb_noisy_grad_f32)."""
+
+    @staticmethod
+    def forward(ctx, h, noise, W, beta, stats_bufs, training, relu, rate, eps):
+        from ._lib import lib, ptr, stream
+        moving_mean, moving_variance = stats_bufs
+        K, J = int(noise.shape[-1]), int(W.shape[0])
+        lead = noise.shape[:-1]
+        n2 = noise.detach().to(torch.float32).reshape(-1, K).contiguous()
+        h2 = h.detach().to(torch.float32).reshape(-1, K).contiguous()
+        R, n_h = int(n2.shape[0]), int(h2.shape[0])
+        dev = n2.device
+        Kp = lib.load().zsb_linear_tc_kpad(K)
+        planes = torch.empty((2, R, Kp), dtype=torch.float16, device=dev)
+        scale = torch.zeros(4, dtype=torch.float32, device=dev)
+        lib.call("zsb_split16_noisy_f32", ptr(h2), n_h, ptr(n2), R, K, ptr(planes), ptr(scale),
+                 stream())
+        wp, ws = _tc_split(W)
+        b = beta.detach().to(torch.float32).contiguous()
+        stats = torch.empty((2, J), dtype=torch.float32, device=dev)
+        y = torch.empty((R, J), dtype=torch.float32, device=dev)
+        a = part = None
+        if training:
+            a = torch.empty((R, J), dtype=torch.float32, device=dev)
+            part = torch.empty(-(-R // 128) * 2 * J, dtype=torch.float32, device=dev)
+        amax = torch.zeros(4, dtype=torch.float32, device=dev)
+        lib.call("zsb_linear_tc_bn_f32", int(training), ptr(wp), ptr(ws), ptr(planes), ptr(scale),
+                 ptr(b), ptr(moving_mean), ptr(moving_variance), rate, eps, ptr(stats), ptr(a),
+                 ptr(part), ptr(y), R, J, K, int(relu), ptr(amax), stream())
+        ctx.save_for_backward(W, y if relu else None, a, stats, h2, n2)
+        ctx.hpl = _Planes(planes, scale, R, K)
+        ctx.wpl = (wp, ws)
+        ctx.meta = (tuple(h.shape), lead, training, relu, R, n_h, K, J)
+        return _tag(y.reshape(tuple(lead) + (J,)), amax)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        from ._lib import lib, ptr, stream
+        W, y, a, stats, h2, n2 = ctx.saved_tensors
+        h_shape, lead, training, relu, R, n_h, K, J = ctx.meta
+        need = ctx.needs_input_grad
+        dev = gy.device
+        g = gy.reshape(R, J).to(torch.float32).contiguous()
+        dbeta = torch.empty(J, dtype=torch.float32, device=dev) if need[3] else None
+        part = torch.empty((-(-R // 128) + 1) * 2 * J, dtype=torch.float32, device=dev)
+        planes = torch.empty((2, R, lib.load().zsb_linear_tc_kpad(J)), dtype=torch.float16,
+                             device=dev)
+        scale = torch.zeros(4, dtype=torch.float32, device=dev)
+        lib.call("zsb_bn_grad_f32", int(training), ptr(g), ptr(y), ptr(a), ptr(stats), int(relu),
+                 R, J, ptr(part), ptr(dbeta), ptr(planes), ptr(scale), stream())
+        gpl = _Planes(planes, scale, R, J)
+        dh = dnoise = None
+        if need[0] or need[1]:
+            dx, _ = _tc_grad_input(gpl, W, R, *ctx.wpl)
+            dnoise = torch.empty((R, K), dtype=torch.float32, device=dev) if need[1] else None
+            dh = torch.empty((n_h, K), dtype=torch.float32, device=dev) if need[0] else None
+            lib.call("zsb_noisy_grad_f32", ptr(dx), ptr(h2), n_h, ptr(n2), R, K, ptr(dnoise),
+                     ptr(dh), stream())
+            dh = None if dh is None else dh.reshape(h_shape)
+            dnoise = None if dnoise is None else dnoise.reshape(tuple(lead) + (K,))
+        dW = _tc_grad_weight(gpl, ctx.hpl, R) if need[2] else None
+        ctx.hpl = None
+        ctx.wpl = None
+        return dh, dnoise, dW, dbeta, None, None, None, None, None
+
+
+def noisy_bn_linear(h, noise, W, beta, moving_mean, moving_variance, training, relu=True,
+                    decay=0.999, epsilon=1e-3):
+    """``relu?(BN((h * noise) @ W.T))``, shape ``noise.shape[:-1] + (J,)``: one layer of
+    examples/bayesian_neural_nets/variational_dropout.py:26-37, ``layers.fully_connected(h * eps,
+    n_out, normalizer_fn=layers.batch_norm)`` with the defaults of tf.contrib.layers:
+
+    * no bias (``fully_connected`` drops it when a normalizer is given);
+    * batch norm with ``center=True`` (``beta`` [J]), ``scale=False`` (no gamma) and ``epsilon``;
+      ``training``: the moments over all ``noise.shape[:-1]`` rows with the population variance, and
+      ``moving_mean`` / ``moving_variance`` (float32 [J]) updated in place as ``m -= (m - batch) *
+      (1 - decay)`` (``updates_collections=None``, no zero-debiasing); otherwise the moving
+      statistics normalise and stay unchanged;
+    * then ``relu``.  ``fully_connected``'s default activation is ReLU, so the example applies it
+      to every layer, the 10-unit logits layer included (its explicit ``tf.nn.relu`` for the hidden
+      layers is redundant): keep ``relu=True`` on the last layer to reproduce it.
+
+    ``noise`` is ``[*lead, K]`` and ``h``'s shape is a suffix of it, so ``x`` [n, K] broadcasts
+    over the particle axis without being tiled; ``h`` may also have ``noise``'s full shape.
+    ``W`` is [J, K] (the kernel transposed, as in ``linear``).  The product of ``h * noise`` is
+    never formed in fp32: its operand planes are made in one pass over ``h`` and ``noise``.
+
+    Differentiable w.r.t. ``h``, ``noise``, ``W`` and ``beta``; the moving statistics receive no
+    gradient.  The batch moments and every gradient's column sums are reduced in a fixed order, so
+    two identical calls give identical bits.  The output carries the max |.| that a following
+    ``linear`` uses for its operand split."""
+    noise_s, h_s = tuple(noise.shape), tuple(h.shape)
+    if noise.dim() < 1 or not noise.is_floating_point():
+        raise ValueError("noise must be a floating tensor [*lead, K], got %s %s"
+                         % (noise.dtype, noise_s))
+    if len(h_s) < 1 or len(h_s) > len(noise_s) or noise_s[len(noise_s) - len(h_s):] != h_s:
+        raise ValueError("the shape of h %s must be a suffix of the shape of noise %s"
+                         % (h_s, noise_s))
+    K = noise_s[-1]
+    if W.dim() != 2 or int(W.shape[1]) != K:
+        raise ValueError("W %s must be [J, %d]" % (tuple(W.shape), K))
+    J = int(W.shape[0])
+    if tuple(beta.shape) != (J,):
+        raise ValueError("beta %s must be [%d]" % (tuple(beta.shape), J))
+    for nm, t in (("moving_mean", moving_mean), ("moving_variance", moving_variance)):
+        if not isinstance(t, torch.Tensor) or tuple(t.shape) != (J,) or \
+                t.dtype != torch.float32 or not t.is_contiguous() or t.device != W.device:
+            raise ValueError("%s must be a contiguous float32 [%d] tensor on %s"
+                             % (nm, J, W.device))
+    if any(int(d) == 0 for d in noise_s) or J == 0:
+        raise ValueError("empty shapes are not supported: noise %s, W %s"
+                         % (noise_s, tuple(W.shape)))
+    return _NoisyBNLinear.apply(h, noise, W, beta, (moving_mean, moving_variance), bool(training),
+                                bool(relu), float(1.0 - decay), float(epsilon))
 
 
 def linear_bernoulli_log_prob(h, W, b, x):
