@@ -19,8 +19,11 @@
 // warp touches 32 consecutive features of one row per instruction: coalesced x loads and out stores.
 #include "tc_common.cuh"
 
+#include <type_traits>
+
 extern "C" int zsb_linear_tc_kpad(int K);
 extern "C" int zsb_linear_tc_slices(int64_t R, int J, int K);
+extern "C" int zsb_linear_tc_nparts(int J);
 
 namespace {
 
@@ -33,16 +36,7 @@ __device__ __forceinline__ float bern_lp(float x, float l) {   // -sigmoid_cross
 // its lo plane is exactly zero.
 constexpr float BIN_SCALE = 2048.f;
 
-// MN (bit 0: operand A, bit 1: operand B; EPI 0 only): the operand is read in a row-major plane
-// layout [contraction rows, features] -- MN-major (transposed) wgmma operand.  MN = 3: weight
-// gradient dW = g^T h from the row-major planes of g and h; MN = 1: input gradient dh = g W with
-// A = the FORWARD planes of W [J, K] (no W^T copy): no product of a dense layer needs a transposed
-// copy of anything.  A stage then holds, per plane, two TMA boxes of 64 contraction rows x 64
-// features (128-byte rows, SWIZZLE_128B; see gmma_desc).  `Kp` is the padded contraction length.
-// ZLO: bit 0 / 1 = the lo plane of operand A / B is zero (a 0/1 sample, see mma_kblock): it is
-// neither loaded nor multiplied.
-//
-// Epilogues with S >= 1 rows of samples per logit row r (sample row s * R + r, k_slices = 1):
+// Epilogues with S >= 1 rows of samples per logit row r (sample row s * R + r):
 //   EPI 4  Bernoulli sampling: h = (u < sigmoidf_(l)) with u injected or drawn from Philox keyed as
 //          zsb_sample_bernoulli_i32 keys element (s R + r) J + j; writes h (float or int32), its fp16
 //          operand plane h * BIN_SCALE [S R][kpad(J)] (pad columns zero) and the epi-1 partial rows
@@ -64,38 +58,69 @@ constexpr float BIN_SCALE = 2048.f;
 //          (sum of squared deviations from the tile mean); the tile's count is min(128, R - 128 t)
 //   EPI 10 out[r, j] = act((l - bn_stats[j]) * bn_stats[J + j] + bn_beta[j]), bn_stats = (mean,
 //          rsqrt(var + eps)) of the moving statistics (evaluation mode)
-template <int EPI, int MN, int Z = 0>
-struct LinW {
+//
+// The descriptor tc_pipeline_kernel runs, LinW<E, EPI, MN, Z>, is a LinCore (the product) plus the
+// fields of one epilogue family E: RowsEpi (EPI 0 - 2), SamplesEpi (4 - 6), ClassEpi (7, 8) or
+// BnEpi (9, 10).
+
+// What a product's units past its first n_tiles are (unit u runs output tile u % n_tiles), as each
+// epilogue family declares it:
+//   K_SLICES       slices of the contraction, kb_per k-blocks each, summed afterwards
+//   SAMPLE_CHUNKS  chunks of s_per sample rows, each over the whole contraction
+//   TILES          none: one unit per tile, over the whole contraction
+enum Units { TILES, K_SLICES, SAMPLE_CHUNKS };
+
+// A unit as one epilogue lane sees it: slice or chunk `sub`, feature block nb and this lane's
+// feature j in it, row tile `tile` and its first row r0
+struct Unit {
+  int sub; int nb; int j; int64_t tile; int64_t r0;
+};
+
+// The product acc[j, r] = sum_k A[j, k] B[r, k] over J features j (operand A: the weight rows of
+// the forward product) and R rows r (operand B), on fp16 hi/lo planes of A and B at the
+// power-of-two scales scale_w[0] and scale_h[0].
+// MN (bit 0: operand A, bit 1: operand B; EPI 0 only): the operand is read in a row-major plane
+// layout [contraction rows, features] -- MN-major (transposed) wgmma operand.  MN = 3: weight
+// gradient dW = g^T h from the row-major planes of g and h; MN = 1: input gradient dh = g W with
+// A = the FORWARD planes of W [J, K] (no W^T copy): no product of a dense layer needs a transposed
+// copy of anything.  A stage then holds, per plane, two TMA boxes of 64 contraction rows x 64
+// features (128-byte rows, SWIZZLE_128B; see gmma_desc).
+// Z: bit 0 / 1 = the lo plane of operand A / B is zero (a 0/1 sample, see mma_kblock): it is
+// neither loaded nor multiplied.
+template <int MN, int Z>
+struct LinCore {
   static constexpr int KIND = 1, RB = 128, MNA = MN & 1, MNB = (MN >> 1) & 1, ZLO = Z;
   static constexpr uint32_t TX = Cfg<RB>::STAGE - ((Z & 1) ? Cfg<RB>::A_TILE : 0) -
                                  ((Z & 2) ? Cfg<RB>::B_TILE : 0);
   CUtensorMap map_whi, map_wlo, map_hhi, map_hlo;
-  const float* bias; const float* x_obs; int64_t n_x; const float* gout;
-  float* out; float* part; int64_t R; int J; int Kp; int relu;
-  const float* scale_w; const float* scale_h; int k_slices; float* amax_scale;
-  int n_blk; int64_t n_tiles; int n_kb_all; int kb_per;
-  // EPI 4 - 6.  EPI 4 / 5 split the S sample rows of a tile into k_slices chunks of s_per rows,
-  // each its own unit, so a layer with few logit rows and many draws still fills every SM.  The
-  // price: each chunk recomputes the tile's whole product (about 125 times for the proposal's first
-  // layer at 100 rows and K = 1000).  EPI 4 also runs one Philox-10 per element, four times the
-  // work of the elementwise sampler, which shares one draw among four elements; it keeps the
-  // sampler's keying so the samples are bit-identical.  Neither cost is measured on its own; the
-  // layer as a whole is (scripts/bench_sbn.py).
-  int S; int s_per; const float* u_in; uint64_t seed; uint32_t iter; const uint32_t* epoch;
-  int h_int; __half* pl_out;
-  const float* ctab; int C; const int32_t* cls; int64_t n_cls;   // EPI 7 / 8
-  const float* bn_stats; const float* bn_beta;                   // EPI 10
-  struct EpiState { float amax = 0.f; };
+  const float* scale_w; const float* scale_h;
+  int64_t R; int J;
+  int n_blk; int64_t n_tiles; int n_kb_all; int kb_per; int k_slices;
 
   __host__ __device__ __forceinline__ int64_t units() const { return n_tiles * k_slices; }
+  template <Units U>
   __device__ __forceinline__ void kb_range(int64_t uu, int& kb0, int& kb1) const {
-    if (EPI >= 4) {
+    if (U != K_SLICES) {
       kb0 = 0;
       kb1 = n_kb_all;
       return;
     }
     kb0 = (int)(uu / n_tiles) * kb_per;
     kb1 = min(kb0 + kb_per, n_kb_all);
+  }
+  template <Units U>
+  __device__ __forceinline__ Unit unit(int64_t uu, int quarter, int lane) const {
+    const int64_t u = U == TILES ? uu : uu % n_tiles;
+    Unit t;
+    t.sub = U == TILES ? 0 : (int)(uu / n_tiles);
+    t.nb = (int)(u % n_blk);
+    t.j = t.nb * BM + quarter * 32 + lane;
+    t.tile = u / n_blk;
+    t.r0 = t.tile * BN;
+    return t;
+  }
+  __device__ __forceinline__ float acc_scale() const {   // powers of two: exact
+    return 1.f / (scale_w[0] * scale_h[0]);
   }
   __device__ __forceinline__ void prefetch() const {
     tma_prefetch_desc(&map_whi); tma_prefetch_desc(&map_wlo);
@@ -130,26 +155,45 @@ struct LinW {
       if (!(Z & 2)) tma_load_2d(sa + 2 * C::A_TILE + C::B_TILE, &map_hlo, fb, kb * 64, r0);
     }
   }
+};
+
+template <class E, int EPI, int MN = 0, int Z = 0>
+struct LinW : LinCore<MN, Z> {
+  E e;
+  struct EpiState { float amax = 0.f; };   // max |stored output|: the consumer's fp16-split scale
+  __device__ __forceinline__ void kb_range(int64_t uu, int& kb0, int& kb1) const {
+    LinCore<MN, Z>::template kb_range<E::UNITS>(uu, kb0, kb1);
+  }
   __device__ __forceinline__ void epilogue(int64_t uu, uint32_t trow, int quarter, int lane,
                                            EpiState& st) const {
-    if constexpr (EPI >= 9)
-      epilogue_bn(uu, trow, quarter, lane, st);
-    else if constexpr (EPI >= 7)
-      epilogue_class(uu, trow, quarter, lane, st);
-    else if constexpr (EPI >= 4)
-      epilogue_samples(uu, trow, quarter, lane, st);
-    else
-      epilogue_rows(uu, trow, quarter, lane, st);
+    e.template run<EPI>(*this, uu, trow, quarter, lane, st.amax);
   }
-  // EPI 9 / 10: this lane's feature j over the tile's rows.  EPI 9 reads the accumulator twice:
-  // once for the tile mean, once for M2 about it (never a sum of squares, which cancels).
-  __device__ __forceinline__ void epilogue_bn(int64_t u, uint32_t trow, int quarter, int lane,
-                                              EpiState& st) const {
-    const float acc_scale = 1.f / (scale_w[0] * scale_h[0]);
-    const int j = (int)(u % n_blk) * BM + quarter * 32 + lane;
+  __device__ __forceinline__ void epi_finish(EpiState& st, int, int lane) const {
+    if (E::folds_amax(EPI) && e.amax_scale)   // NaN / inf never win (fmaxf drops NaN)
+      fold_amax(e.amax_scale, st.amax <= 3.0e38f ? st.amax : 0.f, lane);
+  }
+};
+
+// EPI 9 / 10: this lane's feature j over the tile's rows.  EPI 9 reads the accumulator twice:
+// once for the tile mean, once for M2 about it (never a sum of squares, which cancels).
+struct BnEpi {
+  static constexpr Units UNITS = TILES;
+  // EPI 9 is given no amax_scale
+  __host__ __device__ static constexpr bool folds_amax(int) { return true; }
+  const float* bn_stats; const float* bn_beta;
+  float* out; float* part; int relu; float* amax_scale;
+
+  template <int EPI, class Core>
+  __device__ __forceinline__ void run(const Core& core, int64_t u, uint32_t trow, int quarter,
+                                      int lane, float& amax) const {
+    const int64_t& R = core.R;
+    const int& J = core.J;
+    const float acc_scale = core.acc_scale();
+    const Unit pos = core.template unit<UNITS>(u, quarter, lane);
+    const int j = pos.j;
     const bool j_ok = j < J;
-    const int64_t tile = u / n_blk;
-    const int64_t r0 = tile * BN;
+    const int64_t tile = pos.tile;
+    const int64_t r0 = pos.r0;
     if (EPI == 9) {
       float sum = 0.f;
 #pragma unroll 1
@@ -200,20 +244,31 @@ struct LinW {
             float y = (__uint_as_float(v[jj]) * acc_scale - mu) * rs + bt;
             if (relu) y = fmaxf(y, 0.f);
             out[(rbase + jj) * J + j] = y;
-            st.amax = fmaxf(st.amax, fabsf(y));
+            amax = fmaxf(amax, fabsf(y));
           }
       }
     }
   }
-  // EPI 7 / 8, per 16-row block of this lane's feature j
-  __device__ __forceinline__ void epilogue_class(int64_t u, uint32_t trow, int quarter, int lane,
-                                                 EpiState& st) const {
-    const float acc_scale = 1.f / (scale_w[0] * scale_h[0]);
-    const int nb = (int)(u % n_blk);
-    const int j = nb * BM + quarter * 32 + lane;
+};
+
+// EPI 7 / 8, per 16-row block of this lane's feature j
+struct ClassEpi {
+  static constexpr Units UNITS = TILES;
+  __host__ __device__ static constexpr bool folds_amax(int) { return true; }
+  const float* bias; const float* ctab; int C; const int32_t* cls; int64_t n_cls;
+  float* out; int relu; float* amax_scale;
+
+  template <int EPI, class Core>
+  __device__ __forceinline__ void run(const Core& core, int64_t u, uint32_t trow, int quarter,
+                                      int lane, float& amax) const {
+    const int64_t& R = core.R;
+    const int& J = core.J;
+    const float acc_scale = core.acc_scale();
+    const Unit pos = core.template unit<UNITS>(u, quarter, lane);
+    const int j = pos.j;
     const bool j_ok = j < J;
     const float b_j = (j_ok && bias) ? bias[j] : 0.f;
-    const int64_t r0 = (u / n_blk) * BN;
+    const int64_t r0 = pos.r0;
     const float* __restrict__ tj = ctab + j;                 // ctab[c, j] = tj[c * J]
     // the one rounding order of both forms: (acc * scale + bias) + table entry, then ReLU
     auto act = [&](float l, float t) {
@@ -239,7 +294,7 @@ struct LinW {
             float y;
             if (k >= 0 && k < C) {
               y = act(l[jj], __ldg(tj + (int64_t)k * J));
-              st.amax = fmaxf(st.amax, fabsf(y));
+              amax = fmaxf(amax, fabsf(y));
             } else {
               y = __int_as_float(0x7fffffff);               // NaN: the class is not in the table
             }
@@ -258,26 +313,45 @@ struct LinW {
             if (rbase + jj < R) {
               const float y = act(l[jj], t);
               po[(int64_t)jj * J] = y;
-              st.amax = fmaxf(st.amax, fabsf(y));
+              amax = fmaxf(amax, fabsf(y));
             }
         }
       }
     }
   }
-  // EPI 4 - 6: per 16-row block of this lane's feature j, the logits once, then each of the S
-  // sample rows of those logit rows
-  __device__ __forceinline__ void epilogue_samples(int64_t unit, uint32_t trow, int quarter,
-                                                   int lane, EpiState& st) const {
-    const float acc_scale = 1.f / (scale_w[0] * scale_h[0]);
-    const int s0 = (int)(unit / n_tiles) * s_per, s1 = min(S, s0 + s_per);
-    unit %= n_tiles;
-    const int nb = (int)(unit % n_blk);
-    const int j = nb * BM + quarter * 32 + lane;
+};
+
+// EPI 4 - 6: per 16-row block of this lane's feature j, the logits once, then each of the sample
+// rows s0 .. s1 of the unit's chunk of those logit rows.  EPI 4 / 5 split the S sample rows of a
+// tile into chunks of s_per rows, each its own unit, so a layer with few logit rows and many draws
+// still fills every SM.  The price: each chunk recomputes the tile's whole product (about 125
+// times for the proposal's first layer at 100 rows and K = 1000).  EPI 4 also runs one Philox-10
+// per element, four times the work of the elementwise sampler, which shares one draw among four
+// elements; it keeps the sampler's keying so the samples are bit-identical.  Neither cost is
+// measured on its own; the layer as a whole is (scripts/bench_sbn.py).  EPI 6 sums over all S
+// draws in one chunk.
+struct SamplesEpi {
+  static constexpr Units UNITS = SAMPLE_CHUNKS;
+  __host__ __device__ static constexpr bool folds_amax(int epi) { return epi == 6; }
+  const float* bias; const float* x_obs; const float* gout; float* out; float* part;
+  int S; int s_per; const float* u_in; uint64_t seed; uint32_t iter; const uint32_t* epoch;
+  int h_int; __half* pl_out; float* amax_scale;
+
+  template <int EPI, class Core>
+  __device__ __forceinline__ void run(const Core& core, int64_t uu, uint32_t trow, int quarter,
+                                      int lane, float& amax) const {
+    const int64_t& R = core.R;
+    const int& J = core.J;
+    const float acc_scale = core.acc_scale();
+    const Unit pos = core.template unit<UNITS>(uu, quarter, lane);
+    const int s0 = pos.sub * s_per, s1 = min(S, s0 + s_per);
+    const int nb = pos.nb;
+    const int j = pos.j;
     const bool j_ok = j < J;
     const int Jp = ((J + 63) / 64) * 64;
     const bool col_ok = j < Jp;                    // EPI 4 plane: real and zero-padding columns
     const float b_j = (j_ok && bias) ? bias[j] : 0.f;
-    const int64_t r0 = (unit / n_blk) * BN;
+    const int64_t r0 = pos.r0;
     const int64_t part_row = (int64_t)(nb * 4 + quarter) * ((int64_t)S * R);
     const uint32_t it = (EPI == 4) ? iter + (epoch ? *epoch : 0u) : 0u;
 #pragma unroll 1
@@ -340,24 +414,35 @@ struct LinW {
         for (int jj = 0; jj < 16; ++jj)
           if (j_ok && rbase + jj < R) {
             out[(rbase + jj) * J + j] = dl[jj];
-            st.amax = fmaxf(st.amax, fabsf(dl[jj]));
+            amax = fmaxf(amax, fabsf(dl[jj]));
           }
       }
     }
   }
-  __device__ __forceinline__ void epilogue_rows(int64_t uu, uint32_t trow, int quarter, int lane,
-                                                EpiState& st) const {
-    float& amax = st.amax;   // max |stored output| (EPI 0 / 2): the consumer's fp16-split scale
-    const float acc_scale = 1.f / (scale_w[0] * scale_h[0]);   // powers of two: exact
-    const int64_t u = uu % n_tiles;
-    const int slice = (int)(uu / n_tiles);
-    const bool empty_slice = slice * kb_per >= n_kb_all;   // accumulator never written
+};
+
+// EPI 0 - 2; EPI 0 with K-slices writes slice s of the product to out + s R J
+struct RowsEpi {
+  static constexpr Units UNITS = K_SLICES;
+  __host__ __device__ static constexpr bool folds_amax(int epi) { return epi != 1; }
+  const float* bias; const float* x_obs; int64_t n_x; const float* gout;
+  float* out; float* part; int relu; float* amax_scale;
+
+  template <int EPI, class Core>
+  __device__ __forceinline__ void run(const Core& core, int64_t uu, uint32_t trow, int quarter,
+                                      int lane, float& amax) const {
+    const int64_t& R = core.R;
+    const int& J = core.J;
+    const float acc_scale = core.acc_scale();
+    const Unit pos = core.template unit<UNITS>(uu, quarter, lane);
+    const int slice = pos.sub;
+    const bool empty_slice = slice * core.kb_per >= core.n_kb_all;   // accumulator never written
     float* __restrict__ out_s = (EPI == 0 && out) ? out + (int64_t)slice * R * J : out;
-    const int nb = (int)(u % n_blk);
-    const int j = nb * BM + quarter * 32 + lane;
+    const int nb = pos.nb;
+    const int j = pos.j;
     const bool j_ok = j < J;
     const float b_j = (j_ok && bias) ? bias[j] : 0.f;
-    const int64_t r0 = (u / n_blk) * BN;
+    const int64_t r0 = pos.r0;
     const int64_t part_row = (int64_t)(nb * 4 + quarter) * R;
     const float b_use = (slice == 0) ? b_j : 0.f;           // bias once across the slices
     const bool warp_j_ok = __all_sync(0xffffffffu, j_ok);
@@ -427,68 +512,66 @@ struct LinW {
       process(vb, xb, gb, c + 16);
     }
   }
-  __device__ __forceinline__ void epi_finish(EpiState& st, int, int lane) const {
-    if ((EPI == 0 || EPI == 2 || EPI >= 6) && amax_scale) {   // NaN / inf never win (fmaxf drops NaN)
-      const float m = warp_max(st.amax <= 3.0e38f ? st.amax : 0.f);
-      if (lane == 0 && m > 0.f)
-        atomicMax(reinterpret_cast<unsigned int*>(amax_scale) + 2, __float_as_uint(m));
-    }
-  }
 };
 
-// one product on the tensor cores: A = w planes (J_ features), B = h planes (R rows)
-template <int EPI, int MN, int Z = 0>
-LinW<EPI, MN, Z> make_linw(const CUtensorMap& whi, const CUtensorMap& wlo,
-                           const CUtensorMap& hhi, const CUtensorMap& hlo, const float* bias,
-                           const float* x_obs, int64_t n_x, const float* gout, float* out,
-                           float* part, int64_t R, int J_, int Kp, int relu,
-                           const float* scale_w, const float* scale_h, int k_slices,
-                           float* amax_scale) {
-  const int n_blk = (J_ + BM - 1) / BM;
-  const int64_t n_tiles = ((R + BN - 1) / BN) * n_blk;
-  const int n_kb_all = Kp / 64;
-  const int kb_per = (n_kb_all + k_slices - 1) / k_slices;
-  LinW<EPI, MN, Z> w{whi, wlo, hhi, hlo, bias, x_obs, n_x, gout, out, part, R, J_, Kp,
-                     relu, scale_w, scale_h, k_slices, amax_scale, n_blk, n_tiles,
-                     n_kb_all, kb_per};
-  w.S = 1;
-  w.s_per = 1;
-  return w;
-}
-template <int EPI, int MN, int Z = 0>
-int launch_linear(const CUtensorMap& whi, const CUtensorMap& wlo, const CUtensorMap& hhi,
-                  const CUtensorMap& hlo, const float* bias, const float* x_obs, int64_t n_x,
-                  const float* gout, float* out, float* part, int64_t R, int J_, int Kp, int relu,
-                  const float* scale_w, const float* scale_h, int k_slices, float* amax_scale,
-                  cudaStream_t st, const char* what) {
-  return tc_launch(make_linw<EPI, MN, Z>(whi, wlo, hhi, hlo, bias, x_obs, n_x, gout, out, part,
-                                         R, J_, Kp, relu, scale_w, scale_h, k_slices, amax_scale),
-                   st, what);
+// output tiles of a product over J features and R rows
+inline int64_t lin_tiles(int64_t R, int J) { return ((R + BN - 1) / BN) * ((J + BM - 1) / BM); }
+
+// Tensor maps of one operand's fp16 planes [2][rows][cols] (hi, then lo), in boxes of 64 rows
+// (MN-major) or of the tile's 128 rows (K-major, BM = BN).  A binary operand has its hi plane only;
+// its lo map, never loaded, points at that plane.
+int plane_maps(CUtensorMap* hi, CUtensorMap* lo, const void* planes, int64_t rows, int cols,
+               bool mn_major, bool binary) {
+  const __half* p = reinterpret_cast<const __half*>(planes);
+  const uint32_t box = mn_major ? 64 : BM;
+  const int rc = make_map(hi, p, (uint64_t)rows, (uint64_t)cols, box, 128, 1);
+  if (rc) return rc;
+  return make_map(lo, binary ? p : p + rows * cols, (uint64_t)rows, (uint64_t)cols, box, 128, 1);
 }
 
-// EPI 4 / 5: split the S sample rows into chunks so that the launch has about two units per SM
-template <class W>
-W chunk_samples(W w) {
-  int64_t want = (2 * ZSB_NUM_SMS + w.n_tiles - 1) / w.n_tiles;
-  if (want > w.S) want = w.S;
+// The core of a product over J features, R rows and contraction length K, cut into k_slices
+// units per tile, from the planes of A (w_planes, scale_w) and B (h_planes, scale_h).  A K-major
+// operand's planes are [2][J or R][kpad(K)], an MN-major one's [2][K][kpad(J or R)]; an operand
+// whose bit of Z is set has its hi plane only.
+template <int MN, int Z>
+int make_core(LinCore<MN, Z>& c, const void* w_planes, const float* scale_w, const void* h_planes,
+              const float* scale_h, int J, int64_t R, int64_t K, int k_slices = 1) {
+  const int Kp = zsb_linear_tc_kpad((int)K);
+  int rc = (MN & 1) ? plane_maps(&c.map_whi, &c.map_wlo, w_planes, K, zsb_linear_tc_kpad(J), true,
+                                 Z & 1)
+                    : plane_maps(&c.map_whi, &c.map_wlo, w_planes, J, Kp, false, Z & 1);
+  if (rc) return rc;
+  rc = (MN & 2) ? plane_maps(&c.map_hhi, &c.map_hlo, h_planes, K, zsb_linear_tc_kpad((int)R), true,
+                             Z & 2)
+                : plane_maps(&c.map_hhi, &c.map_hlo, h_planes, R, Kp, false, Z & 2);
+  if (rc) return rc;
+  c.scale_w = scale_w;
+  c.scale_h = scale_h;
+  c.R = R;
+  c.J = J;
+  c.n_blk = (J + BM - 1) / BM;
+  c.n_tiles = lin_tiles(R, J);
+  c.n_kb_all = Kp / 64;
+  c.kb_per = (c.n_kb_all + k_slices - 1) / k_slices;
+  c.k_slices = k_slices;
+  return ZSB_OK;
+}
+
+// EPI 4 / 5: the sample rows per chunk that give a launch about two units per SM
+int sample_chunk(int64_t R, int J, int S) {
+  const int64_t n_tiles = lin_tiles(R, J);
+  int64_t want = (2 * ZSB_NUM_SMS + n_tiles - 1) / n_tiles;
+  if (want > S) want = S;
   if (want < 1) want = 1;
-  w.s_per = (int)((w.S + want - 1) / want);
-  w.k_slices = (w.S + w.s_per - 1) / w.s_per;
-  return w;
+  return (int)((S + want - 1) / want);
 }
 
-// Tensor maps of a forward-layout product: w planes [2][J][Kp] (A) and h planes [R][Kp] (B, hi
-// then lo plane).  binary_h: h has only its hi plane (a 0/1 sample); the lo map is never loaded.
-int linear_maps(const void* w_planes, const void* h_planes, int binary_h, int64_t R, int J, int Kp,
-                CUtensorMap* m) {
-  const __half* wp = reinterpret_cast<const __half*>(w_planes);
-  const __half* hp = reinterpret_cast<const __half*>(h_planes);
-  int rc;
-  if ((rc = make_map(&m[0], wp, (uint64_t)J, (uint64_t)Kp, BM, 128, 1))) return rc;
-  if ((rc = make_map(&m[1], wp + (int64_t)J * Kp, (uint64_t)J, (uint64_t)Kp, BM, 128, 1)))
-    return rc;
-  if ((rc = make_map(&m[2], hp, (uint64_t)R, (uint64_t)Kp, BN, 128, 1))) return rc;
-  return make_map(&m[3], binary_h ? hp : hp + R * Kp, (uint64_t)R, (uint64_t)Kp, BN, 128, 1);
+// f(std::integral_constant<int, Z>()) with Z = 2 when operand B is a 0/1 sample whose planes are
+// its hi plane only (h_binary), else Z = 0
+template <class F>
+int with_h_binary(int h_binary, F f) {
+  if (h_binary) return f(std::integral_constant<int, 2>());
+  return f(std::integral_constant<int, 0>());
 }
 
 // One pass over an activation / gradient matrix that produces its operand planes:
@@ -647,12 +730,7 @@ __global__ void __launch_bounds__(256) split16_class_kernel(
       const int64_t r = rt + i;
 #pragma unroll
       for (int h = 0; h < 2; ++h)
-        if (r < R && col[h] < Kp) {
-          const float x = g[i][h] * s;
-          const __half hi = __float2half_rn(x);
-          planes[r * Kp + col[h]] = hi;
-          planes[n_pl + r * Kp + col[h]] = __float2half_rn(x - __half2float(hi));
-        }
+        if (r < R && col[h] < Kp) store_hilo(planes + r * Kp + col[h], n_pl, g[i][h] * s);
     }
   }
 }
@@ -679,21 +757,11 @@ __global__ void __launch_bounds__(256) noisy_split_kernel(
     const float* __restrict__ nr = noise + r * K;
     for (int k = tx; k < (PLANES ? Kp : K); k += 32) {
       const float x = k < K ? __ldg(hr + k) * nr[k] : 0.f;
-      if (PLANES) {
-        const float xs = x * s;
-        const __half hi = __float2half_rn(xs);
-        planes[r * Kp + k] = hi;
-        planes[n_pl + r * Kp + k] = __float2half_rn(xs - __half2float(hi));
-      } else {
-        const float a = fabsf(x);
-        m = (a <= 3.0e38f) ? fmaxf(m, a) : m;
-      }
+      if (PLANES) store_hilo(planes + r * Kp + k, n_pl, x * s);
+      else m = finite_absmax(m, x);
     }
   }
-  if (!PLANES) {
-    m = warp_max(m);
-    if (tx == 0) atomicMax(reinterpret_cast<unsigned int*>(scale) + 2, __float_as_uint(m));
-  }
+  if (!PLANES) fold_amax(scale, m, tx);
 }
 
 // Chan's update of (count n, mean, M2) with a second set (nb, mb, qb)
@@ -762,11 +830,7 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const float* __restrict__
       out[r * J + j] = y;
       m = fmaxf(m, fabsf(y));
     }
-  if (amax_scale) {
-    m = warp_max(m <= 3.0e38f ? m : 0.f);
-    if (tx == 0 && m > 0.f)
-      atomicMax(reinterpret_cast<unsigned int*>(amax_scale) + 2, __float_as_uint(m));
-  }
+  if (amax_scale) fold_amax(amax_scale, m <= 3.0e38f ? m : 0.f, tx);
 }
 
 // Backward, per 128-row tile t and column j (block: 32 columns x 8 warps, 16 rows per warp, then
@@ -857,20 +921,10 @@ __global__ void __launch_bounds__(256) bn_grad_apply_kernel(
         }
         d = rs * gg;
       }
-      if (PLANES) {
-        const float ds = d * s;
-        const __half hi = __float2half_rn(ds);
-        planes[r * Jp + j] = hi;
-        planes[n_pl + r * Jp + j] = __float2half_rn(ds - __half2float(hi));
-      } else {
-        const float ad = fabsf(d);
-        m = (ad <= 3.0e38f) ? fmaxf(m, ad) : m;
-      }
+      if (PLANES) store_hilo(planes + r * Jp + j, n_pl, d * s);
+      else m = finite_absmax(m, d);
     }
-  if (!PLANES) {
-    m = warp_max(m);
-    if (tx == 0) atomicMax(reinterpret_cast<unsigned int*>(scale) + 2, __float_as_uint(m));
-  }
+  if (!PLANES) fold_amax(scale, m, tx);
 }
 
 // From d = d(h * noise) [R, K]: dnoise[r] = d[r] * h[r % n_h] and dh[i] = sum_s d[s n_h + i] *
@@ -896,10 +950,10 @@ __global__ void __launch_bounds__(256) noisy_grad_kernel(
     }
 }
 
-// blocks of an elementwise 32 x 8 pass over `rows` rows
-inline unsigned row_blocks(int64_t rows) {
-  int64_t b = (rows + 7) / 8;
-  if (b > ZSB_NUM_SMS * 16) b = ZSB_NUM_SMS * 16;
+// blocks of a grid-stride pass over n items at `per` items per block, at most per_sm per SM
+inline unsigned grid_blocks(int64_t n, int64_t per, int per_sm) {
+  int64_t b = zsb_ceil_div(n, per);
+  if (b > ZSB_NUM_SMS * per_sm) b = ZSB_NUM_SMS * per_sm;
   return (unsigned)(b < 1 ? 1 : b);
 }
 
@@ -908,39 +962,22 @@ __global__ void __launch_bounds__(256) absmax2_kernel(const float* __restrict__ 
                                                       float* __restrict__ scale) {
   float m = 0.f;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    const float a = fabsf(src[i]);
-    m = (a == a && a <= 3.0e38f) ? fmaxf(m, a) : m;
-  }
-  m = warp_max(m);
-  if ((threadIdx.x & 31) == 0)
-    atomicMax(reinterpret_cast<unsigned int*>(scale) + 2, __float_as_uint(m));
+       i += (int64_t)gridDim.x * blockDim.x)
+    m = finite_absmax(m, src[i]);
+  fold_amax(scale, m, threadIdx.x & 31);
 }
-// scale[0] = power of two s with max|src| * s in [2^11, 2^12), from the max in scale[2], which
-// it clears again for the next split
-__global__ void pow2_scale_kernel(float* __restrict__ scale) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  const float m = __uint_as_float(reinterpret_cast<unsigned int*>(scale)[2]);
-  int e = 0;
-  if (m > 0.f) frexpf(m, &e);
-  scale[0] = ldexpf(1.f, 12 - e);
-  reinterpret_cast<unsigned int*>(scale)[2] = 0u;
-}
-// As pow2_scale_kernel for the bound mult * max|src| (the class fold of split16_class_kernel adds
-// up to `mult` rows of src)
+// scale[0] = the plane scale of the bound mult * max|src|, from the max in scale[2], which it
+// clears again for the next split (mult > 1: the class fold of split16_class_kernel adds up to
+// `mult` rows of src)
 __global__ void pow2_scale_mult_kernel(float* __restrict__ scale, float mult) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  const float m = __uint_as_float(reinterpret_cast<unsigned int*>(scale)[2]) * mult;
-  int e = 0;
-  if (m > 0.f) frexpf(m, &e);
-  scale[0] = ldexpf(1.f, 12 - e);
+  scale[0] = pow2_plane_scale(__uint_as_float(reinterpret_cast<unsigned int*>(scale)[2]) * mult);
   reinterpret_cast<unsigned int*>(scale)[2] = 0u;
 }
 // max pass of an operand split: leaves scale[0]
-inline void launch_absmax_scale(const float* src, int64_t n, float* scale, unsigned blocks,
-                                cudaStream_t st) {
-  absmax2_kernel<<<blocks, 256, 0, st>>>(src, n, scale);
-  pow2_scale_kernel<<<1, 32, 0, st>>>(scale);
+inline void launch_absmax_scale(const float* src, int64_t n, float* scale, cudaStream_t st) {
+  absmax2_kernel<<<grid_blocks(n, 256 * 8, 16), 256, 0, st>>>(src, n, scale);
+  pow2_scale_mult_kernel<<<1, 32, 0, st>>>(scale, 1.f);
 }
 // src [rows, K] fp32 -> planes [2][rows][Kp] fp16 (hi, lo) of src * scale, zero padded to Kp
 __global__ void __launch_bounds__(256) split16_pad_kernel(const float* __restrict__ src,
@@ -953,10 +990,7 @@ __global__ void __launch_bounds__(256) split16_pad_kernel(const float* __restric
        i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = i / Kp;
     const int k = (int)(i - r * Kp);
-    const float x = (k < K) ? src[r * K + k] * s : 0.f;
-    const __half h = __float2half_rn(x);
-    planes[i] = h;
-    planes[n + i] = __float2half_rn(x - __half2float(h));
+    store_hilo(planes + i, n, (k < K) ? src[r * K + k] * s : 0.f);
   }
 }
 // out[i] = sum_s scratch[s][i]
@@ -980,6 +1014,13 @@ __global__ void __launch_bounds__(256) part_sum_kernel(const float* __restrict__
     out[r] = s;
   }
 }
+// out[r] = the sum of the partial rows part [nparts(J)][rows] that EPI 1 / 4 / 5 write
+int launch_part_sum(const float* part, int J, int64_t rows, float* out, cudaStream_t st,
+                    const char* what) {
+  part_sum_kernel<<<grid_blocks(rows, 256, 8), 256, 0, st>>>(part, zsb_linear_tc_nparts(J), rows,
+                                                             out);
+  return zsb_check_launch(what);
+}
 
 // zsb_linear_tc_amax_f32 (Z = 0) and zsb_linear_tc_bin_f32 (Z = 2: h is a 0/1 sample)
 template <int Z>
@@ -994,26 +1035,15 @@ int linear_tc_amax(int epi, const void* w_planes, const float* scale_w, const vo
   ZSB_REQUIRE(epi == 0 || (x_obs && n_x > 0), "zsb_linear_tc_f32: observations missing");
   ZSB_REQUIRE(epi != 1 || part, "zsb_linear_tc_f32: partial-sum scratch missing");
   ZSB_REQUIRE(epi != 2 || gout, "zsb_linear_tc_f32: upstream gradient missing");
-  const int Kp = zsb_linear_tc_kpad(K);
-  CUtensorMap m[4];
-  int rc;
-  if ((rc = linear_maps(w_planes, h_planes, Z & 2, R, J, Kp, m))) return rc;
-  const CUtensorMap &m_whi = m[0], &m_wlo = m[1], &m_hhi = m[2], &m_hlo = m[3];
-  const int n_blk = (J + BM - 1) / BM;
-  if (epi == 0)
-    rc = launch_linear<0, 0, Z>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out, part, R,
-                                J, Kp, relu, scale_w, scale_h, 1, amax_scale, st, "linear_tc");
-  else if (epi == 1)
-    rc = launch_linear<1, 0, Z>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, nullptr, part,
-                                R, J, Kp, relu, scale_w, scale_h, 1, amax_scale, st, "linear_tc");
-  else
-    rc = launch_linear<2, 0, Z>(m_whi, m_wlo, m_hhi, m_hlo, bias, x_obs, n_x, gout, out, part, R,
-                                J, Kp, relu, scale_w, scale_h, 1, amax_scale, st, "linear_tc");
-  if (rc != ZSB_OK || epi != 1) return rc;
-  int64_t blocks = zsb_ceil_div(R, 256);
-  if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
-  part_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, 4 * n_blk, R, out);
-  return zsb_check_launch("linear_tc_part_sum");
+  LinCore<0, Z> c;
+  int rc = make_core(c, w_planes, scale_w, h_planes, scale_h, J, R, K);
+  if (rc) return rc;
+  const RowsEpi e{.bias = bias, .x_obs = x_obs, .n_x = n_x, .gout = gout, .out = out,
+                  .part = part, .relu = relu, .amax_scale = amax_scale};
+  if (epi == 0) return tc_launch(LinW<RowsEpi, 0, 0, Z>{c, e}, st, "linear_tc");
+  if (epi == 2) return tc_launch(LinW<RowsEpi, 2, 0, Z>{c, e}, st, "linear_tc");
+  rc = tc_launch(LinW<RowsEpi, 1, 0, Z>{c, e}, st, "linear_tc");
+  return rc ? rc : launch_part_sum(part, J, R, out, st, "linear_tc_part_sum");
 }
 
 // zsb_linear_tc_wgrad_f32 (Z = 0) and zsb_linear_tc_wgrad_bin_f32 (Z = 1: h is a 0/1 sample)
@@ -1024,31 +1054,17 @@ int linear_tc_wgrad(const void* h_planes, const float* scale_h, int K, const voi
   ZSB_REQUIRE(h_planes && g_planes && scale_h && scale_g && out && R > 0 && J > 0 && K > 0,
               "zsb_linear_tc_wgrad_f32: bad args");
   ZSB_REQUIRE(R < (1LL << 31) - 64, "zsb_linear_tc_wgrad_f32: too many rows");
-  const int Kp_h = zsb_linear_tc_kpad(K), Jp_g = zsb_linear_tc_kpad(J);
-  const int Rp = zsb_linear_tc_kpad((int)R);                 // padded contraction length
-  const __half* hp = reinterpret_cast<const __half*>(h_planes);
-  const __half* gp = reinterpret_cast<const __half*>(g_planes);
-  CUtensorMap m_whi, m_wlo, m_hhi, m_hlo;                    // "w" = h (rows = k), "h" = g
-  int rc;
-  if ((rc = make_map(&m_whi, hp, (uint64_t)R, (uint64_t)Kp_h, 64, 128, 1))) return rc;
-  if ((rc = make_map(&m_wlo, (Z & 1) ? hp : hp + R * Kp_h, (uint64_t)R, (uint64_t)Kp_h, 64, 128, 1))) return rc;
-  if ((rc = make_map(&m_hhi, gp, (uint64_t)R, (uint64_t)Jp_g, 64, 128, 1))) return rc;
-  if ((rc = make_map(&m_hlo, gp + R * Jp_g, (uint64_t)R, (uint64_t)Jp_g, 64, 128, 1))) return rc;
   const int k_slices = part ? zsb_linear_tc_slices(J, K, (int)R) : 1;
-  rc = launch_linear<0, 3, Z>(m_whi, m_wlo, m_hhi, m_hlo, nullptr, nullptr, 0, nullptr,
-                           k_slices > 1 ? part : out, part, (int64_t)J, K, Rp, 0, scale_h,
-                           scale_g, k_slices, nullptr, st, "linear_tc_wgrad");
-
-  if (rc == ZSB_OK && k_slices > 1) {
-    const int64_t n = (int64_t)J * K;
-    int64_t blocks = zsb_ceil_div(n, 256);
-    if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
-    slice_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, k_slices, n, out);
-    return zsb_check_launch("linear_tc_wgrad_slice_sum");
-  }
-  return rc;
+  LinCore<3, Z> c;              // A = h (K features), B = g (J rows), contraction over the R rows
+  int rc = make_core(c, h_planes, scale_h, g_planes, scale_g, K, J, R, k_slices);
+  if (rc) return rc;
+  rc = tc_launch(LinW<RowsEpi, 0, 3, Z>{c, {.out = k_slices > 1 ? part : out}}, st,
+                 "linear_tc_wgrad");
+  if (rc != ZSB_OK || k_slices == 1) return rc;
+  const int64_t n = (int64_t)J * K;
+  slice_sum_kernel<<<grid_blocks(n, 256, 8), 256, 0, st>>>(part, k_slices, n, out);
+  return zsb_check_launch("linear_tc_wgrad_slice_sum");
 }
-
 
 }  // namespace
 
@@ -1065,15 +1081,9 @@ int zsb_split16_pad_f32(const float* src, int64_t rows, int K, void* planes, flo
   ZSB_REQUIRE(src && planes && scale && rows > 0 && K > 0, "zsb_split16_pad_f32: bad args");
   cudaStream_t st = (cudaStream_t)stream;
   const int Kp = zsb_linear_tc_kpad(K);
-  const int64_t n = rows * (int64_t)K;
-  int64_t blocks = zsb_ceil_div(n, 256 * 8);
-  if (blocks > ZSB_NUM_SMS * 16) blocks = ZSB_NUM_SMS * 16;
-  if (blocks < 1) blocks = 1;
-  launch_absmax_scale(src, n, scale, (unsigned)blocks, st);
-  int64_t blocks2 = zsb_ceil_div(rows * (int64_t)Kp, 256 * 4);
-  if (blocks2 > ZSB_NUM_SMS * 32) blocks2 = ZSB_NUM_SMS * 32;
-  split16_pad_kernel<<<(unsigned)blocks2, 256, 0, st>>>(src, rows, K, Kp,
-                                                        reinterpret_cast<__half*>(planes), scale);
+  launch_absmax_scale(src, rows * (int64_t)K, scale, st);
+  split16_pad_kernel<<<grid_blocks(rows * (int64_t)Kp, 256 * 4, 32), 256, 0, st>>>(
+      src, rows, K, Kp, reinterpret_cast<__half*>(planes), scale);
   return zsb_check_launch("split16_pad");
 }
 
@@ -1087,17 +1097,11 @@ int zsb_split16_dual_f32(const float* src, const float* mask_src, int64_t R, int
               "zsb_split16_dual_f32: bad args (K must be even)");
   cudaStream_t st = (cudaStream_t)stream;
   const int Kp = zsb_linear_tc_kpad(K);
-  if (!have_amax) {
-    const int64_t n = R * (int64_t)K;
-    int64_t blocks = zsb_ceil_div(n, 256 * 8);
-    if (blocks > ZSB_NUM_SMS * 16) blocks = ZSB_NUM_SMS * 16;
-    launch_absmax_scale(src, n, scale, (unsigned)blocks, st);
-  } else {
-    pow2_scale_kernel<<<1, 32, 0, st>>>(scale);    // max|src| left in scale[2] by a GEMM epilogue
-  }
-  int64_t tiles = ((R + 63) / 64) * ((Kp + 63) / 64);
-  if (tiles > ZSB_NUM_SMS * 16) tiles = ZSB_NUM_SMS * 16;
-  split16_dual_kernel<<<(unsigned)tiles, 256, 0, st>>>(
+  if (!have_amax)
+    launch_absmax_scale(src, R * (int64_t)K, scale, st);
+  else
+    pow2_scale_mult_kernel<<<1, 32, 0, st>>>(scale, 1.f);   // max|src| left by a GEMM epilogue
+  split16_dual_kernel<<<grid_blocks(((R + 63) / 64) * (Kp / 64), 1, 16), 256, 0, st>>>(
       src, mask_src, R, K, Kp, reinterpret_cast<__half*>(planes), col_sum, scale);
   return zsb_check_launch("split16_dual");
 }
@@ -1170,27 +1174,18 @@ int zsb_linear_tc_dgrad_f32(const void* w_planes, const float* scale_w, const vo
   ZSB_REQUIRE(w_planes && g_planes && scale_w && scale_g && out && R > 0 && J > 0 && K > 0,
               "zsb_linear_tc_dgrad_f32: bad args");
   ZSB_REQUIRE(R < (1LL << 31), "zsb_linear_tc_dgrad_f32: too many rows");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int Kp_w = zsb_linear_tc_kpad(K), Jp = zsb_linear_tc_kpad(J);
-  const __half* wp = reinterpret_cast<const __half*>(w_planes);
-  const __half* gp = reinterpret_cast<const __half*>(g_planes);
-  CUtensorMap m_whi, m_wlo, m_hhi, m_hlo;
-  int rc;
-  if ((rc = make_map(&m_whi, wp, (uint64_t)J, (uint64_t)Kp_w, 64, 128, 1))) return rc;
-  if ((rc = make_map(&m_wlo, wp + (int64_t)J * Kp_w, (uint64_t)J, (uint64_t)Kp_w, 64, 128, 1)))
-    return rc;
-  if ((rc = make_map(&m_hhi, gp, (uint64_t)R, (uint64_t)Jp, BN, 128, 1))) return rc;
-  if ((rc = make_map(&m_hlo, gp + R * Jp, (uint64_t)R, (uint64_t)Jp, BN, 128, 1))) return rc;
-  return launch_linear<0, 1>(m_whi, m_wlo, m_hhi, m_hlo, nullptr, nullptr, 0, nullptr, out,
-                             nullptr, R, K, Jp, 0, scale_w, scale_g, 1, amax_scale, st,
-                             "linear_tc_dgrad");
+  LinCore<1, 0> c;              // A = W (K features), B = g (R rows), contraction over J
+  const int rc = make_core(c, w_planes, scale_w, g_planes, scale_g, K, R, J);
+  if (rc) return rc;
+  return tc_launch(LinW<RowsEpi, 0, 1>{c, {.out = out, .amax_scale = amax_scale}},
+                   (cudaStream_t)stream, "linear_tc_dgrad");
 }
 
 // Weight gradient of a dense layer WITHOUT transposed operands:
 //   out [J, K] = sum_r g[r, j] * h[r, k]            (dW = g^T h, tf.gradients of tf.layers.dense)
 // h_planes [2][R][Kp(K)], g_planes [2][R][Kp(J)]: the row-major fp16 hi/lo planes the forward /
 // input-gradient products already use (zsb_split16_pad_f32 / zsb_split16_dual_f32).  The contraction
-// runs over the rows, so both operands are MN-major wgmma operands (LinW<0, 3>);
+// runs over the rows, so both operands are MN-major wgmma operands (MN = 3);
 // split-K over the SMs (part = zsb_linear_tc_slices(J, K, R) * J * K floats, or NULL for a single
 // slice).
 int zsb_linear_tc_wgrad_f32(const void* h_planes, const float* scale_h, int K,
@@ -1224,28 +1219,19 @@ int zsb_linear_tc_bern_sample_f32(const void* w_planes, const float* scale_w, co
               "zsb_linear_tc_bern_sample_f32: bad args");
   ZSB_REQUIRE((int64_t)S * R < (1LL << 31), "zsb_linear_tc_bern_sample_f32: too many rows");
   cudaStream_t st = (cudaStream_t)stream;
-  const int Kp = zsb_linear_tc_kpad(K);
-  CUtensorMap m[4];
-  int rc;
-  if ((rc = linear_maps(w_planes, h_planes, h_binary, R, J, Kp, m))) return rc;
-  auto fill = [&](auto w) {
-    w.S = S; w.u_in = u_in; w.seed = seed; w.iter = iter; w.epoch = zsb_epoch_ptr();
-    w.h_int = h_int; w.pl_out = reinterpret_cast<__half*>(h_planes_out);
-    return tc_launch(chunk_samples(w), st, "linear_tc_bern_sample");
-  };
-  float* ho = reinterpret_cast<float*>(h_out);
-  if (h_binary)
-    rc = fill(make_linw<4, 0, 2>(m[0], m[1], m[2], m[3], bias, nullptr, 0, nullptr, ho, part, R,
-                                 J, Kp, 0, scale_w, scale_h, 1, nullptr));
-  else
-    rc = fill(make_linw<4, 0, 0>(m[0], m[1], m[2], m[3], bias, nullptr, 0, nullptr, ho, part, R,
-                                 J, Kp, 0, scale_w, scale_h, 1, nullptr));
-  if (rc != ZSB_OK) return rc;
-  const int64_t SR = (int64_t)S * R;
-  int64_t blocks = zsb_ceil_div(SR, 256);
-  if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
-  part_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, 4 * ((J + BM - 1) / BM), SR, logq);
-  return zsb_check_launch("linear_tc_bern_sample_part_sum");
+  const int s_per = sample_chunk(R, J, S);
+  const SamplesEpi e{.bias = bias, .out = reinterpret_cast<float*>(h_out), .part = part, .S = S,
+                     .s_per = s_per, .u_in = u_in, .seed = seed, .iter = iter,
+                     .epoch = zsb_epoch_ptr(), .h_int = h_int,
+                     .pl_out = reinterpret_cast<__half*>(h_planes_out)};
+  return with_h_binary(h_binary, [&](auto z) {
+    LinCore<0, z> c;
+    int rc = make_core(c, w_planes, scale_w, h_planes, scale_h, J, R, K, (S + s_per - 1) / s_per);
+    if (rc) return rc;
+    rc = tc_launch(LinW<SamplesEpi, 4, 0, z>{c, e}, st, "linear_tc_bern_sample");
+    if (rc) return rc;
+    return launch_part_sum(part, J, (int64_t)S * R, logq, st, "linear_tc_bern_sample_part_sum");
+  });
 }
 
 // Bernoulli layer against S given rows per logit row, l[r] = (h W^T + bias)[r]:
@@ -1264,30 +1250,18 @@ int zsb_linear_tc_bern_given_f32(int epi, const void* w_planes, const float* sca
               "zsb_linear_tc_bern_given_f32: bad args");
   ZSB_REQUIRE((int64_t)S * R < (1LL << 31), "zsb_linear_tc_bern_given_f32: too many rows");
   cudaStream_t st = (cudaStream_t)stream;
-  const int Kp = zsb_linear_tc_kpad(K);
-  CUtensorMap m[4];
-  int rc;
-  if ((rc = linear_maps(w_planes, h_planes, h_binary, R, J, Kp, m))) return rc;
-  auto fill = [&](auto w) {
-    w.S = S;
-    w.s_per = S;                          // EPI 6 sums over the draws: one chunk
-    return tc_launch(epi == 1 ? chunk_samples(w) : w, st, "linear_tc_bern_given");
-  };
-#define ZSB_GIVEN(E, Z)                                                                       \
-  fill(make_linw<E, 0, Z>(m[0], m[1], m[2], m[3], bias, given, (int64_t)S * R, gout,          \
-                          epi == 2 ? out : nullptr, part, R, J, Kp, 0, scale_w, scale_h, 1,    \
-                          epi == 2 ? amax_scale : nullptr))
-  if (epi == 1)
-    rc = h_binary ? ZSB_GIVEN(5, 2) : ZSB_GIVEN(5, 0);
-  else
-    rc = h_binary ? ZSB_GIVEN(6, 2) : ZSB_GIVEN(6, 0);
-#undef ZSB_GIVEN
-  if (rc != ZSB_OK || epi != 1) return rc;
-  const int64_t SR = (int64_t)S * R;
-  int64_t blocks = zsb_ceil_div(SR, 256);
-  if (blocks > ZSB_NUM_SMS * 8) blocks = ZSB_NUM_SMS * 8;
-  part_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, 4 * ((J + BM - 1) / BM), SR, out);
-  return zsb_check_launch("linear_tc_bern_given_part_sum");
+  const int s_per = epi == 1 ? sample_chunk(R, J, S) : S;   // EPI 6 sums over the draws: one chunk
+  const SamplesEpi e{.bias = bias, .x_obs = given, .gout = gout, .out = out, .part = part, .S = S,
+                     .s_per = s_per, .amax_scale = amax_scale};
+  return with_h_binary(h_binary, [&](auto z) {
+    LinCore<0, z> c;
+    int rc = make_core(c, w_planes, scale_w, h_planes, scale_h, J, R, K, (S + s_per - 1) / s_per);
+    if (rc) return rc;
+    if (epi == 2) return tc_launch(LinW<SamplesEpi, 6, 0, z>{c, e}, st, "linear_tc_bern_given");
+    rc = tc_launch(LinW<SamplesEpi, 5, 0, z>{c, e}, st, "linear_tc_bern_given");
+    if (rc) return rc;
+    return launch_part_sum(part, J, (int64_t)S * R, out, st, "linear_tc_bern_given_part_sum");
+  });
 }
 
 // Class-conditioned dense layer (EPI 7 / 8): l = h W^T + bias plus row y of the class table
@@ -1306,23 +1280,15 @@ int zsb_linear_tc_class_f32(const void* w_planes, const float* scale_w, const vo
               "zsb_linear_tc_class_f32: bad args");
   ZSB_REQUIRE(R < (1LL << 31), "zsb_linear_tc_class_f32: too many rows");
   cudaStream_t st = (cudaStream_t)stream;
-  const int Kp = zsb_linear_tc_kpad(K);
-  CUtensorMap m[4];
-  int rc;
-  if ((rc = linear_maps(w_planes, h_planes, h_binary, R, J, Kp, m))) return rc;
-  auto fill = [&](auto w) {
-    w.ctab = ctab; w.C = C; w.cls = cls; w.n_cls = n_cls;
-    return tc_launch(w, st, "linear_tc_class");
-  };
-#define ZSB_CLASS(E, Z)                                                                        \
-  fill(make_linw<E, 0, Z>(m[0], m[1], m[2], m[3], bias, nullptr, 0, nullptr, out, nullptr, R, J, \
-                          Kp, relu, scale_w, scale_h, 1, amax_scale))
-  if (cls)
-    rc = h_binary ? ZSB_CLASS(7, 2) : ZSB_CLASS(7, 0);
-  else
-    rc = h_binary ? ZSB_CLASS(8, 2) : ZSB_CLASS(8, 0);
-#undef ZSB_CLASS
-  return rc;
+  const ClassEpi e{.bias = bias, .ctab = ctab, .C = C, .cls = cls, .n_cls = n_cls, .out = out,
+                   .relu = relu, .amax_scale = amax_scale};
+  return with_h_binary(h_binary, [&](auto z) {
+    LinCore<0, z> c;
+    const int rc = make_core(c, w_planes, scale_w, h_planes, scale_h, J, R, K);
+    if (rc) return rc;
+    if (cls) return tc_launch(LinW<ClassEpi, 7, 0, z>{c, e}, st, "linear_tc_class");
+    return tc_launch(LinW<ClassEpi, 8, 0, z>{c, e}, st, "linear_tc_class");
+  });
 }
 
 // The backward pass of zsb_linear_tc_class_f32 in one pass (split16_class_kernel) over the upstream
@@ -1341,17 +1307,11 @@ int zsb_split16_class_f32(const float* src, const float* mask_src, int64_t R, in
   cudaStream_t st = (cudaStream_t)stream;
   const int Kp = zsb_linear_tc_kpad(K);
   const int64_t n = (cls ? 1 : C) * R * (int64_t)K;
-  if (!have_amax) {
-    int64_t blocks = zsb_ceil_div(n, 256 * 8);
-    if (blocks > ZSB_NUM_SMS * 16) blocks = ZSB_NUM_SMS * 16;
-    absmax2_kernel<<<(unsigned)blocks, 256, 0, st>>>(src, n, scale);
-  }
+  if (!have_amax) absmax2_kernel<<<grid_blocks(n, 256 * 8, 16), 256, 0, st>>>(src, n, scale);
   pow2_scale_mult_kernel<<<1, 32, 0, st>>>(scale, cls ? 1.f : (float)C);
-  int64_t tiles = ((R + 63) / 64) * ((Kp + 63) / 64);
-  if (tiles > ZSB_NUM_SMS * 16) tiles = ZSB_NUM_SMS * 16;
-  split16_class_kernel<<<(unsigned)tiles, 256, 0, st>>>(src, mask_src, R, K, Kp, cls, n_cls, C,
-                                                        reinterpret_cast<__half*>(planes), col_sum,
-                                                        dtab, scale);
+  split16_class_kernel<<<grid_blocks(((R + 63) / 64) * (Kp / 64), 1, 16), 256, 0, st>>>(
+      src, mask_src, R, K, Kp, cls, n_cls, C, reinterpret_cast<__half*>(planes), col_sum, dtab,
+      scale);
   return zsb_check_launch("split16_class");
 }
 
@@ -1365,9 +1325,10 @@ int zsb_split16_noisy_f32(const float* h, int64_t n_h, const float* noise, int64
   cudaStream_t st = (cudaStream_t)stream;
   const int Kp = zsb_linear_tc_kpad(K);
   __half* pl = reinterpret_cast<__half*>(planes);
-  noisy_split_kernel<false><<<row_blocks(R), 256, 0, st>>>(h, n_h, noise, R, K, Kp, pl, scale);
-  pow2_scale_kernel<<<1, 32, 0, st>>>(scale);
-  noisy_split_kernel<true><<<row_blocks(R), 256, 0, st>>>(h, n_h, noise, R, K, Kp, pl, scale);
+  const unsigned blocks = grid_blocks(R, 8, 16);
+  noisy_split_kernel<false><<<blocks, 256, 0, st>>>(h, n_h, noise, R, K, Kp, pl, scale);
+  pow2_scale_mult_kernel<<<1, 32, 0, st>>>(scale, 1.f);
+  noisy_split_kernel<true><<<blocks, 256, 0, st>>>(h, n_h, noise, R, K, Kp, pl, scale);
   return zsb_check_launch("split16_noisy");
 }
 
@@ -1390,27 +1351,24 @@ int zsb_linear_tc_bn_f32(int training, const void* w_planes, const float* scale_
               "zsb_linear_tc_bn_f32: bad args");
   ZSB_REQUIRE(R < (1LL << 31), "zsb_linear_tc_bn_f32: too many rows");
   cudaStream_t st = (cudaStream_t)stream;
-  const int Kp = zsb_linear_tc_kpad(K);
-  CUtensorMap m[4];
-  int rc;
-  if ((rc = linear_maps(w_planes, h_planes, 0, R, J, Kp, m))) return rc;
+  LinCore<0, 0> c;
+  int rc = make_core(c, w_planes, scale_w, h_planes, scale_h, J, R, K);
+  if (rc) return rc;
   const unsigned col_blocks = (unsigned)((J + 7) / 8);
   if (!training) {
     bn_stats_kernel<<<col_blocks, 256, 0, st>>>(nullptr, R, J, moving_mean, moving_var, rate, eps,
                                                 0, stats);
     if ((rc = zsb_check_launch("linear_tc_bn_stats")) != ZSB_OK) return rc;
-    auto w = make_linw<10, 0>(m[0], m[1], m[2], m[3], nullptr, nullptr, 0, nullptr, out, nullptr,
-                              R, J, Kp, relu, scale_w, scale_h, 1, amax_scale);
-    w.bn_stats = stats;
-    w.bn_beta = beta;
-    return tc_launch(w, st, "linear_tc_bn_eval");
+    const BnEpi e{.bn_stats = stats, .bn_beta = beta, .out = out, .relu = relu,
+                  .amax_scale = amax_scale};
+    return tc_launch(LinW<BnEpi, 10>{c, e}, st, "linear_tc_bn_eval");
   }
-  rc = launch_linear<9, 0>(m[0], m[1], m[2], m[3], nullptr, nullptr, 0, nullptr, a, part, R, J,
-                           Kp, relu, scale_w, scale_h, 1, nullptr, st, "linear_tc_bn_train");
+  rc = tc_launch(LinW<BnEpi, 9>{c, {.out = a, .part = part}}, st, "linear_tc_bn_train");
   if (rc != ZSB_OK) return rc;
   bn_stats_kernel<<<col_blocks, 256, 0, st>>>(part, R, J, moving_mean, moving_var, rate, eps, 1,
                                               stats);
-  bn_apply_kernel<<<row_blocks(R), 256, 0, st>>>(a, R, J, stats, beta, relu, out, amax_scale);
+  bn_apply_kernel<<<grid_blocks(R, 8, 16), 256, 0, st>>>(a, R, J, stats, beta, relu, out,
+                                                         amax_scale);
   return zsb_check_launch("linear_tc_bn_apply");
 }
 
@@ -1438,11 +1396,12 @@ int zsb_bn_grad_f32(int training, const float* g, const float* y, const float* a
       g, y, at, stats, relu, R, J, part);
   bn_grad_combine_kernel<<<(unsigned)((J + 7) / 8), 256, 0, st>>>(part, R, J, dbeta, coef);
   __half* pl = reinterpret_cast<__half*>(planes);
-  bn_grad_apply_kernel<false><<<row_blocks(R), 256, 0, st>>>(g, y, at, stats, coef, relu, R, J, Jp,
-                                                             pl, scale);
-  pow2_scale_kernel<<<1, 32, 0, st>>>(scale);
-  bn_grad_apply_kernel<true><<<row_blocks(R), 256, 0, st>>>(g, y, at, stats, coef, relu, R, J, Jp,
-                                                            pl, scale);
+  const unsigned blocks = grid_blocks(R, 8, 16);
+  bn_grad_apply_kernel<false><<<blocks, 256, 0, st>>>(g, y, at, stats, coef, relu, R, J, Jp, pl,
+                                                      scale);
+  pow2_scale_mult_kernel<<<1, 32, 0, st>>>(scale, 1.f);
+  bn_grad_apply_kernel<true><<<blocks, 256, 0, st>>>(g, y, at, stats, coef, relu, R, J, Jp, pl,
+                                                     scale);
   return zsb_check_launch("bn_grad");
 }
 
@@ -1453,8 +1412,8 @@ int zsb_noisy_grad_f32(const float* d, const float* h, int64_t n_h, const float*
                        int K, float* dnoise, float* dh, void* stream) {
   ZSB_REQUIRE(d && h && noise && R > 0 && K > 0 && n_h > 0 && R % n_h == 0,
               "zsb_noisy_grad_f32: bad args");
-  noisy_grad_kernel<<<row_blocks(n_h), 256, 0, (cudaStream_t)stream>>>(d, h, n_h, noise, R, K,
-                                                                       dnoise, dh);
+  noisy_grad_kernel<<<grid_blocks(n_h, 8, 16), 256, 0, (cudaStream_t)stream>>>(d, h, n_h, noise, R,
+                                                                             K, dnoise, dh);
   return zsb_check_launch("noisy_grad");
 }
 

@@ -38,11 +38,6 @@ constexpr float kHalfOverflow = 65520.f;   // fp16 round-to-nearest gives inf fr
 __device__ __forceinline__ const float* scale_rec(const float* scales, int pass) {
   return scales + kScaleHdr + kScaleRec * pass;
 }
-__device__ __forceinline__ float pow2_plane_scale(float m) {
-  int e = 0;
-  if (m > 0.f) frexpf(m, &e);             // m = f * 2^e, f in [0.5, 1)  ->  m < 2^e
-  return ldexpf(1.f, 12 - e);             // m * sq in [2^11, 2^12)
-}
 // impl 5: pass `pass` reads the spare copy of its planes
 __device__ __forceinline__ bool plane_spare_in(const float* scales, int pass) {
   return pass > 0 && __float_as_uint(scale_rec(scales, pass)[3]) != 0u;
@@ -62,11 +57,6 @@ __device__ __forceinline__ float next_plane_scale(const float* __restrict__ scal
   // rejected
   if (bound * sq < kPlaneKeep || !(bound <= 3.0e38f)) return sq;
   return pow2_plane_scale(bound);
-}
-// max over finite |x| (NaN / inf are left to the chain that produced them)
-__device__ __forceinline__ float finite_absmax(float m, float x) {
-  const float a = fabsf(x);
-  return (a <= 3.0e38f) ? fmaxf(m, a) : m;
 }
 // end of a pass that wrote planes: the warp's bound of max|q_next| (and overflow flag) into record
 // pass + 1; block 0 publishes the scales of those planes and clears record pass + 2

@@ -240,6 +240,31 @@ __device__ __forceinline__ float warp_transpose_sum16(float v[16], int lane) {
   return v[0];
 }
 
+// The fp16 operand-plane format of every fp32 matrix the products read: planes [2][rows][cols] of
+// x * s, hi = fp16(x s) and lo = fp16(x s - hi), for a power of two s that puts max |x| in
+// [2^11, 2^12).  A split finds max |x| by folding it into word 2 of its scale slot.
+__device__ __forceinline__ float pow2_plane_scale(float m) {
+  int e = 0;
+  if (m > 0.f) frexpf(m, &e);             // m = f * 2^e, f in [0.5, 1)  ->  m < 2^e
+  return ldexpf(1.f, 12 - e);             // m * sq in [2^11, 2^12)
+}
+// max over finite |x| (NaN / inf are left to the chain that produced them)
+__device__ __forceinline__ float finite_absmax(float m, float x) {
+  const float a = fabsf(x);
+  return (a <= 3.0e38f) ? fmaxf(m, a) : m;
+}
+// p[0] = hi, p[lo] = lo of the already scaled x (lo: offset of the lo plane)
+__device__ __forceinline__ void store_hilo(__half* p, int64_t lo, float x) {
+  const __half h = __float2half_rn(x);
+  p[0] = h;
+  p[lo] = __float2half_rn(x - __half2float(h));
+}
+// the warp's max of m (finite, >= 0) into scale[2] as uint bits, which order as the floats do
+__device__ __forceinline__ void fold_amax(float* scale, float m, int lane) {
+  m = warp_max(m);
+  if (lane == 0 && m > 0.f) atomicMax(reinterpret_cast<unsigned int*>(scale) + 2, __float_as_uint(m));
+}
+
 // One k-block (RB bytes of contraction per operand row) of the three split products for both
 // 64-row halves of the tile.  KIND 0: TF32 operands, 1: fp16.  MNA / MNB: operand read MN-major.
 // ZLO (fp16 only): bit 0 / bit 1 = the lo plane of operand A / B is identically zero (a 0/1

@@ -765,6 +765,26 @@ def _tag(t, amax):
     return t
 
 
+def _grad_weight_release(ctx, gpl, R, need):
+    """dW from the planes ``gpl`` of d/d(pre-activation) and the layer's saved input planes
+    ``ctx.hpl``; the layer then drops its saved planes."""
+    dW = _tc_grad_weight(gpl, ctx.hpl, R) if need else None
+    ctx.hpl = None
+    ctx.wpl = None
+    return dW
+
+
+def _grad_products(ctx, gpl, W, R, wpl, dh_shape, need_dh, need_dW):
+    """The backward products of a dense layer from the planes ``gpl`` of d/d(pre-activation): dh
+    (shaped ``dh_shape`` and tagged with its max |.|, from the forward planes ``wpl`` of W) and
+    dW (_grad_weight_release)."""
+    dh = None
+    if need_dh:
+        dh2, amax = _tc_grad_input(gpl, W, R, *wpl)
+        dh = _tag(dh2.reshape(dh_shape), amax)
+    return dh, _grad_weight_release(ctx, gpl, R, need_dW)
+
+
 class _Linear(torch.autograd.Function):
     """y = relu?(h W^T + b): forward and both backward products on the wgmma kernel at fp32
     accuracy (epi 0; the weight gradient reads the same row-major planes as MN-major operands, split-K).
@@ -799,13 +819,8 @@ class _Linear(torch.autograd.Function):
             if (has_b and need[2]) else None
         gpl = _tc_split_dual(g, mask=y if relu else None, amax=getattr(gy, "_zsb_amax", None),
                              col_sum=db)
-        dh = None
-        if need[0]:
-            dh2, amax = _tc_grad_input(gpl, W, R, *(ctx.wpl or (None, None)))
-            dh = _tag(dh2.reshape(tuple(lead) + (K,)), amax)
-        dW = _tc_grad_weight(gpl, ctx.hpl, R) if need[1] else None
-        ctx.hpl = None
-        ctx.wpl = None
+        dh, dW = _grad_products(ctx, gpl, W, R, ctx.wpl or (None, None), tuple(lead) + (K,),
+                                need[0], need[1])
         return dh, dW, db, None
 
 
@@ -852,12 +867,7 @@ class _LinearBernoulliLogProb(torch.autograd.Function):
         dl = _tc_linear(2, wp, ws, hpl.planes, hpl.scale, bias, x2, g, R, J, K, amax=amax,
                         binary=hpl.binary)
         dlpl = _tc_split_dual(dl, amax=amax, col_sum=db)
-        dh = None
-        if need[0]:
-            dh2, a2 = _tc_grad_input(dlpl, W, R, wp, ws)
-            dh = _tag(dh2.reshape(tuple(lead) + (K,)), a2)
-        dW = _tc_grad_weight(dlpl, hpl, R) if need[1] else None
-        ctx.hpl = None
+        dh, dW = _grad_products(ctx, dlpl, W, R, (wp, ws), tuple(lead) + (K,), need[0], need[1])
         return dh, dW, db, None
 
 
@@ -942,13 +952,7 @@ class _ClassLinear(torch.autograd.Function):
         dtab = torch.zeros((C, J), dtype=torch.float32, device=dev) if need[2] else None
         gpl = _tc_split_class(gy.reshape(-1, J), R, ctx.cls, C, mask=y if relu else None,
                               amax=getattr(gy, "_zsb_amax", None), col_sum=db, dtab=dtab)
-        dh = None
-        if need[0]:
-            dh2, amax = _tc_grad_input(gpl, W, R, *ctx.wpl)
-            dh = _tag(dh2.reshape(tuple(lead) + (K,)), amax)
-        dW = _tc_grad_weight(gpl, ctx.hpl, R) if need[1] else None
-        ctx.hpl = None
-        ctx.wpl = None
+        dh, dW = _grad_products(ctx, gpl, W, R, ctx.wpl, tuple(lead) + (K,), need[0], need[1])
         return dh, dW, None if dtab is None else dtab.t(), db, None, None
 
 
@@ -1045,9 +1049,7 @@ class _NoisyBNLinear(torch.autograd.Function):
                      ptr(dh), stream())
             dh = None if dh is None else dh.reshape(h_shape)
             dnoise = None if dnoise is None else dnoise.reshape(tuple(lead) + (K,))
-        dW = _tc_grad_weight(gpl, ctx.hpl, R) if need[2] else None
-        ctx.hpl = None
-        ctx.wpl = None
+        dW = _grad_weight_release(ctx, gpl, R, need[2])
         return dh, dnoise, dW, dbeta, None, None, None, None, None
 
 
@@ -1165,12 +1167,7 @@ class _LinearBernoulliGiven(torch.autograd.Function):
                  ptr(hpl.scale), int(hpl.binary), ptr(bias), ptr(x2), S, ptr(g), ptr(dl), None,
                  R, J, K, ptr(amax), stream())
         dlpl = _tc_split_dual(dl, amax=amax, col_sum=db)
-        dh = None
-        if need[0]:
-            dh2, a2 = _tc_grad_input(dlpl, W, R, wp, ws)
-            dh = _tag(dh2.reshape(tuple(lead) + (K,)), a2)
-        dW = _tc_grad_weight(dlpl, hpl, R) if need[1] else None
-        ctx.hpl = None
+        dh, dW = _grad_products(ctx, dlpl, W, R, (wp, ws), tuple(lead) + (K,), need[0], need[1])
         return dh, dW, db, None, None, None, None, None, None
 
 
