@@ -487,6 +487,31 @@ int zsb_pmf_logjoint_f32(const float* lat, const float* fixed, const int64_t* ro
                          int64_t K, int64_t n_rows, int64_t n_cols, int64_t D, int64_t chunk_size,
                          void* stream);
 
+/* ---- Planar normalizing flows (csrc/flows.cu; zhusuan/transform.py:70-198) --------------------
+ * A stack of n_iters planar flows along the last axis of z [R, d], parameters b [n_iters],
+ * aux_u [n_iters, d], w [n_iters, d] (the reference's param_b_i, aux_u_i, para_w_i stacked,
+ * transform.py:148-168).  Per flow (transform.py:161-194):
+ *   u = aux_u + w / (w.w) * (softplus(w.aux_u) - 1 - w.aux_u),  psi = u.w = softplus(w.aux_u) - 1
+ *   a = tanh(z.w + b),  log_q -= log(1 + psi (1 - a^2)),  z += a u
+ * with a stable softplus and no invertibility assert (psi > -1 by construction).  1 <= d <= 1024,
+ * n_iters >= 1, R >= 0.  No floating-point atomics: deterministic. */
+/* Forward, one launch (transform.py:148-194): z_out [R, d], lq_out [R] from z_in, lq_in.  ck: NULL,
+ * or [n_iters, R, d] receiving every flow's input z_{k-1}, which zsb_planar_flow_bwd_f32 reads. */
+int zsb_planar_flow_fwd_f32(const float* z_in, const float* lq_in, const float* b,
+                            const float* aux_u, const float* w, float* z_out, float* lq_out,
+                            float* ck, int64_t R, int64_t d, int64_t n_iters, void* stream);
+/* Warps of the backward sweep for these sizes; its `part` scratch is
+ * warps * n_iters * (2 d + 2) floats. */
+int zsb_planar_flow_warps(int64_t R, int64_t d, int64_t n_iters);
+/* Backward of transform.py:170-194, one sweep plus one merge launch.  gz_out [R, d] and glq [R]:
+ * upstream gradients of z_out and lq_out; gz_in [R, d] = d / d z_in (d / d lq_in is glq itself);
+ * db [n_iters], daux_u and dw [n_iters, d]: the parameter gradients through the reparameterisation
+ * of u (transform.py:161-164).  ck as written by the forward pass. */
+int zsb_planar_flow_bwd_f32(const float* ck, const float* gz_out, const float* glq,
+                            const float* b, const float* aux_u, const float* w, float* gz_in,
+                            float* part, float* db, float* daux_u, float* dw, int64_t R,
+                            int64_t d, int64_t n_iters, void* stream);
+
 /* ---- K5: SG-MCMC updates (zhusuan/sgmcmc.py) ------------------------------------------------ */
 int zsb_sgmcmc_parts(void);   /* capacity (floats) of every `part` scratch */
 int zsb_sgmcmc_sgld_f32(float* q, const float* g, const float* noise, float lr, int64_t chains,

@@ -1,0 +1,26 @@
+"""The planar-flow kernels of csrc/flows.cu keep everything in registers: in the built library every
+instance has no stack frame and no local memory, so none of them spills.  CPU only (reads the
+library's resource usage with cuobjdump)."""
+import os
+import re
+import subprocess
+
+import pytest
+
+from test_sass_mainloop import _cuobjdump
+from zhusuan_b200 import _lib
+
+
+def test_no_planar_flow_kernel_spills():
+    exe = _cuobjdump()
+    if exe is None:
+        pytest.skip("cuobjdump not found (CUDA toolkit bin/ not on PATH)")
+    assert os.path.exists(_lib.LIB_PATH), "library not built: " + _lib.LIB_PATH
+    out = subprocess.run([exe, "-res-usage", _lib.LIB_PATH], check=True, capture_output=True,
+                         text=True).stdout
+    found = re.findall(r"Function (\S*planar_flow_\w+):\s*\n\s*REG:(\d+) STACK:(\d+) SHARED:\d+ "
+                       r"LOCAL:(\d+)", out)
+    kinds = {re.search(r"planar_flow_(fwd|bwd|merge)_kernel", name).group(1) for name, *_ in found}
+    assert kinds == {"fwd", "bwd", "merge"}, kinds
+    for name, reg, stack, local in found:
+        assert int(stack) == 0 and int(local) == 0, (name, reg, stack, local)

@@ -18,6 +18,7 @@ from .framework import utils as _fw_utils
 from .hmc import *
 from .sgmcmc import *
 from .evaluation import *
+from .transform import *
 from .utils import (TensorArithmeticMixin, log_mean_exp, log_sum_exp,
                     merge_dicts)
 from .random import set_random_seed

@@ -825,8 +825,9 @@ class _Linear(torch.autograd.Function):
 
 
 def linear(h, W, b=None, relu=False):
-    """``relu?(h @ W.T + b)`` (``tf.layers.dense``) on the wgmma kernel."""
-    return _Linear.apply(h, W, b, bool(relu))
+    """``relu?(h @ W.T + b)`` (``tf.layers.dense``) on the wgmma kernel.  ``h`` may be a
+    ``StochasticTensor``, as a model's node fed straight to a dense layer is (vae_nf.py:23-24)."""
+    return _Linear.apply(_unwrap(h), W, b, bool(relu))
 
 
 class _LinearBernoulliLogProb(torch.autograd.Function):
