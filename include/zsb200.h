@@ -512,6 +512,33 @@ int zsb_planar_flow_bwd_f32(const float* ck, const float* gz_out, const float* g
                             float* part, float* db, float* daux_u, float* dw, int64_t R,
                             int64_t d, int64_t n_iters, void* stream);
 
+/* ---- Sparse-GP conditional moments (csrc/gp.cu; examples/gaussian_process/utils.py:52-90) -----
+ * gp_conditional(z, fz, x, full_cov=False, RBFKernel) for x [B, d], inducing points z [M, d],
+ * kernel scales s [d] (softplus(k_raw_scale), utils.py:16), Li = chol(Kzz)^-1 [M, M] (only its lower
+ * triangle is read) and V = fz Li^T [K, M].  With Kxz[b, m] = exp(-sum_j (x_bj - z_mj)^2 / s_j / 2)
+ * (utils.py:35-39) and A = Kxz Li^T:
+ *   mean = V A^T [K, B]  (utils.py:69-73, re-associated: the same product up to rounding)
+ *   std  = sqrt(1 - rowsum(A^2)) [B]  (utils.py:84-87, Kdiag = 1; no clamp)
+ * Replaces the [B, M, d] broadcast of utils.py:35-39 and the products of utils.py:70-86.
+ * 1 <= M <= 256, 1 <= d <= 64, B >= 0, K >= 0; B = 0 returns without a launch.  No floating-point
+ * atomics: deterministic. */
+/* Forward, one launch: mean (may be NULL when K = 0) and std.  A_out: NULL, or [B, M] receiving A,
+ * which zsb_gp_cond_bwd_f32 reads. */
+int zsb_gp_cond_fwd_f32(const float* x, const float* z, const float* s, const float* Li,
+                        const float* V, float* mean, float* stdv, float* A_out, int64_t B,
+                        int64_t M, int64_t d, int64_t K, void* stream);
+/* Slices of the backward sweep for these sizes; its `part` scratch is
+ * slices * (K*M + M*M + M*d + d) floats.  0 when B = 0. */
+int zsb_gp_cond_parts(int64_t B, int64_t M, int64_t d, int64_t K);
+/* Backward of the moments, one sweep plus one merge launch.  g_mean [K, B] and g_std [B]: upstream
+ * gradients, either may be NULL (zero).  Outputs dz [M, d], ds [d], dLi [M, M] (zero above the
+ * diagonal) and dV [K, M].  A and stdv as written by the forward pass.  B = 0 returns without a
+ * launch and leaves the outputs untouched. */
+int zsb_gp_cond_bwd_f32(const float* x, const float* z, const float* s, const float* Li,
+                        const float* V, const float* A, const float* stdv, const float* g_mean,
+                        const float* g_std, float* part, float* dz, float* ds, float* dLi,
+                        float* dV, int64_t B, int64_t M, int64_t d, int64_t K, void* stream);
+
 /* ---- K5: SG-MCMC updates (zhusuan/sgmcmc.py) ------------------------------------------------ */
 int zsb_sgmcmc_parts(void);   /* capacity (floats) of every `part` scratch */
 int zsb_sgmcmc_sgld_f32(float* q, const float* g, const float* noise, float lr, int64_t chains,

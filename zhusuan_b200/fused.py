@@ -8,8 +8,13 @@ import numpy as np
 import torch
 from torch.autograd.function import once_differentiable
 
+from .distributions.base import Distribution
+from .distributions.multivariate import MultivariateNormalCholesky
+from .distributions.univariate import Normal
+
 __all__ = ["GaussianLogJoint", "BNNRegressionLogJoint", "LNTMLogJoint", "PMFLogJoint", "linear",
-           "class_linear", "noisy_bn_linear", "linear_bernoulli_log_prob", "LinearBernoulli"]
+           "class_linear", "noisy_bn_linear", "linear_bernoulli_log_prob", "LinearBernoulli",
+           "RBFKernel", "gp_conditional"]
 
 
 class GaussianLogJoint(object):
@@ -1304,3 +1309,211 @@ class LinearBernoulli(object):
 
     def prob(self, given):
         return torch.exp(self.log_prob(given))
+
+
+# ---- Sparse GP conditional (examples/gaussian_process/utils.py) on csrc/gp.cu ---------------------
+
+GP_MAX_M = 256
+GP_MAX_D = 64
+
+
+class RBFKernel(object):
+    """utils.py:10-49.  Owns ``k_raw_scale`` [n_covariates], a zeros leaf with ``requires_grad``
+    (the reference's ``k_log_scale_<name>`` variable and initialiser); ``k_scale`` is its softplus,
+    recomputed on each access so it follows optimiser steps.  ``device`` defaults to the current
+    CUDA device.  ``gp_conditional`` runs this kernel on the fused path; ``__call__`` is the
+    reference's broadcast formula in torch, the generic path and the cross-check."""
+
+    def __init__(self, n_covariates, name='rbf_kernel', dtype=torch.float32, device=None):
+        device = torch.device("cuda") if device is None else torch.device(device)
+        self.name = name
+        self.k_raw_scale = torch.zeros(int(n_covariates), dtype=dtype, device=device,
+                                       requires_grad=True)
+
+    @property
+    def k_scale(self):
+        return torch.nn.functional.softplus(self.k_raw_scale)
+
+    def __call__(self, x, y):
+        """K(x, y) [..., n_x, n_y] for x [..., n_x, n_covariates], y [..., n_y, n_covariates]."""
+        if x.dim() < 2:
+            raise ValueError("RBFKernel: rank(x) should be static and >=2")
+        if x.dim() != y.dim():
+            raise ValueError("RBFKernel: x and y should have the same rank")
+        diff = x.unsqueeze(-2) - y.unsqueeze(-3)
+        return torch.exp(-(diff * diff / self.k_scale).sum(-1) / 2)
+
+    def Kdiag(self, x):
+        """diag_part(self(x, x)): ones of x.shape[:-1] (rank 2 or 3, as in the reference)."""
+        shape = (x.shape[0],) if x.dim() == 2 else (x.shape[0], x.shape[1])
+        return torch.ones(shape, dtype=x.dtype, device=x.device)
+
+
+class _GPCondMoments(torch.autograd.Function):
+    """(mean [K, B], std [B]) of utils.py:69-87 with full_cov=False on zsb_gp_cond_fwd_f32, as
+    functions of (z, s, Li, V); x is data.  When a gradient is needed the forward pass also keeps
+    A = Kxz Li^T ([B, M] floats); the backward pass (zsb_gp_cond_bwd_f32) recomputes Kxz from x
+    and z, and sums over B in a fixed order."""
+
+    @staticmethod
+    def forward(ctx, x, z, s, Li, V, need_grad):
+        from ._lib import lib, ptr, stream
+        B, d = int(x.shape[0]), int(x.shape[1])
+        M, K = int(z.shape[0]), int(V.shape[0])
+        xx, zz, ss, LL, VV = (t.detach().contiguous() for t in (x, z, s, Li, V))
+        mean = torch.empty((K, B), dtype=torch.float32, device=x.device)
+        std = torch.empty((B,), dtype=torch.float32, device=x.device)
+        A = torch.empty((B, M), dtype=torch.float32, device=x.device) if need_grad else None
+        if B > 0:
+            lib.call("zsb_gp_cond_fwd_f32", ptr(xx), ptr(zz), ptr(ss), ptr(LL), ptr(VV),
+                     ptr(mean), ptr(std), ptr(A), B, M, d, K, stream())
+        if need_grad:
+            ctx.save_for_backward(xx, zz, ss, LL, VV, A, std)
+        ctx.set_materialize_grads(False)
+        return mean, std
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_mean, g_std):
+        from ._lib import lib, ptr, stream
+        xx, zz, ss, LL, VV, A, std = ctx.saved_tensors
+        B, d = int(xx.shape[0]), int(xx.shape[1])
+        M, K = int(zz.shape[0]), int(VV.shape[0])
+        if B == 0 or (g_mean is None and g_std is None):
+            return None, torch.zeros_like(zz), torch.zeros_like(ss), torch.zeros_like(LL), \
+                torch.zeros_like(VV), None
+        dz, ds = torch.empty_like(zz), torch.empty_like(ss)          # the merge writes every entry
+        dLi, dV = torch.empty_like(LL), torch.empty_like(VV)
+        gm = None if g_mean is None else g_mean.to(torch.float32).contiguous()
+        gs = None if g_std is None else g_std.to(torch.float32).contiguous()
+        part = torch.empty((lib.load().zsb_gp_cond_parts(B, M, d, K), K * M + M * M + M * d + d),
+                           dtype=torch.float32, device=xx.device)
+        lib.call("zsb_gp_cond_bwd_f32", ptr(xx), ptr(zz), ptr(ss), ptr(LL), ptr(VV), ptr(A),
+                 ptr(std), ptr(gm), ptr(gs), ptr(part), ptr(dz), ptr(ds), ptr(dLi), ptr(dV),
+                 B, M, d, K, stream())
+        return None, dz, ds, dLi, dV, None
+
+
+def _gp_factors(z, fz, kernel, Kzz_chol):
+    """Li = chol(Kzz)^-1 and V = fz Li^T in torch (utils.py:63-69), so autograd carries the
+    gradients of Li and V back to Kzz_chol, fz, z and the kernel's scales.  Without ``Kzz_chol``
+    the factor comes from ``cholesky_ex``: no host sync, and a Kzz that is not positive definite
+    gives NaN moments rather than an error."""
+    if Kzz_chol is None:
+        Kzz_chol = torch.linalg.cholesky_ex(kernel(z, z))[0]
+    eye = torch.eye(int(z.shape[0]), dtype=z.dtype, device=z.device)
+    Li = torch.linalg.solve_triangular(Kzz_chol, eye, upper=False)
+    return Li, torch.matmul(fz, Li.transpose(-1, -2))
+
+
+class GPConditionalNormal(Normal):
+    """The registry ``Normal(mean, std, group_ndims=1)`` of a fused ``gp_conditional``, whose
+    moments are computed on first use (sampling, ``log_prob``, ``.mean`` / ``.std``) and then
+    kept.  Building it launches nothing, so a conditional that is never read costs nothing.
+
+    The moments use the values of z, fz, Kzz_chol and the kernel's scales at first use: an
+    in-place optimiser step between building the conditional and reading it changes them.  When
+    they were first computed without a gradient (under ``no_grad`` or ``inference_mode``) and
+    are read again with grad mode on and an input that requires a gradient, they are computed
+    again, so the later read carries the gradient."""
+
+    def __init__(self, z, fz, x, kernel, Kzz_chol):
+        self._args = (z, fz, x, kernel, Kzz_chol)
+        self._moments = None
+        self._moments_grad = False
+        self._check_numerics = False
+        Distribution.__init__(self, dtype=torch.float32, param_dtype=torch.float32,
+                              is_continuous=True, is_reparameterized=True, group_ndims=1)
+
+    def _compute(self):
+        z, fz, x, kernel, Kzz_chol = self._args
+        wants_grad = torch.is_grad_enabled() and any(
+            t is not None and t.requires_grad for t in (z, fz, Kzz_chol, kernel.k_raw_scale))
+        if self._moments is None or (wants_grad and not self._moments_grad):
+            s = kernel.k_scale
+            Li, V = _gp_factors(z, fz, kernel, Kzz_chol)
+            need_grad = torch.is_grad_enabled() and any(t.requires_grad for t in (z, s, Li, V))
+            mean, std = _GPCondMoments.apply(x, z, s, Li, V, need_grad)
+            self._moments = (mean, std, torch.log(std))
+            self._moments_grad = need_grad
+        return self._moments
+
+    _mean = property(lambda self: self._compute()[0])
+    _std = property(lambda self: self._compute()[1])
+    _logstd = property(lambda self: self._compute()[2])
+
+    def _get_batch_shape(self):
+        return torch.Size([int(self._args[1].shape[0]), int(self._args[2].shape[0])])
+
+
+def _gp_fused_ok(z, fz, x, full_cov, kernel, Kzz_chol):
+    """The one eligibility check of the fused path; anything else runs the reference's torch
+    arithmetic."""
+    if full_cov or not isinstance(kernel, RBFKernel):
+        return False
+    ts = [z, fz, x, kernel.k_raw_scale] + ([] if Kzz_chol is None else [Kzz_chol])
+    if any(t.dtype != torch.float32 or not t.is_cuda or t.device != z.device for t in ts):
+        return False
+    if x.requires_grad or fz.dim() != 2:
+        return False
+    M, d = int(z.shape[0]), int(z.shape[1])
+    return 1 <= M <= GP_MAX_M and 1 <= d <= GP_MAX_D
+
+
+def gp_conditional(z, fz, x, full_cov, kernel, Kzz_chol=None):
+    """GP conditional f(x) | f(z) = fz (utils.py:52-90): z [n_z, n_covariates], fz
+    [n_particles, n_z] (a tensor or a ``StochasticTensor``, whose value is taken now), x
+    [n_x, n_covariates].  Returns ``Normal(mean, std, group_ndims=1)`` [n_particles, n_x] for
+    ``full_cov=False`` and ``MultivariateNormalCholesky`` for ``full_cov=True``.
+
+    With an ``RBFKernel``, ``full_cov=False``, float32 CUDA inputs on one device, an ``x`` that
+    needs no gradient, a rank-2 ``fz``, 1 <= n_z <= 256 and 1 <= n_covariates <= 64, the moments
+    run on csrc/gp.cu and are computed lazily, on first use of the returned ``Normal``.  With
+    A = Kxz Li^T and V = fz Li^T (Li = Kzz_chol^-1) they are mean = V A^T and
+    var = 1 - rowsum(A^2): the reference's products re-associated, equal up to rounding.  var is
+    not clamped, as in the reference.  Without ``Kzz_chol`` the Cholesky factor comes from
+    ``torch.linalg.cholesky_ex``, so a Kzz that is not positive definite gives NaN, not an error.
+    Everything else runs the reference's arithmetic in torch."""
+    fz = _unwrap(fz)
+    x = _unwrap(x)
+    if z.dim() != 2:
+        raise ValueError("RBFKernel: rank(x) should be static and >=2" if z.dim() < 2 else
+                         "gp_conditional: z should have shape [n_z, n_covariates], got %s"
+                         % (tuple(z.shape),))
+    if x.dim() != z.dim():
+        raise ValueError("RBFKernel: x and y should have the same rank")
+    n_z, n_cov = int(z.shape[0]), int(z.shape[1])
+    if int(x.shape[-1]) != n_cov:
+        raise ValueError("gp_conditional: x has %d covariates, z has %d"
+                         % (int(x.shape[-1]), n_cov))
+    if fz.dim() < 1 or int(fz.shape[-1]) != n_z:
+        raise ValueError("gp_conditional: fz should have shape [n_particles, %d], got %s"
+                         % (n_z, tuple(fz.shape)))
+    if isinstance(kernel, RBFKernel) and int(kernel.k_raw_scale.shape[0]) != n_cov:
+        raise ValueError("gp_conditional: the kernel has %d covariates, z has %d"
+                         % (int(kernel.k_raw_scale.shape[0]), n_cov))
+    if Kzz_chol is not None and tuple(Kzz_chol.shape) != (n_z, n_z):
+        raise ValueError("gp_conditional: Kzz_chol should have shape [%d, %d], got %s"
+                         % (n_z, n_z, tuple(Kzz_chol.shape)))
+    if _gp_fused_ok(z, fz, x, full_cov, kernel, Kzz_chol):
+        return GPConditionalNormal(z, fz, x, kernel, Kzz_chol)
+    return _gp_conditional_generic(z, fz, x, full_cov, kernel, Kzz_chol)
+
+
+def _gp_conditional_generic(z, fz, x, full_cov, kernel, Kzz_chol=None):
+    """utils.py:60-90 in torch ops, the Kzz_inv form included."""
+    if Kzz_chol is None:
+        Kzz_chol = torch.linalg.cholesky_ex(kernel(z, z))[0]
+    eye = torch.eye(int(z.shape[0]), dtype=z.dtype, device=z.device)
+    Kzz_chol_inv = torch.linalg.solve_triangular(Kzz_chol, eye, upper=False)
+    Kzz_inv = torch.matmul(Kzz_chol_inv.t(), Kzz_chol_inv)
+    Kxz = kernel(x, z)
+    Kxziz = torch.matmul(Kxz, Kzz_inv)
+    mean = torch.matmul(fz, Kxziz.transpose(-1, -2))
+    if full_cov:
+        cov = kernel(x, x) - torch.matmul(Kxziz, Kxz.t())
+        tril = torch.linalg.cholesky_ex(cov)[0]
+        tril = tril.unsqueeze(0).expand((int(fz.shape[0]),) + tuple(tril.shape))
+        return MultivariateNormalCholesky(mean, tril)
+    var = kernel.Kdiag(x) - (torch.matmul(Kxz, Kzz_chol_inv.transpose(-1, -2)) ** 2).sum(-1)
+    return Normal(mean=mean, std=torch.sqrt(var), group_ndims=1)
