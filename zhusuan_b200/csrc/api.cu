@@ -35,7 +35,7 @@ __global__ void epoch_bump_kernel(uint32_t* e, uint32_t by) {
 
 extern "C" {
 
-int zsb_version(void) { return 101; }  // 0.1.1
+int zsb_version(void) { return 102; }  // 0.1.2
 
 // Registers (or, with NULL, removes) a device uint32 that the samplers add to their Philox
 // iteration word: draws become a function of (seed, iter + *epoch, ...).  The stand-in for the

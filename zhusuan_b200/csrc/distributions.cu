@@ -270,6 +270,8 @@ __global__ void __launch_bounds__(256) categorical_lp_kernel(const int32_t* __re
   }
 }
 // d lp / d logits = gout * (onehot(given) - softmax(logits)); written at full (row, C) size.
+// A class outside [0, C) gives a NaN row, like its NaN log-prob (and the reference's
+// sparse_softmax_cross_entropy_with_logits on a GPU).
 __global__ void __launch_bounds__(256) categorical_bwd_kernel(
     const int32_t* __restrict__ given, int64_t given_n, const float* __restrict__ logits,
     int64_t logits_rows, int64_t C, const float* __restrict__ gout, float* __restrict__ dlogits,
@@ -280,9 +282,10 @@ __global__ void __launch_bounds__(256) categorical_bwd_kernel(
     const float* l = logits + (row % logits_rows) * C;
     const float lse = warp_row_lse(l, C, lane);
     const int32_t k = given[row % given_n];
+    const bool in = k >= 0 && k < C;
     const float g = gout[row];
     for (int64_t j = lane; j < C; j += 32)
-      dlogits[row * C + j] = g * ((j == k ? 1.f : 0.f) - expf(l[j] - lse));
+      dlogits[row * C + j] = in ? g * ((j == k ? 1.f : 0.f) - expf(l[j] - lse)) : NAN;
   }
 }
 

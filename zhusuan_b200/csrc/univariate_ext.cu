@@ -89,10 +89,19 @@ int launch_uni(float* out, int64_t n_out, int64_t group, Ops3 ops, F f, cudaStre
 __device__ __forceinline__ float softplusf_(float t) {       // tf.nn.softplus
   return fmaxf(t, 0.f) + log1pf(expf(-fabsf(t)));
 }
-// psi(x) for x > 0: recurrence up to x >= 6, then the asymptotic series
+// psi(x): for x <= 0 the reflection psi(x) = psi(1 - x) - pi cot(pi x) (as Eigen and torch do;
+// infinite at 0 and the negative integers, NaN at -inf), then for x > 0 the recurrence up to
+// x >= 6 -- at most 6 steps, so no argument can keep it looping -- and the asymptotic series.
+// NaN and +inf pass straight through.
 __device__ __forceinline__ float digammaf_(float x) {
   float r = 0.f;
-  while (x < 6.f) { r -= 1.f / x; x += 1.f; }
+  if (x <= 0.f) {
+    float s, c;
+    sincospif(x, &s, &c);
+    r = -3.14159265358979f * c / s;
+    x = 1.f - x;
+  }
+  for (int k = 0; k < 6 && x < 6.f; ++k) { r -= 1.f / x; x += 1.f; }
   const float i = 1.f / x, i2 = i * i;
   return r + logf(x) - 0.5f * i - i2 * (1.f / 12.f - i2 * (1.f / 120.f - i2 * (1.f / 252.f)));
 }
