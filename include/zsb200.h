@@ -539,6 +539,38 @@ int zsb_gp_cond_bwd_f32(const float* x, const float* z, const float* s, const fl
                         const float* g_std, float* part, float* dz, float* ds, float* dLi,
                         float* dV, int64_t B, int64_t M, int64_t d, int64_t K, void* stream);
 
+/* ---- 3x3 SAME convolutions, NHWC (csrc/conv.cu; examples/variational_autoencoders/vae_conv.py) --
+ * conv: tf.layers.conv2d(x, Cout, 3, strides=stride, padding="same") (vae_conv.py:39-53, 80) with
+ * W [3, 3, Cin, Cout]; transpose: tf.nn.conv2d_transpose(..., padding="SAME") + bias_add of
+ * examples/utils/utils.py:74-113 (vae_conv.py:20-36, 63-68) with W [3, 3, Cout, Cin].  Geometry is
+ * given on the convolution's side: Hc x Wc is the conv input grid ("big"), Hs = ceil(Hc / stride)
+ * x Ws its output grid ("small"); pads before are max((Hs - 1) stride + 3 - Hc, 0) / 2.  R images;
+ * stride 1 or 2; 1 <= Cin, Cout <= 64; R*H*W*C < 2^31 on both grids.  No floating-point atomics:
+ * deterministic. */
+/* One layer, one launch: y = relu?(conv(x) + b + residual), replacing conv + bias_add + add + relu
+ * (vae_conv.py:40-53, utils.py:101-111).  transpose = 0: x [R, Hc, Wc, Cin] -> y [R, Hs, Ws, Cout];
+ * transpose = 1: x [R, Hs, Ws, Cin] -> y [R, Hc, Wc, Cout] (stride 2 by output parity: a
+ * warp skips the taps none of its pixels needs).  b, residual (y's shape) may be NULL.  gate: NULL, or x's shape, and x
+ * counts as 0 where gate <= 0 (the ReLU mask of a backward pass).  The input gradient of either
+ * mode is the other mode on the output gradient with the same W.  R = 0 returns without a launch. */
+int zsb_conv3x3_fwd_f32(const float* x, const float* gate, const float* W, const float* b,
+                        const float* residual, float* y, int64_t R, int64_t Hc, int64_t Wc,
+                        int64_t Cin, int64_t Cout, int stride, int transpose, int relu,
+                        void* stream);
+/* Slices of the weight-gradient sweep for these sizes; its `part` scratch is slices * Ca * Cb
+ * floats.  0 when R = 0. */
+int zsb_conv3x3_wgrad_parts(int64_t R, int64_t Hc, int64_t Wc, int stride);
+/* Weight and bias gradient, one persistent sweep plus one merge launch (the tf.gradients of
+ * vae_conv.py's convolutions): dW[kh, kw, a, b] = sum big[n, s i + kh - pt, s j + kw - pl, a]
+ * small[n, i, j, b] over the small grid, big [R, Hc, Wc, Ca], small [R, Hs, Ws, Cb].  conv2d:
+ * big = x, small = g, grad_big = 0, dW [3, 3, Cin, Cout]; conv2d_transpose: big = g, small = x,
+ * grad_big = 1, dW [3, 3, Cout, Cin].  db (may be NULL): the output gradient summed over pixels.
+ * dW may be NULL when only db is wanted: then only the bias sums run.  Not both NULL.
+ * gate: NULL, or the gradient's shape, masking it where gate <= 0.  R >= 1. */
+int zsb_conv3x3_wgrad_f32(const float* big, const float* small, const float* gate, int grad_big,
+                          float* part, float* dW, float* db, int64_t R, int64_t Hc, int64_t Wc,
+                          int64_t Ca, int64_t Cb, int stride, void* stream);
+
 /* ---- K5: SG-MCMC updates (zhusuan/sgmcmc.py) ------------------------------------------------ */
 int zsb_sgmcmc_parts(void);   /* capacity (floats) of every `part` scratch */
 int zsb_sgmcmc_sgld_f32(float* q, const float* g, const float* noise, float lr, int64_t chains,

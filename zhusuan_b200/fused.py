@@ -14,7 +14,7 @@ from .distributions.univariate import Normal
 
 __all__ = ["GaussianLogJoint", "BNNRegressionLogJoint", "LNTMLogJoint", "PMFLogJoint", "linear",
            "class_linear", "noisy_bn_linear", "linear_bernoulli_log_prob", "LinearBernoulli",
-           "RBFKernel", "gp_conditional"]
+           "RBFKernel", "gp_conditional", "conv2d", "conv2d_transpose"]
 
 
 class GaussianLogJoint(object):
@@ -1517,3 +1517,209 @@ def _gp_conditional_generic(z, fz, x, full_cov, kernel, Kzz_chol=None):
         return MultivariateNormalCholesky(mean, tril)
     var = kernel.Kdiag(x) - (torch.matmul(Kxz, Kzz_chol_inv.transpose(-1, -2)) ** 2).sum(-1)
     return Normal(mean=mean, std=torch.sqrt(var), group_ndims=1)
+
+
+# ---- 3x3 SAME convolutions (examples/variational_autoencoders/vae_conv.py) on csrc/conv.cu -------
+
+CONV_MAX_C = 64
+
+
+def _same_pads(big, small, stride):
+    """TensorFlow "SAME" padding of a 3x3 window: (before, after) for an input of ``big`` rows
+    giving ``small = ceil(big / stride)`` rows."""
+    total = max((small - 1) * stride + 3 - big, 0)
+    return total // 2, total - total // 2
+
+
+def _conv_launch(x, gate, W, b, res, R, Hc, Wc, Cin, Cout, stride, transpose, relu, out_shape):
+    from ._lib import lib, ptr, stream
+    y = torch.empty(out_shape, dtype=torch.float32, device=x.device)
+    lib.call("zsb_conv3x3_fwd_f32", ptr(x), ptr(gate), ptr(W), ptr(b), ptr(res), ptr(y), R, Hc,
+             Wc, Cin, Cout, int(stride), int(transpose), int(bool(relu)), stream())
+    return y
+
+
+class _Conv3x3(torch.autograd.Function):
+    """relu?(conv(x) + b + residual) on zsb_conv3x3_fwd_f32, as a function of (x, W, b, residual).
+    ``geom`` = (transpose, stride, R, Hc, Wc, Hs, Ws, Cin, Cout): the convolution's big grid
+    Hc x Wc and small grid Hs x Ws, as in include/zsb200.h.  Backward: the input gradient is the
+    other mode on the output gradient, masked by y > 0 as it is loaded; dW and db come from
+    zsb_conv3x3_wgrad_f32.  The masked gradient is written only when the residual needs it."""
+
+    @staticmethod
+    def forward(ctx, x, W, b, res, geom, relu):
+        transpose, stride, R, Hc, Wc, Hs, Ws, Cin, Cout = geom
+        out = (R, Hc, Wc, Cout) if transpose else (R, Hs, Ws, Cout)
+        xx, WW = x.detach().contiguous(), W.detach().contiguous()
+        bb = None if b is None else b.detach().contiguous()
+        rr = None if res is None else res.detach().contiguous()
+        y = _conv_launch(xx, None, WW, bb, rr, R, Hc, Wc, Cin, Cout, stride, transpose, relu, out)
+        ctx.save_for_backward(xx, WW, y if relu else None)
+        ctx.meta = (geom, relu, b is not None, res is not None)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        from ._lib import lib, ptr, stream
+        xx, WW, y = ctx.saved_tensors
+        geom, relu, has_b, has_r = ctx.meta
+        transpose, stride, R, Hc, Wc, Hs, Ws, Cin, Cout = geom
+        need = ctx.needs_input_grad
+        g = gy.to(torch.float32).contiguous()
+        gate = y if relu else None
+        dres = None
+        if has_r and need[3]:
+            dres = torch.where(y > 0, g, torch.zeros((), dtype=g.dtype, device=g.device)) \
+                if relu else g
+            if relu:
+                g, gate = dres, None
+        dx = dW = db = None
+        if need[0]:
+            # the adjoint: conv2d's input gradient is the transpose on g, and the reverse
+            dx = _conv_launch(g, gate, WW, None, None, R, Hc, Wc, Cout, Cin, stride,
+                              not transpose, False, tuple(xx.shape))
+        if need[1] or (has_b and need[2]):
+            big, small = (g, xx) if transpose else (xx, g)
+            Ca, Cb = (Cout, Cin) if transpose else (Cin, Cout)
+            # the merge writes every entry; without dW only the bias sums run
+            dW = torch.empty_like(WW) if need[1] else None
+            db = torch.empty((Cout,), dtype=torch.float32, device=g.device) \
+                if (has_b and need[2]) else None
+            part = torch.empty((lib.load().zsb_conv3x3_wgrad_parts(R, Hc, Wc, stride), Ca * Cb),
+                               dtype=torch.float32, device=g.device)
+            lib.call("zsb_conv3x3_wgrad_f32", ptr(big), ptr(small), ptr(gate), int(transpose),
+                     ptr(part), ptr(dW), ptr(db), R, Hc, Wc, Ca, Cb, stride, stream())
+        return dx, dW, db, dres, None, None
+
+
+def _conv_check(name, x, W, b, residual, stride, Cin, Cout, in_hw):
+    if not isinstance(x, torch.Tensor) or not isinstance(W, torch.Tensor):
+        raise ValueError("%s: x and W should be tensors" % name)
+    ts = [x, W] + [t for t in (b, residual) if t is not None]
+    for t in ts:
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or not t.is_cuda \
+                or t.device != x.device:
+            raise ValueError("%s: x, W, b and residual should be float32 tensors on one CUDA "
+                             "device" % name)
+    if x.dim() < 3:
+        raise ValueError("%s: x should have shape [..., H, W, C], got %s"
+                         % (name, tuple(x.shape)))
+    if isinstance(stride, bool) or stride not in (1, 2):
+        raise ValueError("%s: stride should be 1 or 2, got %r" % (name, stride))
+    if W.dim() != 4 or tuple(W.shape[:2]) != (3, 3):
+        raise ValueError("%s: W should be a 3x3 kernel [3, 3, ., .], got %s"
+                         % (name, tuple(W.shape)))
+    if not (1 <= Cin <= CONV_MAX_C and 1 <= Cout <= CONV_MAX_C):
+        raise ValueError("%s: channels should be in [1, %d], got Cin %d, Cout %d"
+                         % (name, CONV_MAX_C, Cin, Cout))
+    if int(x.shape[-1]) != Cin:
+        raise ValueError("%s: x has %d channels, W expects %d" % (name, int(x.shape[-1]), Cin))
+    if min(in_hw) < 1:
+        raise ValueError("%s: H and W should be >= 1, got %s" % (name, tuple(in_hw)))
+    if b is not None and tuple(b.shape) != (Cout,):
+        raise ValueError("%s: b should have shape [%d], got %s" % (name, Cout, tuple(b.shape)))
+
+
+def _conv_apply(name, x, W, b, residual, geom, relu, lead, out_hw):
+    transpose, stride, R, Hc, Wc, Hs, Ws, Cin, Cout = geom
+    out_shape = tuple(lead) + tuple(out_hw) + (Cout,)
+    if residual is not None and tuple(residual.shape) != out_shape:
+        raise ValueError("%s: residual should have the output's shape %s, got %s"
+                         % (name, out_shape, tuple(residual.shape)))
+    if max(R * Hc * Wc * (Cout if transpose else Cin),
+           R * Hs * Ws * (Cin if transpose else Cout)) >= 2 ** 31:
+        raise ValueError("%s: R*H*W*C should be below 2^31" % name)
+    if R == 0:
+        return torch.empty(out_shape, dtype=torch.float32, device=x.device)
+    x4 = x.reshape((R,) + tuple(x.shape[-3:]))
+    r4 = None if residual is None else residual.reshape((R,) + tuple(out_hw) + (Cout,))
+    ts = [t for t in (x, W, b, residual) if t is not None]
+    if torch.is_grad_enabled() and any(t.requires_grad for t in ts):
+        y = _Conv3x3.apply(x4, W, b, r4, geom, bool(relu))
+    else:
+        y = _conv_launch(x4.contiguous(), None, W.contiguous(),
+                         None if b is None else b.contiguous(),
+                         None if r4 is None else r4.contiguous(), R, Hc, Wc, Cin, Cout, stride,
+                         transpose, relu, (R,) + tuple(out_hw) + (Cout,))
+    return y.reshape(out_shape)
+
+
+def conv2d(x, W, b=None, stride=1, relu=False, residual=None):
+    """``relu?(tf.layers.conv2d(x, Cout, 3, strides=stride, padding="same") + residual)``
+    (vae_conv.py:39-53, 80) on csrc/conv.cu, in FP32 FFMA.
+
+    x [..., H, W, Cin] is NHWC, any leading shape flattened to R images; W [3, 3, Cin, Cout] is
+    the ``tf.layers.conv2d`` kernel layout; b [Cout]; ``residual`` has the output's shape and is
+    added before the ReLU.  The output is [..., Ho, Wo, Cout] with Ho = ceil(H / stride) and
+
+        y[n, i, j, co] = b[co] + sum_{kh, kw, ci} x[n, s i + kh - pt, s j + kw - pl, ci] W[kh, kw, ci, co]
+
+    where out-of-range x counts as 0 and the pads are TensorFlow's SAME rule:
+    pad_total = max((Ho - 1) s + 3 - H, 0), pt = pad_total // 2 (pl likewise).  So stride 1 pads
+    1 before and 1 after; stride 2 pads 0 before and 1 after an even H, and 1 and 1 an odd H --
+    unlike torch's symmetric ``padding=1``.
+
+    Differentiable w.r.t. x, W, b and residual; under ``inference_mode`` nothing is kept.  The
+    gradients are deterministic: two identical calls give identical bits.  Supported: float32
+    CUDA tensors on one device, stride 1 or 2, 1 <= Cin, Cout <= 64, H, W >= 1 and
+    R*H*W*C < 2^31; anything else raises ValueError before any launch."""
+    x = _unwrap(x)
+    Cin = int(W.shape[2]) if isinstance(W, torch.Tensor) and W.dim() == 4 else 0
+    Cout = int(W.shape[3]) if isinstance(W, torch.Tensor) and W.dim() == 4 else 0
+    hw = tuple(int(v) for v in x.shape[-3:-1]) if isinstance(x, torch.Tensor) \
+        and x.dim() >= 3 else (0, 0)
+    _conv_check("conv2d", x, W, b, residual, stride, Cin, Cout, hw)
+    H, Wd = hw
+    lead = tuple(x.shape[:-3])
+    R = 1
+    for d in lead:
+        R *= int(d)
+    Hs, Ws = -(-H // stride), -(-Wd // stride)
+    geom = (False, int(stride), R, H, Wd, Hs, Ws, Cin, Cout)
+    return _conv_apply("conv2d", x, W, b, residual, geom, relu, lead, (Hs, Ws))
+
+
+def conv2d_transpose(x, W, out_shape, stride=1, b=None, relu=False, residual=None):
+    """``relu?(conv2d_transpose(x, out_shape, (3, 3), stride) + residual)`` of
+    examples/utils/utils.py:74-113 (``tf.nn.conv2d_transpose(..., padding="SAME")`` plus
+    ``bias_add``; vae_conv.py:20-36, 63-68) on csrc/conv.cu, in FP32 FFMA.
+
+    x [..., Hi, Wi, Cin] is NHWC; W [3, 3, Cout, Cin] is that helper's ``weights`` layout;
+    ``out_shape`` = (Ho, Wo, Cout) with ceil(Ho / stride) == Hi and ceil(Wo / stride) == Wi (TF
+    rejects anything else too); b [Cout]; ``residual`` has the output's shape, added before the
+    ReLU.  The map is the adjoint of ``conv2d`` from [Ho, Wo, Cout] to [Hi, Wi, Cin] with the
+    same W and the SAME pads of (Ho -> Hi):
+
+        y[n, h, w, co] = b[co] + sum x[n, i, j, ci] W[kh, kw, co, ci]  over h = s i + kh - pt,
+                                                                      w = s j + kw - pl
+
+    i.e. ``F.conv_transpose2d(..., padding=0)`` cropped by pt rows and pl columns at the start and
+    cut to Ho x Wo.  At stride 2 the kernel enumerates output pixels by parity, and a warp
+    skips the taps none of its pixels needs.  Gradients, determinism, inference mode and the supported range
+    are those of ``conv2d``."""
+    x = _unwrap(x)
+    if not isinstance(W, torch.Tensor) or W.dim() != 4:
+        raise ValueError("conv2d_transpose: W should be a 3x3 kernel [3, 3, Cout, Cin]")
+    Cout, Cin = int(W.shape[2]), int(W.shape[3])
+    try:
+        Ho, Wo, Co = (int(v) for v in out_shape)
+    except (TypeError, ValueError):
+        raise ValueError("conv2d_transpose: out_shape should be (Ho, Wo, Cout), got %r"
+                         % (out_shape,))
+    hw = tuple(int(v) for v in x.shape[-3:-1]) if isinstance(x, torch.Tensor) \
+        and x.dim() >= 3 else (0, 0)
+    _conv_check("conv2d_transpose", x, W, b, residual, stride, Cin, Cout, hw)
+    if Co != Cout:
+        raise ValueError("conv2d_transpose: out_shape has %d channels, W has %d" % (Co, Cout))
+    Hi, Wi = hw
+    if Ho < 1 or Wo < 1 or -(-Ho // stride) != Hi or -(-Wo // stride) != Wi:
+        raise ValueError("conv2d_transpose: out_shape %s does not give the input's %dx%d at "
+                         "stride %d (ceil(Ho / stride) must equal Hi)" % ((Ho, Wo, Co), Hi, Wi,
+                                                                          stride))
+    lead = tuple(x.shape[:-3])
+    R = 1
+    for d in lead:
+        R *= int(d)
+    geom = (True, int(stride), R, Ho, Wo, Hi, Wi, Cin, Cout)
+    return _conv_apply("conv2d_transpose", x, W, b, residual, geom, relu, lead, (Ho, Wo))
