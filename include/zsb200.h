@@ -306,6 +306,26 @@ int zsb_linear_tc_bn_f32(int training, const void* w_planes, const float* scale_
 int zsb_bn_grad_f32(int training, const float* g, const float* y, const float* a,
                     const float* stats, int relu, int64_t R, int J, float* part, float* dbeta,
                     void* planes, float* scale, void* stream);
+/* Dense layer without bias + batch norm with a learned scale gamma [J] (tf.layers.dense(use_bias=
+ * False) + tf.layers.batch_normalization; replaces bernoulli_latent_vae.py:25-30 and 39-44): as
+ * zsb_linear_tc_bn_f32 with out = act(xhat * gamma + beta), xhat = (a - mean) rstd, rate = 1 -
+ * momentum.  h_binary: h_planes is the one plane of a 0/1 sample (zsb_linear_tc_bern_sample_f32).
+ * In evaluation, a [R, J] (may be NULL) receives the pre-activation, which the gradient of gamma
+ * reads. */
+int zsb_linear_tc_bn_gamma_f32(int training, const void* w_planes, const float* scale_w,
+                               const void* h_planes, const float* scale_h, int h_binary,
+                               const float* gamma, const float* beta, float* moving_mean,
+                               float* moving_var, float rate, float eps, float* stats, float* a,
+                               float* part, float* out, int64_t R, int J, int K, int relu,
+                               float* amax_scale, void* stream);
+/* Its backward pass: g' = g [y > 0] (relu) or g; dbeta [J] = sum_r g', dgamma [J] = sum_r g' xhat
+ * (either may be NULL; a is needed in training and for dgamma); the planes of da = gamma rstd (g' -
+ * mean_r g' - xhat mean_r(g' xhat)) in training, of da = gamma rstd g' otherwise.  part and scale as
+ * in zsb_bn_grad_f32; the column sums are deterministic. */
+int zsb_bn_grad_gamma_f32(int training, const float* g, const float* y, const float* a,
+                          const float* stats, const float* gamma, int relu, int64_t R, int J,
+                          float* part, float* dbeta, float* dgamma, void* planes, float* scale,
+                          void* stream);
 /* From d = d(h * noise) [R, K]: dnoise [R, K] = d * h[r % n_h], dh [n_h, K] = sum over the R / n_h
  * particle rows of d * noise (either may be NULL). */
 int zsb_noisy_grad_f32(const float* d, const float* h, int64_t n_h, const float* noise, int64_t R,

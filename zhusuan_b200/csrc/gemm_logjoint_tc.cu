@@ -58,6 +58,11 @@ constexpr float BIN_SCALE = 2048.f;
 //          (sum of squared deviations from the tile mean); the tile's count is min(128, R - 128 t)
 //   EPI 10 out[r, j] = act((l - bn_stats[j]) * bn_stats[J + j] + bn_beta[j]), bn_stats = (mean,
 //          rsqrt(var + eps)) of the moving statistics (evaluation mode)
+//   EPI 11 EPI 10 with batch norm's learned scale gamma (tf.layers.batch_normalization,
+//          bernoulli_latent_vae.py:26-43):
+//          out[r, j] = act(xhat * bn_gamma[j] + bn_beta[j]), xhat = (l - mean) rstd, and, when pre
+//          is not NULL, pre[r, j] = l: what the gradient of gamma needs (xhat is never rebuilt
+//          from out, which the ReLU and gamma = 0 lose)
 //
 // The descriptor tc_pipeline_kernel runs, LinW<E, EPI, MN, Z>, is a LinCore (the product) plus the
 // fields of one epilogue family E: RowsEpi (EPI 0 - 2), SamplesEpi (4 - 6), ClassEpi (7, 8) or
@@ -174,7 +179,7 @@ struct LinW : LinCore<MN, Z> {
   }
 };
 
-// EPI 9 / 10: this lane's feature j over the tile's rows.  EPI 9 reads the accumulator twice:
+// EPI 9 - 11: this lane's feature j over the tile's rows.  EPI 9 reads the accumulator twice:
 // once for the tile mean, once for M2 about it (never a sum of squares, which cancels).
 struct BnEpi {
   static constexpr Units UNITS = TILES;
@@ -182,6 +187,7 @@ struct BnEpi {
   __host__ __device__ static constexpr bool folds_amax(int) { return true; }
   const float* bn_stats; const float* bn_beta;
   float* out; float* part; int relu; float* amax_scale;
+  const float* bn_gamma; float* pre;                          // EPI 11 only
 
   template <int EPI, class Core>
   __device__ __forceinline__ void run(const Core& core, int64_t u, uint32_t trow, int quarter,
@@ -232,6 +238,7 @@ struct BnEpi {
     } else {
       const float mu = j_ok ? bn_stats[j] : 0.f, rs = j_ok ? bn_stats[J + j] : 0.f;
       const float bt = j_ok ? bn_beta[j] : 0.f;
+      const float gm = (EPI == 11 && j_ok) ? bn_gamma[j] : 1.f;
 #pragma unroll 1
       for (int c = 0; c < BN; c += 16) {
         const int64_t rbase = r0 + c;
@@ -241,7 +248,14 @@ struct BnEpi {
 #pragma unroll
         for (int jj = 0; jj < 16; ++jj)
           if (j_ok && rbase + jj < R) {
-            float y = (__uint_as_float(v[jj]) * acc_scale - mu) * rs + bt;
+            const float l = __uint_as_float(v[jj]) * acc_scale;
+            float y;
+            if (EPI == 11) {
+              y = fmaf((l - mu) * rs, gm, bt);
+              if (pre) pre[(rbase + jj) * J + j] = l;
+            } else {
+              y = (l - mu) * rs + bt;
+            }
             if (relu) y = fmaxf(y, 0.f);
             out[(rbase + jj) * J + j] = y;
             amax = fmaxf(amax, fabsf(y));
@@ -815,22 +829,44 @@ __global__ void __launch_bounds__(256) bn_stats_kernel(const float* __restrict__
   }
 }
 
-// Training forward after EPI 9: out = act((a - mean) * rstd + beta), max |out| into scale[2]
-__global__ void __launch_bounds__(256) bn_apply_kernel(const float* __restrict__ a, int64_t R,
-                                                       int J, const float* __restrict__ stats,
-                                                       const float* __restrict__ beta, int relu,
-                                                       float* __restrict__ out,
-                                                       float* __restrict__ amax_scale) {
+// Training forward after EPI 9: out = act((a - mean) * rstd + beta), or with GAMMA act(xhat *
+// gamma + beta), xhat = (a - mean) * rstd (the rounding order of EPI 10 / 11); max |out| into
+// scale[2]
+template <bool GAMMA>
+__device__ __forceinline__ void bn_apply_rows(const float* __restrict__ a, int64_t R, int J,
+                                              const float* __restrict__ stats,
+                                              const float* __restrict__ gamma,
+                                              const float* __restrict__ beta, int relu,
+                                              float* __restrict__ out,
+                                              float* __restrict__ amax_scale) {
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   float m = 0.f;
   for (int64_t r = (int64_t)blockIdx.x * 8 + ty; r < R; r += (int64_t)gridDim.x * 8)
     for (int j = tx; j < J; j += 32) {
-      float y = (a[r * J + j] - __ldg(stats + j)) * __ldg(stats + J + j) + __ldg(beta + j);
+      float y;
+      if (GAMMA)
+        y = fmaf((a[r * J + j] - __ldg(stats + j)) * __ldg(stats + J + j), __ldg(gamma + j),
+                 __ldg(beta + j));
+      else
+        y = (a[r * J + j] - __ldg(stats + j)) * __ldg(stats + J + j) + __ldg(beta + j);
       if (relu) y = fmaxf(y, 0.f);
       out[r * J + j] = y;
       m = fmaxf(m, fabsf(y));
     }
   if (amax_scale) fold_amax(amax_scale, m <= 3.0e38f ? m : 0.f, tx);
+}
+__global__ void __launch_bounds__(256) bn_apply_kernel(const float* __restrict__ a, int64_t R,
+                                                       int J, const float* __restrict__ stats,
+                                                       const float* __restrict__ beta, int relu,
+                                                       float* __restrict__ out,
+                                                       float* __restrict__ amax_scale) {
+  bn_apply_rows<false>(a, R, J, stats, nullptr, beta, relu, out, amax_scale);
+}
+__global__ void __launch_bounds__(256) bn_apply_gamma_kernel(
+    const float* __restrict__ a, int64_t R, int J, const float* __restrict__ stats,
+    const float* __restrict__ gamma, const float* __restrict__ beta, int relu,
+    float* __restrict__ out, float* __restrict__ amax_scale) {
+  bn_apply_rows<true>(a, R, J, stats, gamma, beta, relu, out, amax_scale);
 }
 
 // Backward, per 128-row tile t and column j (block: 32 columns x 8 warps, 16 rows per warp, then
@@ -870,11 +906,12 @@ __global__ void __launch_bounds__(256) bn_grad_sums_kernel(
 
 // One warp per column: the tile sums of bn_grad_sums_kernel in a fixed order (lane-strided runs,
 // then a fixed shuffle tree) -> dbeta[j] = sum g' (may be NULL), coef = (sum g' / R,
-// sum g' xhat / R)
-__global__ void __launch_bounds__(256) bn_grad_combine_kernel(const float* __restrict__ part,
-                                                              int64_t R, int J,
-                                                              float* __restrict__ dbeta,
-                                                              float* __restrict__ coef) {
+// sum g' xhat / R), and with DGAMMA dgamma[j] = sum g' xhat (may be NULL)
+template <bool DGAMMA>
+__device__ __forceinline__ void bn_grad_combine_cols(const float* __restrict__ part, int64_t R,
+                                                     int J, float* __restrict__ dbeta,
+                                                     float* __restrict__ dgamma,
+                                                     float* __restrict__ coef) {
   const int lane = threadIdx.x & 31;
   const int j = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (j >= J) return;
@@ -891,19 +928,32 @@ __global__ void __launch_bounds__(256) bn_grad_combine_kernel(const float* __res
   }
   if (lane == 0) {
     if (dbeta) dbeta[j] = s1;
+    if (DGAMMA && dgamma) dgamma[j] = s2;
     coef[j] = s1 / (float)R;
     coef[J + j] = s2 / (float)R;
   }
 }
+__global__ void __launch_bounds__(256) bn_grad_combine_kernel(const float* __restrict__ part,
+                                                              int64_t R, int J,
+                                                              float* __restrict__ dbeta,
+                                                              float* __restrict__ coef) {
+  bn_grad_combine_cols<false>(part, R, J, dbeta, nullptr, coef);
+}
+__global__ void __launch_bounds__(256) bn_grad_combine_gamma_kernel(
+    const float* __restrict__ part, int64_t R, int J, float* __restrict__ dbeta,
+    float* __restrict__ dgamma, float* __restrict__ coef) {
+  bn_grad_combine_cols<true>(part, R, J, dbeta, dgamma, coef);
+}
 
-// da = rstd (g' - coef[0] - xhat coef[1]) in training (a != NULL), rstd g' in evaluation.
-// PLANES = false: max |da| into scale[2]; PLANES = true: planes [2][R][Jp] = fp16 hi/lo of
-// da * scale[0], pad columns zero -- the operand zsb_linear_tc_dgrad_f32 / _wgrad_f32 read.
-template <bool PLANES>
-__global__ void __launch_bounds__(256) bn_grad_apply_kernel(
+// da = rstd (g' - coef[0] - xhat coef[1]) in training, rstd g' in evaluation; with GAMMA, rstd is
+// gamma rstd.  PLANES = false: max |da| into scale[2]; PLANES = true: planes [2][R][Jp] = fp16
+// hi/lo of da * scale[0], pad columns zero -- the operand zsb_linear_tc_dgrad_f32 / _wgrad_f32 read.
+template <bool PLANES, bool GAMMA>
+__device__ __forceinline__ void bn_grad_apply_rows(
     const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ a,
-    const float* __restrict__ stats, const float* __restrict__ coef, int relu, int64_t R, int J,
-    int Jp, __half* __restrict__ planes, float* __restrict__ scale) {
+    bool training, const float* __restrict__ stats, const float* __restrict__ gamma,
+    const float* __restrict__ coef, int relu, int64_t R, int J, int Jp,
+    __half* __restrict__ planes, float* __restrict__ scale) {
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const float s = PLANES ? scale[0] : 0.f;
   const int64_t n_pl = R * (int64_t)Jp;
@@ -915,16 +965,34 @@ __global__ void __launch_bounds__(256) bn_grad_apply_kernel(
         float gg = g[r * J + j];
         if (relu && !(y[r * J + j] > 0.f)) gg = 0.f;
         const float rs = __ldg(stats + J + j);
-        if (a) {
+        if (training) {
           const float xh = (a[r * J + j] - __ldg(stats + j)) * rs;
           gg = gg - __ldg(coef + j) - xh * __ldg(coef + J + j);
         }
-        d = rs * gg;
+        d = (GAMMA ? __ldg(gamma + j) * rs : rs) * gg;
       }
       if (PLANES) store_hilo(planes + r * Jp + j, n_pl, d * s);
       else m = finite_absmax(m, d);
     }
   if (!PLANES) fold_amax(scale, m, tx);
+}
+// training: a != NULL
+template <bool PLANES>
+__global__ void __launch_bounds__(256) bn_grad_apply_kernel(
+    const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ a,
+    const float* __restrict__ stats, const float* __restrict__ coef, int relu, int64_t R, int J,
+    int Jp, __half* __restrict__ planes, float* __restrict__ scale) {
+  bn_grad_apply_rows<PLANES, false>(g, y, a, a != nullptr, stats, nullptr, coef, relu, R, J, Jp,
+                                    planes, scale);
+}
+template <bool PLANES>
+__global__ void __launch_bounds__(256) bn_grad_apply_gamma_kernel(
+    const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ a,
+    int training, const float* __restrict__ stats, const float* __restrict__ gamma,
+    const float* __restrict__ coef, int relu, int64_t R, int J, int Jp,
+    __half* __restrict__ planes, float* __restrict__ scale) {
+  bn_grad_apply_rows<PLANES, true>(g, y, a, training != 0, stats, gamma, coef, relu, R, J, Jp,
+                                   planes, scale);
 }
 
 // From d = d(h * noise) [R, K]: dnoise[r] = d[r] * h[r % n_h] and dh[i] = sum_s d[s n_h + i] *
@@ -1403,6 +1471,77 @@ int zsb_bn_grad_f32(int training, const float* g, const float* y, const float* a
   bn_grad_apply_kernel<true><<<blocks, 256, 0, st>>>(g, y, at, stats, coef, relu, R, J, Jp, pl,
                                                      scale);
   return zsb_check_launch("bn_grad");
+}
+
+// Dense layer without bias followed by batch norm with a learned scale (tf.layers.dense(use_bias=
+// False) + tf.layers.batch_normalization, bernoulli_latent_vae.py:25-30, 39-44): as
+// zsb_linear_tc_bn_f32, with out = act(xhat * gamma + beta), xhat = (a - mean) rstd, and h_binary as
+// in zsb_linear_tc_bern_sample_f32.  In evaluation, `a` (may be NULL) receives the pre-activation
+// for the gradient of gamma.
+int zsb_linear_tc_bn_gamma_f32(int training, const void* w_planes, const float* scale_w,
+                               const void* h_planes, const float* scale_h, int h_binary,
+                               const float* gamma, const float* beta, float* moving_mean,
+                               float* moving_var, float rate, float eps, float* stats, float* a,
+                               float* part, float* out, int64_t R, int J, int K, int relu,
+                               float* amax_scale, void* stream) {
+  ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && gamma && beta && moving_mean &&
+                  moving_var && stats && out && R > 0 && J > 0 && K > 0 &&
+                  (!training || (a && part)),
+              "zsb_linear_tc_bn_gamma_f32: bad args");
+  ZSB_REQUIRE(R < (1LL << 31), "zsb_linear_tc_bn_gamma_f32: too many rows");
+  cudaStream_t st = (cudaStream_t)stream;
+  const unsigned col_blocks = (unsigned)((J + 7) / 8);
+  return with_h_binary(h_binary, [&](auto z) {
+    LinCore<0, z> c;
+    int rc = make_core(c, w_planes, scale_w, h_planes, scale_h, J, R, K);
+    if (rc) return rc;
+    if (!training) {
+      bn_stats_kernel<<<col_blocks, 256, 0, st>>>(nullptr, R, J, moving_mean, moving_var, rate,
+                                                  eps, 0, stats);
+      if ((rc = zsb_check_launch("linear_tc_bn_gamma_stats")) != ZSB_OK) return rc;
+      const BnEpi e{.bn_stats = stats, .bn_beta = beta, .out = out, .relu = relu,
+                    .amax_scale = amax_scale, .bn_gamma = gamma, .pre = a};
+      return tc_launch(LinW<BnEpi, 11, 0, z>{c, e}, st, "linear_tc_bn_gamma_eval");
+    }
+    rc = tc_launch(LinW<BnEpi, 9, 0, z>{c, {.out = a, .part = part}}, st, "linear_tc_bn_gamma_train");
+    if (rc != ZSB_OK) return rc;
+    bn_stats_kernel<<<col_blocks, 256, 0, st>>>(part, R, J, moving_mean, moving_var, rate, eps, 1,
+                                                stats);
+    bn_apply_gamma_kernel<<<grid_blocks(R, 8, 16), 256, 0, st>>>(a, R, J, stats, gamma, beta, relu,
+                                                                 out, amax_scale);
+    return zsb_check_launch("linear_tc_bn_gamma_apply");
+  });
+}
+
+// Backward of zsb_linear_tc_bn_gamma_f32 from the upstream gradient g [R, J], its output y (read
+// when relu), the pre-activation a (training, or when dgamma is wanted) and stats:
+//   g' = g [y > 0] (relu) or g;  dbeta [J] = sum_r g',  dgamma [J] = sum_r g' xhat (either may be
+//   NULL), xhat = (a - mean) rstd
+//   training: da = gamma rstd (g' - mean_r g' - xhat mean_r(g' xhat));  else: da = gamma rstd g'
+// then the planes of da as zsb_bn_grad_f32 writes them; part and scale as there.
+int zsb_bn_grad_gamma_f32(int training, const float* g, const float* y, const float* a,
+                          const float* stats, const float* gamma, int relu, int64_t R, int J,
+                          float* part, float* dbeta, float* dgamma, void* planes, float* scale,
+                          void* stream) {
+  ZSB_REQUIRE(g && stats && gamma && part && planes && scale && R > 0 && J > 0 && (!relu || y) &&
+                  (!(training || dgamma) || a),
+              "zsb_bn_grad_gamma_f32: bad args");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Jp = zsb_linear_tc_kpad(J);
+  const int64_t n_t = (R + BN_TILE - 1) / BN_TILE;
+  float* coef = part + 2 * n_t * J;
+  bn_grad_sums_kernel<<<dim3((unsigned)n_t, (unsigned)((J + 31) / 32)), 256, 0, st>>>(
+      g, y, a, stats, relu, R, J, part);
+  bn_grad_combine_gamma_kernel<<<(unsigned)((J + 7) / 8), 256, 0, st>>>(part, R, J, dbeta, dgamma,
+                                                                        coef);
+  __half* pl = reinterpret_cast<__half*>(planes);
+  const unsigned blocks = grid_blocks(R, 8, 16);
+  bn_grad_apply_gamma_kernel<false><<<blocks, 256, 0, st>>>(g, y, a, training, stats, gamma, coef,
+                                                            relu, R, J, Jp, pl, scale);
+  pow2_scale_mult_kernel<<<1, 32, 0, st>>>(scale, 1.f);
+  bn_grad_apply_gamma_kernel<true><<<blocks, 256, 0, st>>>(g, y, a, training, stats, gamma, coef,
+                                                           relu, R, J, Jp, pl, scale);
+  return zsb_check_launch("bn_grad_gamma");
 }
 
 // Gradients of x = h[r % n_h] * noise[r] from d = dL/dx [R, K]: dnoise [R, K] = d * h[r % n_h] and

@@ -13,8 +13,8 @@ from .distributions.multivariate import MultivariateNormalCholesky
 from .distributions.univariate import Normal
 
 __all__ = ["GaussianLogJoint", "BNNRegressionLogJoint", "LNTMLogJoint", "PMFLogJoint", "linear",
-           "class_linear", "noisy_bn_linear", "linear_bernoulli_log_prob", "LinearBernoulli",
-           "RBFKernel", "gp_conditional", "conv2d", "conv2d_transpose"]
+           "class_linear", "noisy_bn_linear", "bn_linear", "linear_bernoulli_log_prob",
+           "LinearBernoulli", "RBFKernel", "gp_conditional", "conv2d", "conv2d_transpose"]
 
 
 class GaussianLogJoint(object):
@@ -1107,6 +1107,123 @@ def noisy_bn_linear(h, noise, W, beta, moving_mean, moving_variance, training, r
                          % (noise_s, tuple(W.shape)))
     return _NoisyBNLinear.apply(h, noise, W, beta, (moving_mean, moving_variance), bool(training),
                                 bool(relu), float(1.0 - decay), float(epsilon))
+
+
+class _BNLinear(torch.autograd.Function):
+    """relu?(BN(h W^T) * gamma + beta) on the batch-norm epilogues of the wgmma kernel
+    (zsb_linear_tc_bn_gamma_f32), from the cached operand planes of h -- a 0/1 sample's one plane
+    included.  Backward: one pass gives d beta, d gamma and the planes of the pre-activation
+    gradient (zsb_bn_grad_gamma_f32), which the unchanged input- and weight-gradient products
+    read."""
+
+    @staticmethod
+    def forward(ctx, h, W, gamma, beta, stats_bufs, training, relu, rate, eps, keep_pre):
+        from ._lib import lib, ptr, stream
+        moving_mean, moving_variance = stats_bufs
+        lead = h.shape[:-1]
+        K, J = int(h.shape[-1]), int(W.shape[0])
+        h2 = h.reshape(-1, K)
+        R = int(h2.shape[0])
+        dev = W.device
+        hpl = _planes_of(h2, h)
+        wp, ws = _tc_split(W)
+        gm = gamma.detach().to(torch.float32).contiguous()
+        b = beta.detach().to(torch.float32).contiguous()
+        stats = torch.empty((2, J), dtype=torch.float32, device=dev)
+        y = torch.empty((R, J), dtype=torch.float32, device=dev)
+        a = part = None
+        if training or keep_pre:
+            a = torch.empty((R, J), dtype=torch.float32, device=dev)
+        if training:
+            part = torch.empty(-(-R // 128) * 2 * J, dtype=torch.float32, device=dev)
+        amax = torch.zeros(4, dtype=torch.float32, device=dev)
+        lib.call("zsb_linear_tc_bn_gamma_f32", int(training), ptr(wp), ptr(ws), ptr(hpl.planes),
+                 ptr(hpl.scale), int(hpl.binary), ptr(gm), ptr(b), ptr(moving_mean),
+                 ptr(moving_variance), rate, eps, ptr(stats), ptr(a), ptr(part), ptr(y), R, J, K,
+                 int(relu), ptr(amax), stream())
+        ctx.save_for_backward(W, gm, y if relu else None, a, stats)
+        ctx.hpl = hpl
+        ctx.wpl = (wp, ws)
+        ctx.meta = (lead, training, relu, R, K, J)
+        return _tag(y.reshape(tuple(lead) + (J,)), amax)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        from ._lib import lib, ptr, stream
+        W, gm, y, a, stats = ctx.saved_tensors
+        lead, training, relu, R, K, J = ctx.meta
+        need = ctx.needs_input_grad
+        dev = gy.device
+        g = gy.reshape(R, J).to(torch.float32).contiguous()
+        dgamma = torch.empty(J, dtype=torch.float32, device=dev) if need[2] else None
+        dbeta = torch.empty(J, dtype=torch.float32, device=dev) if need[3] else None
+        part = torch.empty((-(-R // 128) + 1) * 2 * J, dtype=torch.float32, device=dev)
+        planes = torch.empty((2, R, lib.load().zsb_linear_tc_kpad(J)), dtype=torch.float16,
+                             device=dev)
+        scale = torch.zeros(4, dtype=torch.float32, device=dev)
+        lib.call("zsb_bn_grad_gamma_f32", int(training), ptr(g), ptr(y), ptr(a), ptr(stats),
+                 ptr(gm), int(relu), R, J, ptr(part), ptr(dbeta), ptr(dgamma), ptr(planes),
+                 ptr(scale), stream())
+        gpl = _Planes(planes, scale, R, J)
+        dh, dW = _grad_products(ctx, gpl, W, R, ctx.wpl, tuple(lead) + (K,), need[0], need[1])
+        return dh, dW, dgamma, dbeta, None, None, None, None, None, None
+
+
+def bn_linear(h, W, gamma, beta, moving_mean, moving_variance, training, relu=True, momentum=0.99,
+              epsilon=1e-3):
+    """``relu?(BN(h @ W.T))``, shape ``h.shape[:-1] + (J,)``: ``tf.layers.dense(h, J,
+    use_bias=False)`` followed by ``tf.layers.batch_normalization(..., training=training)`` and
+    ``tf.nn.relu``, as in examples/variational_autoencoders/bernoulli_latent_vae.py:25-30 and 39-44,
+    with the defaults of ``tf.layers.batch_normalization`` on its non-fused path (TF 1.x fuses only
+    4-D inputs):
+
+    * ``center=True`` and ``scale=True``: ``y = xhat * gamma + beta`` with ``xhat = (a - mean) *
+      rsqrt(var + epsilon)``, ``a = h @ W.T``;
+    * ``training``: the moments over all ``h.shape[:-1]`` rows with the population variance, and
+      ``moving_mean`` / ``moving_variance`` (contiguous float32 [J]) updated in place as ``m -= (m -
+      batch) * (1 - momentum)``, with no zero-debiasing; otherwise the moving statistics normalise
+      and stay unchanged.
+
+    ``h`` [*lead, K] may be an activation of another fused layer, a ``StochasticTensor``, or a
+    ``LinearBernoulli`` sample, whose one 0/1 operand plane is multiplied as it is (never split
+    again).  ``W`` is [J, K] (the kernel transposed, as in ``linear``); ``gamma`` and ``beta`` are
+    [J].  Differentiable w.r.t. ``h``, ``W``, ``gamma`` and ``beta``; the moving statistics receive
+    no gradient.  In evaluation with a ``gamma`` that requires a gradient, the forward also keeps
+    the pre-activation, from which the gradient of gamma is computed.  The batch moments and every
+    gradient's column sums are reduced in a fixed order, so two identical calls give identical
+    bits.  The output carries the max |.| that a following fused layer uses for its operand
+    split."""
+    h = _unwrap(h)
+    if not isinstance(h, torch.Tensor) or h.dim() < 1:
+        raise ValueError("h must be a tensor [*lead, K], got %r" % (type(h),))
+    if h.dtype != torch.float32 and (h.is_floating_point() or h.is_complex()):
+        raise ValueError("h must be float32 or a 0/1 integer sample, got %s" % h.dtype)
+    K = int(h.shape[-1])
+    if not isinstance(W, torch.Tensor) or W.dim() != 2 or int(W.shape[1]) != K or \
+            W.dtype != torch.float32:
+        raise ValueError("W %s must be a float32 [J, %d] tensor"
+                         % (tuple(getattr(W, "shape", ())), K))
+    dev = W.device
+    if dev.type != "cuda":
+        raise ValueError("bn_linear runs on a CUDA device; W is on %s" % dev)
+    J = int(W.shape[0])
+    if h.device != dev:
+        raise ValueError("h is on %s and W on %s" % (h.device, dev))
+    for nm, t in (("gamma", gamma), ("beta", beta)):
+        if not isinstance(t, torch.Tensor) or tuple(t.shape) != (J,) or \
+                t.dtype != torch.float32 or t.device != dev:
+            raise ValueError("%s must be a float32 [%d] tensor on %s" % (nm, J, dev))
+    for nm, t in (("moving_mean", moving_mean), ("moving_variance", moving_variance)):
+        if not isinstance(t, torch.Tensor) or tuple(t.shape) != (J,) or \
+                t.dtype != torch.float32 or not t.is_contiguous() or t.device != dev:
+            raise ValueError("%s must be a contiguous float32 [%d] tensor on %s" % (nm, J, dev))
+    if h.numel() == 0 or J == 0:
+        raise ValueError("empty shapes are not supported: h %s, W %s"
+                         % (tuple(h.shape), tuple(W.shape)))
+    keep_pre = (not training) and torch.is_grad_enabled() and gamma.requires_grad
+    return _BNLinear.apply(h, W, gamma, beta, (moving_mean, moving_variance), bool(training),
+                           bool(relu), float(1.0 - momentum), float(epsilon), bool(keep_pre))
 
 
 def linear_bernoulli_log_prob(h, W, b, x):
