@@ -326,6 +326,31 @@ int zsb_bn_grad_gamma_f32(int training, const float* g, const float* y, const fl
                           const float* stats, const float* gamma, int relu, int64_t R, int J,
                           float* part, float* dbeta, float* dgamma, void* planes, float* scale,
                           void* stream);
+/* The same layer with the batch norm of 4-D inputs (TF 1.x's fused_batch_norm path, the
+ * convolutions of the GAN examples): as zsb_linear_tc_bn_gamma_f32, except that in training the
+ * moving variance moves towards the Bessel-corrected batch variance R / (R - 1) var (towards 0 when
+ * R = 1); the output still normalises with the population variance var. */
+int zsb_linear_tc_bn_gamma_fused_f32(int training, const void* w_planes, const float* scale_w,
+                                     const void* h_planes, const float* scale_h, int h_binary,
+                                     const float* gamma, const float* beta, float* moving_mean,
+                                     float* moving_var, float rate, float eps, float* stats,
+                                     float* a, float* part, float* out, int64_t R, int J, int K,
+                                     int relu, float* amax_scale, void* stream);
+/* The training step of that batch norm after a pass that left the pre-activation a [R, J] and its
+ * per-128-row-tile moment partials part [ceil(R / 128)][2][J] (mean, M2): the deterministic merge,
+ * stats = (mean, rstd), the moving statistics updated as in zsb_linear_tc_bn_gamma_fused_f32, and
+ * out = act(xhat * gamma + beta); max |out| into amax_scale[2] (may be NULL). */
+int zsb_bn_finish_fused_f32(const float* a, const float* part, int64_t R, int J,
+                            const float* gamma, const float* beta, float* moving_mean,
+                            float* moving_var, float rate, float eps, float* stats, float* out,
+                            int relu, float* amax_scale, void* stream);
+/* As zsb_bn_grad_gamma_f32, but da [R, J] is written in fp32 and max |da| is folded into
+ * scale[2] (scale = device float[4] with scale[2] zero): for a consumer that gathers da (the
+ * transposed convolution) before splitting it into planes. */
+int zsb_bn_grad_gamma_f32out(int training, const float* g, const float* y, const float* a,
+                             const float* stats, const float* gamma, int relu, int64_t R, int J,
+                             float* part, float* dbeta, float* dgamma, float* da, float* scale,
+                             void* stream);
 /* From d = d(h * noise) [R, K]: dnoise [R, K] = d * h[r % n_h], dh [n_h, K] = sum over the R / n_h
  * particle rows of d * noise (either may be NULL). */
 int zsb_noisy_grad_f32(const float* d, const float* h, int64_t n_h, const float* noise, int64_t R,
@@ -590,6 +615,40 @@ int zsb_conv3x3_wgrad_parts(int64_t R, int64_t Hc, int64_t Wc, int stride);
 int zsb_conv3x3_wgrad_f32(const float* big, const float* small, const float* gate, int grad_big,
                           float* part, float* dW, float* db, int64_t R, int64_t Hc, int64_t Wc,
                           int64_t Ca, int64_t Cb, int stride, void* stream);
+
+/* ---- k x k convolutions on the tensor-core products, NHWC (csrc/conv_tc.cu; the GAN examples) --
+ * The memory passes around the dense products that make a k x k convolution (1 <= k <= 7, stride 1
+ * or 2).  Geometry on the convolution's side: the big grid Hb x Wb is its input (the transposed
+ * convolution's output), the small grid Hs x Ws its output, N images, C channels of the tensor the
+ * pass reads or writes, and big pixel (s i + kh - pt, s j + kw - pl) meets small pixel (i, j) at
+ * tap (kh, kw); big pixels outside the grid count as zero.  TF's SAME and VALID are the caller's
+ * choice of Hs, Ws and the pads (0 <= pt, pl < k).  N Hb Wb C and N Hs Ws k k C below 2^31.
+ * Gather-split: x [N, Hb, Wb, C] -> planes [2][N Hs Ws][kpad(k k C)], the fp16 hi/lo operand
+ * planes of the im2col matrix (column (kh k + kw) C + c) at the power-of-two scale of max |x|,
+ * which is taken from scale[2] when have_amax (a producer's max |.| tag) or found by a max pass;
+ * the fp32 matrix is never written.  scale = device float[4] with scale[2] zero or the tag. */
+int zsb_conv_gather_split_f32(const float* x, int64_t N, int64_t Hb, int64_t Wb, int64_t C,
+                              int64_t Hs, int64_t Ws, int k, int stride, int pt, int pl,
+                              void* planes, float* scale, int have_amax, void* stream);
+/* Col2im-sum: the big-grid tensor [N, Hb, Wb, C] whose entry is the sum, over the taps that land
+ * on it (kh, then kw, ascending: deterministic, no atomics), of cols [N Hs Ws, k k C] fp32.
+ *   epi 0: out = the sum (a convolution's input gradient)
+ *   epi 1: out = sigmoid(sum + bias[c])
+ *   epi 2: batch norm training: pre = the sum and part [ceil(N Hb Wb / 128)][2][C] its per-tile
+ *          moments, for zsb_bn_finish_fused_f32 (out unused)
+ *   epi 3: batch norm evaluation: out = act(xhat gamma + beta), xhat = (sum - moving_mean)
+ *          rsqrt(moving_var + eps); stats [2][C] = (moving_mean, rstd); pre (may be NULL) = sum
+ * max |out| into amax_scale[2] (may be NULL; epi 0, 1, 3). */
+int zsb_conv_col2im_f32(int epi, const float* cols, int64_t N, int64_t Hb, int64_t Wb, int64_t C,
+                        int64_t Hs, int64_t Ws, int k, int stride, int pt, int pl,
+                        const float* bias, const float* gamma, const float* beta,
+                        const float* moving_mean, const float* moving_var, float eps, int relu,
+                        float* stats, float* pre, float* part, float* out, float* amax_scale,
+                        void* stream);
+/* Backward through a sigmoid output y [R, C]: gp = g y (1 - y), max |gp| into scale[2], and db [C]
+ * (may be NULL) = the column sums of gp, merged in a fixed order from part [ceil(R / 128)][C]. */
+int zsb_conv_sigmoid_grad_f32(const float* g, const float* y, int64_t R, int C, float* gp,
+                              float* part, float* db, float* scale, void* stream);
 
 /* ---- K5: SG-MCMC updates (zhusuan/sgmcmc.py) ------------------------------------------------ */
 int zsb_sgmcmc_parts(void);   /* capacity (floats) of every `part` scratch */

@@ -792,7 +792,10 @@ __device__ __forceinline__ void chan_merge(double& n, double& mean, double& m2, 
 // order (lane l folds tiles l, l + 32, ... in turn, then a fixed shuffle tree), so two identical
 // calls give identical bits; stats = (mean, rsqrt(var + eps)) with the population variance, and
 // the moving statistics move towards the batch's: m -= (m - batch) * rate (rate = 1 - decay).
+// BESSEL (TF 1.x's fused batch norm, the path of 4-D inputs): the moving variance moves towards the
+// Bessel-corrected batch variance M2 / (R - 1) instead, and towards M2 / R = 0 when R = 1.
 // Evaluation: stats from the moving statistics, which stay as they are.
+template <bool BESSEL>
 __global__ void __launch_bounds__(256) bn_stats_kernel(const float* __restrict__ part, int64_t R,
                                                        int J, float* __restrict__ mmean,
                                                        float* __restrict__ mvar, float rate,
@@ -822,10 +825,11 @@ __global__ void __launch_bounds__(256) bn_stats_kernel(const float* __restrict__
   }
   if (lane == 0) {
     const float mu = (float)mean, var = (float)(m2 / n);
+    const float var_mv = BESSEL ? (float)(m2 / (n > 1.0 ? n - 1.0 : n)) : var;
     stats[j] = mu;
     stats[J + j] = rsqrtf(var + eps);
     mmean[j] -= (mmean[j] - mu) * rate;
-    mvar[j] -= (mvar[j] - var) * rate;
+    mvar[j] -= (mvar[j] - var_mv) * rate;
   }
 }
 
@@ -948,12 +952,13 @@ __global__ void __launch_bounds__(256) bn_grad_combine_gamma_kernel(
 // da = rstd (g' - coef[0] - xhat coef[1]) in training, rstd g' in evaluation; with GAMMA, rstd is
 // gamma rstd.  PLANES = false: max |da| into scale[2]; PLANES = true: planes [2][R][Jp] = fp16
 // hi/lo of da * scale[0], pad columns zero -- the operand zsb_linear_tc_dgrad_f32 / _wgrad_f32 read.
-template <bool PLANES, bool GAMMA>
+// F32: da [R, J] itself in fp32 (planes = NULL), and max |da| into scale[2].
+template <bool PLANES, bool GAMMA, bool F32 = false>
 __device__ __forceinline__ void bn_grad_apply_rows(
     const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ a,
     bool training, const float* __restrict__ stats, const float* __restrict__ gamma,
     const float* __restrict__ coef, int relu, int64_t R, int J, int Jp,
-    __half* __restrict__ planes, float* __restrict__ scale) {
+    __half* __restrict__ planes, float* __restrict__ scale, float* __restrict__ da = nullptr) {
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const float s = PLANES ? scale[0] : 0.f;
   const int64_t n_pl = R * (int64_t)Jp;
@@ -971,8 +976,12 @@ __device__ __forceinline__ void bn_grad_apply_rows(
         }
         d = (GAMMA ? __ldg(gamma + j) * rs : rs) * gg;
       }
-      if (PLANES) store_hilo(planes + r * Jp + j, n_pl, d * s);
-      else m = finite_absmax(m, d);
+      if (PLANES) {
+        store_hilo(planes + r * Jp + j, n_pl, d * s);
+      } else {
+        if (F32) da[r * J + j] = d;
+        m = finite_absmax(m, d);
+      }
     }
   if (!PLANES) fold_amax(scale, m, tx);
 }
@@ -993,6 +1002,15 @@ __global__ void __launch_bounds__(256) bn_grad_apply_gamma_kernel(
     __half* __restrict__ planes, float* __restrict__ scale) {
   bn_grad_apply_rows<PLANES, true>(g, y, a, training != 0, stats, gamma, coef, relu, R, J, Jp,
                                    planes, scale);
+}
+
+__global__ void __launch_bounds__(256) bn_grad_apply_gamma_f32_kernel(
+    const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ a,
+    int training, const float* __restrict__ stats, const float* __restrict__ gamma,
+    const float* __restrict__ coef, int relu, int64_t R, int J, float* __restrict__ da,
+    float* __restrict__ scale) {
+  bn_grad_apply_rows<false, true, true>(g, y, a, training != 0, stats, gamma, coef, relu, R, J, J,
+                                        nullptr, scale, da);
 }
 
 // From d = d(h * noise) [R, K]: dnoise[r] = d[r] * h[r % n_h] and dh[i] = sum_s d[s n_h + i] *
@@ -1132,6 +1150,42 @@ int linear_tc_wgrad(const void* h_planes, const float* scale_h, int K, const voi
   const int64_t n = (int64_t)J * K;
   slice_sum_kernel<<<grid_blocks(n, 256, 8), 256, 0, st>>>(part, k_slices, n, out);
   return zsb_check_launch("linear_tc_wgrad_slice_sum");
+}
+
+// zsb_linear_tc_bn_gamma_f32 (BESSEL = false) and zsb_linear_tc_bn_gamma_fused_f32 (true)
+template <bool BESSEL>
+int linear_tc_bn_gamma(int training, const void* w_planes, const float* scale_w,
+                       const void* h_planes, const float* scale_h, int h_binary,
+                       const float* gamma, const float* beta, float* moving_mean, float* moving_var,
+                       float rate, float eps, float* stats, float* a, float* part, float* out,
+                       int64_t R, int J, int K, int relu, float* amax_scale, void* stream) {
+  ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && gamma && beta && moving_mean &&
+                  moving_var && stats && out && R > 0 && J > 0 && K > 0 &&
+                  (!training || (a && part)),
+              "zsb_linear_tc_bn_gamma_f32: bad args");
+  ZSB_REQUIRE(R < (1LL << 31), "zsb_linear_tc_bn_gamma_f32: too many rows");
+  cudaStream_t st = (cudaStream_t)stream;
+  const unsigned col_blocks = (unsigned)((J + 7) / 8);
+  return with_h_binary(h_binary, [&](auto z) {
+    LinCore<0, z> c;
+    int rc = make_core(c, w_planes, scale_w, h_planes, scale_h, J, R, K);
+    if (rc) return rc;
+    if (!training) {
+      bn_stats_kernel<false><<<col_blocks, 256, 0, st>>>(nullptr, R, J, moving_mean, moving_var,
+                                                         rate, eps, 0, stats);
+      if ((rc = zsb_check_launch("linear_tc_bn_gamma_stats")) != ZSB_OK) return rc;
+      const BnEpi e{.bn_stats = stats, .bn_beta = beta, .out = out, .relu = relu,
+                    .amax_scale = amax_scale, .bn_gamma = gamma, .pre = a};
+      return tc_launch(LinW<BnEpi, 11, 0, z>{c, e}, st, "linear_tc_bn_gamma_eval");
+    }
+    rc = tc_launch(LinW<BnEpi, 9, 0, z>{c, {.out = a, .part = part}}, st, "linear_tc_bn_gamma_train");
+    if (rc != ZSB_OK) return rc;
+    bn_stats_kernel<BESSEL><<<col_blocks, 256, 0, st>>>(part, R, J, moving_mean, moving_var, rate,
+                                                        eps, 1, stats);
+    bn_apply_gamma_kernel<<<grid_blocks(R, 8, 16), 256, 0, st>>>(a, R, J, stats, gamma, beta, relu,
+                                                                 out, amax_scale);
+    return zsb_check_launch("linear_tc_bn_gamma_apply");
+  });
 }
 
 }  // namespace
@@ -1424,8 +1478,8 @@ int zsb_linear_tc_bn_f32(int training, const void* w_planes, const float* scale_
   if (rc) return rc;
   const unsigned col_blocks = (unsigned)((J + 7) / 8);
   if (!training) {
-    bn_stats_kernel<<<col_blocks, 256, 0, st>>>(nullptr, R, J, moving_mean, moving_var, rate, eps,
-                                                0, stats);
+    bn_stats_kernel<false><<<col_blocks, 256, 0, st>>>(nullptr, R, J, moving_mean, moving_var, rate,
+                                                       eps, 0, stats);
     if ((rc = zsb_check_launch("linear_tc_bn_stats")) != ZSB_OK) return rc;
     const BnEpi e{.bn_stats = stats, .bn_beta = beta, .out = out, .relu = relu,
                   .amax_scale = amax_scale};
@@ -1433,8 +1487,8 @@ int zsb_linear_tc_bn_f32(int training, const void* w_planes, const float* scale_
   }
   rc = tc_launch(LinW<BnEpi, 9>{c, {.out = a, .part = part}}, st, "linear_tc_bn_train");
   if (rc != ZSB_OK) return rc;
-  bn_stats_kernel<<<col_blocks, 256, 0, st>>>(part, R, J, moving_mean, moving_var, rate, eps, 1,
-                                              stats);
+  bn_stats_kernel<false><<<col_blocks, 256, 0, st>>>(part, R, J, moving_mean, moving_var, rate,
+                                                     eps, 1, stats);
   bn_apply_kernel<<<grid_blocks(R, 8, 16), 256, 0, st>>>(a, R, J, stats, beta, relu, out,
                                                          amax_scale);
   return zsb_check_launch("linear_tc_bn_apply");
@@ -1484,33 +1538,23 @@ int zsb_linear_tc_bn_gamma_f32(int training, const void* w_planes, const float* 
                                float* moving_var, float rate, float eps, float* stats, float* a,
                                float* part, float* out, int64_t R, int J, int K, int relu,
                                float* amax_scale, void* stream) {
-  ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && gamma && beta && moving_mean &&
-                  moving_var && stats && out && R > 0 && J > 0 && K > 0 &&
-                  (!training || (a && part)),
-              "zsb_linear_tc_bn_gamma_f32: bad args");
-  ZSB_REQUIRE(R < (1LL << 31), "zsb_linear_tc_bn_gamma_f32: too many rows");
-  cudaStream_t st = (cudaStream_t)stream;
-  const unsigned col_blocks = (unsigned)((J + 7) / 8);
-  return with_h_binary(h_binary, [&](auto z) {
-    LinCore<0, z> c;
-    int rc = make_core(c, w_planes, scale_w, h_planes, scale_h, J, R, K);
-    if (rc) return rc;
-    if (!training) {
-      bn_stats_kernel<<<col_blocks, 256, 0, st>>>(nullptr, R, J, moving_mean, moving_var, rate,
-                                                  eps, 0, stats);
-      if ((rc = zsb_check_launch("linear_tc_bn_gamma_stats")) != ZSB_OK) return rc;
-      const BnEpi e{.bn_stats = stats, .bn_beta = beta, .out = out, .relu = relu,
-                    .amax_scale = amax_scale, .bn_gamma = gamma, .pre = a};
-      return tc_launch(LinW<BnEpi, 11, 0, z>{c, e}, st, "linear_tc_bn_gamma_eval");
-    }
-    rc = tc_launch(LinW<BnEpi, 9, 0, z>{c, {.out = a, .part = part}}, st, "linear_tc_bn_gamma_train");
-    if (rc != ZSB_OK) return rc;
-    bn_stats_kernel<<<col_blocks, 256, 0, st>>>(part, R, J, moving_mean, moving_var, rate, eps, 1,
-                                                stats);
-    bn_apply_gamma_kernel<<<grid_blocks(R, 8, 16), 256, 0, st>>>(a, R, J, stats, gamma, beta, relu,
-                                                                 out, amax_scale);
-    return zsb_check_launch("linear_tc_bn_gamma_apply");
-  });
+  return linear_tc_bn_gamma<false>(training, w_planes, scale_w, h_planes, scale_h, h_binary,
+                                   gamma, beta, moving_mean, moving_var, rate, eps, stats, a,
+                                   part, out, R, J, K, relu, amax_scale, stream);
+}
+// As zsb_linear_tc_bn_gamma_f32 with the moving-variance update of TF 1.x's fused batch norm
+// (4-D inputs): in training the moving variance moves towards the Bessel-corrected batch variance
+// R / (R - 1) var (towards var = 0 when R = 1); the output still normalises with the population
+// variance.
+int zsb_linear_tc_bn_gamma_fused_f32(int training, const void* w_planes, const float* scale_w,
+                                     const void* h_planes, const float* scale_h, int h_binary,
+                                     const float* gamma, const float* beta, float* moving_mean,
+                                     float* moving_var, float rate, float eps, float* stats,
+                                     float* a, float* part, float* out, int64_t R, int J, int K,
+                                     int relu, float* amax_scale, void* stream) {
+  return linear_tc_bn_gamma<true>(training, w_planes, scale_w, h_planes, scale_h, h_binary,
+                                  gamma, beta, moving_mean, moving_var, rate, eps, stats, a,
+                                  part, out, R, J, K, relu, amax_scale, stream);
 }
 
 // Backward of zsb_linear_tc_bn_gamma_f32 from the upstream gradient g [R, J], its output y (read
@@ -1542,6 +1586,47 @@ int zsb_bn_grad_gamma_f32(int training, const float* g, const float* y, const fl
   bn_grad_apply_gamma_kernel<true><<<blocks, 256, 0, st>>>(g, y, a, training, stats, gamma, coef,
                                                            relu, R, J, Jp, pl, scale);
   return zsb_check_launch("bn_grad_gamma");
+}
+
+// The training step of TF 1.x's fused batch norm (4-D inputs) after a pass that left the
+// pre-activation a [R, J] and its per-128-row-tile moment partials part (EPI 9's layout): the
+// deterministic merge, stats = (mean, rstd), the moving statistics updated as in
+// zsb_linear_tc_bn_gamma_fused_f32, then out = act(xhat * gamma + beta), max |out| into
+// amax_scale[2] (may be NULL).
+int zsb_bn_finish_fused_f32(const float* a, const float* part, int64_t R, int J,
+                            const float* gamma, const float* beta, float* moving_mean,
+                            float* moving_var, float rate, float eps, float* stats, float* out,
+                            int relu, float* amax_scale, void* stream) {
+  ZSB_REQUIRE(a && part && gamma && beta && moving_mean && moving_var && stats && out && R > 0 &&
+                  J > 0,
+              "zsb_bn_finish_fused_f32: bad args");
+  cudaStream_t st = (cudaStream_t)stream;
+  bn_stats_kernel<true><<<(unsigned)((J + 7) / 8), 256, 0, st>>>(part, R, J, moving_mean,
+                                                                 moving_var, rate, eps, 1, stats);
+  bn_apply_gamma_kernel<<<grid_blocks(R, 8, 16), 256, 0, st>>>(a, R, J, stats, gamma, beta, relu,
+                                                               out, amax_scale);
+  return zsb_check_launch("bn_finish_fused");
+}
+
+// As zsb_bn_grad_gamma_f32, but da [R, J] is written in fp32 and max |da| folded into scale[2]
+// (device float[4] with scale[2] zero), for a consumer that gathers da before splitting it.
+int zsb_bn_grad_gamma_f32out(int training, const float* g, const float* y, const float* a,
+                             const float* stats, const float* gamma, int relu, int64_t R, int J,
+                             float* part, float* dbeta, float* dgamma, float* da, float* scale,
+                             void* stream) {
+  ZSB_REQUIRE(g && stats && gamma && part && da && scale && R > 0 && J > 0 && (!relu || y) &&
+                  (!(training || dgamma) || a),
+              "zsb_bn_grad_gamma_f32out: bad args");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t n_t = (R + BN_TILE - 1) / BN_TILE;
+  float* coef = part + 2 * n_t * J;
+  bn_grad_sums_kernel<<<dim3((unsigned)n_t, (unsigned)((J + 31) / 32)), 256, 0, st>>>(
+      g, y, a, stats, relu, R, J, part);
+  bn_grad_combine_gamma_kernel<<<(unsigned)((J + 7) / 8), 256, 0, st>>>(part, R, J, dbeta, dgamma,
+                                                                        coef);
+  bn_grad_apply_gamma_f32_kernel<<<grid_blocks(R, 8, 16), 256, 0, st>>>(
+      g, y, a, training, stats, gamma, coef, relu, R, J, da, scale);
+  return zsb_check_launch("bn_grad_gamma_f32out");
 }
 
 // Gradients of x = h[r % n_h] * noise[r] from d = dL/dx [R, K]: dnoise [R, K] = d * h[r % n_h] and

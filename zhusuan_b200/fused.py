@@ -14,7 +14,8 @@ from .distributions.univariate import Normal
 
 __all__ = ["GaussianLogJoint", "BNNRegressionLogJoint", "LNTMLogJoint", "PMFLogJoint", "linear",
            "class_linear", "noisy_bn_linear", "bn_linear", "linear_bernoulli_log_prob",
-           "LinearBernoulli", "RBFKernel", "gp_conditional", "conv2d", "conv2d_transpose"]
+           "LinearBernoulli", "RBFKernel", "gp_conditional", "conv2d", "conv2d_transpose",
+           "bn_conv2d", "bn_conv2d_transpose", "sigmoid_conv2d_transpose"]
 
 
 class GaussianLogJoint(object):
@@ -1840,3 +1841,449 @@ def conv2d_transpose(x, W, out_shape, stride=1, b=None, relu=False, residual=Non
         R *= int(d)
     geom = (True, int(stride), R, Ho, Wo, Hi, Wi, Cin, Cout)
     return _conv_apply("conv2d_transpose", x, W, b, residual, geom, relu, lead, (Ho, Wo))
+
+
+# ---------------------------------------------------------------------------
+# k x k convolutions on the tensor-core products (csrc/conv_tc.cu): the GAN examples
+# ---------------------------------------------------------------------------
+CONV_TC_MAX_K = 7
+
+
+class _ConvGeom(object):
+    """A k x k convolution from the big grid Hb x Wb (its input) to the small grid Hs x Ws (its
+    output) over N images, with TF's pads before (pt, pl); the transposed convolution runs the
+    same geometry the other way.  Cin / Cout are the channels of the layer's input / output."""
+    __slots__ = ("N", "Hb", "Wb", "Hs", "Ws", "k", "s", "pt", "pl", "Cin", "Cout")
+
+    def __init__(self, N, Hb, Wb, Hs, Ws, k, s, pt, pl, Cin, Cout):
+        self.N, self.Hb, self.Wb, self.Hs, self.Ws = N, Hb, Wb, Hs, Ws
+        self.k, self.s, self.pt, self.pl, self.Cin, self.Cout = k, s, pt, pl, Cin, Cout
+
+    def args(self, C):
+        """(N, Hb, Wb, C, Hs, Ws, k, s, pt, pl) of a conv_tc.cu pass over C channels."""
+        return (self.N, self.Hb, self.Wb, C, self.Hs, self.Ws, self.k, self.s, self.pt, self.pl)
+
+
+def _tf_pad_before(big, small, k, s, padding):
+    """TF's pad before the first row: SAME pads pad_total = max((small - 1) s + k - big, 0) rows,
+    pad_total // 2 of them before (asymmetric for even k and at stride 2); VALID pads nothing."""
+    return max((small - 1) * s + k - big, 0) // 2 if padding == "SAME" else 0
+
+
+def _conv_tc_geom(name, x, W, stride, padding, transpose):
+    """Validate the arguments of a tensor-core convolution before any launch and return its
+    _ConvGeom and the leading shape of x."""
+    if not isinstance(x, torch.Tensor) or not isinstance(W, torch.Tensor):
+        raise ValueError("%s: x and W should be tensors" % name)
+    if x.dtype != torch.float32 or W.dtype != torch.float32:
+        raise ValueError("%s: x and W should be float32, got %s and %s" % (name, x.dtype, W.dtype))
+    if not x.is_cuda or x.device != W.device:
+        raise ValueError("%s: x and W should be on one CUDA device, got %s and %s"
+                         % (name, x.device, W.device))
+    if x.dim() < 3:
+        raise ValueError("%s: x should be NHWC [..., H, W, C], got %s" % (name, tuple(x.shape)))
+    if W.dim() != 4 or int(W.shape[0]) != int(W.shape[1]) or \
+            not 1 <= int(W.shape[0]) <= CONV_TC_MAX_K:
+        raise ValueError("%s: W should be a square k x k kernel [k, k, ., .] with 1 <= k <= %d, "
+                         "got %s" % (name, CONV_TC_MAX_K, tuple(W.shape)))
+    if isinstance(stride, bool) or stride not in (1, 2):
+        raise ValueError("%s: stride should be 1 or 2, got %r" % (name, stride))
+    if not isinstance(padding, str) or padding.upper() not in ("SAME", "VALID"):
+        raise ValueError("%s: padding should be 'SAME' or 'VALID', got %r" % (name, padding))
+    padding = padding.upper()
+    k, s = int(W.shape[0]), int(stride)
+    # tf.layers kernels: conv2d [k, k, Cin, Cout], conv2d_transpose [k, k, Cout, Cin]
+    Cin, Cout = (int(W.shape[3]), int(W.shape[2])) if transpose else \
+        (int(W.shape[2]), int(W.shape[3]))
+    if int(x.shape[-1]) != Cin:
+        raise ValueError("%s: x has %d channels, W expects %d" % (name, int(x.shape[-1]), Cin))
+    if x.numel() == 0 or W.numel() == 0:
+        raise ValueError("%s: empty shapes are not supported: x %s, W %s"
+                         % (name, tuple(x.shape), tuple(W.shape)))
+    lead = tuple(int(d) for d in x.shape[:-3])
+    N = 1
+    for d in lead:
+        N *= d
+    H, Wd = int(x.shape[-3]), int(x.shape[-2])
+    if transpose:
+        Hs, Ws = H, Wd
+        grow = 0 if padding == "SAME" else max(k - s, 0)
+        Hb, Wb = Hs * s + grow, Ws * s + grow
+    else:
+        Hb, Wb = H, Wd
+        if padding == "SAME":
+            Hs, Ws = -(-Hb // s), -(-Wb // s)
+        else:
+            Hs, Ws = -(-(Hb - k + 1) // s), -(-(Wb - k + 1) // s)
+        if Hs < 1 or Ws < 1:
+            raise ValueError("%s: a %dx%d input is smaller than the %dx%d kernel (VALID)"
+                             % (name, Hb, Wb, k, k))
+    pt, pl = _tf_pad_before(Hb, Hs, k, s, padding), _tf_pad_before(Wb, Ws, k, s, padding)
+    kk = k * k
+    big, small = N * Hb * Wb, N * Hs * Ws
+    C_big, C_small = (Cout, Cin) if transpose else (Cin, Cout)
+    if max(big * C_big, small * C_small, small * kk * C_big,
+           small * (-(-(kk * C_big) // 64) * 64), big * (-(-C_big // 64) * 64)) >= 2 ** 31:
+        raise ValueError("%s: too large: every tensor and operand of the layer must have fewer "
+                         "than 2^31 entries (N*H*W*k*k*C)" % name)
+    return _ConvGeom(N, Hb, Wb, Hs, Ws, k, s, pt, pl, Cin, Cout), lead
+
+
+def _conv_bn_check(name, Cout, dev, gamma, beta, moving_mean, moving_variance):
+    for nm, t, opt in (("gamma", gamma, True), ("beta", beta, False)):
+        if t is None and opt:
+            continue
+        if not isinstance(t, torch.Tensor) or tuple(t.shape) != (Cout,) or \
+                t.dtype != torch.float32 or t.device != dev:
+            raise ValueError("%s: %s must be a float32 [%d] tensor on %s" % (name, nm, Cout, dev))
+    for nm, t in (("moving_mean", moving_mean), ("moving_variance", moving_variance)):
+        if not isinstance(t, torch.Tensor) or tuple(t.shape) != (Cout,) or \
+                t.dtype != torch.float32 or not t.is_contiguous() or t.device != dev:
+            raise ValueError("%s: %s must be a contiguous float32 [%d] tensor on %s"
+                             % (name, nm, Cout, dev))
+
+
+def _gather_planes(x4, g, C, tag=None):
+    """The fp16 operand planes of the im2col matrix [N Hs Ws, k k C] of x4 [N, Hb, Wb, C]
+    (zsb_conv_gather_split_f32), at the scale of ``tag`` (a scale slot holding max |x4|) when
+    given, else of one max pass."""
+    from ._lib import lib, ptr, stream
+    R, K = g.N * g.Hs * g.Ws, g.k * g.k * C
+    planes = torch.empty((2, R, lib.load().zsb_linear_tc_kpad(K)), dtype=torch.float16,
+                         device=x4.device)
+    scale = tag if tag is not None else torch.zeros(4, dtype=torch.float32, device=x4.device)
+    lib.call("zsb_conv_gather_split_f32", ptr(x4), *g.args(C), ptr(planes), ptr(scale),
+             int(tag is not None), stream())
+    return _Planes(planes, scale, R, K)
+
+
+def _take_tag(x):
+    """The max |.| scale slot a producing fused layer left on x (consumed: its word 2 is cleared
+    by the split that reads it), or None."""
+    tag = getattr(x, "_zsb_amax", None)
+    if tag is not None:
+        try:
+            del x._zsb_amax
+        except (AttributeError, RuntimeError):
+            pass
+    return tag
+
+
+def _col2im(epi, cols, g, C, out=None, bias=None, gamma=None, beta=None, mm=None, mv=None,
+            eps=0.0, relu=False, stats=None, pre=None, part=None, amax=None):
+    from ._lib import lib, ptr, stream
+    lib.call("zsb_conv_col2im_f32", epi, ptr(cols), *g.args(C), ptr(bias), ptr(gamma), ptr(beta),
+             ptr(mm), ptr(mv), float(eps), int(bool(relu)), ptr(stats), ptr(pre), ptr(part),
+             ptr(out), ptr(amax), stream())
+
+
+def _ones_like_gamma(gamma, Cout, dev):
+    return gamma.detach().contiguous() if gamma is not None else \
+        torch.ones(Cout, dtype=torch.float32, device=dev)
+
+
+class _BNConv2d(torch.autograd.Function):
+    """relu?(BN(conv(x, W)) * gamma + beta): the gather-split of x, then the batch-norm product of
+    the dense layers with TF's fused-batch-norm update (zsb_linear_tc_bn_gamma_fused_f32) over
+    R = N Ho Wo rows, J = Cout features and K = k k Cin.  Backward: zsb_bn_grad_gamma_f32 gives
+    d beta, d gamma and the planes of G = d/d(pre-activation); dx is the col2im-sum of G W (the
+    MN-major input-gradient product) and dW the weight-gradient product of G and the saved
+    gather planes."""
+
+    @staticmethod
+    def forward(ctx, x, W, gamma, beta, stats_bufs, g, training, relu, rate, eps, keep_pre):
+        from ._lib import lib, ptr, stream
+        moving_mean, moving_variance = stats_bufs
+        dev = W.device
+        tag = _take_tag(x)
+        x4 = x.detach().reshape(g.N, g.Hb, g.Wb, g.Cin).contiguous()
+        hpl = _gather_planes(x4, g, g.Cin, tag)
+        R, K, J = hpl.rows, hpl.K, g.Cout
+        Wt = W.detach().reshape(K, J).t()
+        wp, ws = _tc_split(Wt)
+        gm = _ones_like_gamma(gamma, J, dev)
+        b = beta.detach().contiguous()
+        stats = torch.empty((2, J), dtype=torch.float32, device=dev)
+        y = torch.empty((R, J), dtype=torch.float32, device=dev)
+        a = part = None
+        if training or keep_pre:
+            a = torch.empty((R, J), dtype=torch.float32, device=dev)
+        if training:
+            part = torch.empty(-(-R // 128) * 2 * J, dtype=torch.float32, device=dev)
+        amax = torch.zeros(4, dtype=torch.float32, device=dev)
+        lib.call("zsb_linear_tc_bn_gamma_fused_f32", int(training), ptr(wp), ptr(ws),
+                 ptr(hpl.planes), ptr(hpl.scale), 0, ptr(gm), ptr(b), ptr(moving_mean),
+                 ptr(moving_variance), rate, eps, ptr(stats), ptr(a), ptr(part), ptr(y), R, J, K,
+                 int(relu), ptr(amax), stream())
+        ctx.save_for_backward(gm, y if relu else None, a, stats)
+        ctx.hpl, ctx.wpl, ctx.Wt_shape = hpl, (wp, ws), (J, K)
+        ctx.meta = (g, tuple(x.shape), training, relu, gamma is not None)
+        return _tag(y.reshape(tuple(x.shape[:-3]) + (g.Hs, g.Ws, J)), amax)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        from ._lib import lib, ptr, stream
+        gm, y, a, stats = ctx.saved_tensors
+        g, x_shape, training, relu, has_gamma = ctx.meta
+        need = ctx.needs_input_grad
+        dev = gy.device
+        R, J = g.N * g.Hs * g.Ws, g.Cout
+        gg = gy.reshape(R, J).to(torch.float32).contiguous()
+        dgamma = torch.empty(J, dtype=torch.float32, device=dev) if need[2] else None
+        dbeta = torch.empty(J, dtype=torch.float32, device=dev) if need[3] else None
+        part = torch.empty((-(-R // 128) + 1) * 2 * J, dtype=torch.float32, device=dev)
+        planes = torch.empty((2, R, lib.load().zsb_linear_tc_kpad(J)), dtype=torch.float16,
+                             device=dev)
+        scale = torch.zeros(4, dtype=torch.float32, device=dev)
+        lib.call("zsb_bn_grad_gamma_f32", int(training), ptr(gg), ptr(y), ptr(a), ptr(stats),
+                 ptr(gm), int(relu), R, J, ptr(part), ptr(dbeta), ptr(dgamma), ptr(planes),
+                 ptr(scale), stream())
+        gpl = _Planes(planes, scale, R, J)
+        dx = dW = None
+        if need[0]:
+            wp, ws = ctx.wpl
+            dcols, _ = _tc_grad_input(gpl, _ShapeOnly(ctx.Wt_shape, dev), R, wp, ws)
+            dx = torch.empty((g.N, g.Hb, g.Wb, g.Cin), dtype=torch.float32, device=dev)
+            amax = torch.zeros(4, dtype=torch.float32, device=dev)
+            _col2im(0, dcols, g, g.Cin, out=dx, amax=amax)
+            del dcols
+            dx = _tag(dx.reshape(x_shape), amax)
+        if need[1]:
+            dW = _tc_grad_weight(gpl, ctx.hpl, R).t().reshape(g.k, g.k, g.Cin, g.Cout)
+        ctx.hpl = ctx.wpl = None
+        return dx, dW, dgamma, dbeta, None, None, None, None, None, None, None
+
+
+class _ShapeOnly(object):
+    """Stands for a weight matrix whose operand planes the caller already has: _tc_grad_input
+    reads only its shape and device."""
+    __slots__ = ("shape", "device")
+
+    def __init__(self, shape, device):
+        self.shape, self.device = shape, device
+
+
+def _conv_t_product(x, W, g):
+    """cols [N Hs Ws, k k Cout] = x W'^T with W' = W.reshape(k k Cout, Cin) on the epi-0 product,
+    from the planes of x (scaled by its max |.| tag when it has one); returns cols, the planes of
+    x and of W'.  The planes are not cached on x: only the layer's backward keeps them."""
+    kk = g.k * g.k
+    x2 = x.detach().reshape(-1, g.Cin)
+    tag = _take_tag(x)
+    hpl = _tc_split_dual(x2, amax=None if g.Cin % 2 else tag)
+    wp, ws = _tc_split(W.detach().reshape(kk * g.Cout, g.Cin))
+    cols = _tc_linear(0, wp, ws, hpl.planes, hpl.scale, None, None, None, hpl.rows,
+                      kk * g.Cout, g.Cin)
+    return cols, hpl, (wp, ws)
+
+
+def _conv_t_grads(ctx, gp, gscale, g, need_x, need_W, x_shape):
+    """dx and dW of a transposed convolution from gp = d/d(its output) [N Hb Wb, Cout] in fp32
+    with its max |.| in gscale: the gather-split of gp on the small grid, then the input-gradient
+    product with the forward planes of W' and the weight-gradient product with the planes of x."""
+    R = g.N * g.Hs * g.Ws
+    gpl = _gather_planes(gp.reshape(g.N, g.Hb, g.Wb, g.Cout), g, g.Cout, gscale)
+    dx = dW = None
+    if need_x:
+        wp, ws = ctx.wpl
+        dx2, amax = _tc_grad_input(gpl, _ShapeOnly((gpl.K, g.Cin), gp.device), R, wp, ws)
+        dx = _tag(dx2.reshape(x_shape), amax)
+    if need_W:
+        dW = _tc_grad_weight(gpl, ctx.hpl, R).reshape(g.k, g.k, g.Cout, g.Cin)
+    ctx.hpl = ctx.wpl = None
+    return dx, dW
+
+
+class _BNConv2dT(torch.autograd.Function):
+    """relu?(BN(conv_transpose(x, W)) * gamma + beta): the epi-0 product x W'^T gives the columns
+    [N Hi Wi, k k Cout]; their col2im-sum onto the output grid runs the batch-norm epilogue
+    (training: pre-activation and moment partials, then zsb_bn_finish_fused_f32; evaluation:
+    the affine step in place).  Backward: zsb_bn_grad_gamma_f32out gives d beta, d gamma and
+    da in fp32, then _conv_t_grads."""
+
+    @staticmethod
+    def forward(ctx, x, W, gamma, beta, stats_bufs, g, training, relu, rate, eps, keep_pre):
+        from ._lib import lib, ptr, stream
+        moving_mean, moving_variance = stats_bufs
+        dev = W.device
+        J, Rb = g.Cout, g.N * g.Hb * g.Wb
+        cols, hpl, wpl = _conv_t_product(x, W, g)
+        gm = _ones_like_gamma(gamma, J, dev)
+        b = beta.detach().contiguous()
+        stats = torch.empty((2, J), dtype=torch.float32, device=dev)
+        y = torch.empty((Rb, J), dtype=torch.float32, device=dev)
+        a = torch.empty((Rb, J), dtype=torch.float32, device=dev) if training or keep_pre \
+            else None
+        amax = torch.zeros(4, dtype=torch.float32, device=dev)
+        if training:
+            part = torch.empty(-(-Rb // 128) * 2 * J, dtype=torch.float32, device=dev)
+            _col2im(2, cols, g, J, pre=a, part=part)
+            del cols
+            lib.call("zsb_bn_finish_fused_f32", ptr(a), ptr(part), Rb, J, ptr(gm), ptr(b),
+                     ptr(moving_mean), ptr(moving_variance), rate, eps, ptr(stats), ptr(y),
+                     int(relu), ptr(amax), stream())
+        else:
+            _col2im(3, cols, g, J, out=y, gamma=gm, beta=b, mm=moving_mean, mv=moving_variance,
+                    eps=eps, relu=relu, stats=stats, pre=a, amax=amax)
+            del cols
+        ctx.save_for_backward(gm, y if relu else None, a, stats)
+        ctx.hpl, ctx.wpl = hpl, wpl
+        ctx.meta = (g, tuple(x.shape), training, relu)
+        return _tag(y.reshape(tuple(x.shape[:-3]) + (g.Hb, g.Wb, J)), amax)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        from ._lib import lib, ptr, stream
+        gm, y, a, stats = ctx.saved_tensors
+        g, x_shape, training, relu = ctx.meta
+        need = ctx.needs_input_grad
+        dev = gy.device
+        J, Rb = g.Cout, g.N * g.Hb * g.Wb
+        gg = gy.reshape(Rb, J).to(torch.float32).contiguous()
+        dgamma = torch.empty(J, dtype=torch.float32, device=dev) if need[2] else None
+        dbeta = torch.empty(J, dtype=torch.float32, device=dev) if need[3] else None
+        part = torch.empty((-(-Rb // 128) + 1) * 2 * J, dtype=torch.float32, device=dev)
+        da = torch.empty((Rb, J), dtype=torch.float32, device=dev)
+        scale = torch.zeros(4, dtype=torch.float32, device=dev)
+        lib.call("zsb_bn_grad_gamma_f32out", int(training), ptr(gg), ptr(y), ptr(a), ptr(stats),
+                 ptr(gm), int(relu), Rb, J, ptr(part), ptr(dbeta), ptr(dgamma), ptr(da),
+                 ptr(scale), stream())
+        dx, dW = _conv_t_grads(ctx, da, scale, g, need[0], need[1], x_shape)
+        return dx, dW, dgamma, dbeta, None, None, None, None, None, None, None
+
+
+class _SigmoidConv2dT(torch.autograd.Function):
+    """sigmoid(conv_transpose(x, W) + b): the epi-0 product, then the col2im-sum with the bias +
+    sigmoid epilogue.  Backward: gp = g y (1 - y) and db from zsb_conv_sigmoid_grad_f32, then
+    _conv_t_grads."""
+
+    @staticmethod
+    def forward(ctx, x, W, b, g):
+        J, Rb = g.Cout, g.N * g.Hb * g.Wb
+        dev = W.device
+        cols, hpl, wpl = _conv_t_product(x, W, g)
+        bias = b.detach().contiguous() if b is not None else \
+            torch.zeros(J, dtype=torch.float32, device=dev)
+        y = torch.empty((Rb, J), dtype=torch.float32, device=dev)
+        amax = torch.zeros(4, dtype=torch.float32, device=dev)
+        _col2im(1, cols, g, J, out=y, bias=bias, amax=amax)
+        del cols
+        ctx.save_for_backward(y)
+        ctx.hpl, ctx.wpl = hpl, wpl
+        ctx.meta = (g, tuple(x.shape))
+        return _tag(y.reshape(tuple(x.shape[:-3]) + (g.Hb, g.Wb, J)), amax)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        from ._lib import lib, ptr, stream
+        y, = ctx.saved_tensors
+        g, x_shape = ctx.meta
+        need = ctx.needs_input_grad
+        dev = gy.device
+        J, Rb = g.Cout, g.N * g.Hb * g.Wb
+        gg = gy.reshape(Rb, J).to(torch.float32).contiguous()
+        gp = torch.empty((Rb, J), dtype=torch.float32, device=dev)
+        part = torch.empty(-(-Rb // 128) * J, dtype=torch.float32, device=dev)
+        db = torch.empty(J, dtype=torch.float32, device=dev) if need[2] else None
+        scale = torch.zeros(4, dtype=torch.float32, device=dev)
+        lib.call("zsb_conv_sigmoid_grad_f32", ptr(gg), ptr(y), Rb, J, ptr(gp), ptr(part), ptr(db),
+                 ptr(scale), stream())
+        dx, dW = _conv_t_grads(ctx, gp, scale, g, need[0], need[1], x_shape)
+        return dx, dW, db, None
+
+
+
+
+def _bn_conv_apply(fn, name, x, W, gamma, beta, moving_mean, moving_variance, training, stride,
+                   padding, relu, momentum, epsilon, transpose):
+    x = _unwrap(x)
+    g, _ = _conv_tc_geom(name, x, W, stride, padding, transpose)
+    _conv_bn_check(name, g.Cout, W.device, gamma, beta, moving_mean, moving_variance)
+    keep_pre = (not training) and torch.is_grad_enabled() and gamma is not None and \
+        gamma.requires_grad
+    return fn.apply(x, W, gamma, beta, (moving_mean, moving_variance), g, bool(training),
+                    bool(relu), float(1.0 - momentum), float(epsilon), bool(keep_pre))
+
+
+def bn_conv2d(x, W, gamma, beta, moving_mean, moving_variance, training, stride=1,
+              padding="SAME", relu=True, momentum=0.99, epsilon=1e-3):
+    """``relu?(BN(tf.layers.conv2d(x, Cout, k, stride, padding, use_bias=False)))``, the conv ->
+    batch norm -> ReLU layer of examples/generative_adversarial_nets (dcgan.py, wasserstein_gan.py)
+    on the tensor-core products at fp32 accuracy.
+
+    x [..., H, W, Cin] is NHWC, any leading shape flattened to images; W [k, k, Cin, Cout] is the
+    ``tf.layers.conv2d`` kernel, 1 <= k <= 7; gamma (or None) and beta [Cout].  The output is
+    [..., Ho, Wo, Cout] with Ho = ceil(H / s) (SAME) or ceil((H - k + 1) / s) (VALID), and
+
+        a[n, i, j, co] = sum_{kh, kw, ci} x[n, s i + kh - pt, s j + kw - pl, ci] W[kh, kw, ci, co]
+
+    where out-of-range x counts as 0.  SAME pads by TF's rule, pad_total = max((Ho - 1) s + k - H,
+    0) and pt = pad_total // 2 (pl likewise): asymmetric for even k and at stride 2.  VALID pads
+    nothing.
+
+    Batch norm is ``tf.layers.batch_normalization(training=training)`` with its defaults
+    (``center=True``, ``scale=True``: ``y = xhat * gamma + beta``, ``xhat = (a - mean) *
+    rsqrt(var + epsilon)``) on TF 1.x's FUSED path, which ``tf.layers`` takes for 4-D inputs
+    (``BatchNormalization._fused_batch_norm`` with ``_bessels_correction_test_only = True``, its
+    default).  This differs from ``bn_linear``, which keeps the non-fused rule of 2-D inputs:
+
+    * ``training``: ``mean`` and the population variance ``var`` over all N*H*W pixels normalise
+      the output, but the moving variance moves towards the Bessel-corrected ``var * R / (R - 1)``
+      (``R = N*H*W``); the moving mean towards ``mean``.  Both in place, as ``m -= (m - batch) *
+      (1 - momentum)``, with no zero-debiasing.  At ``R = 1`` the moving variance moves towards
+      ``var = 0``: the factor is 1 there, as in the CPU kernel of TF's ``fused_batch_norm``.
+    * otherwise the moving statistics normalise and stay unchanged.
+
+    ``gamma=None`` is ``scale=False`` (wasserstein_gan.py) and gives the bits of ``gamma = ones``.
+    ``moving_mean`` / ``moving_variance`` are contiguous float32 [Cout] and get no gradient.
+
+    Differentiable w.r.t. x, W, gamma and beta; under ``inference_mode`` nothing is kept.  The
+    batch moments and every gradient are reduced in a fixed order with no float atomics, so two
+    identical calls give identical bits.  The output carries the max |.| that a following fused
+    layer uses for its operand split.  Supported: float32 CUDA tensors on one device, stride 1 or
+    2, padding "SAME" or "VALID", no empty shapes, fewer than 2^31 entries in every tensor and
+    operand; anything else raises ValueError before any launch."""
+    return _bn_conv_apply(_BNConv2d, "bn_conv2d", x, W, gamma, beta, moving_mean, moving_variance,
+                          training, stride, padding, relu, momentum, epsilon, False)
+
+
+def bn_conv2d_transpose(x, W, gamma, beta, moving_mean, moving_variance, training, stride=1,
+                        padding="SAME", relu=True, momentum=0.99, epsilon=1e-3):
+    """``relu?(BN(tf.layers.conv2d_transpose(x, Cout, k, stride, padding, use_bias=False)))``, the
+    generators' deconv -> batch norm -> ReLU layer of examples/generative_adversarial_nets, on the
+    tensor-core products at fp32 accuracy.
+
+    x [..., Hi, Wi, Cin] is NHWC; W [k, k, Cout, Cin] is the ``tf.layers.conv2d_transpose``
+    kernel, 1 <= k <= 7.  The output is [..., Ho, Wo, Cout] as ``tf.layers`` sizes it: Ho = Hi s
+    (SAME) or Hi s + max(k - s, 0) (VALID).  The map is the adjoint of ``bn_conv2d``'s
+    convolution from [Ho, Wo, Cout] to [Hi, Wi, Cin] with the same W and pads:
+
+        a[n, h, w, co] = sum x[n, i, j, ci] W[kh, kw, co, ci]  over h = s i + kh - pt, w = s j + kw - pl
+
+    computed as the product x W'^T (W' = W.reshape(k k Cout, Cin)) followed by a gather of its
+    columns onto the output grid, so no structural zero is multiplied.  Batch norm, ``gamma=None``
+    and the moving statistics are those of ``bn_conv2d`` (TF's fused rule for 4-D inputs, not
+    ``bn_linear``'s).  Gradients, determinism, inference mode, the amax tag and the supported
+    range are those of ``bn_conv2d``."""
+    return _bn_conv_apply(_BNConv2dT, "bn_conv2d_transpose", x, W, gamma, beta, moving_mean,
+                          moving_variance, training, stride, padding, relu, momentum, epsilon,
+                          True)
+
+
+def sigmoid_conv2d_transpose(x, W, b=None, stride=1, padding="SAME"):
+    """``tf.layers.conv2d_transpose(x, Cout, k, stride, padding, activation=tf.sigmoid)`` with its
+    bias b [Cout] (None: no bias), the generators' output layers of
+    examples/generative_adversarial_nets.  Geometry and W as in ``bn_conv2d_transpose``.
+    Differentiable w.r.t. x, W and b; the bias gradient is a column sum merged in a fixed order.
+    Determinism, inference mode, the amax tag and the supported range are those of
+    ``bn_conv2d``."""
+    x = _unwrap(x)
+    g, _ = _conv_tc_geom("sigmoid_conv2d_transpose", x, W, stride, padding, True)
+    if b is not None and (not isinstance(b, torch.Tensor) or tuple(b.shape) != (g.Cout,) or
+                          b.dtype != torch.float32 or b.device != W.device):
+        raise ValueError("sigmoid_conv2d_transpose: b must be a float32 [%d] tensor on %s"
+                         % (g.Cout, W.device))
+    return _SigmoidConv2dT.apply(x, W, b, g)
