@@ -557,6 +557,30 @@ int zsb_planar_flow_bwd_f32(const float* ck, const float* gz_out, const float* g
                             float* part, float* db, float* daux_u, float* dw, int64_t R,
                             int64_t d, int64_t n_iters, void* stream);
 
+/* ---- Inverse autoregressive flows (csrc/iaf.cu; zhusuan/transform.py:17-67, :200-282) ---------
+ * A stack of n_iters IAF flows with linear_ar's network along the last axis of z [R, d], weights
+ * m_w and s_w [n_iters, d, d] (linear_ar's m_w and s_w of every flow, stacked; only the entries
+ * i < j are read, transform.py:38-43, :55-56).  Per flow (transform.py:58-61, :263-275):
+ *   m = z (mask * m_w),  t = z (mask * s_w),  s = exp(t)
+ *   update 0 ('normal'): z = s z + m,                  log_q -= sum_j t_j
+ *   update 1 ('gru'):    g = sigmoid(s), z = g z + (1 - g) m,  log_q += sum_j log1p(exp(-s_j))
+ *   z = reverse(z)
+ * 1 <= d <= 256, n_iters >= 1, R >= 0.  No floating-point atomics: deterministic. */
+/* Forward, one launch: z_out [R, d], lq_out [R] from z_in, lq_in.  ck: NULL, or [n_iters, R, d]
+ * receiving every flow's input z, which zsb_iaf_bwd_f32 reads. */
+int zsb_iaf_fwd_f32(const float* z_in, const float* lq_in, const float* m_w, const float* s_w,
+                    float* z_out, float* lq_out, float* ck, int64_t R, int64_t d,
+                    int64_t n_iters, int update, void* stream);
+/* Slices of the backward sweep for these sizes; its `part` scratch is
+ * slices * n_iters * 2 * d * d floats.  0 when R = 0. */
+int zsb_iaf_slices(int64_t R, int64_t d, int64_t n_iters);
+/* Backward of the stack, one sweep plus one merge launch.  gz_out [R, d] and glq [R]: upstream
+ * gradients of z_out and lq_out; gz_in [R, d] = d / d z_in (d / d lq_in is glq itself); dm_w and
+ * ds_w [n_iters, d, d], zero at i >= j.  ck as written by the forward pass. */
+int zsb_iaf_bwd_f32(const float* ck, const float* gz_out, const float* glq, const float* m_w,
+                    const float* s_w, float* gz_in, float* part, float* dm_w, float* ds_w,
+                    int64_t R, int64_t d, int64_t n_iters, int update, void* stream);
+
 /* ---- Sparse-GP conditional moments (csrc/gp.cu; examples/gaussian_process/utils.py:52-90) -----
  * gp_conditional(z, fz, x, full_cov=False, RBFKernel) for x [B, d], inducing points z [M, d],
  * kernel scales s [d] (softplus(k_raw_scale), utils.py:16), Li = chol(Kzz)^-1 [M, M] (only its lower
