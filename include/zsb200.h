@@ -233,6 +233,30 @@ int zsb_linear_tc_bern_given_f32(int epi, const void* w_planes, const float* sca
                                  const float* bias, const float* given, int S, const float* gout,
                                  float* out, float* part, int64_t R, int J, int K,
                                  float* amax_scale, void* stream);
+/* One-hot categorical layer over C classes (1 <= C <= 128), logits l = h W^T + bias never written
+ * (replaces tf.layers.dense + bn.onehot_categorical, vae_ssl_adaptive_is.py:61-68, with
+ * OnehotCategorical._sample / _log_prob, multivariate.py:522-562).  Draw d = s R + r of S per
+ * logit row; S R < 2^31.
+ *   cls [S R] int32: the class drawn from softmax(l[r]) exactly as zsb_sample_categorical_i32 draws
+ *   it (u_in [S R], or word 0 of Philox block (0, d, iter, stream 6)); onehot [S R, C] its one-hot
+ *   row, float (h_int = 0) or int32; logq [S R] = l[r, cls] - logsumexp(l[r]).
+ * h_binary: h_planes is itself a binary plane. */
+int zsb_linear_tc_cat_sample_f32(const void* w_planes, const float* scale_w, const void* h_planes,
+                                 const float* scale_h, int h_binary, const float* bias,
+                                 const float* u_in, uint64_t seed, uint32_t iter, int S,
+                                 int32_t* cls, void* onehot, int h_int, float* logq, int64_t R,
+                                 int C, int K, void* stream);
+/* The same layer against given [n_g, C] float rows, draw d scored against row d % n_g (n_g divides
+ * S R; OnehotCategorical._log_prob = unnormalized_multinomial_log_prob with normalized logits,
+ * multivariate.py:435-443, 547-556):
+ *   epi 1: out [S R] = sum_j given_j (l[r, j] - logsumexp(l[r]))
+ *   epi 2: out [R, C] = sum_s gout[d] (given_j - (sum_i given_i) softmax(l[r])_j)  (d/dl of the
+ *          sum), max |out| folded into amax_scale[2] (may be NULL) */
+int zsb_linear_tc_cat_given_f32(int epi, const void* w_planes, const float* scale_w,
+                                const void* h_planes, const float* scale_h, int h_binary,
+                                const float* bias, const float* given, int64_t n_g, int S,
+                                const float* gout, float* out, int64_t R, int C, int K,
+                                float* amax_scale, void* stream);
 /* zsb_linear_tc_amax_f32 / zsb_linear_tc_wgrad_f32 with a binary activation h (h_planes = its one
  * plane, scale_h[0] = 2048): the forward, epi 1 / 2 and weight-gradient products of a layer fed a
  * sample (sbn_vimco.py:25-30, 40-43). */

@@ -64,9 +64,19 @@ constexpr float BIN_SCALE = 2048.f;
 //          is not NULL, pre[r, j] = l: what the gradient of gamma needs (xhat is never rebuilt
 //          from out, which the ReLU and gamma = 0 lose)
 //
+// Categorical epilogues (J = C classes, 1 <= C <= 128, so one feature block holds a whole logit
+// row; S draws per logit row, draw d = s R + r; onehot_categorical of a dense layer,
+// vae_ssl_adaptive_is.py:61-68):
+//   EPI 12 one-hot sampling: cls[d] = the class drawn from softmax(l[r]), one uniform per draw
+//          (u_in[d], or word 0 of the Philox block zsb_sample_categorical_i32 keys on d), onehot
+//          [S R, C] (float or int32) and logq[d] = l[y] - logsumexp(l[r])
+//   EPI 13 out[d] = sum_j given[d % n_g, j] (l[r, j] - logsumexp(l[r]))
+//   EPI 14 out[r, j] = sum_s gout[d] (given_j - (sum_i given_i) softmax(l[r])_j), given = row
+//          d % n_g (d/dl of EPI 13)
+//
 // The descriptor tc_pipeline_kernel runs, LinW<E, EPI, MN, Z>, is a LinCore (the product) plus the
-// fields of one epilogue family E: RowsEpi (EPI 0 - 2), SamplesEpi (4 - 6), ClassEpi (7, 8) or
-// BnEpi (9, 10).
+// fields of one epilogue family E: RowsEpi (EPI 0 - 2), SamplesEpi (4 - 6), ClassEpi (7, 8),
+// BnEpi (9 - 11) or CatEpi (12 - 14).
 
 // What a product's units past its first n_tiles are (unit u runs output tile u % n_tiles), as each
 // epilogue family declares it:
@@ -429,6 +439,192 @@ struct SamplesEpi {
           if (j_ok && rbase + jj < R) {
             out[(rbase + jj) * J + j] = dl[jj];
             amax = fmaxf(amax, fabsf(dl[jj]));
+          }
+      }
+    }
+  }
+};
+
+// ZSB_STREAM_CATEGORICAL of samplers.cu: EPI 12 draws what zsb_sample_categorical_i32 draws
+constexpr uint32_t CAT_STREAM = 6u;
+constexpr int CAT_MAX_C = 128;
+constexpr int CAT_PER_LANE = CAT_MAX_C / 32;
+
+// EPI 12 - 14.  The accumulator's natural layout gives a lane one class of 16 rows; a draw needs
+// all C logits of one row, laid out as categorical_sample_kernel (samplers.cu) lays them out: one
+// warp per draw, lane l holding the ceil(C / 32) contiguous classes from l * ceil(C / 32).  So each
+// epilogue warp takes 32 of the tile's rows (the tile is complete once tfull has fired, and no warp
+// overwrites it before all four have arrived on tempty) and reads each row's logits from the whole
+// tile in the sampler's layout.  Per row the max, the sum of exps and its prefix scan are formed
+// once, in the sampler's order; each draw of the unit's chunk then needs only its uniform.
+// Cost (H100, 4e5 rows, 500 -> 10, scripts/bench_ssl_ais.py): the EPI 12 and EPI 13 launches
+// take 0.83 ms where EPI 0 over the same operands takes 0.38 ms, and EPI 14 takes 0.90 ms.  Rows go
+// one at a time, each a chain of dependent shuffles, and the reads of one row's classes are bank
+// conflicts (class pitch ACC_LD = 132 words: 4-way for C <= 32, 16-way at C = 128).  Several rows
+// in flight per warp would hide that latency; not done.
+struct CatEpi {
+  static constexpr Units UNITS = SAMPLE_CHUNKS;
+  __host__ __device__ static constexpr bool folds_amax(int epi) { return epi == 14; }
+  const float* bias; const float* given; int64_t n_g; const float* gout; float* out;
+  int32_t* cls; void* onehot; int h_int; float* logq;
+  int S; int s_per; const float* u_in; uint64_t seed; uint32_t iter; const uint32_t* epoch;
+  float* amax_scale;
+
+  template <int EPI, class Core>
+  __device__ __forceinline__ void run(const Core& core, int64_t uu, uint32_t trow, int quarter,
+                                      int lane, float& amax) const {
+    const int64_t& R = core.R;
+    const int& C = core.J;
+    const float acc_scale = core.acc_scale();
+    const Unit pos = core.template unit<UNITS>(uu, quarter, lane);
+    const int s0 = pos.sub * s_per, s1 = min(S, s0 + s_per);
+    const uint32_t acc0 = trow - (uint32_t)((quarter * 32 + lane) * ACC_LD * 4);
+    const int chunk = (C + 31) / 32;
+    const int c0 = lane * chunk, c1 = min(C, c0 + chunk);
+    const uint32_t it = (EPI == 12) ? iter + (epoch ? *epoch : 0u) : 0u;
+    float b[CAT_PER_LANE];
+#pragma unroll
+    for (int t = 0; t < CAT_PER_LANE; ++t)
+      b[t] = (c0 + t < c1 && bias) ? __ldg(bias + c0 + t) : 0.f;
+#pragma unroll 1
+    for (int i = 0; i < 32; ++i) {
+      const int rl = quarter * 32 + i;
+      const int64_t r = pos.r0 + rl;
+      if (r >= R) break;                                     // warp-uniform
+      float l[CAT_PER_LANE], e[CAT_PER_LANE];
+      float m = -INFINITY;
+#pragma unroll
+      for (int t = 0; t < CAT_PER_LANE; ++t) {
+        l[t] = 0.f;
+        if (c0 + t < c1) {
+          float a;
+          asm volatile("ld.shared.f32 %0, [%1];"
+                       : "=f"(a) : "r"(acc0 + (uint32_t)(((c0 + t) * ACC_LD + rl) * 4)));
+          l[t] = fmaf(a, acc_scale, b[t]);
+          m = fmaxf(m, l[t]);
+        }
+      }
+      m = warp_max(m);
+      float s = 0.f;
+#pragma unroll
+      for (int t = 0; t < CAT_PER_LANE; ++t) {
+        e[t] = 0.f;
+        if (c0 + t < c1) {
+          e[t] = expf(l[t] - m);
+          s += e[t];
+        }
+      }
+      float pre = s;                                         // inclusive prefix of the lane sums
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const float v = __shfl_up_sync(0xffffffffu, pre, o);
+        if (lane >= o) pre += v;
+      }
+      const float total = __shfl_sync(0xffffffffu, pre, 31);
+      const float log_total = logf(total);
+      if (EPI == 12) {
+        int last = -1;                                       // last class with non-zero mass
+#pragma unroll
+        for (int t = 0; t < CAT_PER_LANE; ++t)
+          if (c0 + t < c1 && e[t] > 0.f) last = c0 + t;
+#pragma unroll 1
+        for (int sd = s0; sd < s1; ++sd) {
+          const int64_t d = (int64_t)sd * R + r;
+          float u;
+          if (u_in) {
+            u = __ldg(u_in + d);
+          } else {
+            const Philox4 p = philox4x32_10(0u, (uint32_t)d, it ^ (uint32_t)((uint64_t)d >> 32),
+                                            CAT_STREAM, (uint32_t)seed, (uint32_t)(seed >> 32));
+            u = u32_to_uniform(p.x);
+          }
+          const float target = u * total;
+          // first lane whose inclusive prefix exceeds the target
+          const unsigned hit = __ballot_sync(0xffffffffu, pre > target && s > 0.f);
+          int pick;
+          if (hit) {
+            const int src = __ffs(hit) - 1;
+            const float base = __shfl_sync(0xffffffffu, pre - s, src);
+            pick = -1;
+            if (lane == src) {
+              float acc = base;
+              int lst = c0;
+#pragma unroll
+              for (int t = 0; t < CAT_PER_LANE; ++t) {
+                if (c0 + t < c1 && pick < 0) {
+                  if (e[t] > 0.f) lst = c0 + t;
+                  acc += e[t];
+                  if (acc > target) pick = c0 + t;
+                }
+              }
+              if (pick < 0) pick = lst;                      // round-off at the chunk's end
+            }
+            pick = __shfl_sync(0xffffffffu, pick, src);
+          } else {
+            // u * total rounded up to the total: last class with non-zero mass
+            int lst = last;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) lst = max(lst, __shfl_xor_sync(0xffffffffu, lst, o));
+            pick = lst < 0 ? 0 : lst;
+          }
+          // l[pick] - logsumexp(l) = (l[pick] - m) - log(total), from the lane that holds it
+          float lp = 0.f;
+#pragma unroll
+          for (int t = 0; t < CAT_PER_LANE; ++t)
+            if (c0 + t == pick) lp = (l[t] - m) - log_total;
+          lp = __shfl_sync(0xffffffffu, lp, min(pick / chunk, 31));
+          if (lane == 0) {
+            cls[d] = pick;
+            logq[d] = lp;
+          }
+#pragma unroll
+          for (int t = 0; t < CAT_PER_LANE; ++t)
+            if (c0 + t < c1) {
+              const int64_t k = d * C + c0 + t;
+              if (h_int) reinterpret_cast<int32_t*>(onehot)[k] = (c0 + t == pick) ? 1 : 0;
+              else reinterpret_cast<float*>(onehot)[k] = (c0 + t == pick) ? 1.f : 0.f;
+            }
+        }
+      } else if (EPI == 13) {
+#pragma unroll 1
+        for (int sd = s0; sd < s1; ++sd) {
+          const int64_t d = (int64_t)sd * R + r;
+          const float* __restrict__ gr = given + (d % n_g) * C;
+          float lp = 0.f;
+#pragma unroll
+          for (int t = 0; t < CAT_PER_LANE; ++t)
+            if (c0 + t < c1) lp = fmaf(__ldg(gr + c0 + t), (l[t] - m) - log_total, lp);
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) lp += __shfl_xor_sync(0xffffffffu, lp, o);
+          if (lane == 0) out[d] = lp;
+        }
+      } else {
+        const float inv_total = 1.f / total;
+        float dl[CAT_PER_LANE];
+#pragma unroll
+        for (int t = 0; t < CAT_PER_LANE; ++t) dl[t] = 0.f;
+#pragma unroll 1
+        for (int sd = 0; sd < S; ++sd) {
+          const int64_t d = (int64_t)sd * R + r;
+          const float* __restrict__ gr = given + (d % n_g) * C;
+          const float g = __ldg(gout + d);
+          float x[CAT_PER_LANE], n = 0.f;
+#pragma unroll
+          for (int t = 0; t < CAT_PER_LANE; ++t) {
+            x[t] = (c0 + t < c1) ? __ldg(gr + c0 + t) : 0.f;
+            n += x[t];
+          }
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
+#pragma unroll
+          for (int t = 0; t < CAT_PER_LANE; ++t)
+            dl[t] = fmaf(g, x[t] - n * (e[t] * inv_total), dl[t]);
+        }
+#pragma unroll
+        for (int t = 0; t < CAT_PER_LANE; ++t)
+          if (c0 + t < c1) {
+            out[r * C + c0 + t] = dl[t];
+            amax = fmaxf(amax, fabsf(dl[t]));
           }
       }
     }
@@ -1383,6 +1579,71 @@ int zsb_linear_tc_bern_given_f32(int epi, const void* w_planes, const float* sca
     rc = tc_launch(LinW<SamplesEpi, 5, 0, z>{c, e}, st, "linear_tc_bern_given");
     if (rc) return rc;
     return launch_part_sum(part, J, (int64_t)S * R, out, st, "linear_tc_bern_given_part_sum");
+  });
+}
+
+// One-hot categorical layer with S draws per logit row, l = h W^T + bias never leaving the epilogue
+// (EPI 12; replaces dense + OnehotCategorical._sample + log_prob, vae_ssl_adaptive_is.py:61-68 and
+// multivariate.py:522-562):
+//   cls [S R] int32     the class of draw d = s R + r, drawn as zsb_sample_categorical_i32 draws it
+//                       from the logits l[r] for (seed, iter), or from the uniform u_in[d]
+//   onehot [S R, C]     its one-hot row, float (h_int = 0) or int32
+//   logq [S R]          l[r, cls] - logsumexp(l[r])
+// 1 <= C <= 128 classes; h_binary as in zsb_linear_tc_bern_sample_f32.
+int zsb_linear_tc_cat_sample_f32(const void* w_planes, const float* scale_w, const void* h_planes,
+                                 const float* scale_h, int h_binary, const float* bias,
+                                 const float* u_in, uint64_t seed, uint32_t iter, int S,
+                                 int32_t* cls, void* onehot, int h_int, float* logq, int64_t R,
+                                 int C, int K, void* stream) {
+  ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && cls && onehot && logq && R > 0 &&
+                  K > 0 && S >= 1,
+              "zsb_linear_tc_cat_sample_f32: bad args");
+  ZSB_REQUIRE(C >= 1 && C <= CAT_MAX_C, "zsb_linear_tc_cat_sample_f32: C must be in [1, 128]");
+  ZSB_REQUIRE((int64_t)S * R < (1LL << 31), "zsb_linear_tc_cat_sample_f32: too many rows");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int s_per = sample_chunk(R, C, S);
+  const CatEpi e{.bias = bias, .cls = cls, .onehot = onehot, .h_int = h_int, .logq = logq, .S = S,
+                 .s_per = s_per, .u_in = u_in, .seed = seed, .iter = iter,
+                 .epoch = zsb_epoch_ptr()};
+  return with_h_binary(h_binary, [&](auto z) {
+    LinCore<0, z> c;
+    const int rc = make_core(c, w_planes, scale_w, h_planes, scale_h, C, R, K, (S + s_per - 1) / s_per);
+    if (rc) return rc;
+    return tc_launch(LinW<CatEpi, 12, 0, z>{c, e}, st, "linear_tc_cat_sample");
+  });
+}
+
+// One-hot categorical layer against S given rows per logit row, l[r] = (h W^T + bias)[r], given
+// [n_g, C] float, draw d = s R + r scored against given row d % n_g (n_g divides S R)
+// (OnehotCategorical._log_prob, multivariate.py:542-562 = unnormalized_multinomial_log_prob with
+// normalize_logits, multivariate.py:435-443):
+//   epi 1: out [S R] = sum_j given_j (l[r, j] - logsumexp(l[r]))
+//   epi 2: out [R, C] = sum_s gout[d] (given_j - (sum_i given_i) softmax(l[r])_j), the gradient of
+//          sum gout * (epi 1) wrt the logits; max |out| folded into amax_scale[2] (may be NULL)
+// 1 <= C <= 128; h_binary as in zsb_linear_tc_bern_sample_f32.
+int zsb_linear_tc_cat_given_f32(int epi, const void* w_planes, const float* scale_w,
+                                const void* h_planes, const float* scale_h, int h_binary,
+                                const float* bias, const float* given, int64_t n_g, int S,
+                                const float* gout, float* out, int64_t R, int C, int K,
+                                float* amax_scale, void* stream) {
+  ZSB_REQUIRE(epi == 1 || epi == 2, "zsb_linear_tc_cat_given_f32: epi must be 1 or 2");
+  ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && given && out && R > 0 && K > 0 &&
+                  S >= 1 && n_g > 0 && (epi != 2 || gout),
+              "zsb_linear_tc_cat_given_f32: bad args");
+  ZSB_REQUIRE(C >= 1 && C <= CAT_MAX_C, "zsb_linear_tc_cat_given_f32: C must be in [1, 128]");
+  ZSB_REQUIRE((int64_t)S * R < (1LL << 31), "zsb_linear_tc_cat_given_f32: too many rows");
+  ZSB_REQUIRE(((int64_t)S * R) % n_g == 0,
+              "zsb_linear_tc_cat_given_f32: given rows must divide the draws");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int s_per = epi == 1 ? sample_chunk(R, C, S) : S;   // EPI 14 sums over the draws: one chunk
+  const CatEpi e{.bias = bias, .given = given, .n_g = n_g, .gout = gout, .out = out, .S = S,
+                 .s_per = s_per, .amax_scale = amax_scale};
+  return with_h_binary(h_binary, [&](auto z) {
+    LinCore<0, z> c;
+    const int rc = make_core(c, w_planes, scale_w, h_planes, scale_h, C, R, K, (S + s_per - 1) / s_per);
+    if (rc) return rc;
+    if (epi == 2) return tc_launch(LinW<CatEpi, 14, 0, z>{c, e}, st, "linear_tc_cat_given");
+    return tc_launch(LinW<CatEpi, 13, 0, z>{c, e}, st, "linear_tc_cat_given");
   });
 }
 

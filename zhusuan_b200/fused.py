@@ -14,8 +14,8 @@ from .distributions.univariate import Normal
 
 __all__ = ["GaussianLogJoint", "BNNRegressionLogJoint", "LNTMLogJoint", "PMFLogJoint", "linear",
            "class_linear", "noisy_bn_linear", "bn_linear", "linear_bernoulli_log_prob",
-           "LinearBernoulli", "RBFKernel", "gp_conditional", "conv2d", "conv2d_transpose",
-           "bn_conv2d", "bn_conv2d_transpose", "sigmoid_conv2d_transpose"]
+           "LinearBernoulli", "LinearOnehotCategorical", "RBFKernel", "gp_conditional", "conv2d",
+           "conv2d_transpose", "bn_conv2d", "bn_conv2d_transpose", "sigmoid_conv2d_transpose"]
 
 
 class GaussianLogJoint(object):
@@ -881,8 +881,9 @@ class _LinearBernoulliLogProb(torch.autograd.Function):
 def _class_indices(y, lead, C):
     """``y`` as the int32 class indices [n_y] the class kernel reads (row r of the flattened
     ``lead`` takes index r % n_y): int indices whose shape is a suffix of ``lead``, or a one-hot
-    ``[..., C]`` whose leading shape is (turned into indices on the device, no host sync).  A
-    shape that fits both is read as indices."""
+    ``[..., C]`` whose leading shape is (turned into indices on the device, no host sync; an
+    unchanged LinearOnehotCategorical sample brings its own).  A shape that fits both is read as
+    indices."""
     lead = tuple(int(d) for d in lead)
     ys = tuple(int(d) for d in y.shape)
 
@@ -891,6 +892,9 @@ def _class_indices(y, lead, C):
     if not y.is_floating_point() and suffix(ys):
         idx = y
     elif ys and ys[-1] == C and suffix(ys[:-1]):
+        own = getattr(y, "_zsb_cls", None)     # the class indices of a LinearOnehotCategorical draw
+        if own is not None and own[1] is not None and own[1] == _version(y):
+            return own[0]
         idx = y.detach().argmax(-1)
     else:
         raise ValueError("y %s is neither class indices whose shape is a suffix of %s nor a "
@@ -1424,6 +1428,220 @@ class LinearBernoulli(object):
                 raise ValueError("given %s is not a suffix-broadcast of the "
                                  "batch shape %s" % (tuple(given.shape), lead + (J,)))
         return linear_bernoulli_log_prob(self._h, self._W, self._b, g)
+
+    def prob(self, given):
+        return torch.exp(self.log_prob(given))
+
+
+CAT_MAX_C = 128
+
+
+class _LinearCategoricalGiven(torch.autograd.Function):
+    """OnehotCategorical(logits = h W^T + b).log_prob(given) for S draws per logit row, [S R]: draw
+    d = s R + r against given row d % n_g (g2 = [n_g, C] float).  Forward: the given epilogue, or --
+    for the layer's own sample -- the log q its sampling launch already wrote (``lq``).  Backward:
+    d/dlogits summed over the S draws in one launch, then the input and weight gradients as products
+    over the rows of h."""
+
+    @staticmethod
+    def forward(ctx, h, W, b, g2, S, lq, wp, ws, hpl):
+        R, K, C = hpl.rows, hpl.K, int(W.shape[0])
+        bias = b.detach().to(torch.float32).contiguous() if b is not None else None
+        if lq is None:
+            lq = torch.empty(S * R, dtype=torch.float32, device=g2.device)
+            _cat_given(1, wp, ws, hpl, bias, g2, S, None, lq, R, C, K, None)
+        else:
+            lq = lq.clone()
+        ctx.save_for_backward(W, bias, g2, wp, ws)
+        ctx.hpl = hpl
+        ctx.meta = (tuple(h.shape[:-1]), S, R, C, K, b is not None)
+        return lq
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, glq):
+        W, bias, g2, wp, ws = ctx.saved_tensors
+        lead, S, R, C, K, has_b = ctx.meta
+        need = ctx.needs_input_grad
+        g = glq.reshape(-1).to(torch.float32).contiguous()
+        db = torch.zeros(C, dtype=torch.float32, device=g.device) if (has_b and need[2]) else None
+        amax = torch.zeros(4, dtype=torch.float32, device=g.device)
+        dl = torch.empty((R, C), dtype=torch.float32, device=g.device)
+        _cat_given(2, wp, ws, ctx.hpl, bias, g2, S, g, dl, R, C, K, amax)
+        dlpl = _tc_split_dual(dl, amax=amax, col_sum=db)
+        dh, dW = _grad_products(ctx, dlpl, W, R, (wp, ws), lead + (K,), need[0], need[1])
+        return dh, dW, db, None, None, None, None, None, None
+
+
+def _cat_given(epi, wp, ws, hpl, bias, g2, S, gout, out, R, C, K, amax):
+    from ._lib import lib, ptr, stream
+    lib.call("zsb_linear_tc_cat_given_f32", epi, ptr(wp), ptr(ws), ptr(hpl.planes),
+             ptr(hpl.scale), int(hpl.binary), ptr(bias), ptr(g2), int(g2.shape[0]), S, ptr(gout),
+             ptr(out), R, C, K, ptr(amax), stream())
+
+
+class LinearOnehotCategorical(object):
+    """Drop-in for ``OnehotCategorical(logits=dense(h))`` as a distribution plugin of
+    ``bn.stochastic`` (the ``y`` of vae_ssl_adaptive_is.py:61-68), with the logits never leaving the
+    dense layer's epilogue.  ``W`` [C, H] and ``b`` [C] are the ``tf.layers.dense`` kernel
+    transposed and its bias, as in ``linear``.
+
+    ``sample(n_samples)`` is one launch (zsb_linear_tc_cat_sample_f32) that draws the one-hot sample
+    -- element for element what ``OnehotCategorical(linear(h, W, b)).sample(n_samples)`` draws from
+    the same ``zs.random`` state -- together with its log-probability and its class indices.
+    ``log_prob`` of that very sample returns the stored log-probability (no second product);
+    ``log_prob`` of any other ``given`` ([S, *h.shape[:-1], C] with leading sample axes, or a
+    suffix-broadcast [..., C] such as labels [N, C] against h [K, N, H]; one-hot or not) runs the
+    given epilogue.  Both are differentiable w.r.t. h, W and b.  The sample carries its class
+    indices, so ``class_linear(x, W, W_class, y)`` reads them instead of taking an argmax.
+
+    Outside the fused domain -- more than 128 classes, parameters that are not float32, tensors not
+    on one CUDA device -- the layer is ``OnehotCategorical(linear(h, W, b))`` (``F.linear`` for
+    tensors off the GPU), which draws the same samples by construction."""
+
+    def __init__(self, h, W, b=None, dtype=torch.int32, group_ndims=0):
+        h = _unwrap(h)
+        self._h, self._W, self._b = h, W, b
+        self.dtype = dtype
+        self.param_dtype = torch.float32
+        self.is_continuous = False
+        self.is_reparameterized = False
+        self.group_ndims = group_ndims
+        self._n_categories = int(W.shape[0])
+        ts = [t for t in (h, W, b) if t is not None]
+        self._hpl = None
+        self._fused = (1 <= self._n_categories <= CAT_MAX_C and h.numel() > 0
+                       and all(t.is_cuda and t.dtype == torch.float32 and t.device == W.device
+                               for t in ts))
+
+    n_categories = property(lambda self: self._n_categories)
+
+    @property
+    def logits(self):
+        if self._W.is_cuda:
+            return linear(self._h, self._W, self._b)
+        return torch.nn.functional.linear(self._h, self._W, self._b)
+
+    def _registry(self):
+        from .distributions.multivariate import OnehotCategorical
+        return OnehotCategorical(self.logits, dtype=self.dtype, group_ndims=self.group_ndims)
+
+    def _h_planes(self):
+        """The operand planes of h.  The planes cached on h do not track its version, so the layer
+        keeps the planes it last read with h's version: while that version holds it reuses them;
+        once h has been rewritten in place it splits h afresh and caches the new planes on h as
+        well, so the next reader (this layer or another) does not find the old ones.  An inference
+        tensor has no version and is read through the cache on h, as ``linear`` reads it."""
+        h2 = self._h.reshape(-1, int(self._h.shape[-1]))
+        v = _version(self._h)
+        if v is not None and self._hpl is not None and self._hpl[1] == v:
+            return self._hpl[0]
+        if v is not None and self._hpl is not None:
+            pl = _tc_split_dual(h2)
+            try:
+                self._h._zsb_pl = pl
+            except (AttributeError, RuntimeError):
+                pass
+        else:
+            pl = _planes_of(h2, self._h)
+        self._hpl = (pl, v)
+        return pl
+
+    def get_batch_shape(self):
+        return torch.Size(tuple(self._h.shape[:-1]))
+
+    def get_value_shape(self):
+        return torch.Size([self._n_categories])
+
+    batch_shape = property(lambda self: self.get_batch_shape())
+    value_shape = property(lambda self: self.get_value_shape())
+
+    def sample(self, n_samples=None, u=None):
+        """``n_samples`` as in ``OnehotCategorical.sample``; ``u``: injected uniforms, one per draw,
+        that broadcast to ``[n_samples, *batch_shape]`` (those of ``ops.sample_categorical``), else
+        the Philox stream of ``zs.random``."""
+        from . import random as zrandom
+        from ._lib import lib, ptr, stream
+        if isinstance(n_samples, torch.Tensor):
+            n_samples = int(n_samples.item())
+        S = 1 if n_samples is None else int(n_samples)
+        if not self._fused:
+            if u is None:
+                out = self._registry().sample(n_samples)
+            else:
+                from . import ops
+                draws = ops.sample_categorical(self.logits, S, u=u.to(torch.float32),
+                                               seed=zrandom.get_seed(), it=zrandom.next_counter())
+                out = torch.nn.functional.one_hot(draws.long(), self._n_categories).to(self.dtype)
+                if n_samples is None:
+                    out = out.squeeze(0)
+            self._own = None
+            return out
+        h, W, b = self._h, self._W, self._b
+        lead = tuple(h.shape[:-1])
+        C, K = self._n_categories, int(h.shape[-1])
+        R = h.numel() // K
+        dev = W.device
+        hpl = self._h_planes()
+        wp, ws = _tc_split(W)
+        bias = b.detach().to(torch.float32).contiguous() if b is not None else None
+        seed, it = zrandom.get_seed(), zrandom.next_counter()
+        h_int = self.dtype != torch.float32
+        ys = torch.empty((S,) + lead + (C,), dtype=torch.int32 if h_int else torch.float32,
+                         device=dev)
+        cls = torch.empty(S * R, dtype=torch.int32, device=dev)
+        lq = torch.empty(S * R, dtype=torch.float32, device=dev)
+        uu = None if u is None else u.to(torch.float32).expand((S,) + lead).contiguous()
+        lib.call("zsb_linear_tc_cat_sample_f32", ptr(wp), ptr(ws), ptr(hpl.planes),
+                 ptr(hpl.scale), int(hpl.binary), ptr(bias), ptr(uu), int(seed), int(it), S,
+                 ptr(cls), ptr(ys), int(h_int), ptr(lq), R, C, K, stream())
+        if self.dtype not in (torch.int32, torch.float32):
+            ys = ys.to(self.dtype)
+        if n_samples is None:
+            ys = ys.squeeze(0)
+        vs = _versions(ys, h, W, b)
+        if all(v is not None for t, v in zip((ys, h, W, b), vs) if t is not None):
+            # (inference tensors of torch.inference_mode() have no version: nothing is cached)
+            ys._zsb_cls = (cls, vs[0])
+            self._own = (ys, lq, S, wp, ws, hpl, vs)
+        else:
+            self._own = None
+        return ys
+
+    def log_prob(self, given):
+        if not self._fused:
+            return self._registry().log_prob(given)
+        from . import ops
+        C = self._n_categories
+        lead = tuple(self._h.shape[:-1])
+        own = getattr(self, "_own", None)
+        if own is not None and given is own[0] and \
+                own[6] == _versions(given, self._h, self._W, self._b):
+            ys, lq, S, wp, ws, hpl, _ = own
+            g2 = ys.reshape(-1, C).to(torch.float32).contiguous()
+            lp = _LinearCategoricalGiven.apply(self._h, self._W, self._b, g2, S, lq, wp, ws, hpl)
+            return ops.group_sum(lp.reshape(tuple(given.shape[:-1])), self.group_ndims)
+        gs = tuple(given.shape)
+        nd = len(lead)
+        if not gs or gs[-1] != C:
+            raise ValueError("given %s is not a one-hot over the %d classes" % (gs, C))
+        gb = gs[:-1]
+        if len(gb) >= nd and gb[len(gb) - nd:] == lead:
+            S = 1                   # [S..., *lead, C]: leading sample axes against the shared logits
+            for d in gb[:len(gb) - nd]:
+                S *= int(d)
+            out_shape = gb
+        elif gb == lead[nd - len(gb):]:
+            S, out_shape = 1, lead  # suffix broadcast: given row r % n_g for logit row r
+        else:
+            return self._registry().log_prob(given)
+        if given.numel() == 0:
+            return self._registry().log_prob(given)
+        hpl = self._h_planes()
+        wp, ws = _tc_split(self._W)
+        g2 = given.reshape(-1, C).to(torch.float32).contiguous()
+        lp = _LinearCategoricalGiven.apply(self._h, self._W, self._b, g2, S, None, wp, ws, hpl)
+        return ops.group_sum(lp.reshape(out_shape), self.group_ndims)
 
     def prob(self, given):
         return torch.exp(self.log_prob(given))
