@@ -307,74 +307,55 @@ int zsb_split16_class_f32(const float* src, const float* mask_src, int64_t R, in
  * written in fp32.  scale = device float[4], zero-initialised. */
 int zsb_split16_noisy_f32(const float* h, int64_t n_h, const float* noise, int64_t R, int K,
                           void* planes, float* scale, void* stream);
-/* a = x W^T from those planes and the planes of W; out [R, J] = act((a - mean) rstd + beta) (act =
- * ReLU if relu), stats [2][J] = (mean, rstd).
+/* Dense layer without bias + batch norm (tf.layers.dense(use_bias=False) +
+ * tf.layers.batch_normalization, bernoulli_latent_vae.py:25-30 and 39-44; the convolutions of the
+ * GAN examples; with gamma = NULL, the layers of variational_dropout.py): a = h W^T from the planes
+ * of h (those of zsb_split16_noisy_f32, or with h_binary the one plane of a 0/1 sample,
+ * zsb_linear_tc_bern_sample_f32, which needs gamma), out [R, J] = act(xhat * gamma + beta), xhat =
+ * (a - mean) rstd (act = ReLU if relu), stats [2][J] = (mean, rstd).  gamma = NULL: out = act((a -
+ * mean) rstd + beta), rounded as such rather than as gamma = 1.
  *   training: mean and population variance of a over its R rows, rstd = rsqrt(var + eps); a [R, J]
  *     is written, part = ceil(R / 128) * 2 J floats of moment partials (per 128-row tile: mean and
  *     sum of squared deviations), merged in a fixed order (Chan); moving_mean / moving_var -=
- *     (moving - batch) * rate, rate = 1 - decay.
+ *     (moving - batch) * rate, rate = 1 - decay.  bessel (TF 1.x's fused_batch_norm, the path of
+ *     4-D inputs): the moving variance moves towards the Bessel-corrected R / (R - 1) var (towards
+ *     0 when R = 1); the output still normalises with var.
  *   else: mean / rstd of the moving statistics (unchanged), applied in the product's epilogue;
- *     a and part are not used.
+ *     part is not used, and with gamma a (may be NULL) receives the pre-activation, which the
+ *     gradient of gamma reads.
  * max |out| is folded into amax_scale[2] (may be NULL) as in zsb_linear_tc_amax_f32. */
-int zsb_linear_tc_bn_f32(int training, const void* w_planes, const float* scale_w,
-                         const void* h_planes, const float* scale_h, const float* beta,
-                         float* moving_mean, float* moving_var, float rate, float eps,
-                         float* stats, float* a, float* part, float* out, int64_t R, int J, int K,
-                         int relu, float* amax_scale, void* stream);
-/* Its backward pass from the upstream gradient g [R, J], the output y (read when relu), a
- * (training) and stats: g' = g [y > 0] (relu) or g, dbeta [J] = sum_r g' (may be NULL), and the
- * planes [2][R][kpad(J)] of da = rstd (g' - mean_r g' - xhat mean_r(g' xhat)), xhat = (a - mean)
- * rstd, in training, or of da = rstd g' otherwise -- the operand of zsb_linear_tc_dgrad_f32 /
- * zsb_linear_tc_wgrad_f32.  Column sums are deterministic.  part = (ceil(R / 128) + 1) * 2 J floats;
- * scale = device float[4] with scale[2] zero. */
-int zsb_bn_grad_f32(int training, const float* g, const float* y, const float* a,
-                    const float* stats, int relu, int64_t R, int J, float* part, float* dbeta,
-                    void* planes, float* scale, void* stream);
-/* Dense layer without bias + batch norm with a learned scale gamma [J] (tf.layers.dense(use_bias=
- * False) + tf.layers.batch_normalization; replaces bernoulli_latent_vae.py:25-30 and 39-44): as
- * zsb_linear_tc_bn_f32 with out = act(xhat * gamma + beta), xhat = (a - mean) rstd, rate = 1 -
- * momentum.  h_binary: h_planes is the one plane of a 0/1 sample (zsb_linear_tc_bern_sample_f32).
- * In evaluation, a [R, J] (may be NULL) receives the pre-activation, which the gradient of gamma
- * reads. */
-int zsb_linear_tc_bn_gamma_f32(int training, const void* w_planes, const float* scale_w,
-                               const void* h_planes, const float* scale_h, int h_binary,
-                               const float* gamma, const float* beta, float* moving_mean,
-                               float* moving_var, float rate, float eps, float* stats, float* a,
-                               float* part, float* out, int64_t R, int J, int K, int relu,
-                               float* amax_scale, void* stream);
-/* Its backward pass: g' = g [y > 0] (relu) or g; dbeta [J] = sum_r g', dgamma [J] = sum_r g' xhat
- * (either may be NULL; a is needed in training and for dgamma); the planes of da = gamma rstd (g' -
- * mean_r g' - xhat mean_r(g' xhat)) in training, of da = gamma rstd g' otherwise.  part and scale as
- * in zsb_bn_grad_f32; the column sums are deterministic. */
-int zsb_bn_grad_gamma_f32(int training, const float* g, const float* y, const float* a,
-                          const float* stats, const float* gamma, int relu, int64_t R, int J,
-                          float* part, float* dbeta, float* dgamma, void* planes, float* scale,
-                          void* stream);
-/* The same layer with the batch norm of 4-D inputs (TF 1.x's fused_batch_norm path, the
- * convolutions of the GAN examples): as zsb_linear_tc_bn_gamma_f32, except that in training the
- * moving variance moves towards the Bessel-corrected batch variance R / (R - 1) var (towards 0 when
- * R = 1); the output still normalises with the population variance var. */
-int zsb_linear_tc_bn_gamma_fused_f32(int training, const void* w_planes, const float* scale_w,
-                                     const void* h_planes, const float* scale_h, int h_binary,
-                                     const float* gamma, const float* beta, float* moving_mean,
-                                     float* moving_var, float rate, float eps, float* stats,
-                                     float* a, float* part, float* out, int64_t R, int J, int K,
-                                     int relu, float* amax_scale, void* stream);
-/* The training step of that batch norm after a pass that left the pre-activation a [R, J] and its
- * per-128-row-tile moment partials part [ceil(R / 128)][2][J] (mean, M2): the deterministic merge,
- * stats = (mean, rstd), the moving statistics updated as in zsb_linear_tc_bn_gamma_fused_f32, and
- * out = act(xhat * gamma + beta); max |out| into amax_scale[2] (may be NULL). */
+int zsb_linear_tc_bn_f32(int training, int bessel, const void* w_planes, const float* scale_w,
+                         const void* h_planes, const float* scale_h, int h_binary,
+                         const float* gamma, const float* beta, float* moving_mean,
+                         float* moving_var, float rate, float eps, float* stats, float* a,
+                         float* part, float* out, int64_t R, int J, int K, int relu,
+                         float* amax_scale, void* stream);
+/* The training step of zsb_linear_tc_bn_f32 with bessel after a pass that left the pre-activation
+ * a [R, J] and its per-128-row-tile moment partials part [ceil(R / 128)][2][J] (mean, M2): the
+ * deterministic merge, stats = (mean, rstd), the moving statistics updated, and out = act(xhat *
+ * gamma + beta); max |out| into amax_scale[2] (may be NULL). */
 int zsb_bn_finish_fused_f32(const float* a, const float* part, int64_t R, int J,
                             const float* gamma, const float* beta, float* moving_mean,
                             float* moving_var, float rate, float eps, float* stats, float* out,
                             int relu, float* amax_scale, void* stream);
-/* As zsb_bn_grad_gamma_f32, but da [R, J] is written in fp32 and max |da| is folded into
- * scale[2] (scale = device float[4] with scale[2] zero): for a consumer that gathers da (the
- * transposed convolution) before splitting it into planes. */
-int zsb_bn_grad_gamma_f32out(int training, const float* g, const float* y, const float* a,
-                             const float* stats, const float* gamma, int relu, int64_t R, int J,
-                             float* part, float* dbeta, float* dgamma, float* da, float* scale,
-                             void* stream);
+/* The backward pass of zsb_linear_tc_bn_f32 from the upstream gradient g [R, J], the output y
+ * (read when relu), a and stats: g' = g [y > 0] (relu) or g, dbeta [J] = sum_r g', dgamma [J] = sum_r g' xhat (either may
+ * be NULL; a is needed in training and for dgamma), and the planes [2][R][kpad(J)] of da = gamma
+ * rstd (g' - mean_r g' - xhat mean_r(g' xhat)) in training, of da = gamma rstd g' otherwise (rstd
+ * alone when gamma is NULL) -- the operand of zsb_linear_tc_dgrad_f32 / zsb_linear_tc_wgrad_f32.
+ * Column sums are deterministic.  part = (ceil(R / 128) + 1) * 2 J floats; scale = device float[4]
+ * with scale[2] zero. */
+int zsb_bn_grad_f32(int training, const float* g, const float* y, const float* a,
+                    const float* stats, const float* gamma, int relu, int64_t R, int J,
+                    float* part, float* dbeta, float* dgamma, void* planes, float* scale,
+                    void* stream);
+/* As zsb_bn_grad_f32, but da [R, J] is written in fp32 and max |da| is folded into scale[2]
+ * (scale = device float[4] with scale[2] zero): for a consumer that gathers da (the transposed
+ * convolution) before splitting it into planes. */
+int zsb_bn_grad_f32out(int training, const float* g, const float* y, const float* a,
+                       const float* stats, const float* gamma, int relu, int64_t R, int J,
+                       float* part, float* dbeta, float* dgamma, float* da, float* scale,
+                       void* stream);
 /* From d = d(h * noise) [R, K]: dnoise [R, K] = d * h[r % n_h], dh [n_h, K] = sum over the R / n_h
  * particle rows of d * noise (either may be NULL). */
 int zsb_noisy_grad_f32(const float* d, const float* h, int64_t n_h, const float* noise, int64_t R,

@@ -1,7 +1,6 @@
 """The passes of csrc/conv_tc.cu around the tensor-core products (gather-split, col2im-sum with
-its epilogues, the sigmoid gradient) and the batch-norm kernels the GAN layers added to
-gemm_logjoint_tc.cu exist in the built library with no stack frame and no local memory, so none of
-them spills.  CPU only (reads the library's resource usage with cuobjdump)."""
+its epilogues, the sigmoid gradient) exist in the built library with no stack frame and no local
+memory, so none of them spills.  CPU only (reads the library's resource usage with cuobjdump)."""
 import os
 import re
 import subprocess
@@ -24,12 +23,10 @@ def test_no_conv_tc_kernel_spills():
     out = subprocess.run([exe, "-res-usage", _lib.LIB_PATH], check=True, capture_output=True,
                          text=True).stdout
     found = re.findall(r"Function (\S+):\s*\n\s*REG:(\d+) STACK:(\d+) SHARED:\d+ LOCAL:(\d+)", out)
-    mine = [(n, r, st, lo) for n, r, st, lo in found
-            if "conv_tc" in n or "bn_grad_apply_gamma_f32_kernel" in n
-            or "bn_stats_kernelILb1" in n]
+    mine = [(n, r, st, lo) for n, r, st, lo in found if "conv_tc" in n]
     kinds = {k for n, *_ in mine for k in CONV_TC if k in n}
     assert kinds == CONV_TC, kinds
-    # three col2im_flat instances (epilogues 0, 1, 3), the fp32 BN gradient, the fused BN merge
-    assert len(mine) == len(CONV_TC) + 2 + 2, [n for n, *_ in mine]
+    # three col2im_flat instances (epilogues 0, 1, 3)
+    assert len(mine) == len(CONV_TC) + 2, [n for n, *_ in mine]
     for name, reg, stack, local in mine:
         assert int(stack) == 0 and int(local) == 0, (name, reg, stack, local)

@@ -1029,44 +1029,29 @@ __global__ void __launch_bounds__(256) bn_stats_kernel(const float* __restrict__
   }
 }
 
-// Training forward after EPI 9: out = act((a - mean) * rstd + beta), or with GAMMA act(xhat *
-// gamma + beta), xhat = (a - mean) * rstd (the rounding order of EPI 10 / 11); max |out| into
-// scale[2]
+// Training forward after EPI 9, in the rounding order of EPI 10 / 11: out = act(fma(a - mean,
+// rstd, beta)) without GAMMA (not the same bits as gamma = 1), act(fma(xhat, gamma, beta)), xhat =
+// (a - mean) * rstd, with it; max |out| into amax_scale[2] (may be NULL).  GAMMA is a template
+// argument rather than a NULL test, which took this pass from 40 to 48 registers.
 template <bool GAMMA>
-__device__ __forceinline__ void bn_apply_rows(const float* __restrict__ a, int64_t R, int J,
-                                              const float* __restrict__ stats,
-                                              const float* __restrict__ gamma,
-                                              const float* __restrict__ beta, int relu,
-                                              float* __restrict__ out,
-                                              float* __restrict__ amax_scale) {
+__global__ void __launch_bounds__(256) bn_apply_kernel(const float* __restrict__ a, int64_t R,
+                                                       int J, const float* __restrict__ stats,
+                                                       const float* __restrict__ gamma,
+                                                       const float* __restrict__ beta, int relu,
+                                                       float* __restrict__ out,
+                                                       float* __restrict__ amax_scale) {
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   float m = 0.f;
   for (int64_t r = (int64_t)blockIdx.x * 8 + ty; r < R; r += (int64_t)gridDim.x * 8)
     for (int j = tx; j < J; j += 32) {
-      float y;
-      if (GAMMA)
-        y = fmaf((a[r * J + j] - __ldg(stats + j)) * __ldg(stats + J + j), __ldg(gamma + j),
-                 __ldg(beta + j));
-      else
-        y = (a[r * J + j] - __ldg(stats + j)) * __ldg(stats + J + j) + __ldg(beta + j);
+      const float d = a[r * J + j] - __ldg(stats + j), rs = __ldg(stats + J + j);
+      float y = GAMMA ? fmaf(d * rs, __ldg(gamma + j), __ldg(beta + j))
+                      : fmaf(d, rs, __ldg(beta + j));
       if (relu) y = fmaxf(y, 0.f);
       out[r * J + j] = y;
       m = fmaxf(m, fabsf(y));
     }
   if (amax_scale) fold_amax(amax_scale, m <= 3.0e38f ? m : 0.f, tx);
-}
-__global__ void __launch_bounds__(256) bn_apply_kernel(const float* __restrict__ a, int64_t R,
-                                                       int J, const float* __restrict__ stats,
-                                                       const float* __restrict__ beta, int relu,
-                                                       float* __restrict__ out,
-                                                       float* __restrict__ amax_scale) {
-  bn_apply_rows<false>(a, R, J, stats, nullptr, beta, relu, out, amax_scale);
-}
-__global__ void __launch_bounds__(256) bn_apply_gamma_kernel(
-    const float* __restrict__ a, int64_t R, int J, const float* __restrict__ stats,
-    const float* __restrict__ gamma, const float* __restrict__ beta, int relu,
-    float* __restrict__ out, float* __restrict__ amax_scale) {
-  bn_apply_rows<true>(a, R, J, stats, gamma, beta, relu, out, amax_scale);
 }
 
 // Backward, per 128-row tile t and column j (block: 32 columns x 8 warps, 16 rows per warp, then
@@ -1105,13 +1090,13 @@ __global__ void __launch_bounds__(256) bn_grad_sums_kernel(
 }
 
 // One warp per column: the tile sums of bn_grad_sums_kernel in a fixed order (lane-strided runs,
-// then a fixed shuffle tree) -> dbeta[j] = sum g' (may be NULL), coef = (sum g' / R,
-// sum g' xhat / R), and with DGAMMA dgamma[j] = sum g' xhat (may be NULL)
-template <bool DGAMMA>
-__device__ __forceinline__ void bn_grad_combine_cols(const float* __restrict__ part, int64_t R,
-                                                     int J, float* __restrict__ dbeta,
-                                                     float* __restrict__ dgamma,
-                                                     float* __restrict__ coef) {
+// then a fixed shuffle tree) -> dbeta[j] = sum g', dgamma[j] = sum g' xhat (either may be NULL),
+// coef = (sum g' / R, sum g' xhat / R)
+__global__ void __launch_bounds__(256) bn_grad_combine_kernel(const float* __restrict__ part,
+                                                              int64_t R, int J,
+                                                              float* __restrict__ dbeta,
+                                                              float* __restrict__ dgamma,
+                                                              float* __restrict__ coef) {
   const int lane = threadIdx.x & 31;
   const int j = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (j >= J) return;
@@ -1128,33 +1113,28 @@ __device__ __forceinline__ void bn_grad_combine_cols(const float* __restrict__ p
   }
   if (lane == 0) {
     if (dbeta) dbeta[j] = s1;
-    if (DGAMMA && dgamma) dgamma[j] = s2;
+    if (dgamma) dgamma[j] = s2;
     coef[j] = s1 / (float)R;
     coef[J + j] = s2 / (float)R;
   }
 }
-__global__ void __launch_bounds__(256) bn_grad_combine_kernel(const float* __restrict__ part,
-                                                              int64_t R, int J,
-                                                              float* __restrict__ dbeta,
-                                                              float* __restrict__ coef) {
-  bn_grad_combine_cols<false>(part, R, J, dbeta, nullptr, coef);
-}
-__global__ void __launch_bounds__(256) bn_grad_combine_gamma_kernel(
-    const float* __restrict__ part, int64_t R, int J, float* __restrict__ dbeta,
-    float* __restrict__ dgamma, float* __restrict__ coef) {
-  bn_grad_combine_cols<true>(part, R, J, dbeta, dgamma, coef);
-}
 
-// da = rstd (g' - coef[0] - xhat coef[1]) in training, rstd g' in evaluation; with GAMMA, rstd is
-// gamma rstd.  PLANES = false: max |da| into scale[2]; PLANES = true: planes [2][R][Jp] = fp16
-// hi/lo of da * scale[0], pad columns zero -- the operand zsb_linear_tc_dgrad_f32 / _wgrad_f32 read.
-// F32: da [R, J] itself in fp32 (planes = NULL), and max |da| into scale[2].
-template <bool PLANES, bool GAMMA, bool F32 = false>
-__device__ __forceinline__ void bn_grad_apply_rows(
+// What bn_grad_apply_kernel writes of da
+enum BnGradOut {
+  BN_GRAD_AMAX,     // nothing: max |da| into scale[2]
+  BN_GRAD_PLANES,   // planes [2][R][Jp] = fp16 hi/lo of da * scale[0], pad columns zero -- the
+                    // operand zsb_linear_tc_dgrad_f32 / _wgrad_f32 read
+  BN_GRAD_F32       // da [R, J] in fp32, and max |da| into scale[2]
+};
+// da = gamma rstd (g' - coef[0] - xhat coef[1]) in training, gamma rstd g' in evaluation, with
+// rstd in place of gamma rstd when gamma is NULL
+template <BnGradOut OUT>
+__global__ void __launch_bounds__(256) bn_grad_apply_kernel(
     const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ a,
-    bool training, const float* __restrict__ stats, const float* __restrict__ gamma,
+    int training, const float* __restrict__ stats, const float* __restrict__ gamma,
     const float* __restrict__ coef, int relu, int64_t R, int J, int Jp,
-    __half* __restrict__ planes, float* __restrict__ scale, float* __restrict__ da = nullptr) {
+    __half* __restrict__ planes, float* __restrict__ da, float* __restrict__ scale) {
+  constexpr bool PLANES = OUT == BN_GRAD_PLANES;
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const float s = PLANES ? scale[0] : 0.f;
   const int64_t n_pl = R * (int64_t)Jp;
@@ -1170,43 +1150,16 @@ __device__ __forceinline__ void bn_grad_apply_rows(
           const float xh = (a[r * J + j] - __ldg(stats + j)) * rs;
           gg = gg - __ldg(coef + j) - xh * __ldg(coef + J + j);
         }
-        d = (GAMMA ? __ldg(gamma + j) * rs : rs) * gg;
+        d = (gamma ? __ldg(gamma + j) * rs : rs) * gg;
       }
       if (PLANES) {
         store_hilo(planes + r * Jp + j, n_pl, d * s);
       } else {
-        if (F32) da[r * J + j] = d;
+        if (OUT == BN_GRAD_F32) da[r * J + j] = d;
         m = finite_absmax(m, d);
       }
     }
   if (!PLANES) fold_amax(scale, m, tx);
-}
-// training: a != NULL
-template <bool PLANES>
-__global__ void __launch_bounds__(256) bn_grad_apply_kernel(
-    const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ a,
-    const float* __restrict__ stats, const float* __restrict__ coef, int relu, int64_t R, int J,
-    int Jp, __half* __restrict__ planes, float* __restrict__ scale) {
-  bn_grad_apply_rows<PLANES, false>(g, y, a, a != nullptr, stats, nullptr, coef, relu, R, J, Jp,
-                                    planes, scale);
-}
-template <bool PLANES>
-__global__ void __launch_bounds__(256) bn_grad_apply_gamma_kernel(
-    const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ a,
-    int training, const float* __restrict__ stats, const float* __restrict__ gamma,
-    const float* __restrict__ coef, int relu, int64_t R, int J, int Jp,
-    __half* __restrict__ planes, float* __restrict__ scale) {
-  bn_grad_apply_rows<PLANES, true>(g, y, a, training != 0, stats, gamma, coef, relu, R, J, Jp,
-                                   planes, scale);
-}
-
-__global__ void __launch_bounds__(256) bn_grad_apply_gamma_f32_kernel(
-    const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ a,
-    int training, const float* __restrict__ stats, const float* __restrict__ gamma,
-    const float* __restrict__ coef, int relu, int64_t R, int J, float* __restrict__ da,
-    float* __restrict__ scale) {
-  bn_grad_apply_rows<false, true, true>(g, y, a, training != 0, stats, gamma, coef, relu, R, J, J,
-                                        nullptr, scale, da);
 }
 
 // From d = d(h * noise) [R, K]: dnoise[r] = d[r] * h[r % n_h] and dh[i] = sum_s d[s n_h + i] *
@@ -1348,40 +1301,55 @@ int linear_tc_wgrad(const void* h_planes, const float* scale_h, int K, const voi
   return zsb_check_launch("linear_tc_wgrad_slice_sum");
 }
 
-// zsb_linear_tc_bn_gamma_f32 (BESSEL = false) and zsb_linear_tc_bn_gamma_fused_f32 (true)
-template <bool BESSEL>
-int linear_tc_bn_gamma(int training, const void* w_planes, const float* scale_w,
-                       const void* h_planes, const float* scale_h, int h_binary,
-                       const float* gamma, const float* beta, float* moving_mean, float* moving_var,
-                       float rate, float eps, float* stats, float* a, float* part, float* out,
-                       int64_t R, int J, int K, int relu, float* amax_scale, void* stream) {
-  ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && gamma && beta && moving_mean &&
-                  moving_var && stats && out && R > 0 && J > 0 && K > 0 &&
-                  (!training || (a && part)),
-              "zsb_linear_tc_bn_gamma_f32: bad args");
-  ZSB_REQUIRE(R < (1LL << 31), "zsb_linear_tc_bn_gamma_f32: too many rows");
-  cudaStream_t st = (cudaStream_t)stream;
+// The training step of batch norm after a pass that left the pre-activation a [R, J] and its
+// moment partials part (EPI 9's layout): the merge into stats and the moving statistics (bessel:
+// the moving variance of TF's fused batch norm), then the affine step and ReLU
+int bn_finish(const float* a, const float* part, int64_t R, int J, const float* gamma,
+              const float* beta, float* moving_mean, float* moving_var, float rate, float eps,
+              int bessel, float* stats, float* out, int relu, float* amax_scale, cudaStream_t st) {
   const unsigned col_blocks = (unsigned)((J + 7) / 8);
-  return with_h_binary(h_binary, [&](auto z) {
-    LinCore<0, z> c;
-    int rc = make_core(c, w_planes, scale_w, h_planes, scale_h, J, R, K);
-    if (rc) return rc;
-    if (!training) {
-      bn_stats_kernel<false><<<col_blocks, 256, 0, st>>>(nullptr, R, J, moving_mean, moving_var,
-                                                         rate, eps, 0, stats);
-      if ((rc = zsb_check_launch("linear_tc_bn_gamma_stats")) != ZSB_OK) return rc;
-      const BnEpi e{.bn_stats = stats, .bn_beta = beta, .out = out, .relu = relu,
-                    .amax_scale = amax_scale, .bn_gamma = gamma, .pre = a};
-      return tc_launch(LinW<BnEpi, 11, 0, z>{c, e}, st, "linear_tc_bn_gamma_eval");
-    }
-    rc = tc_launch(LinW<BnEpi, 9, 0, z>{c, {.out = a, .part = part}}, st, "linear_tc_bn_gamma_train");
-    if (rc != ZSB_OK) return rc;
-    bn_stats_kernel<BESSEL><<<col_blocks, 256, 0, st>>>(part, R, J, moving_mean, moving_var, rate,
-                                                        eps, 1, stats);
-    bn_apply_gamma_kernel<<<grid_blocks(R, 8, 16), 256, 0, st>>>(a, R, J, stats, gamma, beta, relu,
-                                                                 out, amax_scale);
-    return zsb_check_launch("linear_tc_bn_gamma_apply");
-  });
+  if (bessel)
+    bn_stats_kernel<true><<<col_blocks, 256, 0, st>>>(part, R, J, moving_mean, moving_var, rate,
+                                                      eps, 1, stats);
+  else
+    bn_stats_kernel<false><<<col_blocks, 256, 0, st>>>(part, R, J, moving_mean, moving_var, rate,
+                                                       eps, 1, stats);
+  const unsigned blocks = grid_blocks(R, 8, 16);
+  if (gamma)
+    bn_apply_kernel<true><<<blocks, 256, 0, st>>>(a, R, J, stats, gamma, beta, relu, out,
+                                                  amax_scale);
+  else
+    bn_apply_kernel<false><<<blocks, 256, 0, st>>>(a, R, J, stats, gamma, beta, relu, out,
+                                                   amax_scale);
+  return zsb_check_launch("bn_finish");
+}
+
+// The backward passes of zsb_bn_grad_f32 (OUT = BN_GRAD_PLANES) and zsb_bn_grad_f32out
+// (BN_GRAD_F32): the per-tile column sums, their merge into dbeta, dgamma and coef, then da
+template <BnGradOut OUT>
+int bn_grad(int training, const float* g, const float* y, const float* a, const float* stats,
+            const float* gamma, int relu, int64_t R, int J, float* part, float* dbeta,
+            float* dgamma, void* planes, float* da, float* scale, cudaStream_t st) {
+  const int64_t n_t = (R + BN_TILE - 1) / BN_TILE;
+  float* coef = part + 2 * n_t * J;
+  bn_grad_sums_kernel<<<dim3((unsigned)n_t, (unsigned)((J + 31) / 32)), 256, 0, st>>>(
+      g, y, training || dgamma ? a : nullptr, stats, relu, R, J, part);
+  bn_grad_combine_kernel<<<(unsigned)((J + 7) / 8), 256, 0, st>>>(part, R, J, dbeta, dgamma,
+                                                                  coef);
+  const unsigned blocks = grid_blocks(R, 8, 16);
+  if constexpr (OUT == BN_GRAD_F32) {
+    bn_grad_apply_kernel<BN_GRAD_F32><<<blocks, 256, 0, st>>>(
+        g, y, a, training, stats, gamma, coef, relu, R, J, J, nullptr, da, scale);
+  } else {
+    const int Jp = zsb_linear_tc_kpad(J);
+    __half* pl = reinterpret_cast<__half*>(planes);
+    bn_grad_apply_kernel<BN_GRAD_AMAX><<<blocks, 256, 0, st>>>(
+        g, y, a, training, stats, gamma, coef, relu, R, J, Jp, pl, nullptr, scale);
+    pow2_scale_mult_kernel<<<1, 32, 0, st>>>(scale, 1.f);
+    bn_grad_apply_kernel<BN_GRAD_PLANES><<<blocks, 256, 0, st>>>(
+        g, y, a, training, stats, gamma, coef, relu, R, J, Jp, pl, nullptr, scale);
+  }
+  return zsb_check_launch("bn_grad");
 }
 
 }  // namespace
@@ -1715,145 +1683,57 @@ int zsb_split16_noisy_f32(const float* h, int64_t n_h, const float* noise, int64
   return zsb_check_launch("split16_noisy");
 }
 
-// Batch-normalised dense layer, no bias: a = h W^T from the planes of zsb_split16_noisy_f32, then
-// out [R, J] = act((a - mean) rstd + beta) (act = ReLU if relu), stats [2][J] = (mean, rstd).
+// Batch-normalised dense layer, no bias: a = h W^T from the planes of h (h_binary: the one plane
+// of a 0/1 sample, as in zsb_linear_tc_bern_sample_f32), then out [R, J] = act(xhat * gamma +
+// beta), xhat = (a - mean) rstd (act = ReLU if relu), stats [2][J] = (mean, rstd).  gamma = NULL:
+// out = act((a - mean) rstd + beta), rounded as such, not as gamma = 1.
 //   training != 0: mean and the population variance over the R rows (EPI 9 writes a [R, J] and
 //     the moment partials part [ceil(R / 128) * 2 J], merged in a fixed order), rstd =
-//     rsqrt(var + eps); moving_mean / moving_var -= (moving - batch) * rate; a pass applies the
-//     affine step and ReLU.
+//     rsqrt(var + eps); moving_mean / moving_var -= (moving - batch) * rate, where with bessel
+//     (TF 1.x's fused batch norm, 4-D inputs) the moving variance moves towards R / (R - 1) var
+//     (towards var = 0 when R = 1); a pass applies the affine step and ReLU.
 //   training == 0: mean / rstd of the moving statistics, which are not changed; the product's
-//     epilogue writes out (EPI 10): a and part are not used.
+//     epilogue writes out (EPI 10, or 11 with gamma) and, with gamma, the pre-activation into a
+//     (may be NULL) for the gradient of gamma; part is not used.
 // max |out| is folded into amax_scale[2] (may be NULL).
-int zsb_linear_tc_bn_f32(int training, const void* w_planes, const float* scale_w,
-                         const void* h_planes, const float* scale_h, const float* beta,
-                         float* moving_mean, float* moving_var, float rate, float eps,
-                         float* stats, float* a, float* part, float* out, int64_t R, int J, int K,
-                         int relu, float* amax_scale, void* stream) {
+int zsb_linear_tc_bn_f32(int training, int bessel, const void* w_planes, const float* scale_w,
+                         const void* h_planes, const float* scale_h, int h_binary,
+                         const float* gamma, const float* beta, float* moving_mean,
+                         float* moving_var, float rate, float eps, float* stats, float* a,
+                         float* part, float* out, int64_t R, int J, int K, int relu,
+                         float* amax_scale, void* stream) {
   ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && beta && moving_mean && moving_var &&
                   stats && out && R > 0 && J > 0 && K > 0 && (!training || (a && part)),
               "zsb_linear_tc_bn_f32: bad args");
   ZSB_REQUIRE(R < (1LL << 31), "zsb_linear_tc_bn_f32: too many rows");
+  // EPI 10 is built on the two-plane mainloop only
+  ZSB_REQUIRE(gamma || !h_binary, "zsb_linear_tc_bn_f32: a 0/1 sample needs gamma");
   cudaStream_t st = (cudaStream_t)stream;
-  LinCore<0, 0> c;
-  int rc = make_core(c, w_planes, scale_w, h_planes, scale_h, J, R, K);
-  if (rc) return rc;
-  const unsigned col_blocks = (unsigned)((J + 7) / 8);
-  if (!training) {
-    bn_stats_kernel<false><<<col_blocks, 256, 0, st>>>(nullptr, R, J, moving_mean, moving_var, rate,
-                                                       eps, 0, stats);
+  return with_h_binary(h_binary, [&](auto z) {
+    LinCore<0, z> c;
+    int rc = make_core(c, w_planes, scale_w, h_planes, scale_h, J, R, K);
+    if (rc) return rc;
+    if (training) {
+      rc = tc_launch(LinW<BnEpi, 9, 0, z>{c, {.out = a, .part = part}}, st, "linear_tc_bn_train");
+      return rc ? rc : bn_finish(a, part, R, J, gamma, beta, moving_mean, moving_var, rate, eps,
+                                 bessel, stats, out, relu, amax_scale, st);
+    }
+    bn_stats_kernel<false><<<(unsigned)((J + 7) / 8), 256, 0, st>>>(nullptr, R, J, moving_mean,
+                                                                    moving_var, rate, eps, 0,
+                                                                    stats);
     if ((rc = zsb_check_launch("linear_tc_bn_stats")) != ZSB_OK) return rc;
     const BnEpi e{.bn_stats = stats, .bn_beta = beta, .out = out, .relu = relu,
-                  .amax_scale = amax_scale};
-    return tc_launch(LinW<BnEpi, 10>{c, e}, st, "linear_tc_bn_eval");
-  }
-  rc = tc_launch(LinW<BnEpi, 9>{c, {.out = a, .part = part}}, st, "linear_tc_bn_train");
-  if (rc != ZSB_OK) return rc;
-  bn_stats_kernel<false><<<col_blocks, 256, 0, st>>>(part, R, J, moving_mean, moving_var, rate,
-                                                     eps, 1, stats);
-  bn_apply_kernel<<<grid_blocks(R, 8, 16), 256, 0, st>>>(a, R, J, stats, beta, relu, out,
-                                                         amax_scale);
-  return zsb_check_launch("linear_tc_bn_apply");
+                  .amax_scale = amax_scale, .bn_gamma = gamma, .pre = a};
+    if constexpr (decltype(z)::value == 0)
+      if (!gamma) return tc_launch(LinW<BnEpi, 10>{c, e}, st, "linear_tc_bn_eval");
+    return tc_launch(LinW<BnEpi, 11, 0, z>{c, e}, st, "linear_tc_bn_eval");
+  });
 }
 
-// Backward of zsb_linear_tc_bn_f32 from the upstream gradient g [R, J], its output y (the ReLU
-// mask, read when relu), a (training) and stats:
-//   g' = g [y > 0] (relu) or g;  dbeta [J] = sum_r g' (may be NULL)
-//   training: da = rstd (g' - mean_r g' - xhat mean_r(g' xhat)), xhat = (a - mean) rstd
-//   else:     da = rstd g'
-// The column sums run per 128-row tile and are merged in a fixed order (deterministic).
-// planes [2][R][kpad(J)] = fp16 hi/lo of da times scale[0], a power of two picked from max |da|:
-// the operand of zsb_linear_tc_dgrad_f32 / zsb_linear_tc_wgrad_f32.  part = (ceil(R / 128) + 1)
-// * 2 J floats of scratch; scale = device float[4] with scale[2] zero.
-int zsb_bn_grad_f32(int training, const float* g, const float* y, const float* a,
-                    const float* stats, int relu, int64_t R, int J, float* part, float* dbeta,
-                    void* planes, float* scale, void* stream) {
-  ZSB_REQUIRE(g && stats && part && planes && scale && R > 0 && J > 0 && (!relu || y) &&
-                  (!training || a),
-              "zsb_bn_grad_f32: bad args");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int Jp = zsb_linear_tc_kpad(J);
-  const int64_t n_t = (R + BN_TILE - 1) / BN_TILE;
-  const float* at = training ? a : nullptr;
-  float* coef = part + 2 * n_t * J;
-  bn_grad_sums_kernel<<<dim3((unsigned)n_t, (unsigned)((J + 31) / 32)), 256, 0, st>>>(
-      g, y, at, stats, relu, R, J, part);
-  bn_grad_combine_kernel<<<(unsigned)((J + 7) / 8), 256, 0, st>>>(part, R, J, dbeta, coef);
-  __half* pl = reinterpret_cast<__half*>(planes);
-  const unsigned blocks = grid_blocks(R, 8, 16);
-  bn_grad_apply_kernel<false><<<blocks, 256, 0, st>>>(g, y, at, stats, coef, relu, R, J, Jp, pl,
-                                                      scale);
-  pow2_scale_mult_kernel<<<1, 32, 0, st>>>(scale, 1.f);
-  bn_grad_apply_kernel<true><<<blocks, 256, 0, st>>>(g, y, at, stats, coef, relu, R, J, Jp, pl,
-                                                     scale);
-  return zsb_check_launch("bn_grad");
-}
-
-// Dense layer without bias followed by batch norm with a learned scale (tf.layers.dense(use_bias=
-// False) + tf.layers.batch_normalization, bernoulli_latent_vae.py:25-30, 39-44): as
-// zsb_linear_tc_bn_f32, with out = act(xhat * gamma + beta), xhat = (a - mean) rstd, and h_binary as
-// in zsb_linear_tc_bern_sample_f32.  In evaluation, `a` (may be NULL) receives the pre-activation
-// for the gradient of gamma.
-int zsb_linear_tc_bn_gamma_f32(int training, const void* w_planes, const float* scale_w,
-                               const void* h_planes, const float* scale_h, int h_binary,
-                               const float* gamma, const float* beta, float* moving_mean,
-                               float* moving_var, float rate, float eps, float* stats, float* a,
-                               float* part, float* out, int64_t R, int J, int K, int relu,
-                               float* amax_scale, void* stream) {
-  return linear_tc_bn_gamma<false>(training, w_planes, scale_w, h_planes, scale_h, h_binary,
-                                   gamma, beta, moving_mean, moving_var, rate, eps, stats, a,
-                                   part, out, R, J, K, relu, amax_scale, stream);
-}
-// As zsb_linear_tc_bn_gamma_f32 with the moving-variance update of TF 1.x's fused batch norm
-// (4-D inputs): in training the moving variance moves towards the Bessel-corrected batch variance
-// R / (R - 1) var (towards var = 0 when R = 1); the output still normalises with the population
-// variance.
-int zsb_linear_tc_bn_gamma_fused_f32(int training, const void* w_planes, const float* scale_w,
-                                     const void* h_planes, const float* scale_h, int h_binary,
-                                     const float* gamma, const float* beta, float* moving_mean,
-                                     float* moving_var, float rate, float eps, float* stats,
-                                     float* a, float* part, float* out, int64_t R, int J, int K,
-                                     int relu, float* amax_scale, void* stream) {
-  return linear_tc_bn_gamma<true>(training, w_planes, scale_w, h_planes, scale_h, h_binary,
-                                  gamma, beta, moving_mean, moving_var, rate, eps, stats, a,
-                                  part, out, R, J, K, relu, amax_scale, stream);
-}
-
-// Backward of zsb_linear_tc_bn_gamma_f32 from the upstream gradient g [R, J], its output y (read
-// when relu), the pre-activation a (training, or when dgamma is wanted) and stats:
-//   g' = g [y > 0] (relu) or g;  dbeta [J] = sum_r g',  dgamma [J] = sum_r g' xhat (either may be
-//   NULL), xhat = (a - mean) rstd
-//   training: da = gamma rstd (g' - mean_r g' - xhat mean_r(g' xhat));  else: da = gamma rstd g'
-// then the planes of da as zsb_bn_grad_f32 writes them; part and scale as there.
-int zsb_bn_grad_gamma_f32(int training, const float* g, const float* y, const float* a,
-                          const float* stats, const float* gamma, int relu, int64_t R, int J,
-                          float* part, float* dbeta, float* dgamma, void* planes, float* scale,
-                          void* stream) {
-  ZSB_REQUIRE(g && stats && gamma && part && planes && scale && R > 0 && J > 0 && (!relu || y) &&
-                  (!(training || dgamma) || a),
-              "zsb_bn_grad_gamma_f32: bad args");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int Jp = zsb_linear_tc_kpad(J);
-  const int64_t n_t = (R + BN_TILE - 1) / BN_TILE;
-  float* coef = part + 2 * n_t * J;
-  bn_grad_sums_kernel<<<dim3((unsigned)n_t, (unsigned)((J + 31) / 32)), 256, 0, st>>>(
-      g, y, a, stats, relu, R, J, part);
-  bn_grad_combine_gamma_kernel<<<(unsigned)((J + 7) / 8), 256, 0, st>>>(part, R, J, dbeta, dgamma,
-                                                                        coef);
-  __half* pl = reinterpret_cast<__half*>(planes);
-  const unsigned blocks = grid_blocks(R, 8, 16);
-  bn_grad_apply_gamma_kernel<false><<<blocks, 256, 0, st>>>(g, y, a, training, stats, gamma, coef,
-                                                            relu, R, J, Jp, pl, scale);
-  pow2_scale_mult_kernel<<<1, 32, 0, st>>>(scale, 1.f);
-  bn_grad_apply_gamma_kernel<true><<<blocks, 256, 0, st>>>(g, y, a, training, stats, gamma, coef,
-                                                           relu, R, J, Jp, pl, scale);
-  return zsb_check_launch("bn_grad_gamma");
-}
-
-// The training step of TF 1.x's fused batch norm (4-D inputs) after a pass that left the
-// pre-activation a [R, J] and its per-128-row-tile moment partials part (EPI 9's layout): the
-// deterministic merge, stats = (mean, rstd), the moving statistics updated as in
-// zsb_linear_tc_bn_gamma_fused_f32, then out = act(xhat * gamma + beta), max |out| into
-// amax_scale[2] (may be NULL).
+// The training step of zsb_linear_tc_bn_f32 with bessel after a pass that left the pre-activation
+// a [R, J] and its per-128-row-tile moment partials part (EPI 9's layout): the deterministic
+// merge, stats = (mean, rstd), the moving statistics updated, then out = act(xhat * gamma + beta),
+// max |out| into amax_scale[2] (may be NULL).
 int zsb_bn_finish_fused_f32(const float* a, const float* part, int64_t R, int J,
                             const float* gamma, const float* beta, float* moving_mean,
                             float* moving_var, float rate, float eps, float* stats, float* out,
@@ -1861,33 +1741,42 @@ int zsb_bn_finish_fused_f32(const float* a, const float* part, int64_t R, int J,
   ZSB_REQUIRE(a && part && gamma && beta && moving_mean && moving_var && stats && out && R > 0 &&
                   J > 0,
               "zsb_bn_finish_fused_f32: bad args");
-  cudaStream_t st = (cudaStream_t)stream;
-  bn_stats_kernel<true><<<(unsigned)((J + 7) / 8), 256, 0, st>>>(part, R, J, moving_mean,
-                                                                 moving_var, rate, eps, 1, stats);
-  bn_apply_gamma_kernel<<<grid_blocks(R, 8, 16), 256, 0, st>>>(a, R, J, stats, gamma, beta, relu,
-                                                               out, amax_scale);
-  return zsb_check_launch("bn_finish_fused");
+  return bn_finish(a, part, R, J, gamma, beta, moving_mean, moving_var, rate, eps, 1, stats, out,
+                   relu, amax_scale, (cudaStream_t)stream);
 }
 
-// As zsb_bn_grad_gamma_f32, but da [R, J] is written in fp32 and max |da| folded into scale[2]
-// (device float[4] with scale[2] zero), for a consumer that gathers da before splitting it.
-int zsb_bn_grad_gamma_f32out(int training, const float* g, const float* y, const float* a,
-                             const float* stats, const float* gamma, int relu, int64_t R, int J,
-                             float* part, float* dbeta, float* dgamma, float* da, float* scale,
-                             void* stream) {
-  ZSB_REQUIRE(g && stats && gamma && part && da && scale && R > 0 && J > 0 && (!relu || y) &&
+// Backward of zsb_linear_tc_bn_f32 from the upstream gradient g [R, J], its output y (the ReLU
+// mask, read when relu), the pre-activation a (training, or when dgamma is wanted) and stats:
+//   g' = g [y > 0] (relu) or g;  dbeta [J] = sum_r g',  dgamma [J] = sum_r g' xhat (either may be
+//   NULL), xhat = (a - mean) rstd
+//   training: da = gamma rstd (g' - mean_r g' - xhat mean_r(g' xhat));  else: da = gamma rstd g'
+//   (rstd in place of gamma rstd when gamma is NULL)
+// The column sums run per 128-row tile and are merged in a fixed order (deterministic).
+// planes [2][R][kpad(J)] = fp16 hi/lo of da times scale[0], a power of two picked from max |da|:
+// the operand of zsb_linear_tc_dgrad_f32 / zsb_linear_tc_wgrad_f32.  part = (ceil(R / 128) + 1)
+// * 2 J floats of scratch; scale = device float[4] with scale[2] zero.
+int zsb_bn_grad_f32(int training, const float* g, const float* y, const float* a,
+                    const float* stats, const float* gamma, int relu, int64_t R, int J,
+                    float* part, float* dbeta, float* dgamma, void* planes, float* scale,
+                    void* stream) {
+  ZSB_REQUIRE(g && stats && part && planes && scale && R > 0 && J > 0 && (!relu || y) &&
                   (!(training || dgamma) || a),
-              "zsb_bn_grad_gamma_f32out: bad args");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t n_t = (R + BN_TILE - 1) / BN_TILE;
-  float* coef = part + 2 * n_t * J;
-  bn_grad_sums_kernel<<<dim3((unsigned)n_t, (unsigned)((J + 31) / 32)), 256, 0, st>>>(
-      g, y, a, stats, relu, R, J, part);
-  bn_grad_combine_gamma_kernel<<<(unsigned)((J + 7) / 8), 256, 0, st>>>(part, R, J, dbeta, dgamma,
-                                                                        coef);
-  bn_grad_apply_gamma_f32_kernel<<<grid_blocks(R, 8, 16), 256, 0, st>>>(
-      g, y, a, training, stats, gamma, coef, relu, R, J, da, scale);
-  return zsb_check_launch("bn_grad_gamma_f32out");
+              "zsb_bn_grad_f32: bad args");
+  return bn_grad<BN_GRAD_PLANES>(training, g, y, a, stats, gamma, relu, R, J, part, dbeta, dgamma,
+                                 planes, nullptr, scale, (cudaStream_t)stream);
+}
+
+// As zsb_bn_grad_f32, but da [R, J] is written in fp32 and max |da| folded into scale[2]
+// (device float[4] with scale[2] zero), for a consumer that gathers da before splitting it.
+int zsb_bn_grad_f32out(int training, const float* g, const float* y, const float* a,
+                       const float* stats, const float* gamma, int relu, int64_t R, int J,
+                       float* part, float* dbeta, float* dgamma, float* da, float* scale,
+                       void* stream) {
+  ZSB_REQUIRE(g && stats && part && da && scale && R > 0 && J > 0 && (!relu || y) &&
+                  (!(training || dgamma) || a),
+              "zsb_bn_grad_f32out: bad args");
+  return bn_grad<BN_GRAD_F32>(training, g, y, a, stats, gamma, relu, R, J, part, dbeta, dgamma,
+                              nullptr, da, scale, (cudaStream_t)stream);
 }
 
 // Gradients of x = h[r % n_h] * noise[r] from d = dL/dx [R, K]: dnoise [R, K] = d * h[r % n_h] and

@@ -994,17 +994,93 @@ def class_linear(h, W, W_class, y=None, b=None, relu=False):
     return _ClassLinear.apply(h, W, W_class, b, cls, bool(relu))
 
 
+def _bn_check(name, J, dev, gamma, beta, moving_mean, moving_variance):
+    """ValueError naming the first of gamma (None: no learned scale), beta, moving_mean and
+    moving_variance that is not a float32 [J] tensor on dev; the moving statistics, which are
+    updated in place, must also be contiguous."""
+    for nm, t, contig in (("gamma", gamma, False), ("beta", beta, False),
+                          ("moving_mean", moving_mean, True),
+                          ("moving_variance", moving_variance, True)):
+        if t is None and nm == "gamma":
+            continue
+        if not isinstance(t, torch.Tensor) or tuple(t.shape) != (J,) or \
+                t.dtype != torch.float32 or t.device != dev or (contig and not t.is_contiguous()):
+            raise ValueError("%s: %s must be a %sfloat32 [%d] tensor on %s"
+                             % (name, nm, "contiguous " if contig else "", J, dev))
+
+
+def _bn_buffers(R, J, dev, training, keep_pre):
+    """stats [2, J], the output y [R, J], the pre-activation a [R, J] (training, or keep_pre: an
+    evaluation whose gamma needs a gradient; else None), the moment partials of 128-row tiles
+    (training; else None) and the amax slot of a batch-normalised layer's forward."""
+    f32 = dict(dtype=torch.float32, device=dev)
+    a = torch.empty((R, J), **f32) if training or keep_pre else None
+    part = torch.empty(-(-R // 128) * 2 * J, **f32) if training else None
+    return torch.empty((2, J), **f32), torch.empty((R, J), **f32), a, part, torch.zeros(4, **f32)
+
+
+def _bn_save(ctx, training, relu, gm, y, a, stats, *extra):
+    """Keeps what _bn_backward reads, then ``extra`` (ctx.saved_tensors[4:])."""
+    ctx.save_for_backward(gm, y if relu else None, a, stats, *extra)
+    ctx.bn = (training, relu)
+
+
+def _bn_forward(ctx, hpl, wpl, J, gamma, beta, stats_bufs, training, relu, rate, eps, bessel,
+                keep_pre, *extra):
+    """y [R, J] = relu?(BN(h W^T) * gamma + beta) (gamma None: no scale) and its amax slot, from
+    the operand planes hpl of h and wpl of W (zsb_linear_tc_bn_f32; bessel: TF's fused-batch-norm
+    update of the moving variance); saves the layer for _bn_backward."""
+    from ._lib import lib, ptr, stream
+    moving_mean, moving_variance = stats_bufs
+    R, K = hpl.rows, hpl.K
+    gm = None if gamma is None else gamma.detach().to(torch.float32).contiguous()
+    b = beta.detach().to(torch.float32).contiguous()
+    stats, y, a, part, amax = _bn_buffers(R, J, b.device, training, keep_pre)
+    lib.call("zsb_linear_tc_bn_f32", int(training), int(bessel), ptr(wpl[0]), ptr(wpl[1]),
+             ptr(hpl.planes), ptr(hpl.scale), int(hpl.binary), ptr(gm), ptr(b), ptr(moving_mean),
+             ptr(moving_variance), rate, eps, ptr(stats), ptr(a), ptr(part), ptr(y), R, J, K,
+             int(relu), ptr(amax), stream())
+    _bn_save(ctx, training, relu, gm, y, a, stats, *extra)
+    return y, amax
+
+
+def _bn_backward(ctx, gy, need_gamma, need_beta, planes=True):
+    """d gamma, d beta (each None unless needed) and G = d/d(pre-activation) of a layer saved by
+    _bn_save: G's operand planes (zsb_bn_grad_f32), or with planes=False G [R, J] in fp32 and the
+    scale slot holding its max |.| (zsb_bn_grad_f32out)."""
+    from ._lib import lib, ptr, stream
+    gm, y, a, stats = ctx.saved_tensors[:4]
+    training, relu = ctx.bn
+    J = int(stats.shape[1])
+    R = gy.numel() // J
+    f32 = dict(dtype=torch.float32, device=gy.device)
+    g = gy.reshape(R, J).to(torch.float32).contiguous()
+    dgamma = torch.empty(J, **f32) if need_gamma else None
+    dbeta = torch.empty(J, **f32) if need_beta else None
+    part = torch.empty((-(-R // 128) + 1) * 2 * J, **f32)
+    scale = torch.zeros(4, **f32)
+    args = (int(training), ptr(g), ptr(y), ptr(a), ptr(stats), ptr(gm), int(relu), R, J,
+            ptr(part), ptr(dbeta), ptr(dgamma))
+    if planes:
+        pl = torch.empty((2, R, lib.load().zsb_linear_tc_kpad(J)), dtype=torch.float16,
+                         device=gy.device)
+        lib.call("zsb_bn_grad_f32", *args, ptr(pl), ptr(scale), stream())
+        return dgamma, dbeta, _Planes(pl, scale, R, J)
+    da = torch.empty((R, J), **f32)
+    lib.call("zsb_bn_grad_f32out", *args, ptr(da), ptr(scale), stream())
+    return dgamma, dbeta, (da, scale)
+
+
 class _NoisyBNLinear(torch.autograd.Function):
     """relu?(BN((h * noise) W^T)) on the batch-norm epilogues of the wgmma kernel.  Forward: one
-    split pass turns h * noise into operand planes (zsb_split16_noisy_f32), then the product and the
-    batch-norm step (zsb_linear_tc_bn_f32).  Backward: one pass gives d beta and the planes of the
-    pre-activation gradient (zsb_bn_grad_f32), the unchanged input- and weight-gradient products
-    read them, and one pass turns d(h * noise) into d noise and d h (zsb_noisy_grad_f32)."""
+    split pass turns h * noise into operand planes (zsb_split16_noisy_f32), then _bn_forward with
+    no gamma.  Backward: _bn_backward gives d beta and the planes of the pre-activation gradient,
+    the unchanged input- and weight-gradient products read them, and one pass turns d(h * noise)
+    into d noise and d h (zsb_noisy_grad_f32)."""
 
     @staticmethod
     def forward(ctx, h, noise, W, beta, stats_bufs, training, relu, rate, eps):
         from ._lib import lib, ptr, stream
-        moving_mean, moving_variance = stats_bufs
         K, J = int(noise.shape[-1]), int(W.shape[0])
         lead = noise.shape[:-1]
         n2 = noise.detach().to(torch.float32).reshape(-1, K).contiguous()
@@ -1016,41 +1092,22 @@ class _NoisyBNLinear(torch.autograd.Function):
         scale = torch.zeros(4, dtype=torch.float32, device=dev)
         lib.call("zsb_split16_noisy_f32", ptr(h2), n_h, ptr(n2), R, K, ptr(planes), ptr(scale),
                  stream())
-        wp, ws = _tc_split(W)
-        b = beta.detach().to(torch.float32).contiguous()
-        stats = torch.empty((2, J), dtype=torch.float32, device=dev)
-        y = torch.empty((R, J), dtype=torch.float32, device=dev)
-        a = part = None
-        if training:
-            a = torch.empty((R, J), dtype=torch.float32, device=dev)
-            part = torch.empty(-(-R // 128) * 2 * J, dtype=torch.float32, device=dev)
-        amax = torch.zeros(4, dtype=torch.float32, device=dev)
-        lib.call("zsb_linear_tc_bn_f32", int(training), ptr(wp), ptr(ws), ptr(planes), ptr(scale),
-                 ptr(b), ptr(moving_mean), ptr(moving_variance), rate, eps, ptr(stats), ptr(a),
-                 ptr(part), ptr(y), R, J, K, int(relu), ptr(amax), stream())
-        ctx.save_for_backward(W, y if relu else None, a, stats, h2, n2)
         ctx.hpl = _Planes(planes, scale, R, K)
-        ctx.wpl = (wp, ws)
-        ctx.meta = (tuple(h.shape), lead, training, relu, R, n_h, K, J)
+        ctx.wpl = _tc_split(W)
+        y, amax = _bn_forward(ctx, ctx.hpl, ctx.wpl, J, None, beta, stats_bufs, training, relu,
+                              rate, eps, False, False, W, h2, n2)
+        ctx.meta = (tuple(h.shape), lead, R, n_h, K)
         return _tag(y.reshape(tuple(lead) + (J,)), amax)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gy):
         from ._lib import lib, ptr, stream
-        W, y, a, stats, h2, n2 = ctx.saved_tensors
-        h_shape, lead, training, relu, R, n_h, K, J = ctx.meta
+        W, h2, n2 = ctx.saved_tensors[4:]
+        h_shape, lead, R, n_h, K = ctx.meta
         need = ctx.needs_input_grad
         dev = gy.device
-        g = gy.reshape(R, J).to(torch.float32).contiguous()
-        dbeta = torch.empty(J, dtype=torch.float32, device=dev) if need[3] else None
-        part = torch.empty((-(-R // 128) + 1) * 2 * J, dtype=torch.float32, device=dev)
-        planes = torch.empty((2, R, lib.load().zsb_linear_tc_kpad(J)), dtype=torch.float16,
-                             device=dev)
-        scale = torch.zeros(4, dtype=torch.float32, device=dev)
-        lib.call("zsb_bn_grad_f32", int(training), ptr(g), ptr(y), ptr(a), ptr(stats), int(relu),
-                 R, J, ptr(part), ptr(dbeta), ptr(planes), ptr(scale), stream())
-        gpl = _Planes(planes, scale, R, J)
+        _, dbeta, gpl = _bn_backward(ctx, gy, False, need[3])
         dh = dnoise = None
         if need[0] or need[1]:
             dx, _ = _tc_grad_input(gpl, W, R, *ctx.wpl)
@@ -1100,13 +1157,7 @@ def noisy_bn_linear(h, noise, W, beta, moving_mean, moving_variance, training, r
     if W.dim() != 2 or int(W.shape[1]) != K:
         raise ValueError("W %s must be [J, %d]" % (tuple(W.shape), K))
     J = int(W.shape[0])
-    if tuple(beta.shape) != (J,):
-        raise ValueError("beta %s must be [%d]" % (tuple(beta.shape), J))
-    for nm, t in (("moving_mean", moving_mean), ("moving_variance", moving_variance)):
-        if not isinstance(t, torch.Tensor) or tuple(t.shape) != (J,) or \
-                t.dtype != torch.float32 or not t.is_contiguous() or t.device != W.device:
-            raise ValueError("%s must be a contiguous float32 [%d] tensor on %s"
-                             % (nm, J, W.device))
+    _bn_check("noisy_bn_linear", J, W.device, None, beta, moving_mean, moving_variance)
     if any(int(d) == 0 for d in noise_s) or J == 0:
         raise ValueError("empty shapes are not supported: noise %s, W %s"
                          % (noise_s, tuple(W.shape)))
@@ -1115,62 +1166,30 @@ def noisy_bn_linear(h, noise, W, beta, moving_mean, moving_variance, training, r
 
 
 class _BNLinear(torch.autograd.Function):
-    """relu?(BN(h W^T) * gamma + beta) on the batch-norm epilogues of the wgmma kernel
-    (zsb_linear_tc_bn_gamma_f32), from the cached operand planes of h -- a 0/1 sample's one plane
-    included.  Backward: one pass gives d beta, d gamma and the planes of the pre-activation
-    gradient (zsb_bn_grad_gamma_f32), which the unchanged input- and weight-gradient products
-    read."""
+    """relu?(BN(h W^T) * gamma + beta): _bn_forward from the cached operand planes of h -- a 0/1
+    sample's one plane included.  Backward: _bn_backward gives d beta, d gamma and the planes of
+    the pre-activation gradient, which the unchanged input- and weight-gradient products read."""
 
     @staticmethod
     def forward(ctx, h, W, gamma, beta, stats_bufs, training, relu, rate, eps, keep_pre):
-        from ._lib import lib, ptr, stream
-        moving_mean, moving_variance = stats_bufs
         lead = h.shape[:-1]
         K, J = int(h.shape[-1]), int(W.shape[0])
         h2 = h.reshape(-1, K)
         R = int(h2.shape[0])
-        dev = W.device
-        hpl = _planes_of(h2, h)
-        wp, ws = _tc_split(W)
-        gm = gamma.detach().to(torch.float32).contiguous()
-        b = beta.detach().to(torch.float32).contiguous()
-        stats = torch.empty((2, J), dtype=torch.float32, device=dev)
-        y = torch.empty((R, J), dtype=torch.float32, device=dev)
-        a = part = None
-        if training or keep_pre:
-            a = torch.empty((R, J), dtype=torch.float32, device=dev)
-        if training:
-            part = torch.empty(-(-R // 128) * 2 * J, dtype=torch.float32, device=dev)
-        amax = torch.zeros(4, dtype=torch.float32, device=dev)
-        lib.call("zsb_linear_tc_bn_gamma_f32", int(training), ptr(wp), ptr(ws), ptr(hpl.planes),
-                 ptr(hpl.scale), int(hpl.binary), ptr(gm), ptr(b), ptr(moving_mean),
-                 ptr(moving_variance), rate, eps, ptr(stats), ptr(a), ptr(part), ptr(y), R, J, K,
-                 int(relu), ptr(amax), stream())
-        ctx.save_for_backward(W, gm, y if relu else None, a, stats)
-        ctx.hpl = hpl
-        ctx.wpl = (wp, ws)
-        ctx.meta = (lead, training, relu, R, K, J)
+        ctx.hpl = _planes_of(h2, h)
+        ctx.wpl = _tc_split(W)
+        y, amax = _bn_forward(ctx, ctx.hpl, ctx.wpl, J, gamma, beta, stats_bufs, training, relu,
+                              rate, eps, False, keep_pre, W)
+        ctx.meta = (lead, R, K)
         return _tag(y.reshape(tuple(lead) + (J,)), amax)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gy):
-        from ._lib import lib, ptr, stream
-        W, gm, y, a, stats = ctx.saved_tensors
-        lead, training, relu, R, K, J = ctx.meta
+        W, = ctx.saved_tensors[4:]
+        lead, R, K = ctx.meta
         need = ctx.needs_input_grad
-        dev = gy.device
-        g = gy.reshape(R, J).to(torch.float32).contiguous()
-        dgamma = torch.empty(J, dtype=torch.float32, device=dev) if need[2] else None
-        dbeta = torch.empty(J, dtype=torch.float32, device=dev) if need[3] else None
-        part = torch.empty((-(-R // 128) + 1) * 2 * J, dtype=torch.float32, device=dev)
-        planes = torch.empty((2, R, lib.load().zsb_linear_tc_kpad(J)), dtype=torch.float16,
-                             device=dev)
-        scale = torch.zeros(4, dtype=torch.float32, device=dev)
-        lib.call("zsb_bn_grad_gamma_f32", int(training), ptr(g), ptr(y), ptr(a), ptr(stats),
-                 ptr(gm), int(relu), R, J, ptr(part), ptr(dbeta), ptr(dgamma), ptr(planes),
-                 ptr(scale), stream())
-        gpl = _Planes(planes, scale, R, J)
+        dgamma, dbeta, gpl = _bn_backward(ctx, gy, need[2], need[3])
         dh, dW = _grad_products(ctx, gpl, W, R, ctx.wpl, tuple(lead) + (K,), need[0], need[1])
         return dh, dW, dgamma, dbeta, None, None, None, None, None, None
 
@@ -1215,14 +1234,9 @@ def bn_linear(h, W, gamma, beta, moving_mean, moving_variance, training, relu=Tr
     J = int(W.shape[0])
     if h.device != dev:
         raise ValueError("h is on %s and W on %s" % (h.device, dev))
-    for nm, t in (("gamma", gamma), ("beta", beta)):
-        if not isinstance(t, torch.Tensor) or tuple(t.shape) != (J,) or \
-                t.dtype != torch.float32 or t.device != dev:
-            raise ValueError("%s must be a float32 [%d] tensor on %s" % (nm, J, dev))
-    for nm, t in (("moving_mean", moving_mean), ("moving_variance", moving_variance)):
-        if not isinstance(t, torch.Tensor) or tuple(t.shape) != (J,) or \
-                t.dtype != torch.float32 or not t.is_contiguous() or t.device != dev:
-            raise ValueError("%s must be a contiguous float32 [%d] tensor on %s" % (nm, J, dev))
+    if gamma is None:
+        raise ValueError("bn_linear: gamma must be a float32 [%d] tensor on %s" % (J, dev))
+    _bn_check("bn_linear", J, dev, gamma, beta, moving_mean, moving_variance)
     if h.numel() == 0 or J == 0:
         raise ValueError("empty shapes are not supported: h %s, W %s"
                          % (tuple(h.shape), tuple(W.shape)))
@@ -2147,20 +2161,6 @@ def _conv_tc_geom(name, x, W, stride, padding, transpose):
     return _ConvGeom(N, Hb, Wb, Hs, Ws, k, s, pt, pl, Cin, Cout), lead
 
 
-def _conv_bn_check(name, Cout, dev, gamma, beta, moving_mean, moving_variance):
-    for nm, t, opt in (("gamma", gamma, True), ("beta", beta, False)):
-        if t is None and opt:
-            continue
-        if not isinstance(t, torch.Tensor) or tuple(t.shape) != (Cout,) or \
-                t.dtype != torch.float32 or t.device != dev:
-            raise ValueError("%s: %s must be a float32 [%d] tensor on %s" % (name, nm, Cout, dev))
-    for nm, t in (("moving_mean", moving_mean), ("moving_variance", moving_variance)):
-        if not isinstance(t, torch.Tensor) or tuple(t.shape) != (Cout,) or \
-                t.dtype != torch.float32 or not t.is_contiguous() or t.device != dev:
-            raise ValueError("%s: %s must be a contiguous float32 [%d] tensor on %s"
-                             % (name, nm, Cout, dev))
-
-
 def _gather_planes(x4, g, C, tag=None):
     """The fp16 operand planes of the im2col matrix [N Hs Ws, k k C] of x4 [N, Hb, Wb, C]
     (zsb_conv_gather_split_f32), at the scale of ``tag`` (a scale slot holding max |x4|) when
@@ -2201,63 +2201,33 @@ def _ones_like_gamma(gamma, Cout, dev):
 
 
 class _BNConv2d(torch.autograd.Function):
-    """relu?(BN(conv(x, W)) * gamma + beta): the gather-split of x, then the batch-norm product of
-    the dense layers with TF's fused-batch-norm update (zsb_linear_tc_bn_gamma_fused_f32) over
-    R = N Ho Wo rows, J = Cout features and K = k k Cin.  Backward: zsb_bn_grad_gamma_f32 gives
-    d beta, d gamma and the planes of G = d/d(pre-activation); dx is the col2im-sum of G W (the
-    MN-major input-gradient product) and dW the weight-gradient product of G and the saved
-    gather planes."""
+    """relu?(BN(conv(x, W)) * gamma + beta): the gather-split of x, then _bn_forward with TF's
+    fused-batch-norm update over R = N Ho Wo rows, J = Cout features and K = k k Cin.  Backward:
+    _bn_backward gives d beta, d gamma and the planes of G = d/d(pre-activation); dx is the
+    col2im-sum of G W (the MN-major input-gradient product) and dW the weight-gradient product of
+    G and the saved gather planes."""
 
     @staticmethod
     def forward(ctx, x, W, gamma, beta, stats_bufs, g, training, relu, rate, eps, keep_pre):
-        from ._lib import lib, ptr, stream
-        moving_mean, moving_variance = stats_bufs
         dev = W.device
         tag = _take_tag(x)
         x4 = x.detach().reshape(g.N, g.Hb, g.Wb, g.Cin).contiguous()
         hpl = _gather_planes(x4, g, g.Cin, tag)
-        R, K, J = hpl.rows, hpl.K, g.Cout
-        Wt = W.detach().reshape(K, J).t()
-        wp, ws = _tc_split(Wt)
-        gm = _ones_like_gamma(gamma, J, dev)
-        b = beta.detach().contiguous()
-        stats = torch.empty((2, J), dtype=torch.float32, device=dev)
-        y = torch.empty((R, J), dtype=torch.float32, device=dev)
-        a = part = None
-        if training or keep_pre:
-            a = torch.empty((R, J), dtype=torch.float32, device=dev)
-        if training:
-            part = torch.empty(-(-R // 128) * 2 * J, dtype=torch.float32, device=dev)
-        amax = torch.zeros(4, dtype=torch.float32, device=dev)
-        lib.call("zsb_linear_tc_bn_gamma_fused_f32", int(training), ptr(wp), ptr(ws),
-                 ptr(hpl.planes), ptr(hpl.scale), 0, ptr(gm), ptr(b), ptr(moving_mean),
-                 ptr(moving_variance), rate, eps, ptr(stats), ptr(a), ptr(part), ptr(y), R, J, K,
-                 int(relu), ptr(amax), stream())
-        ctx.save_for_backward(gm, y if relu else None, a, stats)
-        ctx.hpl, ctx.wpl, ctx.Wt_shape = hpl, (wp, ws), (J, K)
-        ctx.meta = (g, tuple(x.shape), training, relu, gamma is not None)
+        K, J = hpl.K, g.Cout
+        ctx.hpl, ctx.wpl, ctx.Wt_shape = hpl, _tc_split(W.detach().reshape(K, J).t()), (J, K)
+        y, amax = _bn_forward(ctx, hpl, ctx.wpl, J, _ones_like_gamma(gamma, J, dev), beta,
+                              stats_bufs, training, relu, rate, eps, True, keep_pre)
+        ctx.meta = (g, tuple(x.shape))
         return _tag(y.reshape(tuple(x.shape[:-3]) + (g.Hs, g.Ws, J)), amax)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gy):
-        from ._lib import lib, ptr, stream
-        gm, y, a, stats = ctx.saved_tensors
-        g, x_shape, training, relu, has_gamma = ctx.meta
+        g, x_shape = ctx.meta
         need = ctx.needs_input_grad
         dev = gy.device
-        R, J = g.N * g.Hs * g.Ws, g.Cout
-        gg = gy.reshape(R, J).to(torch.float32).contiguous()
-        dgamma = torch.empty(J, dtype=torch.float32, device=dev) if need[2] else None
-        dbeta = torch.empty(J, dtype=torch.float32, device=dev) if need[3] else None
-        part = torch.empty((-(-R // 128) + 1) * 2 * J, dtype=torch.float32, device=dev)
-        planes = torch.empty((2, R, lib.load().zsb_linear_tc_kpad(J)), dtype=torch.float16,
-                             device=dev)
-        scale = torch.zeros(4, dtype=torch.float32, device=dev)
-        lib.call("zsb_bn_grad_gamma_f32", int(training), ptr(gg), ptr(y), ptr(a), ptr(stats),
-                 ptr(gm), int(relu), R, J, ptr(part), ptr(dbeta), ptr(dgamma), ptr(planes),
-                 ptr(scale), stream())
-        gpl = _Planes(planes, scale, R, J)
+        R = g.N * g.Hs * g.Ws
+        dgamma, dbeta, gpl = _bn_backward(ctx, gy, need[2], need[3])
         dx = dW = None
         if need[0]:
             wp, ws = ctx.wpl
@@ -2317,8 +2287,8 @@ class _BNConv2dT(torch.autograd.Function):
     """relu?(BN(conv_transpose(x, W)) * gamma + beta): the epi-0 product x W'^T gives the columns
     [N Hi Wi, k k Cout]; their col2im-sum onto the output grid runs the batch-norm epilogue
     (training: pre-activation and moment partials, then zsb_bn_finish_fused_f32; evaluation:
-    the affine step in place).  Backward: zsb_bn_grad_gamma_f32out gives d beta, d gamma and
-    da in fp32, then _conv_t_grads."""
+    the affine step in place).  Backward: _bn_backward gives d beta, d gamma and da in fp32, then
+    _conv_t_grads."""
 
     @staticmethod
     def forward(ctx, x, W, gamma, beta, stats_bufs, g, training, relu, rate, eps, keep_pre):
@@ -2329,13 +2299,8 @@ class _BNConv2dT(torch.autograd.Function):
         cols, hpl, wpl = _conv_t_product(x, W, g)
         gm = _ones_like_gamma(gamma, J, dev)
         b = beta.detach().contiguous()
-        stats = torch.empty((2, J), dtype=torch.float32, device=dev)
-        y = torch.empty((Rb, J), dtype=torch.float32, device=dev)
-        a = torch.empty((Rb, J), dtype=torch.float32, device=dev) if training or keep_pre \
-            else None
-        amax = torch.zeros(4, dtype=torch.float32, device=dev)
+        stats, y, a, part, amax = _bn_buffers(Rb, J, dev, training, keep_pre)
         if training:
-            part = torch.empty(-(-Rb // 128) * 2 * J, dtype=torch.float32, device=dev)
             _col2im(2, cols, g, J, pre=a, part=part)
             del cols
             lib.call("zsb_bn_finish_fused_f32", ptr(a), ptr(part), Rb, J, ptr(gm), ptr(b),
@@ -2345,29 +2310,17 @@ class _BNConv2dT(torch.autograd.Function):
             _col2im(3, cols, g, J, out=y, gamma=gm, beta=b, mm=moving_mean, mv=moving_variance,
                     eps=eps, relu=relu, stats=stats, pre=a, amax=amax)
             del cols
-        ctx.save_for_backward(gm, y if relu else None, a, stats)
+        _bn_save(ctx, training, relu, gm, y, a, stats)
         ctx.hpl, ctx.wpl = hpl, wpl
-        ctx.meta = (g, tuple(x.shape), training, relu)
+        ctx.meta = (g, tuple(x.shape))
         return _tag(y.reshape(tuple(x.shape[:-3]) + (g.Hb, g.Wb, J)), amax)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gy):
-        from ._lib import lib, ptr, stream
-        gm, y, a, stats = ctx.saved_tensors
-        g, x_shape, training, relu = ctx.meta
+        g, x_shape = ctx.meta
         need = ctx.needs_input_grad
-        dev = gy.device
-        J, Rb = g.Cout, g.N * g.Hb * g.Wb
-        gg = gy.reshape(Rb, J).to(torch.float32).contiguous()
-        dgamma = torch.empty(J, dtype=torch.float32, device=dev) if need[2] else None
-        dbeta = torch.empty(J, dtype=torch.float32, device=dev) if need[3] else None
-        part = torch.empty((-(-Rb // 128) + 1) * 2 * J, dtype=torch.float32, device=dev)
-        da = torch.empty((Rb, J), dtype=torch.float32, device=dev)
-        scale = torch.zeros(4, dtype=torch.float32, device=dev)
-        lib.call("zsb_bn_grad_gamma_f32out", int(training), ptr(gg), ptr(y), ptr(a), ptr(stats),
-                 ptr(gm), int(relu), Rb, J, ptr(part), ptr(dbeta), ptr(dgamma), ptr(da),
-                 ptr(scale), stream())
+        dgamma, dbeta, (da, scale) = _bn_backward(ctx, gy, need[2], need[3], planes=False)
         dx, dW = _conv_t_grads(ctx, da, scale, g, need[0], need[1], x_shape)
         return dx, dW, dgamma, dbeta, None, None, None, None, None, None, None
 
@@ -2419,7 +2372,7 @@ def _bn_conv_apply(fn, name, x, W, gamma, beta, moving_mean, moving_variance, tr
                    padding, relu, momentum, epsilon, transpose):
     x = _unwrap(x)
     g, _ = _conv_tc_geom(name, x, W, stride, padding, transpose)
-    _conv_bn_check(name, g.Cout, W.device, gamma, beta, moving_mean, moving_variance)
+    _bn_check(name, g.Cout, W.device, gamma, beta, moving_mean, moving_variance)
     keep_pre = (not training) and torch.is_grad_enabled() and gamma is not None and \
         gamma.requires_grad
     return fn.apply(x, W, gamma, beta, (moving_mean, moving_variance), g, bool(training),
