@@ -257,6 +257,39 @@ int zsb_linear_tc_cat_given_f32(int epi, const void* w_planes, const float* scal
                                 const float* bias, const float* given, int64_t n_g, int S,
                                 const float* gout, float* out, int64_t R, int C, int K,
                                 float* amax_scale, void* stream);
+/* Gaussian dense layer over D features (1 <= D <= 256), the heads mu = h W_mean^T + b_mean and
+ * ls = h W_logstd^T + b_logstd never written unless asked for (replaces two tf.layers.dense +
+ * bn.normal(..., logstd=..., n_samples=K), vae_ssl_adaptive_is.py:53-68, with Normal._sample /
+ * _log_prob, univariate.py:161-181).  w_planes: the planes of the packed heads [2 Dp, K], Dp =
+ * zsb_linear_tc_kpad(D), in blocks of 64 rows [mean 0..63 | logstd 0..63 | mean 64..127 | ...],
+ * zero padded; bias: the packed biases [2 Dp] or NULL.  Draw s R + r of S per row; S R < 2^31.
+ *   z [S R, D] = eps * exp(ls) + mu, eps = eps_in [S R D] or element (s R + r) D + j of the normals
+ *   zsb_reparam_normal_f32 draws for (seed, iter): z is that sampler's draw bit for bit;
+ *   logq [S R] = sum_j log N(z; mu, exp(ls)), summed in a fixed order from part (Dp / 32 * S R
+ *   floats of scratch: two partial rows per 64 features);
+ *   mean_out / logstd_out [R, D] (either may be NULL); max |z| folded into amax_scale[2] (may be
+ *   NULL).  h_binary: h_planes is itself a binary plane. */
+int zsb_linear_tc_normal_sample_f32(const void* w_planes, const float* scale_w,
+                                    const void* h_planes, const float* scale_h, int h_binary,
+                                    const float* bias, const float* eps_in, uint64_t seed,
+                                    uint32_t iter, int S, float* z, float* logq, float* part,
+                                    float* mean_out, float* logstd_out, int64_t R, int D, int K,
+                                    float* amax_scale, void* stream);
+/* Its backward pass in one launch, summed over the S draws in order (no float atomics), with eps
+ * recomputed from (seed, iter + *epoch) or read from eps_in.  epoch (may be NULL): a copy of the
+ * device epoch taken when the forward launch ran, so the draws are recomputed as they were drawn
+ * even if the epoch has moved since:
+ *   reparam:   d mu = sum_s gz_s,                d ls = sum_s (gz_s std eps_s - glq_s)
+ *   otherwise: d mu = sum_s glq_s eps_s / std,   d ls = sum_s glq_s (eps_s^2 - 1)
+ * (Normal._sample stop-gradients mean and std when not reparameterised, univariate.py:161-172;
+ * log q keeps its partials).  gz [S R, D] and glq [S R] may each be NULL (zero); logstd [R, D].
+ * dpre [R, 2 Dp]: the gradient of the packed pre-activation, padding columns zero, max |dpre|
+ * folded into amax_scale[2] (must start at zero): the operand of zsb_split16_dual_f32 with
+ * have_amax = 1. */
+int zsb_linear_normal_grad_f32(const float* logstd, const float* gz, const float* glq,
+                               const float* eps_in, uint64_t seed, uint32_t iter,
+                               const uint32_t* epoch, int reparam, int S, int64_t R, int D,
+                               float* dpre, float* amax_scale, void* stream);
 /* zsb_linear_tc_amax_f32 / zsb_linear_tc_wgrad_f32 with a binary activation h (h_planes = its one
  * plane, scale_h[0] = 2048): the forward, epi 1 / 2 and weight-gradient products of a layer fed a
  * sample (sbn_vimco.py:25-30, 40-43). */

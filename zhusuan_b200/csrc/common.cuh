@@ -204,4 +204,15 @@ static inline bool zsb_vec4_ok(int64_t chains, int64_t row_len, std::initializer
 #define ZSB_STREAM_SGMCMC_RESAMPLE 4u
 #define ZSB_STREAM_SAMPLE 5u
 
+// Element i of the standard normals zsb_reparam_normal_f32 draws (component i & 3 of the
+// philox_normal4 block i >> 2 on ZSB_STREAM_SAMPLE), with only the Box-Muller pair it needs
+__device__ __forceinline__ float philox_normal_at(uint64_t seed, uint32_t iter, int64_t i) {
+  const Philox4 p = philox4x32_10((uint32_t)(i >> 2), (uint32_t)((uint64_t)i >> 34), iter,
+                                  ZSB_STREAM_SAMPLE, (uint32_t)seed, (uint32_t)(seed >> 32));
+  float e0, e1;
+  if ((i & 2) == 0) box_muller(p.x, p.y, e0, e1);
+  else box_muller(p.z, p.w, e0, e1);
+  return (i & 1) ? e1 : e0;
+}
+
 #endif  // __CUDACC__

@@ -74,9 +74,16 @@ constexpr float BIN_SCALE = 2048.f;
 //   EPI 14 out[r, j] = sum_s gout[d] (given_j - (sum_i given_i) softmax(l[r])_j), given = row
 //          d % n_g (d/dl of EPI 13)
 //
+// Gaussian-sampling epilogue (D features, 1 <= D <= 256; the two heads packed in blocks of 64
+// columns, [mean 0..63 | logstd 0..63 | mean 64..127 | ...], so one 128-feature tile holds mean_j
+// and logstd_j of the same 64 features; bn.normal of two dense heads, vae_ssl_adaptive_is.py:53-68):
+//   EPI 15 z[s R + r, j] = eps * expf(ls) + mu with eps the standard normal
+//          zsb_reparam_normal_f32 draws for element (s R + r) D + j (or injected), and the partial
+//          rows of log N(z; mu, exp(ls)) summed over the features
+//
 // The descriptor tc_pipeline_kernel runs, LinW<E, EPI, MN, Z>, is a LinCore (the product) plus the
 // fields of one epilogue family E: RowsEpi (EPI 0 - 2), SamplesEpi (4 - 6), ClassEpi (7, 8),
-// BnEpi (9 - 11) or CatEpi (12 - 14).
+// BnEpi (9 - 11), CatEpi (12 - 14) or NormalEpi (15).
 
 // What a product's units past its first n_tiles are (unit u runs output tile u % n_tiles), as each
 // epilogue family declares it:
@@ -626,6 +633,94 @@ struct CatEpi {
             out[r * C + c0 + t] = dl[t];
             amax = fmaxf(amax, fabsf(dl[t]));
           }
+      }
+    }
+  }
+};
+
+constexpr float NORMAL_HALF_LOG_2PI = 0.9189385332046727f;   // kHalfLog2Pi of distributions.cu
+constexpr int NORMAL_MAX_D = 256;
+
+// EPI 15.  The heads of feature j sit in accumulator rows f and 64 + f of the tile (f = j % 64), so
+// a lane takes one feature over half of the tile's rows: warps 0 / 1 features 0 - 31 / 32 - 63 of
+// rows 0 - 63, warps 2 / 3 the same features of rows 64 - 127 (every warp reads rows another warp
+// was given; the tile is complete once tfull has fired, as for CatEpi).  Per 4-row block, mu, std
+// and the log-density's constants once, then each sample row of the unit's chunk.  Each element
+// runs its own Philox-10 and one Box-Muller pair, twice the transcendental work and four times the
+// Philox work of zsb_reparam_normal_f32, which shares one block among four elements; the keying is
+// the same, so z is that sampler's draw bit for bit.  The partial row of warp q for feature block nb
+// is nb * 2 + (q & 1): Dp / 32 rows in all, summed in a fixed order.
+struct NormalEpi {
+  static constexpr Units UNITS = SAMPLE_CHUNKS;
+  __host__ __device__ static constexpr bool folds_amax(int) { return true; }
+  const float* bias; int D; float* z; float* part; float* mean_out; float* logstd_out;
+  int S; int s_per; const float* eps_in; uint64_t seed; uint32_t iter; const uint32_t* epoch;
+  float* amax_scale;
+
+  template <int EPI, class Core>
+  __device__ __forceinline__ void run(const Core& core, int64_t uu, uint32_t trow, int quarter,
+                                      int lane, float& amax) const {
+    const int64_t& R = core.R;
+    const float acc_scale = core.acc_scale();
+    const Unit pos = core.template unit<UNITS>(uu, quarter, lane);
+    const int s0 = pos.sub * s_per, s1 = min(S, s0 + s_per);
+    const int f = (quarter & 1) * 32 + lane;
+    const int j = pos.nb * 64 + f;
+    const bool j_ok = j < D;
+    const int half = quarter >> 1;
+    const uint32_t acc0 = trow - (uint32_t)((quarter * 32 + lane) * ACC_LD * 4);
+    const uint32_t row_mu = acc0 + (uint32_t)((f * ACC_LD + 64 * half) * 4);
+    const uint32_t row_ls = row_mu + (uint32_t)(64 * ACC_LD * 4);
+    const float bm = (j_ok && bias) ? __ldg(bias + pos.nb * 128 + f) : 0.f;
+    const float bl = (j_ok && bias) ? __ldg(bias + pos.nb * 128 + 64 + f) : 0.f;
+    const int64_t SR = (int64_t)S * R;
+    const int64_t part_row = (int64_t)(pos.nb * 2 + (quarter & 1)) * SR;
+    const uint32_t it = iter + (epoch ? *epoch : 0u);
+#pragma unroll 1
+    for (int c = 0; c < 64; c += 4) {
+      const int64_t rbase = pos.r0 + 64 * half + c;
+      if (rbase >= R) break;                                 // warp-uniform
+      float vm[4], vl[4], mu[4], sd[4], c1[4], hv[4];
+      asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+                   : "=f"(vm[0]), "=f"(vm[1]), "=f"(vm[2]), "=f"(vm[3])
+                   : "r"(row_mu + 4u * (uint32_t)c));
+      asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+                   : "=f"(vl[0]), "=f"(vl[1]), "=f"(vl[2]), "=f"(vl[3])
+                   : "r"(row_ls + 4u * (uint32_t)c));
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        mu[jj] = fmaf(vm[jj], acc_scale, bm);
+        const float ls = fmaf(vl[jj], acc_scale, bl);
+        const int64_t r = rbase + jj;
+        if (pos.sub == 0 && j_ok && r < R) {
+          if (mean_out) mean_out[r * D + j] = mu[jj];
+          if (logstd_out) logstd_out[r * D + j] = ls;
+        }
+        sd[jj] = expf(ls);
+        c1[jj] = -NORMAL_HALF_LOG_2PI - ls;
+        hv[jj] = 0.5f * expf(-2.f * ls);
+      }
+#pragma unroll 1
+      for (int s = s0; s < s1; ++s) {
+        float lpv[4];
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int64_t r = rbase + jj;
+          const bool ok = j_ok && r < R;
+          const int64_t i = ((int64_t)s * R + r) * D + j;      // element of the [S, R, D] sample
+          const float e = !ok ? 0.f : eps_in ? __ldg(eps_in + i) : philox_normal_at(seed, it, i);
+          const float zz = e * sd[jj] + mu[jj];                 // zsb_reparam_normal_f32's rounding
+          const float d = zz - mu[jj];
+          lpv[jj] = ok ? c1[jj] - hv[jj] * d * d : 0.f;
+          if (ok) {
+            z[i] = zz;
+            amax = fmaxf(amax, fabsf(zz));
+          }
+        }
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) lpv[jj] = warp_sum(lpv[jj]);
+        const float sum = lane == 0 ? lpv[0] : lane == 1 ? lpv[1] : lane == 2 ? lpv[2] : lpv[3];
+        if (lane < 4 && rbase + lane < R) part[part_row + (int64_t)s * R + rbase + lane] = sum;
       }
     }
   }
@@ -1612,6 +1707,46 @@ int zsb_linear_tc_cat_given_f32(int epi, const void* w_planes, const float* scal
     if (rc) return rc;
     if (epi == 2) return tc_launch(LinW<CatEpi, 14, 0, z>{c, e}, st, "linear_tc_cat_given");
     return tc_launch(LinW<CatEpi, 13, 0, z>{c, e}, st, "linear_tc_cat_given");
+  });
+}
+
+// Gaussian layer with S draws per row, the heads mu = h W_mean^T + b_mean and ls = h W_logstd^T +
+// b_logstd never leaving the epilogue (EPI 15; replaces two dense layers + Normal._sample + log_prob,
+// vae_ssl_adaptive_is.py:53-68 and univariate.py:161-181).  w_planes / bias: the packed heads
+// [2 Dp, K] / [2 Dp], Dp = kpad(D), in blocks of 64 rows [mean | logstd | mean | ...], zero padded.
+//   z [S R, D]       eps * exp(ls) + mu, eps = eps_in [S R D] or the Philox normal
+//                    zsb_reparam_normal_f32 draws for (seed, iter) at element (s R + r) D + j
+//   logq [S R]       sum_j log N(z; mu, exp(ls));  part = Dp / 32 * S R floats of scratch
+//   mean_out, logstd_out [R, D] (either may be NULL)
+// max |z| is folded into amax_scale[2] (may be NULL).  1 <= D <= 256; h_binary as in
+// zsb_linear_tc_bern_sample_f32.
+int zsb_linear_tc_normal_sample_f32(const void* w_planes, const float* scale_w,
+                                    const void* h_planes, const float* scale_h, int h_binary,
+                                    const float* bias, const float* eps_in, uint64_t seed,
+                                    uint32_t iter, int S, float* z, float* logq, float* part,
+                                    float* mean_out, float* logstd_out, int64_t R, int D, int K,
+                                    float* amax_scale, void* stream) {
+  ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && z && logq && part && R > 0 && K > 0 &&
+                  S >= 1,
+              "zsb_linear_tc_normal_sample_f32: bad args");
+  ZSB_REQUIRE(D >= 1 && D <= NORMAL_MAX_D, "zsb_linear_tc_normal_sample_f32: D must be in [1, 256]");
+  ZSB_REQUIRE((int64_t)S * R < (1LL << 31),
+              "zsb_linear_tc_normal_sample_f32: too many rows");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int J = 2 * zsb_linear_tc_kpad(D);
+  const int s_per = sample_chunk(R, J, S);
+  const NormalEpi e{.bias = bias, .D = D, .z = z, .part = part, .mean_out = mean_out,
+                    .logstd_out = logstd_out, .S = S, .s_per = s_per, .eps_in = eps_in,
+                    .seed = seed, .iter = iter, .epoch = zsb_epoch_ptr(), .amax_scale = amax_scale};
+  return with_h_binary(h_binary, [&](auto zb) {
+    LinCore<0, zb> c;
+    int rc = make_core(c, w_planes, scale_w, h_planes, scale_h, J, R, K, (S + s_per - 1) / s_per);
+    if (rc) return rc;
+    rc = tc_launch(LinW<NormalEpi, 15, 0, zb>{c, e}, st, "linear_tc_normal_sample");
+    if (rc) return rc;
+    const int64_t rows = (int64_t)S * R;                 // two partial rows per 64 features
+    part_sum_kernel<<<grid_blocks(rows, 256, 8), 256, 0, st>>>(part, J / 64, rows, logq);
+    return zsb_check_launch("linear_tc_normal_sample_part_sum");
   });
 }
 

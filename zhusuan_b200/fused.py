@@ -14,8 +14,9 @@ from .distributions.univariate import Normal
 
 __all__ = ["GaussianLogJoint", "BNNRegressionLogJoint", "LNTMLogJoint", "PMFLogJoint", "linear",
            "class_linear", "noisy_bn_linear", "bn_linear", "linear_bernoulli_log_prob",
-           "LinearBernoulli", "LinearOnehotCategorical", "RBFKernel", "gp_conditional", "conv2d",
-           "conv2d_transpose", "bn_conv2d", "bn_conv2d_transpose", "sigmoid_conv2d_transpose"]
+           "LinearBernoulli", "LinearOnehotCategorical", "LinearNormal", "RBFKernel",
+           "gp_conditional", "conv2d", "conv2d_transpose", "bn_conv2d", "bn_conv2d_transpose",
+           "sigmoid_conv2d_transpose"]
 
 
 class GaussianLogJoint(object):
@@ -1494,7 +1495,32 @@ def _cat_given(epi, wp, ws, hpl, bias, g2, S, gout, out, R, C, K, amax):
              ptr(out), R, C, K, ptr(amax), stream())
 
 
-class LinearOnehotCategorical(object):
+class _CachedHPlanes(object):
+    """The operand planes of a layer's input ``self._h``, kept with h's version in ``self._hpl``."""
+
+    def _h_planes(self):
+        """The operand planes of h.  The planes cached on h do not track its version, so the layer
+        keeps the planes it last read with h's version: while that version holds it reuses them;
+        once h has been rewritten in place it splits h afresh and caches the new planes on h as
+        well, so the next reader (this layer or another) does not find the old ones.  An inference
+        tensor has no version and is read through the cache on h, as ``linear`` reads it."""
+        h2 = self._h.reshape(-1, int(self._h.shape[-1]))
+        v = _version(self._h)
+        if v is not None and self._hpl is not None and self._hpl[1] == v:
+            return self._hpl[0]
+        if v is not None and self._hpl is not None:
+            pl = _tc_split_dual(h2)
+            try:
+                self._h._zsb_pl = pl
+            except (AttributeError, RuntimeError):
+                pass
+        else:
+            pl = _planes_of(h2, self._h)
+        self._hpl = (pl, v)
+        return pl
+
+
+class LinearOnehotCategorical(_CachedHPlanes):
     """Drop-in for ``OnehotCategorical(logits=dense(h))`` as a distribution plugin of
     ``bn.stochastic`` (the ``y`` of vae_ssl_adaptive_is.py:61-68), with the logits never leaving the
     dense layer's epilogue.  ``W`` [C, H] and ``b`` [C] are the ``tf.layers.dense`` kernel
@@ -1539,27 +1565,6 @@ class LinearOnehotCategorical(object):
     def _registry(self):
         from .distributions.multivariate import OnehotCategorical
         return OnehotCategorical(self.logits, dtype=self.dtype, group_ndims=self.group_ndims)
-
-    def _h_planes(self):
-        """The operand planes of h.  The planes cached on h do not track its version, so the layer
-        keeps the planes it last read with h's version: while that version holds it reuses them;
-        once h has been rewritten in place it splits h afresh and caches the new planes on h as
-        well, so the next reader (this layer or another) does not find the old ones.  An inference
-        tensor has no version and is read through the cache on h, as ``linear`` reads it."""
-        h2 = self._h.reshape(-1, int(self._h.shape[-1]))
-        v = _version(self._h)
-        if v is not None and self._hpl is not None and self._hpl[1] == v:
-            return self._hpl[0]
-        if v is not None and self._hpl is not None:
-            pl = _tc_split_dual(h2)
-            try:
-                self._h._zsb_pl = pl
-            except (AttributeError, RuntimeError):
-                pass
-        else:
-            pl = _planes_of(h2, self._h)
-        self._hpl = (pl, v)
-        return pl
 
     def get_batch_shape(self):
         return torch.Size(tuple(self._h.shape[:-1]))
@@ -1656,6 +1661,225 @@ class LinearOnehotCategorical(object):
         g2 = given.reshape(-1, C).to(torch.float32).contiguous()
         lp = _LinearCategoricalGiven.apply(self._h, self._W, self._b, g2, S, None, wp, ws, hpl)
         return ops.group_sum(lp.reshape(out_shape), self.group_ndims)
+
+    def prob(self, given):
+        return torch.exp(self.log_prob(given))
+
+
+NORMAL_MAX_D = 256
+
+
+def _pack_heads(a, b, D):
+    """The heads ``a``, ``b`` ([D, ...]) stacked along axis 0 in blocks of 64 rows, [a 0..63 |
+    b 0..63 | a 64..127 | ...], each zero padded to Dp = kpad(D) rows: the weight (or bias) layout
+    of zsb_linear_tc_normal_sample_f32.  Differentiable."""
+    Dp = (D + 63) // 64 * 64
+    pad = (0, 0) * (a.dim() - 1) + (0, Dp - D)
+    blocks = [torch.nn.functional.pad(t, pad).reshape((Dp // 64, 64) + tuple(t.shape[1:]))
+              for t in (a, b)]
+    return torch.stack(blocks, 1).reshape((2 * Dp,) + tuple(a.shape[1:]))
+
+
+def _unpack_heads(y, D):
+    """(a, b) of a packed [..., 2 Dp] output, each [..., D]."""
+    Dp = int(y.shape[-1]) // 2
+    y4 = y.reshape(tuple(y.shape[:-1]) + (Dp // 64, 2, 64))
+    lead = tuple(y.shape[:-1])
+    return (y4[..., 0, :].reshape(lead + (Dp,))[..., :D],
+            y4[..., 1, :].reshape(lead + (Dp,))[..., :D])
+
+
+class _LinearNormalSample(torch.autograd.Function):
+    """(z, log q(z)) of S draws per row of h from N(mu, exp(ls)), [mu | ls] = h Wp^T + bp with the
+    packed heads Wp [2 Dp, K], bp [2 Dp]: one launch of the Gaussian-sampling epilogue (EPI 15).
+    Backward receives the gradients of z and log q together and runs one pass over the draws
+    (zsb_linear_normal_grad_f32, eps recomputed from Philox or read when injected) that gives the
+    gradient of the packed pre-activation, then the layer's input- and weight-gradient products.
+    ``reparam`` False: z is a constant (Normal._sample stop-gradients mean and std) and log q keeps
+    its partials w.r.t. mu and ls."""
+
+    @staticmethod
+    def forward(ctx, h, Wp, bp, eps, S, D, reparam, hpl, seed, it, keep):
+        from ._lib import lib, ptr, stream
+        lead = tuple(h.shape[:-1])
+        R, K, J = hpl.rows, hpl.K, int(Wp.shape[0])
+        dev = Wp.device
+        wp, ws = _tc_split(Wp)
+        bias = bp.detach().to(torch.float32).contiguous() if bp is not None else None
+        z = torch.empty((S,) + lead + (D,), dtype=torch.float32, device=dev)
+        lq = torch.empty((S,) + lead, dtype=torch.float32, device=dev)
+        part = torch.empty(J // 64 * S * R, dtype=torch.float32, device=dev)
+        ls = torch.empty((R, D), dtype=torch.float32, device=dev) if keep else None
+        amax = torch.zeros(4, dtype=torch.float32, device=dev)
+        e = None if eps is None else eps.detach().to(torch.float32).expand(z.shape).contiguous()
+        lib.call("zsb_linear_tc_normal_sample_f32", ptr(wp), ptr(ws), ptr(hpl.planes),
+                 ptr(hpl.scale), int(hpl.binary), ptr(bias), ptr(e), int(seed), int(it), S,
+                 ptr(z), ptr(lq), ptr(part), None, ptr(ls), R, D, K, ptr(amax), stream())
+        if keep:
+            # the device epoch the launch added to `it`, copied on the stream right after it: the
+            # backward pass recomputes these draws even if the epoch moves before it runs
+            from . import random as zrandom
+            ep = zrandom._epoch["tensor"]
+            ctx.epoch = None if (ep is None or e is not None) else ep.clone()
+            ctx.save_for_backward(Wp, ls, e)
+            ctx.hpl = hpl
+            ctx.wpl = (wp, ws)
+        ctx.meta = (lead, S, R, D, K, bp is not None, reparam, int(seed), int(it))
+        ctx.set_materialize_grads(False)     # an unused z or log q sends None, not zeros
+        if not reparam:
+            ctx.mark_non_differentiable(z)
+        return _tag(z, amax), lq
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gz, glq):
+        from ._lib import lib, ptr, stream
+        Wp, ls, e = ctx.saved_tensors
+        lead, S, R, D, K, has_b, reparam, seed, it = ctx.meta
+        need = ctx.needs_input_grad
+        dev = Wp.device
+        J = int(Wp.shape[0])
+        g_z = gz.to(torch.float32).contiguous() if (gz is not None and reparam) else None
+        g_lq = glq.to(torch.float32).contiguous() if glq is not None else None
+        dpre = torch.empty((R, J), dtype=torch.float32, device=dev)
+        amax = torch.zeros(4, dtype=torch.float32, device=dev)
+        lib.call("zsb_linear_normal_grad_f32", ptr(ls), ptr(g_z), ptr(g_lq), ptr(e), seed, it,
+                 ptr(ctx.epoch), int(reparam), S, R, D, ptr(dpre), ptr(amax), stream())
+        db = torch.zeros(J, dtype=torch.float32, device=dev) if (has_b and need[2]) else None
+        dpl = _tc_split_dual(dpre, amax=amax, col_sum=db)
+        dh, dW = _grad_products(ctx, dpl, Wp, R, ctx.wpl, lead + (K,), need[0], need[1])
+        return dh, dW, db, None, None, None, None, None, None, None, None
+
+
+class LinearNormal(_CachedHPlanes):
+    """Drop-in for ``Normal(dense(h), logstd=dense(h), ...)`` as a distribution plugin of
+    ``bn.stochastic`` (the z heads of vae_ssl_adaptive_is.py:53-68, and the Gaussian latent head of
+    the VAE examples), with the two heads never leaving the dense layer's epilogue.  ``W_mean``,
+    ``W_logstd`` [D, H] and ``b_mean``, ``b_logstd`` [D] (either bias may be None) are the
+    ``tf.layers.dense`` kernels transposed and their biases, as in ``linear``.
+
+    ``sample(n_samples)`` is one launch (zsb_linear_tc_normal_sample_f32) that draws z -- element
+    for element what ``Normal(layer.mean, logstd=layer.logstd).sample(n_samples)`` draws from the
+    same ``zs.random`` state, or from the same injected ``eps`` -- together with ``log q(z)`` summed
+    over the features; no [n_samples, *batch, D] tensor besides z is written.  ``log_prob`` of that
+    very sample with ``group_ndims >= 1`` returns the stored sum (no second pass); any other
+    ``given``, and ``group_ndims = 0``, is scored by ``Normal`` on ``mean`` / ``logstd``.  Both are
+    differentiable w.r.t. h and the four parameters: z by the reparameterisation when
+    ``is_reparameterized``, else z is a constant and log q keeps its partials (univariate.py:161-172).
+    The sample carries its max |.|, so the next ``linear`` of it skips its max pass.
+
+    ``mean`` / ``logstd`` are one ``linear`` over the packed heads, sliced: they read the operand
+    planes the sampling launch reads.  Outside the fused domain -- more than 256 features,
+    parameters that are not float32, tensors not on one CUDA device -- the layer is
+    ``Normal(linear(h, W_mean, b_mean), logstd=linear(h, W_logstd, b_logstd))`` (``F.linear`` for
+    tensors off the GPU)."""
+
+    def __init__(self, h, W_mean, b_mean, W_logstd, b_logstd, group_ndims=0,
+                 is_reparameterized=True):
+        h = _unwrap(h)
+        self._h = h
+        self._params = (W_mean, b_mean, W_logstd, b_logstd)
+        self._D = int(W_mean.shape[0])
+        if tuple(W_logstd.shape) != tuple(W_mean.shape):
+            raise ValueError("W_mean %s and W_logstd %s differ in shape"
+                             % (tuple(W_mean.shape), tuple(W_logstd.shape)))
+        self.dtype = torch.float32
+        self.param_dtype = torch.float32
+        self.is_continuous = True
+        self.is_reparameterized = bool(is_reparameterized)
+        self.group_ndims = group_ndims
+        self._hpl = None
+        self._heads = None
+        self._own = None
+        ts = [t for t in (h,) + self._params if t is not None]
+        self._fused = (1 <= self._D <= NORMAL_MAX_D and h.numel() > 0
+                       and all(t.is_cuda and t.dtype == torch.float32
+                               and t.device == W_mean.device for t in ts))
+
+    def _packed(self):
+        W_mean, b_mean, W_logstd, b_logstd = self._params
+        Wp = _pack_heads(W_mean, W_logstd, self._D)
+        if b_mean is None and b_logstd is None:
+            return Wp, None
+        zero = torch.zeros(self._D, dtype=torch.float32, device=W_mean.device)
+        return Wp, _pack_heads(zero if b_mean is None else b_mean,
+                               zero if b_logstd is None else b_logstd, self._D)
+
+    def _mean_logstd(self):
+        ts = (self._h,) + self._params
+        vs = _versions(*ts)
+        key = (vs, torch.is_grad_enabled())
+        if not all(v is not None for t, v in zip(ts, vs) if t is not None):
+            key = None                       # an inference tensor: nothing is cached
+        if key is not None and self._heads is not None and self._heads[0] == key:
+            return self._heads[1]
+        W_mean, b_mean, W_logstd, b_logstd = self._params
+        if self._fused:
+            self._h_planes()                 # h's cached planes follow its in-place changes
+            Wp, bp = self._packed()
+            heads = _unpack_heads(linear(self._h, Wp, bp), self._D)
+        elif W_mean.is_cuda:
+            heads = (linear(self._h, W_mean, b_mean), linear(self._h, W_logstd, b_logstd))
+        else:
+            F = torch.nn.functional
+            heads = (F.linear(self._h, W_mean, b_mean), F.linear(self._h, W_logstd, b_logstd))
+        self._heads = (key, heads)
+        return heads
+
+    mean = property(lambda self: self._mean_logstd()[0])
+    logstd = property(lambda self: self._mean_logstd()[1])
+
+    def _registry(self):
+        mean, logstd = self._mean_logstd()
+        return Normal(mean, logstd=logstd, group_ndims=self.group_ndims,
+                      is_reparameterized=self.is_reparameterized)
+
+    def get_batch_shape(self):
+        return torch.Size(tuple(self._h.shape[:-1]) + (self._D,))
+
+    def get_value_shape(self):
+        return torch.Size([])
+
+    batch_shape = property(lambda self: self.get_batch_shape())
+    value_shape = property(lambda self: self.get_value_shape())
+
+    def sample(self, n_samples=None, eps=None):
+        """``n_samples`` as in ``Normal.sample``; ``eps``: injected standard normals that broadcast
+        to ``[n_samples, *batch_shape]`` (``Normal._sample(n, eps=...)``), else the Philox stream of
+        ``zs.random``."""
+        from . import random as zrandom
+        if isinstance(n_samples, torch.Tensor):
+            n_samples = int(n_samples.item())
+        S = 1 if n_samples is None else int(n_samples)
+        self._own = None
+        if not self._fused:
+            out = self._registry()._sample(S, eps=eps)
+            return out.squeeze(0) if n_samples is None else out
+        hpl = self._h_planes()
+        Wp, bp = self._packed()
+        keep = torch.is_grad_enabled() and any(
+            t is not None and t.requires_grad for t in (self._h, Wp, bp))
+        seed, it = zrandom.get_seed(), zrandom.next_counter()
+        z, lq = _LinearNormalSample.apply(self._h, Wp, bp, eps, S, self._D,
+                                          self.is_reparameterized, hpl, seed, it, keep)
+        if n_samples is None:
+            amax = getattr(z, "_zsb_amax", None)
+            z, lq = z.squeeze(0), lq.squeeze(0)
+            if amax is not None:
+                _tag(z, amax)
+        vs = _versions(z, self._h, *self._params)
+        if all(v is not None for t, v in zip((z, self._h) + self._params, vs) if t is not None):
+            # (inference tensors of torch.inference_mode() have no version: nothing is cached)
+            self._own = (z, lq, vs)
+        return z
+
+    def log_prob(self, given):
+        from . import ops
+        own = self._own
+        if (own is not None and self.group_ndims >= 1 and given is own[0]
+                and own[2] == _versions(given, self._h, *self._params)):
+            return ops.group_sum(own[1], self.group_ndims - 1)
+        return self._registry().log_prob(given)
 
     def prob(self, given):
         return torch.exp(self.log_prob(given))
