@@ -540,18 +540,41 @@ int zsb_sample_count_i32(int kind, const float* param, int64_t param_n, int64_t 
                          const float* u, uint64_t seed, uint32_t iter, int32_t* out, int64_t n,
                          void* stream);
 
-/* ---- K8, config 5: Logistic-Normal Topic Model E-step log-joint (csrc/lntm.cu) -----------------
+/* ---- K8, config 5: Logistic-Normal Topic Model E-step log-joint and M-step (csrc/lntm.cu) -------
  * log p = sum_k Normal(eta_k; mean_k, exp(logstd_k)).log_prob + sum_v x[d,v] log(softmax(eta) @ phi)[v]
  * (examples/topic_models/lntm_mcem.py:33-48, e_obj :97-99; UnnormalizedMultinomial._log_prob,
  * multivariate.py:435-443 with normalize_logits=False) and its gradient w.r.t. eta, fused and
  * sparsity-aware: the corpus is CSR, only the words a document contains are formed, the
- * [chains*docs, V] matrix of the reference never exists.  phi_t = softmax(beta)^T [V, K]. */
+ * [chains*docs, V] matrix of the reference never exists.  1 <= n_topics <= 128; the topic axis of
+ * phi_t = softmax(beta)^T is padded to Kp = 16 ceil(n_topics / 16): phi_t [V, Kp], zero pad columns.
+ *
+ * zsb_lntm_logjoint_f32 (lntm_mcem.py:33-48, 97-99; tempered as evaluation.py:91-94):
+ *   doc_ids [docs] (int64, nullable): row d of eta is corpus document doc_ids[d]; NULL = 0..docs-1.
+ *   temperature (device scalar, nullable): returns prior + t * likelihood and its gradient, which is
+ *   log_prior * (1 - t) + log_joint * t when the proposal is the eta prior; NULL = today's result.
+ * zsb_lntm_mstep_f32 / zsb_lntm_mstep_grad_f32 (lntm_mcem.py:106-114, cond_log_prob('x') and
+ * tf.gradients of -log_joint_beta w.r.t. beta): lp [chains, docs] = log p(x_d | eta_c, beta), then
+ * dbeta [K, V] = d/d beta sum_{c,d} g[c,d] lp[c,d].  The forward writes theta [chains, docs, Kp]
+ * and ratio [chains, nnz] for the gradient; the gradient groups the corpus entries by word (CSC:
+ * csc_ptr [V+1], csc_entry [nnz] ascending within a word, entry_doc [nnz]) and sums in a fixed
+ * order, with no atomics.  doc_slot [n_corpus_docs]: batch row of each corpus document, -1 outside
+ * the batch (NULL when doc_ids is NULL).  G [V, Kp] is scratch. */
 int zsb_lntm_phi_t_f32(const float* beta, int64_t n_topics, int64_t n_vocab, float* phi_t,
                        void* stream);
 int zsb_lntm_logjoint_f32(const float* eta, const float* eta_mean, const float* eta_logstd,
                           const float* phi_t, const int64_t* doc_ptr, const int32_t* word_idx,
-                          const float* word_cnt, float* lp_out, float* grad_out, int64_t chains,
-                          int64_t docs, int64_t n_topics, void* stream);
+                          const float* word_cnt, const int64_t* doc_ids, const float* temperature,
+                          float* lp_out, float* grad_out, int64_t chains, int64_t docs,
+                          int64_t n_topics, void* stream);
+int zsb_lntm_mstep_f32(const float* eta, const float* phi_t, const int64_t* doc_ptr,
+                       const int32_t* word_idx, const float* word_cnt, const int64_t* doc_ids,
+                       float* lp_out, float* ratio, float* theta, int64_t chains, int64_t docs,
+                       int64_t nnz, int64_t n_topics, void* stream);
+int zsb_lntm_mstep_grad_f32(const float* g, const float* ratio, const float* theta,
+                            const float* phi_t, const int64_t* csc_ptr, const int32_t* csc_entry,
+                            const int32_t* entry_doc, const int32_t* doc_slot, float* G,
+                            float* dbeta, int64_t chains, int64_t docs, int64_t nnz,
+                            int64_t n_topics, int64_t n_vocab, void* stream);
 
 /* ---- Bayesian PMF, one HMC sweep over every chunk of one factor (csrc/pmf.cu) ------------------
  * The model of examples/probabilistic_matrix_factorization/pmf_hmc.py:19-31 with its log_joint

@@ -89,7 +89,7 @@ class _Lib(object):
     _KERNELS = {"zsb_hmc_mass_stats_f32": 2, "zsb_hmc_dense_traj_prepare_f32": 3, "zsb_hmc_dense_resident_h16_f32": 1, "zsb_sgmcmc_sghmc_f32": 2,
                 "zsb_sgmcmc_mean_sq_f32": 2, "zsb_sgmcmc_sgnht_scalar_f32": 2,
                 "zsb_split16_pad_f32": 3, "zsb_linear_tc_f32": 2, "zsb_planar_flow_bwd_f32": 2,
-                "zsb_iaf_bwd_f32": 2,
+                "zsb_iaf_bwd_f32": 2, "zsb_lntm_mstep_grad_f32": 2,
                 "zsb_gp_cond_bwd_f32": 2, "zsb_conv3x3_wgrad_f32": 2,
                 # the GAN layers' entries, in their common case: a gather-split with its max
                 # pass, a sigmoid gradient with the bias sums

@@ -32,6 +32,12 @@ class AIS(object):
     ``run(noise=f)`` injects the HMC noise of step k as ``f(k)`` (k < n_adapt: adaptation
     iterations, then the temperature iterations) and ``init=[...]`` the two prior draws -- the
     parity surface against oracle/evaluation.py.
+
+    When ``meta_bn`` is a ``zs.fused.LNTMLogJoint`` on the kernels, the tempered log-joint, its
+    gradient and the t = 0 prior density all come from its fused kernel reading ``temperature``
+    on the device (``LNTMLogJoint.tempered``).  That assumes the proposal's log-joint is the eta
+    prior the LNTMLogJoint holds, as lntm_mcem.py:133-136 sets it; ``proposal_meta_bn`` still
+    gives the initial draws.
     """
 
     def __init__(self, meta_bn, proposal_meta_bn, hmc, observed, latent,
@@ -57,6 +63,9 @@ class AIS(object):
         def log_fn(obs):                                  # evaluation.py:91-94
             t = self._temp
             return log_prior(obs) * (1 - t) + log_joint(obs) * t
+        from .fused import LNTMLogJoint
+        if isinstance(meta_bn, LNTMLogJoint) and meta_bn.fused:
+            log_fn = meta_bn.tempered(self._temp)
         self.log_fn = log_fn
         self._observed = dict(observed)
         self.sample_op, self.hmc_info = hmc.sample(log_fn, observed, latent)

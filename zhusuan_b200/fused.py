@@ -393,8 +393,9 @@ class _BNNProvider(object):
 
 
 class LNTMLogJoint(object):
-    """E-step objective of the Logistic-Normal Topic Model, examples/topic_models/
-    lntm_mcem.py:33-48 with ``model.log_joint = e_obj`` (:97-99):
+    """Logistic-Normal Topic Model, examples/topic_models/lntm_mcem.py:33-48: the E-step objective
+    with ``model.log_joint = e_obj`` (:97-99), the M-step likelihood (:106-114) and AIS's tempered
+    log-joint (evaluation.py:91-94):
 
         eta [chains, docs, K] ~ Normal(eta_mean, exp(eta_logstd)), group_ndims=1
         log p = cond_log_prob('eta') + UnnormalizedMultinomial(log(softmax(eta) @ softmax(beta)),
@@ -406,8 +407,22 @@ class LNTMLogJoint(object):
     ``doc_word`` of the reference never exists (335 TB at BASELINE config 5).  As a plain callable
     it is the dense torch restatement of the reference graph (small shapes / cross-check).
 
-    x: dense [docs, V] counts (any float/int tensor); beta: [K, V] (fixed during the E-step; call
-    ``set_beta`` after every M-step); K in {16, 32, 64, 128}.
+    x: dense [n_docs, V] counts (any float/int tensor), the whole corpus; beta: [K, V] (fixed
+    during the E-step; call ``set_beta`` after every M-step); 1 <= K <= 128 on the kernels.  A CPU
+    ``beta`` or K > 128 leaves only the dense restatement: HMC then differentiates ``__call__``.
+
+    ``set_docs(doc_ids)`` selects a batch of corpus rows (a device int64 tensor of distinct rows,
+    or None for all of them) with no host sync: eta is then ``[chains, len(doc_ids), K]`` for the
+    E-step, the dense callable and ``cond_log_px``.  One training batch of the example::
+
+        lj.set_docs(ids)                               # ids = perm[t * 100:(t + 1) * 100]
+        eta.copy_(Eta[:, ids])
+        for _ in range(num_e_steps):
+            sample_op()                                # zs.HMC(...).sample(lj, {}, {"eta": eta})
+        Eta[:, ids] = eta
+        log_px = lj.cond_log_px(eta, beta).mean(0).sum()
+        log_p_beta = Normal(torch.zeros_like(beta), logstd=log_delta).log_prob(beta).sum()
+        (-(log_p_beta + log_px)).backward()            # then the Adam step on beta
     """
 
     def __init__(self, x, beta, eta_mean, eta_logstd, name="eta"):
@@ -424,35 +439,75 @@ class LNTMLogJoint(object):
         idx = nz.nonzero(as_tuple=False)                  # row-major: sorted by document
         self.word_idx = idx[:, 1].to(torch.int32).contiguous()
         self.word_cnt = self.x[idx[:, 0], idx[:, 1]].contiguous()
+        self.nnz = int(idx.shape[0])
+        # the same entries grouped by word, documents ascending (the M-step's fixed summation order)
+        order = torch.sort(idx[:, 1], stable=True)[1]
+        self.csc_entry = order.to(torch.int32).contiguous()
+        self.entry_doc = idx[order, 0].to(torch.int32).contiguous()
+        self.csc_ptr = torch.zeros(self.n_vocab + 1, dtype=torch.int64, device=dev)
+        self.csc_ptr[1:] = torch.cumsum(torch.bincount(idx[:, 1], minlength=self.n_vocab), 0)
         self.eta_mean = eta_mean.detach().to(torch.float32).contiguous()
         self.eta_logstd = eta_logstd.detach().to(torch.float32).contiguous()
         self.n_topics = int(beta.shape[0])
-        if self.n_topics not in (16, 32, 64, 128):
-            raise ValueError("LNTMLogJoint: n_topics must be 16, 32, 64 or 128")
-        self.phi_t = torch.empty((self.n_vocab, self.n_topics), dtype=torch.float32, device=dev)
+        if self.n_topics < 1:
+            raise ValueError("LNTMLogJoint: n_topics must be at least 1")
+        self.n_topics_padded = 16 * -(-self.n_topics // 16)
+        self.fused = dev.type == "cuda" and self.n_topics <= 128
+        self.set_docs(None)
         self.set_beta(beta)
-        self._zsb_fused = {"kind": "provider", "obj": self}
+        if self.fused:
+            self._zsb_fused = {"kind": "provider", "obj": self}
 
     def set_beta(self, beta):
+        """Take ``beta`` for the E-step: phi_t [V, Kp] = softmax(beta)^T with zero pad columns,
+        in a new buffer (a pending ``cond_log_px`` backward keeps the one it read)."""
         from ._lib import lib, ptr, stream
         self.beta = beta.detach().to(torch.float32).contiguous()
+        if not self.fused:
+            return
+        self.phi_t = torch.empty((self.n_vocab, self.n_topics_padded), dtype=torch.float32,
+                                 device=self.beta.device)
         lib.call("zsb_lntm_phi_t_f32", ptr(self.beta), self.n_topics, self.n_vocab,
                  ptr(self.phi_t), stream())
 
-    def _launch(self, eta, want_lp, want_grad):
-        from ._lib import lib, ptr, stream
-        eta = eta.detach()
-        if eta.dim() != 3 or int(eta.shape[1]) != self.n_docs or \
+    def set_docs(self, doc_ids):
+        """Work on corpus rows ``doc_ids`` (int64 tensor on the corpus' device, distinct rows) or,
+        for None, on every row.  No CSR rebuild and no host sync."""
+        if doc_ids is None:
+            self.doc_ids, self._doc_slot, self.n_batch = None, None, self.n_docs
+            return
+        if not isinstance(doc_ids, torch.Tensor) or doc_ids.dim() != 1 or \
+                doc_ids.dtype != torch.int64 or doc_ids.device != self.doc_ptr.device:
+            raise ValueError("doc_ids must be a 1-D int64 tensor on %s" % self.doc_ptr.device)
+        self.doc_ids = doc_ids.contiguous()
+        self.n_batch = int(doc_ids.shape[0])
+        # batch row of each corpus document, -1 outside the batch (the M-step skips those)
+        self._doc_slot = torch.full((self.n_docs,), -1, dtype=torch.int32,
+                                    device=doc_ids.device).scatter_(
+            0, self.doc_ids, torch.arange(self.n_batch, dtype=torch.int32,
+                                          device=doc_ids.device))
+
+    def _check_eta(self, eta):
+        if eta.dim() != 3 or int(eta.shape[1]) != self.n_batch or \
                 int(eta.shape[2]) != self.n_topics:
-            raise ValueError("eta must be [chains, %d, %d]" % (self.n_docs, self.n_topics))
-        eta = eta.to(torch.float32).contiguous()
+            raise ValueError("eta must be [chains, %d, %d]" % (self.n_batch, self.n_topics))
+        return eta.detach().to(torch.float32).contiguous()
+
+    def _launch(self, eta, want_lp, want_grad, temperature=None):
+        from ._lib import lib, ptr, stream
+        if not self.fused:
+            raise ValueError("LNTMLogJoint: the fused kernels need 1 <= n_topics <= 128 and a "
+                             "CUDA beta (got %d topics on %s); call the object for the dense "
+                             "log-joint" % (self.n_topics, self.beta.device))
+        eta = self._check_eta(eta)
         chains = int(eta.shape[0])
-        lp = torch.empty((chains, self.n_docs), dtype=torch.float32, device=eta.device) \
+        lp = torch.empty((chains, self.n_batch), dtype=torch.float32, device=eta.device) \
             if want_lp else None
         g = torch.empty_like(eta) if want_grad else None
         lib.call("zsb_lntm_logjoint_f32", ptr(eta), ptr(self.eta_mean), ptr(self.eta_logstd),
                  ptr(self.phi_t), ptr(self.doc_ptr), ptr(self.word_idx), ptr(self.word_cnt),
-                 ptr(lp), ptr(g), chains, self.n_docs, self.n_topics, stream())
+                 ptr(self.doc_ids), ptr(temperature), ptr(lp), ptr(g), chains, self.n_batch,
+                 self.n_topics, stream())
         return lp, g
 
     # provider interface used by HMC's generic path instead of autograd
@@ -462,17 +517,96 @@ class LNTMLogJoint(object):
     def grad(self, var_list):
         return [self._launch(var_list[0], False, True)[1]]
 
+    def tempered(self, temperature):
+        """The provider of ``prior + t * likelihood`` for a 0-d float32 device tensor ``t`` read
+        by the kernel at every call: AIS's log-joint ``log_prior * (1 - t) + log_joint * t``
+        (evaluation.py:91-94) when the proposal's log-joint is this object's eta prior."""
+        return _LNTMTempered(self, temperature)
+
+    def _batch_x(self):
+        return self.x if self.doc_ids is None else self.x.index_select(0, self.doc_ids)
+
+    def _dense_log_px(self, eta, beta):
+        theta = torch.softmax(eta, -1)
+        phi = torch.softmax(beta, -1)
+        doc_word = theta.reshape(-1, self.n_topics) @ phi
+        doc_word = doc_word.reshape(tuple(eta.shape[:-1]) + (self.n_vocab,))
+        return (self._batch_x().to(doc_word.dtype) * torch.log(doc_word)).sum(-1)
+
+    def cond_log_px(self, eta, beta):
+        """log p(x_d | eta_c, beta) [chains, B] of the selected documents (the reference's
+        ``cond_log_prob('x')``, lntm_mcem.py:106-110), differentiable w.r.t. ``beta`` only: eta
+        is a constant, as ``var_list=[beta]`` makes it.  Refreshes phi_t from ``beta``.  On the
+        kernels (zsb_lntm_mstep_f32, and zsb_lntm_mstep_grad_f32 for the gradient) nothing
+        [chains * B, V]-sized is formed; a float64 or CPU ``beta``, or K > 128, takes the dense
+        restatement."""
+        eta = eta.detach()
+        if not (self.fused and beta.dtype == torch.float32 and beta.is_cuda):
+            return self._dense_log_px(eta.to(beta.dtype), beta)
+        self.set_beta(beta)
+        return _LNTMLogPx.apply(beta, self._check_eta(eta), self)
+
     def __call__(self, observed):
         """Dense restatement of the reference graph in torch (lntm_mcem.py:33-48)."""
         eta = observed[self.name]
-        theta = torch.softmax(eta, -1)
-        phi = torch.softmax(self.beta, -1)
-        doc_word = theta.reshape(-1, self.n_topics) @ phi
-        doc_word = doc_word.reshape(tuple(eta.shape[:-1]) + (self.n_vocab,))
         prec = torch.exp(-2 * self.eta_logstd)
         prior = (-0.5 * math.log(2 * math.pi) - self.eta_logstd
                  - 0.5 * prec * (eta - self.eta_mean) ** 2).sum(-1)
-        return prior + (self.x * torch.log(doc_word)).sum(-1)
+        return prior + self._dense_log_px(eta, self.beta)
+
+
+class _LNTMTempered(object):
+    """HMC's provider interface (and the callable AIS evaluates at t = 0) over
+    ``LNTMLogJoint.tempered``: zsb_lntm_logjoint_f32 with a device temperature."""
+
+    def __init__(self, obj, temperature):
+        self.obj, self.temperature = obj, temperature
+        self._zsb_fused = {"kind": "provider", "obj": self}
+
+    def logp(self, var_list):
+        return self.obj._launch(var_list[0], True, False, self.temperature)[0]
+
+    def grad(self, var_list):
+        return [self.obj._launch(var_list[0], False, True, self.temperature)[1]]
+
+    def __call__(self, observed):
+        return self.logp([observed[self.obj.name]])
+
+
+class _LNTMLogPx(torch.autograd.Function):
+    """lp [chains, B] of LNTMLogJoint.cond_log_px on zsb_lntm_mstep_f32; backward is
+    zsb_lntm_mstep_grad_f32 on the theta / ratio the forward wrote."""
+
+    @staticmethod
+    def forward(ctx, beta, eta, obj):
+        from ._lib import lib, ptr, stream
+        chains, dev = int(eta.shape[0]), eta.device
+        lp = torch.empty((chains, obj.n_batch), dtype=torch.float32, device=dev)
+        ratio = torch.empty((chains, obj.nnz), dtype=torch.float32, device=dev)
+        theta = torch.empty((chains, obj.n_batch, obj.n_topics_padded), dtype=torch.float32,
+                            device=dev)
+        lib.call("zsb_lntm_mstep_f32", ptr(eta), ptr(obj.phi_t), ptr(obj.doc_ptr),
+                 ptr(obj.word_idx), ptr(obj.word_cnt), ptr(obj.doc_ids), ptr(lp), ptr(ratio),
+                 ptr(theta), chains, obj.n_batch, obj.nnz, obj.n_topics, stream())
+        ctx.obj, ctx.phi_t, ctx.doc_slot = obj, obj.phi_t, obj._doc_slot
+        ctx.save_for_backward(ratio, theta)
+        return lp
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, glp):
+        from ._lib import lib, ptr, stream
+        obj = ctx.obj
+        ratio, theta = ctx.saved_tensors
+        glp = glp.to(torch.float32).contiguous()
+        G = torch.empty((obj.n_vocab, obj.n_topics_padded), dtype=torch.float32,
+                        device=glp.device)
+        dbeta = torch.empty((obj.n_topics, obj.n_vocab), dtype=torch.float32, device=glp.device)
+        lib.call("zsb_lntm_mstep_grad_f32", ptr(glp), ptr(ratio), ptr(theta), ptr(ctx.phi_t),
+                 ptr(obj.csc_ptr), ptr(obj.csc_entry), ptr(obj.entry_doc), ptr(ctx.doc_slot),
+                 ptr(G), ptr(dbeta), int(glp.shape[0]), int(glp.shape[1]), obj.nnz,
+                 obj.n_topics, obj.n_vocab, stream())
+        return dbeta, None, None
 
 
 def _as_numpy(a, dtype):
