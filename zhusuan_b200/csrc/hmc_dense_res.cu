@@ -217,10 +217,17 @@ __device__ __forceinline__ void epilogue_planes(const ResEpi& a, uint32_t trow, 
 }
 
 
-// the TMA producer's copy of "this pass reads the spare planes", read from global memory once
-__device__ __forceinline__ int& producer_spare_in() {
-  __shared__ int spare_in;
-  return spare_in;
+// What the TMA producer loads: whether this pass reads the spare planes (read from global memory
+// once), and the first dimension and chain of its current unit, worked out before the unit's first
+// k-block (kb_range starts every unit at 0).  The tensor cores wait on the one producer thread for
+// every k-block, and tile()'s 64-bit division by the run-time number of dimension blocks, done per
+// k-block, made the benchmark's pass about 6% slower on an H100 (README).
+struct ProducerState {
+  int spare_in, n0, c0;
+};
+__device__ __forceinline__ ProducerState& producer_state() {
+  __shared__ ProducerState ps;
+  return ps;
 }
 
 // CX x CY: a cluster takes CX dimension blocks of CY chain blocks.  Its CX CTAs on one chain block
@@ -264,16 +271,20 @@ struct ResW {
     tma_prefetch_desc(&m_phi); tma_prefetch_desc(&m_plo);
     tma_prefetch_desc(&m_qhi); tma_prefetch_desc(&m_qlo);
     tma_prefetch_desc(&m_shi); tma_prefetch_desc(&m_slo);
-    producer_spare_in() = plane_spare_in(scales, pass);   // prefetch runs on the producer thread
+    producer_state().spare_in = plane_spare_in(scales, pass);   // prefetch runs on the producer
   }
   __device__ __forceinline__ void load(int64_t u, int kb, uint32_t sa, uint32_t fb) const {
     using C = Cfg<RB>;
-    int nb;
-    int64_t cb;
-    tile(u, nb, cb);
-    const int n0 = nb * BM;
-    const int c0 = (int)cb * BN;
-    const bool s = producer_spare_in() != 0;
+    ProducerState& ps = producer_state();
+    if (kb == 0) {
+      int nb;
+      int64_t cb;
+      tile(u, nb, cb);
+      ps.n0 = nb * BM;
+      ps.c0 = (int)cb * BN;
+    }
+    const int n0 = ps.n0, c0 = ps.c0;
+    const bool s = ps.spare_in != 0;
     const CUtensorMap* qh = s ? &m_shi : &m_qhi;
     const CUtensorMap* ql = s ? &m_slo : &m_qlo;
     const int r = (int)(u % CLUSTER), rx = r % CX, ry = r / CX;   // this CTA's cluster rank
