@@ -175,8 +175,11 @@ int zsb_linear_tc_f32(int epi, const void* w_planes, const float* scale_w, const
                       const float* scale_h, const float* bias, const float* x_obs, int64_t n_x,
                       const float* gout, float* out, float* part, int64_t R, int J, int K,
                       int relu, void* stream);
-/* As zsb_linear_tc_f32, additionally folding max |out| (epi 0 / 2) into amax_scale[2] so that the
- * consumer's operand split (zsb_split16_dual_f32, have_amax = 1) needs no pass over `out`. */
+/* As zsb_linear_tc_f32, additionally folding max |out| (epi 0 / 2 / 16) into amax_scale[2] so that
+ * the consumer's operand split (zsb_split16_dual_f32, have_amax = 1) needs no pass over `out`.
+ *   epi 16: out [R, J] = act(h W^T + bias + x) with the residual x [R, J] (n_x = R) added before
+ *           the ReLU: tf.layers.conv2d(..., activation=relu) of a resnet block whose shortcut is
+ *           added first (vae_conv.py:39-53), on the im2col planes of zsb_conv_gather_split_f32 */
 int zsb_linear_tc_amax_f32(int epi, const void* w_planes, const float* scale_w,
                            const void* h_planes, const float* scale_h, const float* bias,
                            const float* x_obs, int64_t n_x, const float* gout, float* out,
@@ -723,17 +726,26 @@ int zsb_conv_gather_split_f32(const float* x, int64_t N, int64_t Hb, int64_t Wb,
  *          moments, for zsb_bn_finish_fused_f32 (out unused)
  *   epi 3: batch norm evaluation: out = act(xhat gamma + beta), xhat = (sum - moving_mean)
  *          rsqrt(moving_var + eps); stats [2][C] = (moving_mean, rstd); pre (may be NULL) = sum
- * max |out| into amax_scale[2] (may be NULL; epi 0, 1, 3). */
+ *   epi 4: out = act(sum + bias[c] + residual) with bias [C] and residual [N, Hb, Wb, C] (either
+ *          may be NULL): the transposed convolution of examples/utils/utils.py:74-113 with the
+ *          resnet blocks' residual added before the ReLU (vae_conv.py:20-36)
+ * act = ReLU if relu (epi 3, 4).  max |out| into amax_scale[2] (may be NULL; epi 0, 1, 3, 4). */
 int zsb_conv_col2im_f32(int epi, const float* cols, int64_t N, int64_t Hb, int64_t Wb, int64_t C,
                         int64_t Hs, int64_t Ws, int k, int stride, int pt, int pl,
-                        const float* bias, const float* gamma, const float* beta,
-                        const float* moving_mean, const float* moving_var, float eps, int relu,
-                        float* stats, float* pre, float* part, float* out, float* amax_scale,
-                        void* stream);
+                        const float* bias, const float* residual, const float* gamma,
+                        const float* beta, const float* moving_mean, const float* moving_var,
+                        float eps, int relu, float* stats, float* pre, float* part, float* out,
+                        float* amax_scale, void* stream);
 /* Backward through a sigmoid output y [R, C]: gp = g y (1 - y), max |gp| into scale[2], and db [C]
  * (may be NULL) = the column sums of gp, merged in a fixed order from part [ceil(R / 128)][C]. */
 int zsb_conv_sigmoid_grad_f32(const float* g, const float* y, int64_t R, int C, float* gp,
                               float* part, float* db, float* scale, void* stream);
+/* Backward through relu?(conv + b + residual) with output y [R, C] (the tf.gradients of the ReLU,
+ * bias_add and residual add of vae_conv.py:20-53): gp = g (y > 0), or g when relu = 0 (y may then
+ * be NULL), which is the residual's gradient; max |gp| into scale[2], and db [C] (may be NULL) = the
+ * column sums of gp, merged in a fixed order from part [ceil(R / 128)][C].  C < 2^20. */
+int zsb_conv_relu_grad_f32(const float* g, const float* y, int64_t R, int C, int relu, float* gp,
+                           float* part, float* db, float* scale, void* stream);
 
 /* ---- K5: SG-MCMC updates (zhusuan/sgmcmc.py) ------------------------------------------------ */
 int zsb_sgmcmc_parts(void);   /* capacity (floats) of every `part` scratch */

@@ -1,25 +1,33 @@
 """Convolutional VAE (examples/variational_autoencoders/vae_conv.py) on zs.fused.conv2d /
-conv2d_transpose against cuDNN convolutions with the same SAME padding, on seeded synthetic data.
+conv2d_transpose and on zs.fused.conv2d_tc / conv2d_transpose_tc against cuDNN convolutions with
+the same SAME padding, on seeded synthetic data.
 Arms (alternating in one process; dense layers are zs.fused.linear in every arm):
-  fused       zs.fused.conv2d / conv2d_transpose: one launch per layer, bias, residual and ReLU fused
+  fused       zs.fused.conv2d / conv2d_transpose (FFMA): one launch per layer, bias, residual and
+              ReLU fused; 3 x 3 kernels and 1 - 64 channels only, so it prints nothing elsewhere
+  fused_tc    zs.fused.conv2d_tc / conv2d_transpose_tc: the tensor-core products with the gather
+              split, col2im, bias, residual and ReLU passes around them
   cudnn_fp32  F.conv2d / F.conv_transpose2d with the asymmetric pads, allow_tf32 = False, then
               bias, residual add and ReLU as separate ops: the accuracy-matched arm
   cudnn_tf32  the same with torch's defaults (cuDNN in TF32): NOT accuracy-matched
-Cases:
-  {enc,dec}_{plain,resize}_{fwd,fwdbwd}_{128,4096}  one resnet block of the example (nf = 16):
-      enc_plain 28x28x16 -> 28x28x16, enc_resize 28x28x16 -> 14x14x32,
-      dec_plain 28x28x16 -> 28x28x16, dec_resize 14x14x32 -> 28x28x16
+Cases (nf = 16 unless --nf says otherwise):
+  {enc,dec}_{plain,resize}_{fwd,fwdbwd}_{128,4096}  one resnet block of the example:
+      enc_plain 28x28xnf -> 28x28xnf, enc_resize 28x28xnf -> 14x14x2nf,
+      dec_plain 28x28xnf -> 28x28xnf, dec_resize 14x14x2nf -> 28x28xnf
+  layer_{conv,deconv}_{k3c128,k5c64}_{fwd,fwdbwd}_4096  one stride-1 SAME layer with bias and ReLU
+      outside the FFMA range: 3 x 3 with 128 -> 128 channels and 5 x 5 with 64 -> 64, at 14 x 14
   train_step   one training step at 128 images (bound, sgvb().backward(), Adam(1e-4, beta1 0.5))
   test_bound   the bound over 400 images without a gradient
   generate     x_mean of 100 images from the prior
 Each prints the median, min and max over windows and the CUDA-event time of one call
 (`stream_ms`); launches per call and conv-kernel device time come from a separate torch.profiler
-pass, checked against the conv kernels the library launched: when the profiler recorded a
+pass, checked against the FFMA conv kernels the library launched: when the profiler recorded a
 different number of them (`conv_kernels_profiled` against `conv_kernels_launched`),
-`profile_complete` is false and its device columns are null.
+`profile_complete` is false and its device columns are null.  In the fused_tc arm the conv device
+time counts every tensor-core product, so in train_step, test_bound and generate it includes the
+products of the dense layers too.
 FLOPs and bytes of the convolutions are computed from the shapes.  One JSON line per case and arm, with the card's name and power limit.
 
-    python scripts/bench_vae_conv.py [--windows 7] [--steps 20] [--cases a,b]
+    python scripts/bench_vae_conv.py [--windows 7] [--steps 20] [--cases a,b] [--nf 16]
 """
 import argparse
 import json
@@ -36,7 +44,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import zhusuan_b200 as zs  # noqa: E402
 
 NF, Z_DIM = 16, 32
-ARMS = ("fused", "cudnn_fp32", "cudnn_tf32")
+ARMS = ("fused", "fused_tc", "cudnn_fp32", "cudnn_tf32")
 
 
 def card():
@@ -49,14 +57,19 @@ def card():
     return name, power
 
 
-def _pads(big, small, s):
-    total = max((small - 1) * s + 3 - big, 0)
+def _pads(big, small, s, k=3):
+    total = max((small - 1) * s + k - big, 0)
     return total // 2, total - total // 2
 
 
 class Fused(object):
     conv = staticmethod(zs.fused.conv2d)
     deconv = staticmethod(zs.fused.conv2d_transpose)
+
+
+class FusedTC(object):
+    conv = staticmethod(zs.fused.conv2d_tc)
+    deconv = staticmethod(zs.fused.conv2d_transpose_tc)
 
 
 class Cudnn(object):
@@ -67,9 +80,9 @@ class Cudnn(object):
 
     def conv(self, x, W, b=None, stride=1, relu=False, residual=None):
         torch.backends.cudnn.allow_tf32 = self.tf32
-        H, Wd = int(x.shape[-3]), int(x.shape[-2])
+        H, Wd, k = int(x.shape[-3]), int(x.shape[-2]), int(W.shape[0])
         Ho, Wo = -(-H // stride), -(-Wd // stride)
-        (pt, pb), (pl, pr) = _pads(H, Ho, stride), _pads(Wd, Wo, stride)
+        (pt, pb), (pl, pr) = _pads(H, Ho, stride, k), _pads(Wd, Wo, stride, k)
         xc = x.reshape((-1,) + tuple(x.shape[-3:])).permute(0, 3, 1, 2)
         if pt == pb and pl == pr:
             y = F.conv2d(xc, W.permute(3, 2, 0, 1), stride=stride, padding=(pt, pl))
@@ -79,9 +92,9 @@ class Cudnn(object):
 
     def deconv(self, x, W, out_shape, stride=1, b=None, relu=False, residual=None):
         torch.backends.cudnn.allow_tf32 = self.tf32
-        Ho, Wo = int(out_shape[0]), int(out_shape[1])
-        pt, _ = _pads(Ho, int(x.shape[-3]), stride)
-        pl, _ = _pads(Wo, int(x.shape[-2]), stride)
+        Ho, Wo, k = int(out_shape[0]), int(out_shape[1]), int(W.shape[0])
+        pt, _ = _pads(Ho, int(x.shape[-3]), stride, k)
+        pl, _ = _pads(Wo, int(x.shape[-2]), stride, k)
         xc = x.reshape((-1,) + tuple(x.shape[-3:])).permute(0, 3, 1, 2)
         y = F.conv_transpose2d(xc, W.permute(3, 2, 0, 1), stride=stride)
         return self._epilogue(y[:, :, pt:pt + Ho, pl:pl + Wo].permute(0, 2, 3, 1), b, relu,
@@ -97,7 +110,9 @@ class Cudnn(object):
 
 
 def make_ops(arm):
-    return Fused() if arm == "fused" else Cudnn(arm == "cudnn_tf32")
+    if arm in ("fused", "fused_tc"):
+        return Fused() if arm == "fused" else FusedTC()
+    return Cudnn(arm == "cudnn_tf32")
 
 
 # ---- the example's blocks (vae_conv.py:20-53) ------------------------------------------------------
@@ -120,9 +135,19 @@ def deconv_resnet_block(ops, h, ps, out_shape, resize):
     return ops.deconv(t, ps[2], out_shape, 2, b=ps[3], relu=True, residual=r)
 
 
-ENC = [(NF, False), (2 * NF, True), (2 * NF, False), (2 * NF, True), (2 * NF, False)]
-DEC = [((7, 7, 2 * NF), False), ((14, 14, 2 * NF), True), ((14, 14, 2 * NF), False),
-       ((28, 28, NF), True), ((28, 28, NF), False)]
+def set_nf(nf):
+    """The example's filter count: the encoder / decoder blocks and the block cases."""
+    global NF, ENC, DEC, BLOCKS
+    NF = nf
+    ENC = [(NF, False), (2 * NF, True), (2 * NF, False), (2 * NF, True), (2 * NF, False)]
+    DEC = [((7, 7, 2 * NF), False), ((14, 14, 2 * NF), True), ((14, 14, 2 * NF), False),
+           ((28, 28, NF), True), ((28, 28, NF), False)]
+    BLOCKS = {   # name: (transpose, resize, in [H, W, C], out [H, W, C])
+        "enc_plain": (False, False, (28, 28, NF), (28, 28, NF)),
+        "enc_resize": (False, True, (28, 28, NF), (14, 14, 2 * NF)),
+        "dec_plain": (True, False, (28, 28, NF), (28, 28, NF)),
+        "dec_resize": (True, True, (14, 14, 2 * NF), (28, 28, NF)),
+    }
 
 
 def _param(g, shape, fan_in=None):
@@ -202,16 +227,13 @@ def example(ops, x, q, p):
 
 # ---- cases -------------------------------------------------------------------------------------
 
-BLOCKS = {   # name: (transpose, resize, in [H, W, C], out [H, W, C])
-    "enc_plain": (False, False, (28, 28, NF), (28, 28, NF)),
-    "enc_resize": (False, True, (28, 28, NF), (14, 14, 2 * NF)),
-    "dec_plain": (True, False, (28, 28, NF), (28, 28, NF)),
-    "dec_resize": (True, True, (14, 14, 2 * NF), (28, 28, NF)),
-}
+set_nf(NF)
+LAYERS = {"k3c128": (3, 128), "k5c64": (5, 64)}   # single layers at 14 x 14: (k, channels)
+LAYER_HW = 14
 
 
 def model_layers(encoder, decoder_):
-    """(Cin, Cout, small pixels) of every convolution of the example."""
+    """(Cin, Cout, small pixels) of every (3 x 3) convolution of the example."""
     out = []
     if encoder:
         out.append((1, NF, 784))
@@ -236,9 +258,9 @@ def model_layers(encoder, decoder_):
     return out
 
 
-def conv_cost(layers, R, backward):
-    flops = sum(2 * 9 * ci * co * px * R for ci, co, px in layers)
-    byts = sum(4 * (R * px * (ci + 2 * co) + 9 * ci * co) for ci, co, px in layers)
+def conv_cost(layers, R, backward, k=3):
+    flops = sum(2 * k * k * ci * co * px * R for ci, co, px in layers)
+    byts = sum(4 * (R * px * (ci + 2 * co) + k * k * ci * co) for ci, co, px in layers)
     return (3 * flops, 3 * byts) if backward else (flops, byts)
 
 
@@ -272,10 +294,12 @@ def case_fn(case, arm):
         return step, conv_cost(model_layers(True, True), n, True)
     block, kind, R = case.rsplit("_", 2)
     R = int(R)
+    backward = kind == "fwdbwd"
+    if block.startswith("layer_"):
+        return layer_case(ops, g, block, R, backward)
     transpose, resize, (hi, wi, ci), out = BLOCKS[block]
     ps = block_params(g, ci, out[2], resize, transpose)
     h = torch.randn(R, hi, wi, ci, generator=g, device="cuda")
-    backward = kind == "fwdbwd"
     if backward:
         h.requires_grad_(True)
 
@@ -297,6 +321,28 @@ def case_fn(case, arm):
     return run, conv_cost(layers, R, backward)
 
 
+def layer_case(ops, g, name, R, backward):
+    """One stride-1 SAME layer with bias and ReLU: layer_{conv,deconv}_{k3c128,k5c64}."""
+    _, kind, size = name.split("_")
+    k, c = LAYERS[size]
+    W = _param(g, (k, k, c, c), k * k * c)
+    b = _param(g, (c,))
+    h = torch.randn(R, LAYER_HW, LAYER_HW, c, generator=g, device="cuda")
+    if backward:
+        h.requires_grad_(True)
+
+    def run():
+        with torch.set_grad_enabled(backward):
+            if kind == "deconv":
+                y = ops.deconv(h, W, (LAYER_HW, LAYER_HW, c), 1, b=b, relu=True)
+            else:
+                y = ops.conv(h, W, b, 1, True)
+            if backward:
+                torch.autograd.grad(y.sum(), [h, W, b])
+        return y
+    return run, conv_cost([(c, c, LAYER_HW * LAYER_HW)], R, backward, k)
+
+
 def model_layers_block(block):
     transpose, resize, (hi, wi, ci), (ho, wo, co) = BLOCKS[block]
     small = min(hi * wi, ho * wo)
@@ -311,9 +357,10 @@ CONV_NAMES = ("conv3x3", "conv", "cudnn", "xmma", "implicit", "dgrad", "wgrad", 
               "winograd", "fft")
 
 
-def profile(fn):
-    """(kernel launches, device ms of all kernels, device ms of convolution kernels, conv kernels
-    the library launched, conv kernels the profiler recorded) of one call."""
+def profile(fn, arm):
+    """(kernel launches, device ms of all kernels, device ms of convolution kernels, FFMA conv
+    kernels the library launched, FFMA conv kernels the profiler recorded) of one call.  In the
+    fused_tc arm every tensor-core product counts as a convolution kernel."""
     from torch.profiler import profile as prof_, ProfilerActivity
     from zhusuan_b200._lib import lib
     fn()
@@ -335,8 +382,9 @@ def profile(fn):
     evs = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
     seen = sum(1 for e in evs if "conv3x3" in e.name)
     total = sum(e.device_time_total for e in evs) / 1e3
+    names = CONV_NAMES + (("tc_pipeline_kernel",) if arm == "fused_tc" else ())
     conv = sum(e.device_time_total for e in evs
-               if any(k in e.name.lower() for k in CONV_NAMES)
+               if any(k in e.name.lower() for k in names)
                and "zsb_linear" not in e.name and "split16" not in e.name) / 1e3
     return len(evs), round(total, 4), round(conv, 4), launched[0], seen
 
@@ -362,7 +410,17 @@ def all_cases():
         for kind in ("fwd", "fwdbwd"):
             for R in (128, 4096):
                 out.append("%s_%s_%d" % (block, kind, R))
+    for layer in ("conv_k3c128", "deconv_k3c128", "conv_k5c64", "deconv_k5c64"):
+        for kind in ("fwd", "fwdbwd"):
+            out.append("layer_%s_%s_4096" % (layer, kind))
     return out + ["train_step", "test_bound", "generate"]
+
+
+def fused_supports(case):
+    """The FFMA layers take 3 x 3 kernels and at most 64 channels."""
+    if case.startswith("layer_"):
+        return False
+    return 2 * NF <= 64
 
 
 def main():
@@ -370,13 +428,17 @@ def main():
     ap.add_argument("--windows", type=int, default=7)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--cases", default=",".join(all_cases()))
+    ap.add_argument("--nf", type=int, default=NF, help="the example's filter count (16)")
     args = ap.parse_args()
+    set_nf(args.nf)
     assert torch.cuda.is_available(), "bench_vae_conv.py measures on a CUDA device"
     name, power = card()
     tf32_default = torch.backends.cudnn.allow_tf32
     for case in args.cases.split(","):
         fns, costs = {}, {}
         for arm in ARMS:
+            if arm == "fused" and not fused_supports(case):
+                continue
             fns[arm], costs[arm] = case_fn(case, arm)
         for fn in fns.values():
             for _ in range(3):
@@ -393,11 +455,11 @@ def main():
                 times[arm].append((time.perf_counter() - t0) / args.steps * 1e3)
         for arm, fn in fns.items():
             ts = sorted(times[arm])
-            launches, dev_ms, conv_ms, zsb, seen = profile(fn)
+            launches, dev_ms, conv_ms, zsb, seen = profile(fn, arm)
             complete = seen == zsb
             flops, byts = costs[arm]
             print(json.dumps({
-                "case": case, "arm": arm, "accuracy_matched": arm != "cudnn_tf32",
+                "case": case, "arm": arm, "nf": NF, "accuracy_matched": arm != "cudnn_tf32",
                 "ms_median": round(ts[len(ts) // 2], 4), "ms_min": round(ts[0], 4),
                 "ms_max": round(ts[-1], 4), "stream_ms": stream_ms(fn),
                 "launches_per_call": launches, "conv_kernels_launched": zsb,

@@ -91,9 +91,10 @@ class _Lib(object):
                 "zsb_split16_pad_f32": 3, "zsb_linear_tc_f32": 2, "zsb_planar_flow_bwd_f32": 2,
                 "zsb_iaf_bwd_f32": 2, "zsb_lntm_mstep_grad_f32": 2,
                 "zsb_gp_cond_bwd_f32": 2, "zsb_conv3x3_wgrad_f32": 2,
-                # the GAN layers' entries, in their common case: a gather-split with its max
-                # pass, a sigmoid gradient with the bias sums
+                # the tensor-core conv layers' entries, in their common case: a gather-split
+                # with its max pass, a sigmoid or ReLU gradient with the bias sums
                 "zsb_conv_gather_split_f32": 3, "zsb_conv_sigmoid_grad_f32": 2,
+                "zsb_conv_relu_grad_f32": 2,
                 # the batch-norm entries in training
                 "zsb_linear_tc_bn_f32": 3, "zsb_bn_finish_fused_f32": 2, "zsb_bn_grad_f32": 5,
                 "zsb_bn_grad_f32out": 3}

@@ -14,23 +14,12 @@
 //                 tap) entries that land on each big pixel, gathered in a fixed tap order (kh, then
 //                 kw, ascending): no atomics, deterministic.  Epilogues: none, bias + sigmoid, batch
 //                 norm training (pre-activation + per-128-row moment partials for the merge of
-//                 zsb_bn_finish_fused_f32) and batch norm evaluation.
-#include "tc_common.cuh"
+//                 zsb_bn_finish_fused_f32), batch norm evaluation, and bias + residual + ReLU
+//                 (epi 4, whose kernel is in conv_bias.cu with the other passes of the biased
+//                 layers).
+#include "conv_tc.cuh"
 
 namespace {
-
-constexpr int TILE = 128;        // rows per moment partial (the dense products' row tile)
-
-struct Geo {
-  int64_t N, Hb, Wb, Hs, Ws;
-  int C, k, s, pt, pl;
-};
-
-inline unsigned blocks_for(int64_t n, int64_t per, int per_sm) {
-  int64_t b = zsb_ceil_div(n, per);
-  if (b > ZSB_NUM_SMS * per_sm) b = ZSB_NUM_SMS * per_sm;
-  return (unsigned)(b < 1 ? 1 : b);
-}
 
 // scale[2] = running max |x| bits (NaN and inf skipped)
 __global__ void __launch_bounds__(256) conv_absmax_kernel(const float* __restrict__ x, int64_t n,
@@ -75,31 +64,6 @@ __global__ void __launch_bounds__(256) gather_split_kernel(const float* __restri
       store_hilo(planes + r * Kp + col, n_pl, v * sc);
     }
   }
-}
-
-// y[n, y, x, c] = sum over the taps (kh, kw) with s i + kh - pt = y, s j + kw - pl = x of
-// cols[(n Hs + i) Ws + j, (kh k + kw) C + c], kh then kw ascending
-__device__ __forceinline__ float col2im_at(const float* __restrict__ cols, const Geo& g,
-                                           int64_t r, int c) {
-  const int64_t xo = r % g.Wb, t = r / g.Wb;
-  const int64_t yo = t % g.Hb, n = t / g.Hb;
-  const int64_t KK = (int64_t)g.k * g.k * g.C;
-  const int64_t ny0 = yo + g.pt, nx0 = xo + g.pl;
-  float acc = 0.f;
-  for (int kh = (int)(ny0 % g.s); kh < g.k; kh += g.s) {
-    const int64_t ny = ny0 - kh;
-    if (ny < 0) break;
-    const int64_t i = ny / g.s;
-    if (i >= g.Hs) continue;
-    for (int kw = (int)(nx0 % g.s); kw < g.k; kw += g.s) {
-      const int64_t nx = nx0 - kw;
-      if (nx < 0) break;
-      const int64_t j = nx / g.s;
-      if (j >= g.Ws) continue;
-      acc += cols[((n * g.Hs + i) * g.Ws + j) * KK + (int64_t)(kh * g.k + kw) * g.C + c];
-    }
-  }
-  return acc;
 }
 
 // Flat epilogues over the N Hb Wb x C outputs:
@@ -258,6 +222,11 @@ int check_geo(const Geo& g, const char* what) {
 
 }  // namespace
 
+int conv_col_sum_merge_launch(const float* part, int64_t n_t, int C, float* db, cudaStream_t st) {
+  col_sum_merge_kernel<<<(unsigned)((C + 7) / 8), 256, 0, st>>>(part, n_t, C, db);
+  return zsb_check_launch("conv_col_sum_merge");
+}
+
 extern "C" {
 
 int zsb_conv_gather_split_f32(const float* x, int64_t N, int64_t Hb, int64_t Wb, int64_t C,
@@ -282,21 +251,24 @@ int zsb_conv_gather_split_f32(const float* x, int64_t N, int64_t Hb, int64_t Wb,
 
 int zsb_conv_col2im_f32(int epi, const float* cols, int64_t N, int64_t Hb, int64_t Wb, int64_t C,
                         int64_t Hs, int64_t Ws, int k, int stride, int pt, int pl,
-                        const float* bias, const float* gamma, const float* beta,
-                        const float* moving_mean, const float* moving_var, float eps, int relu,
-                        float* stats, float* pre, float* part, float* out, float* amax_scale,
-                        void* stream) {
-  ZSB_REQUIRE(cols && epi >= 0 && epi <= 3, "zsb_conv_col2im_f32: bad args");
+                        const float* bias, const float* residual, const float* gamma,
+                        const float* beta, const float* moving_mean, const float* moving_var,
+                        float eps, int relu, float* stats, float* pre, float* part, float* out,
+                        float* amax_scale, void* stream) {
+  ZSB_REQUIRE(cols && epi >= 0 && epi <= 4, "zsb_conv_col2im_f32: bad args");
   ZSB_REQUIRE(epi != 1 || (bias && out), "zsb_conv_col2im_f32: epi 1 needs bias and out");
   ZSB_REQUIRE(epi != 2 || (pre && part), "zsb_conv_col2im_f32: epi 2 needs pre and part");
   ZSB_REQUIRE(epi != 3 || (gamma && beta && moving_mean && moving_var && stats && out),
               "zsb_conv_col2im_f32: epi 3 needs gamma, beta, the moving statistics and stats");
-  ZSB_REQUIRE(epi != 0 || out, "zsb_conv_col2im_f32: out missing");
+  ZSB_REQUIRE((epi != 0 && epi != 4) || out, "zsb_conv_col2im_f32: out missing");
   ZSB_REQUIRE(C > 0 && C < (1 << 20), "zsb_conv_col2im_f32: bad channel count");
   const Geo g{N, Hb, Wb, Hs, Ws, (int)C, k, stride, pt, pl};
   int rc = check_geo(g, "zsb_conv_col2im_f32");
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
+  if (epi == 4)
+    return conv_col2im_bias_launch(cols, N, Hb, Wb, (int)C, Hs, Ws, k, stride, pt, pl, bias,
+                                   residual, relu, out, amax_scale, st);
   if (epi == 2) {
     const int64_t n_t = zsb_ceil_div(N * Hb * Wb, TILE);
     col2im_bn_train_kernel<<<dim3((unsigned)n_t, (unsigned)((C + 31) / 32)), 256, 0, st>>>(

@@ -9,6 +9,9 @@
 //          = Bernoulli(logits = l).log_prob(x) summed over the feature axis (univariate.py:398-403
 //            + group_ndims = 1, base.py:303-304) once the partial rows are added up
 //   EPI 2  out[r, j] = g[r] * (x - sigmoid(l))                   d(sum_r g[r] * log_prob[r]) / dl
+//   EPI 16 out[r, j] = act(l + res[r, j])                         biased layer with a residual added
+//          before the ReLU (the resnet blocks of vae_conv.py:39-53); res [R, J] is read through the
+//          observation loads of EPI 1 (x_obs = res, n_x = R)
 //
 // fp32 accuracy on fp16 tensor cores: both operands are pre-split into scaled fp16 hi + lo planes
 // (zsb_split16_pad_f32), three fp16 wgmma products per k-step accumulate hi*hi + hi*lo + lo*hi
@@ -82,7 +85,7 @@ constexpr float BIN_SCALE = 2048.f;
 //          rows of log N(z; mu, exp(ls)) summed over the features
 //
 // The descriptor tc_pipeline_kernel runs, LinW<E, EPI, MN, Z>, is a LinCore (the product) plus the
-// fields of one epilogue family E: RowsEpi (EPI 0 - 2), SamplesEpi (4 - 6), ClassEpi (7, 8),
+// fields of one epilogue family E: RowsEpi (EPI 0 - 2, 16), SamplesEpi (4 - 6), ClassEpi (7, 8),
 // BnEpi (9 - 11), CatEpi (12 - 14) or NormalEpi (15).
 
 // What a product's units past its first n_tiles are (unit u runs output tile u % n_tiles), as each
@@ -726,7 +729,7 @@ struct NormalEpi {
   }
 };
 
-// EPI 0 - 2; EPI 0 with K-slices writes slice s of the product to out + s R J
+// EPI 0 - 2 and 16; EPI 0 with K-slices writes slice s of the product to out + s R J
 struct RowsEpi {
   static constexpr Units UNITS = K_SLICES;
   __host__ __device__ static constexpr bool folds_amax(int epi) { return epi != 1; }
@@ -780,7 +783,8 @@ struct RowsEpi {
       // the row sums in a WARPSYNC.COLLECTIVE sequence (125 SHFL + 70 WARPSYNC -> 63 SHFL)
       const int64_t rbase = r0 + c;
       float lpv[16];
-      float* __restrict__ po = (EPI == 0 || EPI == 2) ? out_s + rbase * J + j : nullptr;
+      float* __restrict__ po =
+          (EPI == 0 || EPI == 2 || EPI == 16) ? out_s + rbase * J + j : nullptr;
       const bool full = warp_j_ok && rbase + 16 <= R;   // no per-element predicates
 #pragma unroll
       for (int jj = 0; jj < 16; ++jj) {
@@ -791,12 +795,16 @@ struct RowsEpi {
           if (ok) { *po = y; amax = fmaxf(amax, fabsf(y)); }
         } else if (EPI == 1) {
           lpv[jj] = ok ? bern_lp(xe[jj], l) : 0.f;
+        } else if (EPI == 16) {
+          const float a = l + xe[jj];
+          const float y = relu ? fmaxf(a, 0.f) : a;
+          if (ok) { *po = y; amax = fmaxf(amax, fabsf(y)); }
         } else {
           const float g = __shfl_sync(0xffffffffu, ge, jj);
           const float y = g * (xe[jj] - __fdividef(1.f, 1.f + __expf(-l)));
           if (ok) { *po = y; amax = fmaxf(amax, fabsf(y)); }
         }
-        if (EPI == 0 || EPI == 2) po += J;
+        if (EPI == 0 || EPI == 2 || EPI == 16) po += J;
       }
       if (EPI == 1) {
         const float sum = warp_transpose_sum16(lpv, lane);
@@ -1358,11 +1366,14 @@ int linear_tc_amax(int epi, const void* w_planes, const float* scale_w, const vo
                    const float* scale_h, const float* bias, const float* x_obs, int64_t n_x,
                    const float* gout, float* out, float* part, int64_t R, int J, int K, int relu,
                    float* amax_scale, cudaStream_t st) {
-  ZSB_REQUIRE(epi >= 0 && epi <= 2, "zsb_linear_tc_f32: unknown epilogue");
+  ZSB_REQUIRE((epi >= 0 && epi <= 2) || (epi == 16 && Z == 0),
+              "zsb_linear_tc_f32: unknown epilogue");
   ZSB_REQUIRE(w_planes && h_planes && scale_w && scale_h && out && R > 0 && J > 0 && K > 0,
               "zsb_linear_tc_f32: bad args");
   ZSB_REQUIRE(R < (1LL << 31), "zsb_linear_tc_f32: too many rows");
   ZSB_REQUIRE(epi == 0 || (x_obs && n_x > 0), "zsb_linear_tc_f32: observations missing");
+  ZSB_REQUIRE(epi != 16 || (n_x == R && R * J < (1LL << 31)),
+              "zsb_linear_tc_f32: epi 16 needs a residual of R x J (n_x = R) below 2^31 entries");
   ZSB_REQUIRE(epi != 1 || part, "zsb_linear_tc_f32: partial-sum scratch missing");
   ZSB_REQUIRE(epi != 2 || gout, "zsb_linear_tc_f32: upstream gradient missing");
   LinCore<0, Z> c;
@@ -1372,6 +1383,8 @@ int linear_tc_amax(int epi, const void* w_planes, const float* scale_w, const vo
                   .part = part, .relu = relu, .amax_scale = amax_scale};
   if (epi == 0) return tc_launch(LinW<RowsEpi, 0, 0, Z>{c, e}, st, "linear_tc");
   if (epi == 2) return tc_launch(LinW<RowsEpi, 2, 0, Z>{c, e}, st, "linear_tc");
+  if constexpr (Z == 0)
+    if (epi == 16) return tc_launch(LinW<RowsEpi, 16, 0, 0>{c, e}, st, "linear_tc_residual");
   rc = tc_launch(LinW<RowsEpi, 1, 0, Z>{c, e}, st, "linear_tc");
   return rc ? rc : launch_part_sum(part, J, R, out, st, "linear_tc_part_sum");
 }
@@ -1493,6 +1506,8 @@ int zsb_split16_dual_f32(const float* src, const float* mask_src, int64_t R, int
 //   epi 1: out [R] = sum_j Bernoulli(logits = h W^T + bias).log_prob(x[r % n_x, j]);
 //          part = scratch of zsb_linear_tc_nparts(J) * R floats
 //   epi 2: out [R, J] = gout[r] * (x - sigmoid(logits))
+//   epi 16 (zsb_linear_tc_amax_f32 only): out [R, J] = act(h W^T + bias + x) with the residual
+//          x [R, J] (n_x = R), added before the ReLU
 // `part` is read by epi 1 only.
 //
 // Split-K slices of the weight-gradient product zsb_linear_tc_wgrad_f32 (R output rows, J

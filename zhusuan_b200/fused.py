@@ -16,7 +16,7 @@ __all__ = ["GaussianLogJoint", "BNNRegressionLogJoint", "LNTMLogJoint", "PMFLogJ
            "class_linear", "noisy_bn_linear", "bn_linear", "linear_bernoulli_log_prob",
            "LinearBernoulli", "LinearOnehotCategorical", "LinearNormal", "RBFKernel",
            "gp_conditional", "conv2d", "conv2d_transpose", "bn_conv2d", "bn_conv2d_transpose",
-           "sigmoid_conv2d_transpose"]
+           "sigmoid_conv2d_transpose", "conv2d_tc", "conv2d_transpose_tc"]
 
 
 class GaussianLogJoint(object):
@@ -2460,9 +2460,12 @@ def _tf_pad_before(big, small, k, s, padding):
     return max((small - 1) * s + k - big, 0) // 2 if padding == "SAME" else 0
 
 
-def _conv_tc_geom(name, x, W, stride, padding, transpose):
+def _conv_tc_geom(name, x, W, stride, padding, transpose, out_hw=None, empty_batch=False):
     """Validate the arguments of a tensor-core convolution before any launch and return its
-    _ConvGeom and the leading shape of x."""
+    _ConvGeom and the leading shape of x.  ``out_hw`` (transposed only): the output's (Ho, Wo), as
+    ``tf.nn.conv2d_transpose``'s ``output_shape`` gives it, instead of the size ``tf.layers``
+    picks; it must satisfy ceil(Ho / s) == Hi (SAME) or ceil((Ho - k + 1) / s) == Hi (VALID), as
+    TF requires.  ``empty_batch``: zero images (a leading dimension of 0) are valid, N = 0."""
     if not isinstance(x, torch.Tensor) or not isinstance(W, torch.Tensor):
         raise ValueError("%s: x and W should be tensors" % name)
     if x.dtype != torch.float32 or W.dtype != torch.float32:
@@ -2487,7 +2490,8 @@ def _conv_tc_geom(name, x, W, stride, padding, transpose):
         (int(W.shape[2]), int(W.shape[3]))
     if int(x.shape[-1]) != Cin:
         raise ValueError("%s: x has %d channels, W expects %d" % (name, int(x.shape[-1]), Cin))
-    if x.numel() == 0 or W.numel() == 0:
+    empty_lead = empty_batch and min(int(d) for d in x.shape[-3:]) > 0
+    if (x.numel() == 0 and not empty_lead) or W.numel() == 0:
         raise ValueError("%s: empty shapes are not supported: x %s, W %s"
                          % (name, tuple(x.shape), tuple(W.shape)))
     lead = tuple(int(d) for d in x.shape[:-3])
@@ -2497,8 +2501,19 @@ def _conv_tc_geom(name, x, W, stride, padding, transpose):
     H, Wd = int(x.shape[-3]), int(x.shape[-2])
     if transpose:
         Hs, Ws = H, Wd
-        grow = 0 if padding == "SAME" else max(k - s, 0)
-        Hb, Wb = Hs * s + grow, Ws * s + grow
+        if out_hw is None:
+            grow = 0 if padding == "SAME" else max(k - s, 0)
+            Hb, Wb = Hs * s + grow, Ws * s + grow
+        else:
+            Hb, Wb = out_hw
+            for big, small in ((Hb, Hs), (Wb, Ws)):
+                n = big if padding == "SAME" else big - k + 1
+                if n < 1 or -(-n // s) != small:
+                    raise ValueError(
+                        "%s: an output of %dx%d does not give the input's %dx%d at stride %d, %s "
+                        "(ceil(%s / stride) must equal Hi)" % (
+                            name, Hb, Wb, Hs, Ws, s, padding,
+                            "Ho" if padding == "SAME" else "(Ho - k + 1)"))
     else:
         Hb, Wb = H, Wd
         if padding == "SAME":
@@ -2546,11 +2561,11 @@ def _take_tag(x):
 
 
 def _col2im(epi, cols, g, C, out=None, bias=None, gamma=None, beta=None, mm=None, mv=None,
-            eps=0.0, relu=False, stats=None, pre=None, part=None, amax=None):
+            eps=0.0, relu=False, stats=None, pre=None, part=None, amax=None, residual=None):
     from ._lib import lib, ptr, stream
-    lib.call("zsb_conv_col2im_f32", epi, ptr(cols), *g.args(C), ptr(bias), ptr(gamma), ptr(beta),
-             ptr(mm), ptr(mv), float(eps), int(bool(relu)), ptr(stats), ptr(pre), ptr(part),
-             ptr(out), ptr(amax), stream())
+    lib.call("zsb_conv_col2im_f32", epi, ptr(cols), *g.args(C), ptr(bias), ptr(residual),
+             ptr(gamma), ptr(beta), ptr(mm), ptr(mv), float(eps), int(bool(relu)), ptr(stats),
+             ptr(pre), ptr(part), ptr(out), ptr(amax), stream())
 
 
 def _ones_like_gamma(gamma, Cout, dev):
@@ -2816,3 +2831,195 @@ def sigmoid_conv2d_transpose(x, W, b=None, stride=1, padding="SAME"):
         raise ValueError("sigmoid_conv2d_transpose: b must be a float32 [%d] tensor on %s"
                          % (g.Cout, W.device))
     return _SigmoidConv2dT.apply(x, W, b, g)
+
+
+# Biased layers relu?(conv(x) + b + residual) on the same products (csrc/conv_bias.cu): the
+# convolutions of vae_conv.py at any k <= 7, channel count and padding
+CONV_TC_MAX_C = 2 ** 20
+
+
+def _relu_grad(gy, y, R, J, relu, need_db):
+    """gp = d/d(pre-activation) [R, J] of relu?(a) with output y (gy itself without ReLU, copied),
+    db [J] (None unless ``need_db``) and the scale slot holding max |gp|
+    (zsb_conv_relu_grad_f32)."""
+    from ._lib import lib, ptr, stream
+    dev = gy.device
+    g = gy.reshape(R, J).to(torch.float32).contiguous()
+    gp = torch.empty((R, J), dtype=torch.float32, device=dev)
+    part = torch.empty(-(-R // 128) * J, dtype=torch.float32, device=dev)
+    db = torch.empty(J, dtype=torch.float32, device=dev) if need_db else None
+    scale = torch.zeros(4, dtype=torch.float32, device=dev)
+    lib.call("zsb_conv_relu_grad_f32", ptr(g), ptr(y if relu else None), R, J, int(relu), ptr(gp),
+             ptr(part), ptr(db), ptr(scale), stream())
+    return gp, db, scale
+
+
+class _Conv2dTC(torch.autograd.Function):
+    """relu?(conv(x, W) + b + residual): the gather-split of x, then the product over R = N Ho Wo
+    rows, J = Cout features and K = k k Cin with the bias + ReLU epilogue (epi 0), or with the
+    residual added before the ReLU (epi 16).  Backward: gp = d/d(pre-activation) and db from
+    zsb_conv_relu_grad_f32 (gp is the residual's gradient too), the plain split of gp at the max
+    |gp| that pass left, then dx as the col2im-sum of G W and dW from the saved gather planes, as
+    in _BNConv2d."""
+
+    @staticmethod
+    def forward(ctx, x, W, b, res, g, relu):
+        dev = W.device
+        tag = _take_tag(x)
+        x4 = x.detach().reshape(g.N, g.Hb, g.Wb, g.Cin).contiguous()
+        hpl = _gather_planes(x4, g, g.Cin, tag)
+        R, K, J = hpl.rows, hpl.K, g.Cout
+        wp, ws = _tc_split(W.detach().reshape(K, J).t())
+        bias = None if b is None else b.detach().contiguous()
+        r2 = None if res is None else res.detach().reshape(R, J).contiguous()
+        amax = torch.zeros(4, dtype=torch.float32, device=dev)
+        y = _tc_linear(0 if r2 is None else 16, wp, ws, hpl.planes, hpl.scale, bias, r2, None, R,
+                       J, K, relu, amax=amax)
+        ctx.save_for_backward(y if relu else None)
+        ctx.hpl, ctx.wpl = hpl, (wp, ws)
+        ctx.meta = (g, tuple(x.shape), relu)
+        return _tag(y.reshape(tuple(x.shape[:-3]) + (g.Hs, g.Ws, J)), amax)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        y, = ctx.saved_tensors
+        g, x_shape, relu = ctx.meta
+        need = ctx.needs_input_grad
+        dev = gy.device
+        R, J, K = g.N * g.Hs * g.Ws, g.Cout, g.k * g.k * g.Cin
+        gp, db, scale = _relu_grad(gy, y, R, J, relu, need[2])
+        dx = dW = None
+        if need[0] or need[1]:
+            gpl = _tc_split_dual(gp, amax=scale)
+            if need[0]:
+                wp, ws = ctx.wpl
+                dcols, _ = _tc_grad_input(gpl, _ShapeOnly((J, K), dev), R, wp, ws)
+                dx = torch.empty((g.N, g.Hb, g.Wb, g.Cin), dtype=torch.float32, device=dev)
+                amax = torch.zeros(4, dtype=torch.float32, device=dev)
+                _col2im(0, dcols, g, g.Cin, out=dx, amax=amax)
+                del dcols
+                dx = _tag(dx.reshape(x_shape), amax)
+            if need[1]:
+                dW = _tc_grad_weight(gpl, ctx.hpl, R).t().reshape(g.k, g.k, g.Cin, g.Cout)
+        ctx.hpl = ctx.wpl = None
+        dres = gp.reshape(gy.shape) if need[3] else None
+        return dx, dW, db, dres, None, None
+
+
+class _Conv2dTransposeTC(torch.autograd.Function):
+    """relu?(conv_transpose(x, W) + b + residual): the epi-0 product x W'^T gives the columns
+    [N Hi Wi, k k Cout]; their col2im-sum onto the output grid adds the bias and the residual and
+    applies the ReLU (epi 4).  Backward: gp and db from zsb_conv_relu_grad_f32 (gp is the
+    residual's gradient too), then _conv_t_grads at the max |gp| that pass left."""
+
+    @staticmethod
+    def forward(ctx, x, W, b, res, g, relu):
+        J, Rb = g.Cout, g.N * g.Hb * g.Wb
+        dev = W.device
+        cols, hpl, wpl = _conv_t_product(x, W, g)
+        bias = None if b is None else b.detach().contiguous()
+        r2 = None if res is None else res.detach().reshape(Rb, J).contiguous()
+        y = torch.empty((Rb, J), dtype=torch.float32, device=dev)
+        amax = torch.zeros(4, dtype=torch.float32, device=dev)
+        _col2im(4, cols, g, J, out=y, bias=bias, residual=r2, relu=relu, amax=amax)
+        del cols
+        ctx.save_for_backward(y if relu else None)
+        ctx.hpl, ctx.wpl = hpl, wpl
+        ctx.meta = (g, tuple(x.shape), relu)
+        return _tag(y.reshape(tuple(x.shape[:-3]) + (g.Hb, g.Wb, J)), amax)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        y, = ctx.saved_tensors
+        g, x_shape, relu = ctx.meta
+        need = ctx.needs_input_grad
+        gp, db, scale = _relu_grad(gy, y, g.N * g.Hb * g.Wb, g.Cout, relu, need[2])
+        dx = dW = None
+        if need[0] or need[1]:
+            dx, dW = _conv_t_grads(ctx, gp, scale, g, need[0], need[1], x_shape)
+        ctx.hpl = ctx.wpl = None
+        dres = gp.reshape(gy.shape) if need[3] else None
+        return dx, dW, db, dres, None, None
+
+
+def _conv_tc_apply(fn, name, x, W, b, residual, g, lead, relu, out_hw):
+    """Check b and residual against the layer's geometry and the channel and weight-operand
+    limits, all before any launch; then zero images give an empty result without a launch."""
+    out_shape = tuple(lead) + tuple(out_hw) + (g.Cout,)
+    for what, t, shape in (("b", b, (g.Cout,)), ("residual", residual, out_shape)):
+        if t is not None and (not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or
+                              t.device != W.device or tuple(t.shape) != shape):
+            raise ValueError("%s: %s should be a float32 tensor of shape %s on %s, got %s"
+                             % (name, what, shape, W.device,
+                                (t.dtype, tuple(t.shape), t.device)
+                                if isinstance(t, torch.Tensor) else type(t).__name__))
+    if max(g.Cin, g.Cout) >= CONV_TC_MAX_C:
+        raise ValueError("%s: channels should be below 2^20, got Cin %d, Cout %d"
+                         % (name, g.Cin, g.Cout))
+    kk = g.k * g.k
+    # the weight operand: W^T [Cout, k k Cin] (conv2d_tc) or W' [k k Cout, Cin] (transposed), in
+    # rows padded to 64 entries
+    w_rows, w_cols = (kk * g.Cout, g.Cin) if fn is _Conv2dTransposeTC else (g.Cout, kk * g.Cin)
+    if w_rows * (-(-w_cols // 64) * 64) >= 2 ** 31:
+        raise ValueError("%s: too large: the weight operand must have fewer than 2^31 entries"
+                         % name)
+    if g.N == 0:
+        return torch.empty(out_shape, dtype=torch.float32, device=x.device)
+    return fn.apply(x, W, b, residual, g, bool(relu))
+
+
+def conv2d_tc(x, W, b=None, stride=1, relu=False, residual=None, padding="SAME"):
+    """``relu?(tf.layers.conv2d(x, Cout, k, stride, padding) + residual)`` with its bias b, the
+    convolutions of vae_conv.py's encoder and resnet blocks (vae_conv.py:39-53, 80), on the
+    tensor-core products at fp32 accuracy: ``conv2d`` beyond the 3 x 3, 64-channel, SAME range of
+    its FFMA kernels.
+
+    x [..., H, W, Cin] is NHWC, any leading shape flattened to images; W [k, k, Cin, Cout] is the
+    ``tf.layers.conv2d`` kernel, 1 <= k <= 7; b [Cout] or None; ``residual`` (or None) has the
+    output's shape and is added before the ReLU.  The output is [..., Ho, Wo, Cout], sized and
+    padded as in ``bn_conv2d``:
+
+        y[n, i, j, co] = b[co] + residual[n, i, j, co]
+                         + sum_{kh, kw, ci} x[n, s i + kh - pt, s j + kw - pl, ci] W[kh, kw, ci, co]
+
+    Differentiable w.r.t. x, W, b and residual; under ``inference_mode`` nothing is kept.  Every
+    reduction runs in a fixed order with no float atomics, so two identical calls give identical
+    bits.  The output carries the max |.| that a following fused layer uses for its operand split,
+    and a tagged x is split at its tag.  Supported: float32 CUDA tensors on one device, stride 1
+    or 2, padding "SAME" or "VALID", 1 <= Cin, Cout < 2^20, fewer than 2^31 entries in every
+    tensor and operand; zero images give an empty result without a launch; anything else raises
+    ValueError before any launch."""
+    x = _unwrap(x)
+    g, lead = _conv_tc_geom("conv2d_tc", x, W, stride, padding, False, empty_batch=True)
+    return _conv_tc_apply(_Conv2dTC, "conv2d_tc", x, W, b, residual, g, lead, relu, (g.Hs, g.Ws))
+
+
+def conv2d_transpose_tc(x, W, out_shape, stride=1, b=None, relu=False, residual=None,
+                        padding="SAME"):
+    """``relu?(conv2d_transpose(x, out_shape, (k, k), stride) + residual)`` of
+    examples/utils/utils.py:74-113 (``tf.nn.conv2d_transpose`` plus ``bias_add``; vae_conv.py:20-36,
+    63-68) on the tensor-core products at fp32 accuracy: ``conv2d_transpose`` beyond the 3 x 3,
+    64-channel, SAME range of its FFMA kernels.
+
+    x [..., Hi, Wi, Cin] is NHWC; W [k, k, Cout, Cin] is that helper's ``weights`` layout, 1 <= k
+    <= 7; ``out_shape`` = (Ho, Wo, Cout) with ceil(Ho / stride) == Hi for SAME and
+    ceil((Ho - k + 1) / stride) == Hi for VALID (Wo likewise), as TF requires; b [Cout] or None;
+    ``residual`` (or None) has the output's shape and is added before the ReLU.  The map is the
+    adjoint of ``conv2d_tc``'s convolution from [Ho, Wo, Cout] to [Hi, Wi, Cin] with the same W
+    and pads, computed as in ``bn_conv2d_transpose``.  Gradients, determinism, inference mode, the
+    max |.| tag and the supported range are those of ``conv2d_tc``."""
+    x = _unwrap(x)
+    try:
+        Ho, Wo, Co = (int(v) for v in out_shape)
+    except (TypeError, ValueError):
+        raise ValueError("conv2d_transpose_tc: out_shape should be (Ho, Wo, Cout), got %r"
+                         % (out_shape,))
+    g, lead = _conv_tc_geom("conv2d_transpose_tc", x, W, stride, padding, True, out_hw=(Ho, Wo),
+                            empty_batch=True)
+    if Co != g.Cout:
+        raise ValueError("conv2d_transpose_tc: out_shape has %d channels, W has %d"
+                         % (Co, g.Cout))
+    return _conv_tc_apply(_Conv2dTransposeTC, "conv2d_transpose_tc", x, W, b, residual, g, lead,
+                          relu, (Ho, Wo))
