@@ -115,6 +115,11 @@ struct Unit {
 template <int MN, int Z>
 struct LinCore {
   static constexpr int KIND = 1, RB = 128, MNA = MN & 1, MNB = (MN >> 1) & 1, ZLO = Z;
+  // the weight gradient (MN = 3) contracts over all the rows of a batch -- 4096 k-blocks in the
+  // IWAE decoder at K = 64, N = 4096, up to 1024 in one split-K slice -- so its units add their
+  // accumulator into the shared tile every 8 k-blocks (PromoteOf in tc_common.cuh); the other
+  // products contract over a layer's width, a few dozen k-blocks at most
+  static constexpr int PROMOTE_KB = MN == 3 ? 8 : 0;
   static constexpr uint32_t TX = Cfg<RB>::STAGE - ((Z & 1) ? Cfg<RB>::A_TILE : 0) -
                                  ((Z & 2) ? Cfg<RB>::B_TILE : 0);
   CUtensorMap map_whi, map_wlo, map_hhi, map_hlo;

@@ -37,8 +37,10 @@ __global__ void __launch_bounds__(256) reduce_cols_kernel(const float* __restric
         const float x2 = p[(k + 2) * inner], x3 = p[(k + 3) * inner];
         const float mm = fmaxf(fmaxf(fmaxf(x0, x1), fmaxf(x2, x3)), m);
         if (mm == -INFINITY || mm == INFINITY) {
-          // all -inf so far (sum stays 0), or a +inf: (inf - inf) = nan as in the reference
-          s = (mm == INFINITY) ? NAN : 0.f;
+          // all -inf (or NaN: fmaxf drops it from mm) so far, the sum stays 0 -- unless a NaN was
+          // among them -- or a +inf: (inf - inf) = nan as in the reference
+          const bool nan_in = isnan(x0) || isnan(x1) || isnan(x2) || isnan(x3);
+          s = (mm == INFINITY || nan_in) ? NAN : s;
         } else {
           s = s * expf(m - mm) + expf(x0 - mm) + expf(x1 - mm) + expf(x2 - mm) + expf(x3 - mm);
         }
@@ -47,7 +49,7 @@ __global__ void __launch_bounds__(256) reduce_cols_kernel(const float* __restric
       for (; k < K; ++k) {
         const float x = p[k * inner];
         const float mm = fmaxf(x, m);
-        if (mm == -INFINITY || mm == INFINITY) s = (mm == INFINITY) ? NAN : 0.f;
+        if (mm == -INFINITY || mm == INFINITY) s = (mm == INFINITY || isnan(x)) ? NAN : s;
         else s = s * expf(m - mm) + expf(x - mm);
         m = mm;
       }

@@ -325,6 +325,49 @@ struct ZloOf<W, decltype((void)W::ZLO)> {
   static constexpr int value = W::ZLO;
 };
 
+// The MMA warpgroup's accumulator d into the shared-memory tile the epilogue reads: stored, or
+// (add) added to what the tile holds.  Each thread touches only its own elements.
+__device__ __forceinline__ void acc_tile_write(uint32_t acc_base, int tid, const float (&d)[2][64],
+                                               bool add) {
+  const int row = 16 * (tid >> 5) + ((tid & 31) >> 2);
+  const int col = 2 * (tid & 3);
+#pragma unroll
+  for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const uint32_t a0 = acc_base + (uint32_t)(((64 * mh + row) * ACC_LD + 8 * j + col) * 4);
+      float v0 = d[mh][4 * j], v1 = d[mh][4 * j + 1], v2 = d[mh][4 * j + 2], v3 = d[mh][4 * j + 3];
+      if (add) {
+        float p0, p1, p2, p3;
+        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(p0), "=f"(p1) : "r"(a0) : "memory");
+        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(p2), "=f"(p3)
+                     : "r"(a0 + 8u * ACC_LD * 4u) : "memory");
+        v0 += p0; v1 += p1; v2 += p2; v3 += p3;
+      }
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a0), "f"(v0), "f"(v1) : "memory");
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a0 + 8u * ACC_LD * 4u), "f"(v2),
+                   "f"(v3) : "memory");
+    }
+}
+
+// PROMOTE_KB (optional, default 0)  every PROMOTE_KB k-blocks of a unit the MMA warpgroup adds
+//                                 its wgmma accumulator into the unit's tile in shared memory
+//                                 (fp32 adds, rounded to nearest) and restarts it from zero.  The
+//                                 tensor core's own fp32 accumulation does not round to nearest:
+//                                 on partial sums of one sign it drifts toward zero by about 6 u
+//                                 per k-block (H100), which over the hundreds of k-blocks of a
+//                                 long contraction grows far past an fp32 sum's error.  The unit
+//                                 then waits for the epilogue to drain the tile before its
+//                                 mainloop instead of after it.
+template <class W, class = void>
+struct PromoteOf {
+  static constexpr int value = 0;
+};
+template <class W>
+struct PromoteOf<W, decltype((void)W::PROMOTE_KB)> {
+  static constexpr int value = W::PROMOTE_KB;
+};
+
 template <class W>
 __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __grid_constant__ W w) {
   using C = Cfg<W::RB>;
@@ -384,6 +427,13 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
 #pragma unroll
         for (int i = 0; i < 64; ++i) d[mh][i] = 0.f;
       int prev = -1;
+      [[maybe_unused]] int since = 0;
+      [[maybe_unused]] bool in_tile = false;            // the tile holds a promoted partial sum
+      if constexpr (PromoteOf<W>::value > 0) {
+        const long long t1 = prof_clock();
+        mbar_wait(tempty_bar, acc_phase ^ 1);          // epilogue drained the previous unit
+        t_tempty += prof_clock() - t1;
+      }
       for (int kb = kb0; kb < kb1; ++kb) {
         const uint32_t sa = smem_base + stage * C::STAGE;
         const long long t0 = prof_clock();
@@ -396,25 +446,29 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_pipeline_kernel(const __gri
         if (prev >= 0 && tid == 0) release(prev);
         prev = stage;
         if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+        if constexpr (PromoteOf<W>::value > 0) {
+          if (++since == PromoteOf<W>::value && kb + 1 < kb1) {
+            wgmma_wait<0>();
+            if (tid == 0) release(prev);
+            prev = -1;
+            acc_tile_write(acc_base, tid, d, in_tile);
+            in_tile = true;
+            since = 0;
+#pragma unroll
+            for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+              for (int i = 0; i < 64; ++i) d[mh][i] = 0.f;
+          }
+        }
       }
       wgmma_wait<0>();
       if (prev >= 0 && tid == 0) release(prev);
       const long long t1 = prof_clock();
-      mbar_wait(tempty_bar, acc_phase ^ 1);           // epilogue drained the previous unit
+      if constexpr (PromoteOf<W>::value == 0)
+        mbar_wait(tempty_bar, acc_phase ^ 1);         // epilogue drained the previous unit
       const long long t2 = prof_clock();
       t_tempty += t2 - t1;
-      const int row = 16 * (tid >> 5) + ((tid & 31) >> 2);
-      const int col = 2 * (tid & 3);
-#pragma unroll
-      for (int mh = 0; mh < 2; ++mh)
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const uint32_t a0 = acc_base + (uint32_t)(((64 * mh + row) * ACC_LD + 8 * j + col) * 4);
-          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a0), "f"(d[mh][4 * j]),
-                       "f"(d[mh][4 * j + 1]) : "memory");
-          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a0 + 8u * ACC_LD * 4u),
-                       "f"(d[mh][4 * j + 2]), "f"(d[mh][4 * j + 3]) : "memory");
-        }
+      acc_tile_write(acc_base, tid, d, in_tile);
       mbar_arrive(tfull_bar);
       acc_phase ^= 1;
       t_store += prof_clock() - t2;
