@@ -844,6 +844,51 @@ int zsb_bnn_logjoint_f32(const float* w0, const float* w1, const float* x, const
                          float n_train, float* lp, float* g0, float* g1, float* g_ylogstd,
                          float* y_mean, float* log_lik, int64_t K, void* stream);
 
+/* ---- BNN regression with L >= 3 weight layers (csrc/bnn_deep.cu) -------------------------------
+ * build_bnn of examples/bayesian_neural_nets/bnn_vi.py:18-35 and bnn_sgmcmc.py:19-35 at
+ * layer_sizes = [n_0, ..., n_{L-1}, 1] (widths[0..L], widths[L] = 1), with the log-joint override
+ * of bnn_vi.py:83-86 / bnn_sgmcmc.py:74-77, replacing the per-layer einsum / concat / relu /
+ * Normal log_prob graph, its tf.gradients (bnn_vi.py:88-89, sgmcmc.py:96-98) and the prediction
+ * fetches (bnn_vi.py:98-103).  Layer i: w[i] [K, widths[i+1], widths[i] + 1], prior
+ * N(0, exp(logstd[i])) read flat over one particle's layer, index modulo logstd_n[i].  The
+ * per-layer arrays (w, g, logstd, logstd_n, ...) are HOST arrays of L entries.  Limits:
+ * 3 <= L <= 8, widths[i] <= 128 for i < L, at most 32768 weights per particle; any B and K >= 1.
+ * No floating-point atomics: deterministic.
+ *
+ * Value, gradients and predictions in one launch; outputs as zsb_bnn_logjoint_f32's, each
+ * written only when non-NULL (g may be NULL, or hold NULL for a layer whose gradient is not
+ * needed).  y_logstd is a DEVICE scalar. */
+int zsb_bnn_deep_logjoint_f32(int L, const int* widths /* host */, const float* const* w /* host */,
+                              const float* x, const float* y, int64_t B,
+                              const float* const* logstd /* host */,
+                              const int* logstd_n /* host */, const float* y_logstd,
+                              float n_train, float* lp, float* const* g /* host */,
+                              float* g_ylogstd, float* y_mean, float* log_lik, int64_t K,
+                              void* stream);
+
+/* One fused SG-MCMC step of `method` (enum zsb_sgmcmc_method) on the same log-joint, gradient and
+ * update of every layer in one launch (sgmcmc.py:195-200, 225-257, 326-371, 460-523), with
+ * zsb_sgmcmc_bnn_step_f32's state per layer (host arrays of L device pointers; NULL arrays where
+ * the method has no such state): v, aux, alpha_eff, mean_k.  The noise of latent i is
+ * (seed + i, iter, row0 + chain), as the element-wise zsb_sgmcmc_*_f32 kernels draw it, or
+ * injected through noise / resample_noise (host arrays, or NULL).  part: L*zsb_sgmcmc_parts()
+ * floats (SGHMC, scalar SGNHT); work: work_n >= min(chains, zsb_sgmcmc_parts()) * (weights per
+ * chain) floats of scratch for the gradient. */
+int zsb_sgmcmc_bnn_deep_step_f32(int method, int L, const int* widths /* host */,
+                                 float* const* w /* host */, float* const* v /* host */,
+                                 float* const* aux /* host */,
+                                 const float* const* alpha_eff /* host */, const float* x,
+                                 const float* y, int64_t B, const float* const* logstd /* host */,
+                                 const int* logstd_n /* host */, float y_logstd, float n_train,
+                                 float lr, float friction, float variance_estimate, float decay,
+                                 float epsilon, float variance_extra, float tune_rate,
+                                 int second_order, int resample,
+                                 const float* const* noise /* host */,
+                                 const float* const* resample_noise /* host */, uint64_t seed,
+                                 uint32_t iter, int64_t row0, float* part,
+                                 float* const* mean_k /* host */, float* work, int64_t work_n,
+                                 int64_t chains, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

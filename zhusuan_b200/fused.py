@@ -136,6 +136,15 @@ class BNNRegressionLogJoint(object):
     gradient.  Under ``torch.no_grad()`` ``fused_log_joint`` launches the
     value-only kernel; its gradient is first order (no double backward).  Anything else: the objectives and
     HMC fall back to ``__call__`` under autograd, ``predictive`` raises.
+
+    Deeper nets: ``names`` and ``logstds`` give one entry per weight layer, L >= 2 of them, at
+    layer sizes [n_0, n_1, ..., n_{L-1}, 1] (layer i: w_i [K, n_{i+1}, n_i + 1], ReLU after every
+    layer but the last).  L = 2 runs on the kernels above.  L >= 3 runs on csrc/bnn_deep.cu with
+    the same consumers and rules -- the SG-MCMC step in one launch, ``fused_log_joint``,
+    ``predictive`` and the HMC provider -- within its limits: L <= 8, n_0 <= 128, hidden widths
+    <= 128, at most 32768 weights per particle, any number of rows B (minibatches included) and
+    particles K.  ``fused_inputs`` then returns the L latents, ``x`` and ``y``.  Shapes past the
+    limits run the generic path.
     """
 
     MAX_IN1, MAX_H = 16, 64      # limits of the fused kernels (n_in + 1, H)
@@ -146,6 +155,10 @@ class BNNRegressionLogJoint(object):
         self._Normal = Normal
         self.x, self.y = x, y
         self.logstds = [l.contiguous() for l in logstds]
+        if len(self.logstds) != len(tuple(names)) or len(self.logstds) < 2:
+            raise ValueError("BNNRegressionLogJoint needs one logstd per weight layer and at "
+                             "least two layers (got %d names, %d logstds)"
+                             % (len(tuple(names)), len(self.logstds)))
         self.n_train = float(n_train)
         if isinstance(y_logstd, torch.Tensor):
             if y_logstd.dim() != 0 or y_logstd.dtype != torch.float32 or \
@@ -209,6 +222,8 @@ class BNNRegressionLogJoint(object):
         None (the caller runs ``__call__`` under autograd).  ``x`` / ``y`` come from
         ``observed``, else from the object; latents that are ``StochasticTensor`` samples of a
         variational net are unwrapped."""
+        if len(self.names) > 2:
+            return self._deep_fused_inputs(observed)
         try:
             w0, w1 = (_unwrap(observed[n]) for n in self.names)
         except KeyError:
@@ -241,6 +256,87 @@ class BNNRegressionLogJoint(object):
             return None
         return w0, w1, x, y
 
+    def _deep_fused_inputs(self, observed):
+        """fused_inputs for L >= 3 layers: ``(w_0, ..., w_{L-1}, x, y)`` or None.  The rules of
+        the two-layer check, per layer, with the deep kernels' limits: L <= DEEP_MAX_L, n_0 and
+        every hidden width <= DEEP_MAX_WIDTH, at most DEEP_MAX_WEIGHTS weights per particle."""
+        try:
+            ws = [_unwrap(observed[n]) for n in self.names]
+        except KeyError:
+            return None
+        x, y = _unwrap(observed.get("x", self.x)), _unwrap(observed.get("y", self.y))
+        if not all(isinstance(t, torch.Tensor) and t.is_cuda for t in ws + [x, y]) or \
+                any(w.dtype != torch.float32 or w.dim() != 3 for w in ws):
+            return None
+        if not self.deep_shape_ok([tuple(int(d) for d in w.shape) for w in ws]):
+            return None
+        if x.dim() != 2 or int(x.shape[1]) + 1 != ws[0].shape[2] or x.shape[0] < 1 or \
+                y.numel() != x.shape[0]:
+            return None
+        dev = ws[0].device
+        if any(t.device != dev for t in ws + [x, y]):
+            return None
+        if any(ls.requires_grad or ls.dtype != torch.float32 or ls.device != dev
+               for ls in self.logstds):
+            return None
+        if isinstance(self.y_logstd, torch.Tensor) and self.y_logstd.device != dev:
+            return None
+        if any(self.fused_prior_logstd(i, w.shape[1:]) is None for i, w in enumerate(ws)):
+            return None
+        return tuple(ws) + (x, y)
+
+    DEEP_MAX_L, DEEP_MAX_WIDTH, DEEP_MAX_WEIGHTS = 8, 128, 32768   # limits of csrc/bnn_deep.cu
+
+    @classmethod
+    def deep_shape_ok(cls, shapes):
+        """Whether latents of these shapes ([K, n_{i+1}, n_i + 1] per layer, L >= 3) chain into
+        one net within the deep kernels' limits."""
+        L = len(shapes)
+        if not 3 <= L <= cls.DEEP_MAX_L:
+            return False
+        K = shapes[0][0]
+        if K < 1 or any(len(s) != 3 or s[0] != K for s in shapes) or shapes[-1][1] != 1:
+            return False
+        widths = [s[2] - 1 for s in shapes]
+        if any(shapes[i][1] != widths[i + 1] for i in range(L - 1)):
+            return False
+        if any(not 1 <= n <= cls.DEEP_MAX_WIDTH for n in widths):
+            return False
+        return sum(s[1] * s[2] for s in shapes) <= cls.DEEP_MAX_WEIGHTS
+
+    def _deep_prior(self, ws):
+        """(logstd tensors, host arrays of their pointers and sizes) as the deep kernels read
+        them; the tensors must outlive the call."""
+        import ctypes
+        from ._lib import ptr
+        lss = [self.fused_prior_logstd(i, w.shape[1:]).detach() for i, w in enumerate(ws)]
+        L = len(ws)
+        return (lss, (ctypes.c_void_p * L)(*[ptr(l) for l in lss]),
+                (ctypes.c_int * L)(*[l.numel() for l in lss]))
+
+    def _launch_deep(self, ws, x, y, ys, lp=False, gs=(), gys=False, ym=False, ll=False):
+        """One zsb_bnn_deep_logjoint_f32 launch; returns ``(lp, [g_i], gys, y_mean, log_lik)``
+        with None where not requested (``gs``: per layer whether its gradient is wanted)."""
+        import ctypes
+        from ._lib import lib, ptr, stream
+        L = len(ws)
+        ws = [w.detach().contiguous() for w in ws]
+        K, B, dev = int(ws[0].shape[0]), int(x.shape[0]), ws[0].device
+        x = x.detach().to(torch.float32).contiguous()
+        y = y.detach().to(torch.float32).contiguous().view(-1)
+        gs = list(gs) + [False] * (L - len(gs))
+        widths = (ctypes.c_int * (L + 1))(*([int(w.shape[2]) - 1 for w in ws] + [1]))
+        lss, ls_p, ls_n = self._deep_prior(ws)
+        e = lambda want, *s: torch.empty(s, dtype=torch.float32, device=dev) if want else None  # noqa: E731
+        g = [e(want, *w.shape) for want, w in zip(gs, ws)]
+        out = (e(lp, K), e(gys, K), e(ym, K, B), e(ll, K, B))
+        w_p = (ctypes.c_void_p * L)(*[ptr(w) for w in ws])
+        g_p = (ctypes.c_void_p * L)(*[ptr(t) for t in g])
+        lib.call("zsb_bnn_deep_logjoint_f32", L, widths, ctypes.addressof(w_p), ptr(x), ptr(y), B,
+                 ctypes.addressof(ls_p), ls_n, ptr(ys.detach()), self.n_train, ptr(out[0]),
+                 ctypes.addressof(g_p), ptr(out[1]), ptr(out[2]), ptr(out[3]), K, stream())
+        return out[0], g, out[1], out[2], out[3]
+
     def _launch(self, w0, w1, x, y, ys, lp=False, g0=False, g1=False, gys=False,
                 ym=False, ll=False):
         """One zsb_bnn_logjoint_f32 launch; returns the requested outputs (None elsewhere)."""
@@ -271,8 +367,13 @@ class BNNRegressionLogJoint(object):
         if got is None:
             raise ValueError("BNNRegressionLogJoint.fused_log_joint: these inputs need the "
                              "generic path (see fused_inputs)")
+        ys = self._y_logstd_dev(got[0].device)
+        if len(got) > 4:
+            ws, x, y = got[:-2], got[-2], got[-1]
+            if not torch.is_grad_enabled():
+                return self._launch_deep(ws, x, y, ys, lp=True)[0]
+            return _BNNDeepLogJoint.apply(ys, self, x, y, *[w.contiguous() for w in ws])
         w0, w1, x, y = got
-        ys = self._y_logstd_dev(w0.device)
         if not torch.is_grad_enabled():        # nothing is recorded: the value-only launch
             return self._launch(w0, w1, x, y, ys, lp=True)[0]
         return _BNNLogJoint.apply(w0.contiguous(), w1.contiguous(), ys, self, x, y)
@@ -287,6 +388,11 @@ class BNNRegressionLogJoint(object):
         if got is None:
             raise ValueError("BNNRegressionLogJoint.predictive: shapes outside the fused "
                              "kernel's limits (see fused_inputs)")
+        if len(got) > 4:
+            _, _, _, ym, ll = self._launch_deep(got[:-2], got[-2], got[-1],
+                                                self._y_logstd_dev(got[0].device), ym=True,
+                                                ll=True)
+            return ym, ll
         w0, w1, x, y = got
         _, _, _, _, ym, ll = self._launch(w0, w1, x, y, self._y_logstd_dev(w0.device),
                                           ym=True, ll=True)
@@ -294,7 +400,8 @@ class BNNRegressionLogJoint(object):
 
     def hmc_provider(self, latent_names, observed, latents):
         """The provider ``zs.HMC`` uses instead of autograd (logp / grad, one launch each) when
-        the latents are (w0, w1) and ``fused_inputs`` accepts them; else None."""
+        the latents are the object's weight layers and ``fused_inputs`` accepts them; else
+        None."""
         if list(latent_names) != list(self.names):
             return None
         obs = dict(observed)
@@ -306,15 +413,15 @@ class BNNRegressionLogJoint(object):
     def __call__(self, observed):
         x = observed.get("x", self.x)
         y = observed.get("y", self.y)
-        w0, w1 = observed[self.names[0]], observed[self.names[1]]
-        C = w0.shape[0]
+        ws = [observed[n] for n in self.names]
+        C = ws[0].shape[0]
         h = x.unsqueeze(0).expand(C, -1, -1)
         lp = 0.0
-        for w, ls in zip((w0, w1), self.logstds):
+        for i, (w, ls) in enumerate(zip(ws, self.logstds)):
             ones = torch.ones(h.shape[:-1] + (1,), device=h.device)
             h = torch.cat([h, ones], -1)
             h = torch.einsum("imk,ijk->ijm", w, h) / math.sqrt(h.shape[2])
-            if w is w0:
+            if i < len(ws) - 1:
                 h = torch.relu(h)
             lp = lp + self._Normal(torch.zeros_like(ls), logstd=ls,
                                    group_ndims=2).log_prob(w)
@@ -356,6 +463,28 @@ class _BNNLogJoint(torch.autograd.Function):
         return d0, d1, dys, None, None, None
 
 
+class _BNNDeepLogJoint(torch.autograd.Function):
+    """lp [K] of an L >= 3 layer BNNRegressionLogJoint over (y_logstd, w_0, ..., w_{L-1}) on
+    zsb_bnn_deep_logjoint_f32; as _BNNLogJoint, the forward launch writes the gradients the
+    inputs need and backward scales them."""
+
+    @staticmethod
+    def forward(ctx, ys, obj, x, y, *ws):
+        need = ctx.needs_input_grad
+        lp, gs, gys, _, _ = obj._launch_deep(ws, x, y, ys, lp=True, gs=need[4:], gys=need[0])
+        ctx.save_for_backward(gys, *gs)
+        return lp
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, glp):
+        gys, *gs = ctx.saved_tensors
+        glp = glp.to(torch.float32)
+        dws = [g * glp.view(-1, 1, 1) if g is not None else None for g in gs]
+        dys = (gys * glp).sum() if gys is not None else None
+        return (dys, None, None, None) + tuple(dws)
+
+
 class _BNNProvider(object):
     """HMC's provider interface over BNNRegressionLogJoint: values and gradients of the latents
     (w0, w1) at the observed rows, one zsb_bnn_logjoint_f32 launch each.  HMC picks the provider
@@ -375,6 +504,9 @@ class _BNNProvider(object):
         got = self.obj.fused_inputs(obs)
         if got is None:
             return self.obj(obs)
+        if len(got) > 4:
+            return self.obj._launch_deep(got[:-2], got[-2], got[-1],
+                                         self.obj._y_logstd_dev(got[0].device), lp=True)[0]
         w0, w1, x, y = got
         return self.obj._launch(w0, w1, x, y, self.obj._y_logstd_dev(w0.device), lp=True)[0]
 
@@ -386,6 +518,11 @@ class _BNNProvider(object):
                 gs = torch.autograd.grad(self.obj(self._obs(xs)).sum(), xs, allow_unused=True)
             return [g.contiguous() if g is not None else torch.zeros_like(x)
                     for g, x in zip(gs, xs)]
+        if len(got) > 4:
+            ws = got[:-2]
+            return self.obj._launch_deep(ws, got[-2], got[-1],
+                                         self.obj._y_logstd_dev(ws[0].device),
+                                         gs=[True] * len(ws))[1]
         w0, w1, x, y = got
         out = self.obj._launch(w0, w1, x, y, self.obj._y_logstd_dev(w0.device), g0=True,
                                g1=True)

@@ -7,9 +7,11 @@ reference feeds through placeholders are passed as
 ``sample_op(observed={...})`` overrides.  Gradients of the user log-joint
 come from torch autograd over the registry kernels (replaces tf.gradients,
 sgmcmc.py:96-98); the update itself is one fused kernel per latent.  On the
-two-layer BNN regression log-joint of ``zs.fused`` every method runs the whole
-step (gradient and update) in one launch instead (csrc/sgmcmc_bnn.cu).
+BNN regression log-joint of ``zs.fused`` every method runs the whole step
+(gradient and update) in one launch instead (csrc/sgmcmc_bnn.cu for two weight
+layers, csrc/bnn_deep.cu for more).
 """
+import ctypes
 from collections import namedtuple
 
 import torch
@@ -169,6 +171,8 @@ class SGMCMC(object):
             return None
         if isinstance(obj.y_logstd, torch.Tensor):   # the step kernel takes y_logstd by value
             return None
+        if len(self._var_list) > 2:
+            return self._fused_bnn_deep(obj)
         w0, w1 = self._var_list
         if w0.dim() != 3 or w1.dim() != 3 or w1.shape[1] != 1 or \
                 w1.shape[2] != w0.shape[1] + 1:
@@ -188,9 +192,26 @@ class SGMCMC(object):
             return None
         return obj
 
+    def _fused_bnn_deep(self, obj):
+        """_fused_bnn for L >= 3 layers (csrc/bnn_deep.cu): any minibatch size."""
+        ws = self._var_list
+        if any(w.dim() != 3 for w in ws) or \
+                not obj.deep_shape_ok([tuple(int(d) for d in w.shape) for w in ws]):
+            return None
+        x, y = obj.x, obj.y
+        if x.dim() != 2 or x.shape[1] + 1 != ws[0].shape[2]:
+            raise ValueError("minibatch x has shape {} but w0 {} needs [B, {}]".format(
+                tuple(x.shape), tuple(ws[0].shape), ws[0].shape[2] - 1))
+        if y.numel() != x.shape[0]:
+            raise ValueError("minibatch y has {} values but x has {} rows".format(
+                y.numel(), x.shape[0]))
+        if any(obj.fused_prior_logstd(i, w.shape[1:]) is None for i, w in enumerate(ws)):
+            return None
+        return obj
+
     def _bnn_part_buf(self):
         if not hasattr(self, "_bnn_part"):
-            self._bnn_part = torch.zeros(2 * lib.load().zsb_sgmcmc_parts(),
+            self._bnn_part = torch.zeros(len(self._var_list) * lib.load().zsb_sgmcmc_parts(),
                                          dtype=_F32, device=self._var_list[0].device)
         return self._bnn_part
 
@@ -198,7 +219,13 @@ class SGMCMC(object):
                   alpha_eff=(None, None), mean_k=(None, None), part=None, friction=0.,
                   variance_estimate=0., decay=0., epsilon=0., variance_extra=0., tune_rate=0.,
                   second_order=False, resample=False):
-        """One zsb_sgmcmc_bnn_step_f32 launch on (w0, w1); state pairs are (w0's, w1's)."""
+        """One zsb_sgmcmc_bnn_step_f32 launch on (w0, w1); state pairs are (w0's, w1's).  With
+        L >= 3 latents, one zsb_sgmcmc_bnn_deep_step_f32 launch; the state holds one entry per
+        latent."""
+        if len(self._var_list) > 2:
+            return self._bnn_deep_step(obj, noise, method, v, aux, alpha_eff, mean_k, part,
+                                       friction, variance_estimate, decay, epsilon,
+                                       variance_extra, tune_rate, second_order, resample)
         w0, w1 = self._var_list
         x, y = obj.x.contiguous(), obj.y.contiguous()
         ls0 = obj.fused_prior_logstd(0, w0.shape[1:])
@@ -213,6 +240,44 @@ class SGMCMC(object):
                  self._noise(noise, "resample", 1), self._seed_now(), self.t & 0xFFFFFFFF,
                  self._row0, ptr(part), ptr(mean_k[0]), ptr(mean_k[1]), self._chains,
                  stream())
+
+    def _bnn_deep_step(self, obj, noise, method, v, aux, alpha_eff, mean_k, part, friction,
+                       variance_estimate, decay, epsilon, variance_extra, tune_rate,
+                       second_order, resample):
+        ws = self._var_list
+        L = len(ws)
+        x, y = obj.x.contiguous(), obj.y.contiguous()
+        parts = lib.load().zsb_sgmcmc_parts()
+        n_w = sum(w.numel() // self._chains for w in ws)
+        need = min(self._chains, parts) * n_w
+        if getattr(self, "_bnn_work", None) is None or self._bnn_work.numel() < need:
+            self._bnn_work = torch.empty(need, dtype=_F32, device=ws[0].device)
+        widths = (ctypes.c_int * (L + 1))(*([int(w.shape[2]) - 1 for w in ws] + [1]))
+        lss, ls_p, ls_n = obj._deep_prior(ws)
+
+        def arr(ts):
+            if ts is None or all(t is None for t in ts):
+                return None, None
+            a = (ctypes.c_void_p * L)(*[ptr(t) for t in ts])
+            return a, ctypes.addressof(a)
+
+        def noise_arr(key):
+            n = noise.get(key)
+            if n is None:
+                return None, None
+            ts = [n[k].contiguous() for k in self._latent_k]
+            a = (ctypes.c_void_p * L)(*[ptr(t) for t in ts])
+            return (a, ts), ctypes.addressof(a)
+        keep = [arr(ws), arr(v), arr(aux), arr(alpha_eff), arr(mean_k), noise_arr("noise"),
+                noise_arr("resample"), (ls_p, ctypes.addressof(ls_p))]
+        w_a, v_a, aux_a, ae_a, mk_a, nz_a, rs_a, ls_a = (k[1] for k in keep)
+        lib.call("zsb_sgmcmc_bnn_deep_step_f32", method, L, widths, w_a, v_a, aux_a, ae_a,
+                 ptr(x), ptr(y), int(x.shape[0]), ls_a, ls_n, obj.y_logstd, obj.n_train,
+                 self.lr, friction, variance_estimate, decay, epsilon, variance_extra, tune_rate,
+                 int(second_order), int(resample), nz_a, rs_a, self._seed_now(),
+                 self.t & 0xFFFFFFFF, self._row0, ptr(part), mk_a, ptr(self._bnn_work),
+                 self._bnn_work.numel(), self._chains, stream())
+        del keep, lss
 
     def _resample_due(self):
         return self.n_iter_resample_v != 0 and \
