@@ -536,6 +536,50 @@ int zsb_sample_gamma_f32(const float* alpha, int64_t alpha_rows, const float* be
  * 1363-1379): Philox block (i / 4, 0, iter, 9), word i % 4. */
 int zsb_sample_base_noise_f32(int kind, float* out, int64_t n, uint64_t seed, uint32_t iter,
                               void* stream);
+/* ---- ExpConcrete / Concrete (multivariate.py:683-958; csrc/concrete.cu) -----------------------
+ * Rows of C categories, 1 <= C <= 1024; value row r reads parameter row r % logits_rows (the
+ * parameters broadcast as a suffix) and given row r % given_rows.  `temperature` is a device
+ * pointer to one float, so no call synchronises with the host.  log_space = 1: ExpConcrete (values
+ * are log-probabilities), 0: Concrete (values on the simplex).
+ *
+ * zsb_sample_concrete_f32 (ExpConcrete._sample multivariate.py:768-782, Concrete._sample
+ * :905-919): out [rows, C] = log_softmax((l + g) / t) or softmax(...), g = -log(-log(u)), u
+ * clamped to [1e-7, 1 - 1e-7].  u = injected uniforms [rows, C], or NULL: element e of the flat
+ * output is word e % 4 of Philox block (e / 4, 0, iter, 9), the draw of zsb_sample_base_noise_f32
+ * kind 0 for the same (seed, iter).
+ * zsb_sample_concrete_bwd_f32: the reparameterisation gradient from the saved sample y [rows, C]
+ * and its cotangent gy alone: dA = gy - exp(y) sum(gy) (log space) or y (gy - sum(y gy));
+ * dlogits [logits_rows, C] = sum over the rows s * logits_rows + lr of dA / t, in a fixed order;
+ * d t = -sum(dA y) / t (log space) or -sum(dA log y) / t, into dtemp [1].  rows must be a
+ * multiple of logits_rows.  Either output may be NULL.
+ * zsb_logprob_concrete_f32 (ExpConcrete._log_prob :800-812, Concrete._log_prob :938-955):
+ * out [rows] = lgamma(C) + (C-1) log t + sum(temp) [- sum(log given)] - C LSE(temp), temp = l - t x,
+ * x = given (log space) or log(given).
+ * zsb_logprob_concrete_bwd_f32: with w = 1 - C softmax(temp) and gout [rows]: dgiven [rows, C] =
+ * gout (-t w) or gout (-t w - 1) / given; dlogits [logits_rows, C] = sum of gout w over the rows
+ * of each parameter row, in a fixed order; d t = sum gout ((C-1)/t - sum(w x)), into dtemp [1].
+ * rows must be a multiple of logits_rows; every output may be NULL.
+ * Both backward entries take `work`, zsb_concrete_bwd_work(logits_rows, C, rows) floats of
+ * scratch: ZSB_CONCRETE_PARTS temperature partials, one per CTA, and, when the sample axis is split
+ * across CTAs (few parameter rows, many samples), each chunk's logits-gradient partial.  A second
+ * launch merges both in a fixed order.  No float atomics: identical calls give identical bits. */
+#define ZSB_CONCRETE_PARTS 1024
+int zsb_sample_concrete_f32(const float* logits, int64_t logits_rows, const float* temperature,
+                            int64_t n_categories, int log_space, const float* u, uint64_t seed,
+                            uint32_t iter, float* out, int64_t rows, void* stream);
+int zsb_sample_concrete_bwd_f32(const float* y, const float* gy, int64_t logits_rows,
+                                const float* temperature, int64_t n_categories, int log_space,
+                                float* dlogits, float* dtemp, float* work, int64_t rows,
+                                void* stream);
+int zsb_logprob_concrete_f32(const float* given, int64_t given_rows, const float* logits,
+                             int64_t logits_rows, const float* temperature, int64_t n_categories,
+                             int log_space, float* out, int64_t rows, void* stream);
+int zsb_logprob_concrete_bwd_f32(const float* given, int64_t given_rows, const float* logits,
+                                 int64_t logits_rows, const float* temperature,
+                                 int64_t n_categories, int log_space, const float* gout,
+                                 float* dgiven, float* dlogits, float* dtemp, float* work,
+                                 int64_t rows, void* stream);
+int zsb_concrete_bwd_work(int64_t logits_rows, int64_t n_categories, int64_t rows);
 /* Poisson._sample (univariate.py:915-920) / Binomial._sample (univariate.py:1025-1045): kind 0 =
  * Poisson(rate = param), 1 = Binomial(n_experiments, sigmoid(param)); one uniform per draw
  * (injected u [n] or Philox), inverse transform enumerating the support outwards from the mode. */

@@ -90,6 +90,7 @@ class _Lib(object):
                 "zsb_sgmcmc_mean_sq_f32": 2, "zsb_sgmcmc_sgnht_scalar_f32": 2,
                 "zsb_split16_pad_f32": 3, "zsb_linear_tc_f32": 2, "zsb_planar_flow_bwd_f32": 2,
                 "zsb_iaf_bwd_f32": 2, "zsb_lntm_mstep_grad_f32": 2,
+                "zsb_sample_concrete_bwd_f32": 2, "zsb_logprob_concrete_bwd_f32": 2,
                 "zsb_gp_cond_bwd_f32": 2, "zsb_conv3x3_wgrad_f32": 2,
                 # the tensor-core conv layers' entries, in their common case: a gather-split
                 # with its max pass, a sigmoid or ReLU gradient with the bias sums

@@ -1,11 +1,15 @@
 """ExpConcrete / Concrete (Gumbel-softmax relaxations, multivariate.py:683-958)
 and MatrixVariateNormalCholesky (multivariate.py:961-1160).
 
-These complete the distribution registry for model code; they are composed
-from the library's reduction kernels (log-sum-exp / sum over the category
-axis through ``ops.reduce_axes``) plus elementwise torch ops, and -- for the
-matrix-variate normal -- torch's triangular solves (cuBLAS: library code).
-None of them is on the accelerated hot path of SURVEY section 8.
+ExpConcrete and Concrete sample and score on the fused kernels of
+csrc/concrete.cu (one pass per direction over the [S, *batch, C] tensor, the
+gradients w.r.t. given, logits and temperature analytic) whenever the logits
+and the temperature are float32 on one CUDA device, ``given`` is float32 and
+1 <= C <= 1024.  Every other input takes the composition kept here: the
+library's reduction kernels (log-sum-exp / sum over the category axis through
+``ops.reduce_axes``) plus elementwise torch ops.  Both draw the same uniforms
+from a given ``zs.random`` state.  The matrix-variate normal stays on torch's
+triangular solves (cuBLAS: library code).
 """
 import math
 
@@ -25,6 +29,7 @@ class ExpConcrete(Distribution):
     log-probabilities on the simplex)."""
     _group_sum_in_log_prob = True
     _name = "ExpConcrete"
+    _log_space = True
 
     def __init__(self, temperature, logits, group_ndims=0,
                  is_reparameterized=True, use_path_derivative=False,
@@ -57,19 +62,42 @@ class ExpConcrete(Distribution):
     def _get_batch_shape(self):
         return self._logits.shape[:-1]
 
-    def _gumbel_logits(self, n_samples):
+    def _fused(self, given=None):
+        """The kernels of csrc/concrete.cu take these inputs (decided from them alone)."""
+        l, t = self._logits, self._temperature
+        return (l.dtype == torch.float32 and t.dtype == torch.float32 and l.is_cuda
+                and t.device == l.device
+                and 1 <= self._n_categories <= ops.CONCRETE_MAX_CATEGORIES
+                and (given is None or (given.dtype == torch.float32
+                                       and given.device == l.device)))
+
+    def _gumbel_logits(self, n_samples, u=None):
         logits, temperature = self._logits, self._temperature
         if not self.is_reparameterized:
             logits, temperature = logits.detach(), temperature.detach()
-        from .. import ops
-        u = ops.base_noise(0, (int(n_samples),) + tuple(logits.shape), logits.device,
-                           *self._next_rng())
+        rng = self._next_rng()
+        if u is None:
+            u = ops.base_noise(0, (int(n_samples),) + tuple(logits.shape), logits.device, *rng)
         u = u.clamp(1e-7, 1.0 - 1e-7)                 # open interval (0, 1)
         gumbel = -torch.log(-torch.log(u))
         return (logits + gumbel) / temperature
 
-    def _sample(self, n_samples):
-        return torch.log_softmax(self._gumbel_logits(n_samples), -1)
+    def _sample(self, n_samples, u=None):
+        """``u``: injected uniforms [n_samples] + logits.shape (clamped as drawn ones are)."""
+        if self._fused():
+            logits, temperature = self._logits, self._temperature
+            if not self.is_reparameterized:
+                logits, temperature = logits.detach(), temperature.detach()
+            seed, it = self._next_rng()
+            return ops.sample_concrete(logits, temperature, n_samples, self._log_space, u=u,
+                                       seed=seed, it=it)
+        a = self._gumbel_logits(n_samples, u)
+        return torch.log_softmax(a, -1) if self._log_space else torch.softmax(a, -1)
+
+    def _finish(self, lp):
+        if self._check_numerics and not bool(torch.isfinite(lp).all()):
+            raise FloatingPointError(self._name + ".log_prob has numeric errors")
+        return ops.group_sum(lp, self._group_ndims)
 
     def _density_terms(self, temp, extra):
         """lgamma(n) + (n-1) log t + sum(temp + extra) - n * LSE(temp)."""
@@ -79,13 +107,17 @@ class ExpConcrete(Distribution):
             ops.reduce_axes(temp + extra if extra is not None else temp,
                             ops.OP_SUM, -1) - \
             n * ops.reduce_axes(temp, ops.OP_LSE, -1)
-        if self._check_numerics and not bool(torch.isfinite(lp).all()):
-            raise FloatingPointError(self._name + ".log_prob has numeric errors")
-        return ops.group_sum(lp, self._group_ndims)
+        return self._finish(lp)
 
     def _log_prob(self, given):
         logits = self.path_param(self._logits)
         t = self.path_param(self._temperature)
+        if self._fused(given):
+            return self._finish(ops.concrete_log_prob(given, logits, t, self._log_space))
+        if not self._log_space:
+            log_given = torch.log(given)
+            temp = (logits - t * log_given).contiguous()
+            return self._density_terms(temp, -log_given)
         temp = (logits - t * given).contiguous()
         return self._density_terms(temp, None)
 
@@ -96,16 +128,7 @@ ExpGumbelSoftmax = ExpConcrete
 class Concrete(ExpConcrete):
     """multivariate.py:820-958: the Gumbel-softmax relaxation on the simplex."""
     _name = "Concrete"
-
-    def _sample(self, n_samples):
-        return torch.softmax(self._gumbel_logits(n_samples), -1)
-
-    def _log_prob(self, given):
-        logits = self.path_param(self._logits)
-        t = self.path_param(self._temperature)
-        log_given = torch.log(given)
-        temp = (logits - t * log_given).contiguous()
-        return self._density_terms(temp, -log_given)
+    _log_space = False
 
 
 GumbelSoftmax = Concrete

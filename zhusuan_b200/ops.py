@@ -619,4 +619,108 @@ def sample_count(kind, param, n_experiments, shape, u=None, seed=0, it=0):
     return out
 
 
+# ------------------------------------------------------- ExpConcrete / Concrete
+CONCRETE_MAX_CATEGORIES = 1024
+
+
+def _concrete_work(logits_rows, C, rows, device):
+    n = lib.load().zsb_concrete_bwd_work(int(logits_rows), int(C), int(rows))
+    if n < 0:
+        raise ZsbError("zsb_concrete_bwd_work: bad sizes")
+    return torch.empty(n, dtype=_F32, device=device)
+
+
+class _ConcreteSample(torch.autograd.Function):
+    """ExpConcrete / Concrete ._sample (multivariate.py:768-782, 905-919) in one pass: y =
+    log_softmax((l + g) / t) or softmax(...), u injected or drawn as base_noise(0, ...) would
+    draw it.  Backward: the reparameterisation gradient from the saved sample alone."""
+
+    @staticmethod
+    def forward(ctx, logits, temperature, n_samples, log_space, u, seed, it):
+        l = _f32c(logits)
+        t = _f32c(temperature)
+        C = int(l.shape[-1])
+        lrows = max(1, l.numel() // C)
+        full = (int(n_samples),) + tuple(l.shape)
+        out = torch.empty(full, dtype=_F32, device=l.device)
+        rows = out.numel() // C
+        uu = None if u is None else _f32c(u.expand(full)).reshape(-1)
+        lib.call("zsb_sample_concrete_f32", ptr(l), lrows, ptr(t), C, int(log_space), ptr(uu),
+                 int(seed), int(it), ptr(out), rows, stream())
+        ctx.save_for_backward(out, t)
+        ctx.meta = (lrows, C, int(log_space), rows, tuple(l.shape))
+        return out
+
+    @staticmethod
+    def backward(ctx, gy):
+        y, t = ctx.saved_tensors
+        lrows, C, log_space, rows, lshape = ctx.meta
+        need = ctx.needs_input_grad
+        if rows == 0:
+            return (torch.zeros(lshape, dtype=_F32, device=y.device) if need[0] else None,
+                    torch.zeros_like(t) if need[1] else None, None, None, None, None, None)
+        dl = torch.empty(lshape, dtype=_F32, device=y.device) if need[0] else None
+        dt = torch.empty((), dtype=_F32, device=y.device) if need[1] else None
+        if need[0] or need[1]:
+            lib.call("zsb_sample_concrete_bwd_f32", ptr(y), ptr(_f32c(gy)), lrows, ptr(t), C,
+                     log_space, ptr(dl), ptr(dt), ptr(_concrete_work(lrows, C, rows, y.device)),
+                     rows, stream())
+        return dl, dt.reshape(t.shape) if dt is not None else None, None, None, None, None, None
+
+
+def sample_concrete(logits, temperature, n_samples, log_space, u=None, seed=0, it=0):
+    """[n_samples] + logits.shape relaxed one-hot draws (log-probabilities when ``log_space``);
+    ``u``: injected uniforms of that shape."""
+    return _ConcreteSample.apply(logits, temperature, int(n_samples), bool(log_space), u,
+                                 seed, it)
+
+
+class _ConcreteLogProb(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, given, logits, temperature, log_space):
+        full = torch.broadcast_shapes(given.shape, logits.shape)
+        C = int(full[-1])
+        bshape = tuple(full[:-1])
+        g, grows = _rows_prep(given, bshape, C)
+        l, lrows = _rows_prep(logits, bshape, C)
+        t = _f32c(temperature)
+        rows = 1
+        for d in bshape:
+            rows *= int(d)
+        out = torch.empty(bshape, dtype=_F32, device=logits.device)
+        if rows > 0:
+            lib.call("zsb_logprob_concrete_f32", ptr(g), grows, ptr(l), lrows, ptr(t), C,
+                     int(log_space), ptr(out), rows, stream())
+        ctx.save_for_backward(g, l, t)
+        ctx.meta = (grows, lrows, C, int(log_space), rows, bshape, given.shape, logits.shape)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        g, l, t = ctx.saved_tensors
+        grows, lrows, C, log_space, rows, bshape, gs, ls = ctx.meta
+        need = ctx.needs_input_grad
+        dev = l.device
+        alloc = torch.empty if rows > 0 else torch.zeros
+        dg = alloc(bshape + (C,), dtype=_F32, device=dev) if need[0] else None
+        dl = alloc(lrows * C, dtype=_F32, device=dev) if need[1] else None
+        dt = alloc((), dtype=_F32, device=dev) if need[2] else None
+        if rows > 0 and any(need[:3]):
+            lib.call("zsb_logprob_concrete_bwd_f32", ptr(g), grows, ptr(l), lrows, ptr(t), C,
+                     log_space, ptr(_f32c(gout)), ptr(dg), ptr(dl), ptr(dt),
+                     ptr(_concrete_work(lrows, C, rows, dev)), rows, stream())
+        if dl is not None:
+            # a suffix-broadcast parameter comes back in its own shape; an expanded one in full
+            dl = dl.reshape(ls) if dl.numel() == math.prod(ls) else \
+                _sum_to(dl.reshape(bshape + (C,)), ls)
+        return (_sum_to(dg, gs) if dg is not None else None, dl,
+                dt.reshape(t.shape) if dt is not None else None, None)
+
+
+def concrete_log_prob(given, logits, temperature, log_space):
+    """ExpConcrete._log_prob (log_space) / Concrete._log_prob (multivariate.py:800-812,
+    938-955), before the group sum."""
+    return _ConcreteLogProb.apply(given, logits, temperature, bool(log_space))
+
+
 LOG_2PI = math.log(2.0 * math.pi)
