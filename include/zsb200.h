@@ -765,31 +765,29 @@ int zsb_conv_gather_split_f32(const float* x, int64_t N, int64_t Hb, int64_t Wb,
 /* Col2im-sum: the big-grid tensor [N, Hb, Wb, C] whose entry is the sum, over the taps that land
  * on it (kh, then kw, ascending: deterministic, no atomics), of cols [N Hs Ws, k k C] fp32.
  *   epi 0: out = the sum (a convolution's input gradient)
- *   epi 1: out = sigmoid(sum + bias[c])
+ *   epi 1: out = act(sum + bias[c] + residual) with bias [C] and residual [N, Hb, Wb, C] (either
+ *          may be NULL): the generators' sigmoid output layers, and the transposed convolution of
+ *          examples/utils/utils.py:74-113 with the resnet blocks' residual added before the ReLU
+ *          (vae_conv.py:20-36)
  *   epi 2: batch norm training: pre = the sum and part [ceil(N Hb Wb / 128)][2][C] its per-tile
  *          moments, for zsb_bn_finish_fused_f32 (out unused)
  *   epi 3: batch norm evaluation: out = act(xhat gamma + beta), xhat = (sum - moving_mean)
  *          rsqrt(moving_var + eps); stats [2][C] = (moving_mean, rstd); pre (may be NULL) = sum
- *   epi 4: out = act(sum + bias[c] + residual) with bias [C] and residual [N, Hb, Wb, C] (either
- *          may be NULL): the transposed convolution of examples/utils/utils.py:74-113 with the
- *          resnet blocks' residual added before the ReLU (vae_conv.py:20-36)
- * act = ReLU if relu (epi 3, 4).  max |out| into amax_scale[2] (may be NULL; epi 0, 1, 3, 4). */
+ * act: 0 none, 1 ReLU, 2 sigmoid; epi 1 takes any, epi 3 none or ReLU, epi 0 and 2 none.  max |out|
+ * into amax_scale[2] (may be NULL; epi 0, 1, 3). */
 int zsb_conv_col2im_f32(int epi, const float* cols, int64_t N, int64_t Hb, int64_t Wb, int64_t C,
                         int64_t Hs, int64_t Ws, int k, int stride, int pt, int pl,
                         const float* bias, const float* residual, const float* gamma,
                         const float* beta, const float* moving_mean, const float* moving_var,
-                        float eps, int relu, float* stats, float* pre, float* part, float* out,
+                        float eps, int act, float* stats, float* pre, float* part, float* out,
                         float* amax_scale, void* stream);
-/* Backward through a sigmoid output y [R, C]: gp = g y (1 - y), max |gp| into scale[2], and db [C]
- * (may be NULL) = the column sums of gp, merged in a fixed order from part [ceil(R / 128)][C]. */
-int zsb_conv_sigmoid_grad_f32(const float* g, const float* y, int64_t R, int C, float* gp,
-                              float* part, float* db, float* scale, void* stream);
-/* Backward through relu?(conv + b + residual) with output y [R, C] (the tf.gradients of the ReLU,
- * bias_add and residual add of vae_conv.py:20-53): gp = g (y > 0), or g when relu = 0 (y may then
- * be NULL), which is the residual's gradient; max |gp| into scale[2], and db [C] (may be NULL) = the
- * column sums of gp, merged in a fixed order from part [ceil(R / 128)][C].  C < 2^20. */
-int zsb_conv_relu_grad_f32(const float* g, const float* y, int64_t R, int C, int relu, float* gp,
-                           float* part, float* db, float* scale, void* stream);
+/* Backward through act(conv + b + residual) with output y [R, C] (the tf.gradients of the
+ * activation, bias_add and residual add): gp = g y (1 - y) (act 2, sigmoid), g (y > 0) (act 1,
+ * ReLU) or g (act 0; y may then be NULL), which is also the residual's gradient; max |gp| into
+ * scale[2], and db [C] (may be NULL) = the column sums of gp, merged in a fixed order from
+ * part [ceil(R / 128)][C].  C < 2^20, R C < 2^31. */
+int zsb_conv_act_grad_f32(const float* g, const float* y, int64_t R, int C, int act, float* gp,
+                          float* part, float* db, float* scale, void* stream);
 
 /* ---- K5: SG-MCMC updates (zhusuan/sgmcmc.py) ------------------------------------------------ */
 int zsb_sgmcmc_parts(void);   /* capacity (floats) of every `part` scratch */

@@ -308,6 +308,12 @@ def test_errors_raise_before_any_launch(zs):
         zs.fused.bn_conv2d_transpose(**conv(x=big, W=T(np.zeros((5, 5, 6, 64))), stride=2))
     with pytest.raises(ValueError, match="2\\^31"):
         zs.fused.sigmoid_conv2d_transpose(big, T(np.zeros((5, 5, 3, 64))), stride=2)
+    # 2^20 output or input channels, shaped without allocating them
+    wide = torch.zeros(1, device="cuda").expand(1, 1, 2 ** 20, 4)
+    with pytest.raises(ValueError, match="2\\^20"):
+        zs.fused.sigmoid_conv2d_transpose(x, wide)
+    with pytest.raises(ValueError, match="2\\^20"):       # x [1, 1, 4, 2^20], W [1, 1, 4, 2^20]
+        zs.fused.sigmoid_conv2d_transpose(wide.permute(0, 1, 3, 2), wide.permute(0, 1, 3, 2))
     assert lib.launches == n0
     n = lib.launches
     with pytest.raises(ValueError):       # a VALID input smaller than the kernel

@@ -93,9 +93,8 @@ class _Lib(object):
                 "zsb_sample_concrete_bwd_f32": 2, "zsb_logprob_concrete_bwd_f32": 2,
                 "zsb_gp_cond_bwd_f32": 2, "zsb_conv3x3_wgrad_f32": 2,
                 # the tensor-core conv layers' entries, in their common case: a gather-split
-                # with its max pass, a sigmoid or ReLU gradient with the bias sums
-                "zsb_conv_gather_split_f32": 3, "zsb_conv_sigmoid_grad_f32": 2,
-                "zsb_conv_relu_grad_f32": 2,
+                # with its max pass, an activation gradient with the bias sums
+                "zsb_conv_gather_split_f32": 3, "zsb_conv_act_grad_f32": 2,
                 # the batch-norm entries in training
                 "zsb_linear_tc_bn_f32": 3, "zsb_bn_finish_fused_f32": 2, "zsb_bn_grad_f32": 5,
                 "zsb_bn_grad_f32out": 3}

@@ -2697,11 +2697,15 @@ def _take_tag(x):
     return tag
 
 
+# the activation codes of zsb_conv_col2im_f32 and zsb_conv_act_grad_f32
+_ACT_NONE, _ACT_RELU, _ACT_SIGMOID = 0, 1, 2
+
+
 def _col2im(epi, cols, g, C, out=None, bias=None, gamma=None, beta=None, mm=None, mv=None,
-            eps=0.0, relu=False, stats=None, pre=None, part=None, amax=None, residual=None):
+            eps=0.0, act=_ACT_NONE, stats=None, pre=None, part=None, amax=None, residual=None):
     from ._lib import lib, ptr, stream
     lib.call("zsb_conv_col2im_f32", epi, ptr(cols), *g.args(C), ptr(bias), ptr(residual),
-             ptr(gamma), ptr(beta), ptr(mm), ptr(mv), float(eps), int(bool(relu)), ptr(stats),
+             ptr(gamma), ptr(beta), ptr(mm), ptr(mv), float(eps), act, ptr(stats),
              ptr(pre), ptr(part), ptr(out), ptr(amax), stream())
 
 
@@ -2711,45 +2715,27 @@ def _ones_like_gamma(gamma, Cout, dev):
 
 
 class _BNConv2d(torch.autograd.Function):
-    """relu?(BN(conv(x, W)) * gamma + beta): the gather-split of x, then _bn_forward with TF's
+    """relu?(BN(conv(x, W)) * gamma + beta): _conv_planes, then _bn_forward with TF's
     fused-batch-norm update over R = N Ho Wo rows, J = Cout features and K = k k Cin.  Backward:
-    _bn_backward gives d beta, d gamma and the planes of G = d/d(pre-activation); dx is the
-    col2im-sum of G W (the MN-major input-gradient product) and dW the weight-gradient product of
-    G and the saved gather planes."""
+    _bn_backward gives d beta, d gamma and the planes of G = d/d(pre-activation), then
+    _conv_grads."""
 
     @staticmethod
     def forward(ctx, x, W, gamma, beta, stats_bufs, g, training, relu, rate, eps, keep_pre):
-        dev = W.device
-        tag = _take_tag(x)
-        x4 = x.detach().reshape(g.N, g.Hb, g.Wb, g.Cin).contiguous()
-        hpl = _gather_planes(x4, g, g.Cin, tag)
-        K, J = hpl.K, g.Cout
-        ctx.hpl, ctx.wpl, ctx.Wt_shape = hpl, _tc_split(W.detach().reshape(K, J).t()), (J, K)
-        y, amax = _bn_forward(ctx, hpl, ctx.wpl, J, _ones_like_gamma(gamma, J, dev), beta,
-                              stats_bufs, training, relu, rate, eps, True, keep_pre)
+        ctx.hpl, ctx.wpl = _conv_planes(x, W, g)
+        y, amax = _bn_forward(ctx, ctx.hpl, ctx.wpl, g.Cout,
+                              _ones_like_gamma(gamma, g.Cout, W.device), beta, stats_bufs,
+                              training, relu, rate, eps, True, keep_pre)
         ctx.meta = (g, tuple(x.shape))
-        return _tag(y.reshape(tuple(x.shape[:-3]) + (g.Hs, g.Ws, J)), amax)
+        return _tag(y.reshape(tuple(x.shape[:-3]) + (g.Hs, g.Ws, g.Cout)), amax)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gy):
         g, x_shape = ctx.meta
         need = ctx.needs_input_grad
-        dev = gy.device
-        R = g.N * g.Hs * g.Ws
         dgamma, dbeta, gpl = _bn_backward(ctx, gy, need[2], need[3])
-        dx = dW = None
-        if need[0]:
-            wp, ws = ctx.wpl
-            dcols, _ = _tc_grad_input(gpl, _ShapeOnly(ctx.Wt_shape, dev), R, wp, ws)
-            dx = torch.empty((g.N, g.Hb, g.Wb, g.Cin), dtype=torch.float32, device=dev)
-            amax = torch.zeros(4, dtype=torch.float32, device=dev)
-            _col2im(0, dcols, g, g.Cin, out=dx, amax=amax)
-            del dcols
-            dx = _tag(dx.reshape(x_shape), amax)
-        if need[1]:
-            dW = _tc_grad_weight(gpl, ctx.hpl, R).t().reshape(g.k, g.k, g.Cin, g.Cout)
-        ctx.hpl = ctx.wpl = None
+        dx, dW = _conv_grads(ctx, gpl, g, need[0], need[1], x_shape)
         return dx, dW, dgamma, dbeta, None, None, None, None, None, None, None
 
 
@@ -2760,6 +2746,37 @@ class _ShapeOnly(object):
 
     def __init__(self, shape, device):
         self.shape, self.device = shape, device
+
+
+def _conv_planes(x, W, g):
+    """The planes of a convolution's product over R = N Ho Wo rows, J = Cout features and K = k k
+    Cin: the gather-split of x (at its max |.| tag when it has one) and the planes of
+    W^T [Cout, k k Cin]."""
+    tag = _take_tag(x)
+    x4 = x.detach().reshape(g.N, g.Hb, g.Wb, g.Cin).contiguous()
+    hpl = _gather_planes(x4, g, g.Cin, tag)
+    return hpl, _tc_split(W.detach().reshape(hpl.K, g.Cout).t())
+
+
+def _conv_grads(ctx, gpl, g, need_x, need_W, x_shape):
+    """dx and dW of a convolution from the planes gpl of G = d/d(its pre-activation)
+    [N Ho Wo, Cout]: dx is the col2im-sum of G W (the MN-major input-gradient product with the
+    forward planes of W^T) and dW the weight-gradient product of G and the saved gather planes."""
+    R, K = g.N * g.Hs * g.Ws, g.k * g.k * g.Cin
+    dev = gpl.planes.device
+    dx = dW = None
+    if need_x:
+        wp, ws = ctx.wpl
+        dcols, _ = _tc_grad_input(gpl, _ShapeOnly((g.Cout, K), dev), R, wp, ws)
+        dx = torch.empty((g.N, g.Hb, g.Wb, g.Cin), dtype=torch.float32, device=dev)
+        amax = torch.zeros(4, dtype=torch.float32, device=dev)
+        _col2im(0, dcols, g, g.Cin, out=dx, amax=amax)
+        del dcols
+        dx = _tag(dx.reshape(x_shape), amax)
+    if need_W:
+        dW = _tc_grad_weight(gpl, ctx.hpl, R).t().reshape(g.k, g.k, g.Cin, g.Cout)
+    ctx.hpl = ctx.wpl = None
+    return dx, dW
 
 
 def _conv_t_product(x, W, g):
@@ -2818,7 +2835,7 @@ class _BNConv2dT(torch.autograd.Function):
                      int(relu), ptr(amax), stream())
         else:
             _col2im(3, cols, g, J, out=y, gamma=gm, beta=b, mm=moving_mean, mv=moving_variance,
-                    eps=eps, relu=relu, stats=stats, pre=a, amax=amax)
+                    eps=eps, act=_ACT_RELU if relu else _ACT_NONE, stats=stats, pre=a, amax=amax)
             del cols
         _bn_save(ctx, training, relu, gm, y, a, stats)
         ctx.hpl, ctx.wpl = hpl, wpl
@@ -2833,49 +2850,6 @@ class _BNConv2dT(torch.autograd.Function):
         dgamma, dbeta, (da, scale) = _bn_backward(ctx, gy, need[2], need[3], planes=False)
         dx, dW = _conv_t_grads(ctx, da, scale, g, need[0], need[1], x_shape)
         return dx, dW, dgamma, dbeta, None, None, None, None, None, None, None
-
-
-class _SigmoidConv2dT(torch.autograd.Function):
-    """sigmoid(conv_transpose(x, W) + b): the epi-0 product, then the col2im-sum with the bias +
-    sigmoid epilogue.  Backward: gp = g y (1 - y) and db from zsb_conv_sigmoid_grad_f32, then
-    _conv_t_grads."""
-
-    @staticmethod
-    def forward(ctx, x, W, b, g):
-        J, Rb = g.Cout, g.N * g.Hb * g.Wb
-        dev = W.device
-        cols, hpl, wpl = _conv_t_product(x, W, g)
-        bias = b.detach().contiguous() if b is not None else \
-            torch.zeros(J, dtype=torch.float32, device=dev)
-        y = torch.empty((Rb, J), dtype=torch.float32, device=dev)
-        amax = torch.zeros(4, dtype=torch.float32, device=dev)
-        _col2im(1, cols, g, J, out=y, bias=bias, amax=amax)
-        del cols
-        ctx.save_for_backward(y)
-        ctx.hpl, ctx.wpl = hpl, wpl
-        ctx.meta = (g, tuple(x.shape))
-        return _tag(y.reshape(tuple(x.shape[:-3]) + (g.Hb, g.Wb, J)), amax)
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, gy):
-        from ._lib import lib, ptr, stream
-        y, = ctx.saved_tensors
-        g, x_shape = ctx.meta
-        need = ctx.needs_input_grad
-        dev = gy.device
-        J, Rb = g.Cout, g.N * g.Hb * g.Wb
-        gg = gy.reshape(Rb, J).to(torch.float32).contiguous()
-        gp = torch.empty((Rb, J), dtype=torch.float32, device=dev)
-        part = torch.empty(-(-Rb // 128) * J, dtype=torch.float32, device=dev)
-        db = torch.empty(J, dtype=torch.float32, device=dev) if need[2] else None
-        scale = torch.zeros(4, dtype=torch.float32, device=dev)
-        lib.call("zsb_conv_sigmoid_grad_f32", ptr(gg), ptr(y), Rb, J, ptr(gp), ptr(part), ptr(db),
-                 ptr(scale), stream())
-        dx, dW = _conv_t_grads(ctx, gp, scale, g, need[0], need[1], x_shape)
-        return dx, dW, db, None
-
-
 
 
 def _bn_conv_apply(fn, name, x, W, gamma, beta, moving_mean, moving_variance, training, stride,
@@ -2960,25 +2934,22 @@ def sigmoid_conv2d_transpose(x, W, b=None, stride=1, padding="SAME"):
     examples/generative_adversarial_nets.  Geometry and W as in ``bn_conv2d_transpose``.
     Differentiable w.r.t. x, W and b; the bias gradient is a column sum merged in a fixed order.
     Determinism, inference mode, the amax tag and the supported range are those of
-    ``bn_conv2d``."""
+    ``bn_conv2d``, and both channel counts must be below 2^20."""
     x = _unwrap(x)
-    g, _ = _conv_tc_geom("sigmoid_conv2d_transpose", x, W, stride, padding, True)
-    if b is not None and (not isinstance(b, torch.Tensor) or tuple(b.shape) != (g.Cout,) or
-                          b.dtype != torch.float32 or b.device != W.device):
-        raise ValueError("sigmoid_conv2d_transpose: b must be a float32 [%d] tensor on %s"
-                         % (g.Cout, W.device))
-    return _SigmoidConv2dT.apply(x, W, b, g)
+    g, lead = _conv_tc_geom("sigmoid_conv2d_transpose", x, W, stride, padding, True)
+    return _conv_tc_apply(_Conv2dTransposeTC, "sigmoid_conv2d_transpose", x, W, b, None, g, lead,
+                          _ACT_SIGMOID, (g.Hb, g.Wb))
 
 
-# Biased layers relu?(conv(x) + b + residual) on the same products (csrc/conv_bias.cu): the
-# convolutions of vae_conv.py at any k <= 7, channel count and padding
+# Biased layers act(conv(x) + b + residual) on the same products: the convolutions of vae_conv.py
+# at any k <= 7, channel count and padding, and the GAN generators' sigmoid output layers
 CONV_TC_MAX_C = 2 ** 20
 
 
-def _relu_grad(gy, y, R, J, relu, need_db):
-    """gp = d/d(pre-activation) [R, J] of relu?(a) with output y (gy itself without ReLU, copied),
-    db [J] (None unless ``need_db``) and the scale slot holding max |gp|
-    (zsb_conv_relu_grad_f32)."""
+def _act_grad(gy, y, R, J, act, need_db):
+    """gp = d/d(pre-activation) [R, J] of act(a) with output y (gy itself without an activation,
+    copied), db [J] (None unless ``need_db``) and the scale slot holding max |gp|
+    (zsb_conv_act_grad_f32)."""
     from ._lib import lib, ptr, stream
     dev = gy.device
     g = gy.reshape(R, J).to(torch.float32).contiguous()
@@ -2986,72 +2957,56 @@ def _relu_grad(gy, y, R, J, relu, need_db):
     part = torch.empty(-(-R // 128) * J, dtype=torch.float32, device=dev)
     db = torch.empty(J, dtype=torch.float32, device=dev) if need_db else None
     scale = torch.zeros(4, dtype=torch.float32, device=dev)
-    lib.call("zsb_conv_relu_grad_f32", ptr(g), ptr(y if relu else None), R, J, int(relu), ptr(gp),
+    lib.call("zsb_conv_act_grad_f32", ptr(g), ptr(y if act else None), R, J, act, ptr(gp),
              ptr(part), ptr(db), ptr(scale), stream())
     return gp, db, scale
 
 
 class _Conv2dTC(torch.autograd.Function):
-    """relu?(conv(x, W) + b + residual): the gather-split of x, then the product over R = N Ho Wo
-    rows, J = Cout features and K = k k Cin with the bias + ReLU epilogue (epi 0), or with the
-    residual added before the ReLU (epi 16).  Backward: gp = d/d(pre-activation) and db from
-    zsb_conv_relu_grad_f32 (gp is the residual's gradient too), the plain split of gp at the max
-    |gp| that pass left, then dx as the col2im-sum of G W and dW from the saved gather planes, as
-    in _BNConv2d."""
+    """act(conv(x, W) + b + residual), act none or ReLU: _conv_planes, then the product over
+    R = N Ho Wo rows, J = Cout features and K = k k Cin with the bias + ReLU epilogue (epi 0), or
+    with the residual added before the ReLU (epi 16).  Backward: gp = d/d(pre-activation) and db
+    from _act_grad (gp is the residual's gradient too), the plain split of gp at the max |gp| that
+    pass left, then _conv_grads."""
 
     @staticmethod
-    def forward(ctx, x, W, b, res, g, relu):
-        dev = W.device
-        tag = _take_tag(x)
-        x4 = x.detach().reshape(g.N, g.Hb, g.Wb, g.Cin).contiguous()
-        hpl = _gather_planes(x4, g, g.Cin, tag)
+    def forward(ctx, x, W, b, res, g, act):
+        hpl, (wp, ws) = _conv_planes(x, W, g)
         R, K, J = hpl.rows, hpl.K, g.Cout
-        wp, ws = _tc_split(W.detach().reshape(K, J).t())
         bias = None if b is None else b.detach().contiguous()
         r2 = None if res is None else res.detach().reshape(R, J).contiguous()
-        amax = torch.zeros(4, dtype=torch.float32, device=dev)
+        amax = torch.zeros(4, dtype=torch.float32, device=W.device)
         y = _tc_linear(0 if r2 is None else 16, wp, ws, hpl.planes, hpl.scale, bias, r2, None, R,
-                       J, K, relu, amax=amax)
-        ctx.save_for_backward(y if relu else None)
+                       J, K, act == _ACT_RELU, amax=amax)
+        ctx.save_for_backward(y if act else None)
         ctx.hpl, ctx.wpl = hpl, (wp, ws)
-        ctx.meta = (g, tuple(x.shape), relu)
+        ctx.meta = (g, tuple(x.shape), act)
         return _tag(y.reshape(tuple(x.shape[:-3]) + (g.Hs, g.Ws, J)), amax)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gy):
         y, = ctx.saved_tensors
-        g, x_shape, relu = ctx.meta
+        g, x_shape, act = ctx.meta
         need = ctx.needs_input_grad
-        dev = gy.device
-        R, J, K = g.N * g.Hs * g.Ws, g.Cout, g.k * g.k * g.Cin
-        gp, db, scale = _relu_grad(gy, y, R, J, relu, need[2])
+        gp, db, scale = _act_grad(gy, y, g.N * g.Hs * g.Ws, g.Cout, act, need[2])
         dx = dW = None
         if need[0] or need[1]:
-            gpl = _tc_split_dual(gp, amax=scale)
-            if need[0]:
-                wp, ws = ctx.wpl
-                dcols, _ = _tc_grad_input(gpl, _ShapeOnly((J, K), dev), R, wp, ws)
-                dx = torch.empty((g.N, g.Hb, g.Wb, g.Cin), dtype=torch.float32, device=dev)
-                amax = torch.zeros(4, dtype=torch.float32, device=dev)
-                _col2im(0, dcols, g, g.Cin, out=dx, amax=amax)
-                del dcols
-                dx = _tag(dx.reshape(x_shape), amax)
-            if need[1]:
-                dW = _tc_grad_weight(gpl, ctx.hpl, R).t().reshape(g.k, g.k, g.Cin, g.Cout)
+            dx, dW = _conv_grads(ctx, _tc_split_dual(gp, amax=scale), g, need[0], need[1],
+                                 x_shape)
         ctx.hpl = ctx.wpl = None
         dres = gp.reshape(gy.shape) if need[3] else None
         return dx, dW, db, dres, None, None
 
 
 class _Conv2dTransposeTC(torch.autograd.Function):
-    """relu?(conv_transpose(x, W) + b + residual): the epi-0 product x W'^T gives the columns
+    """act(conv_transpose(x, W) + b + residual): the epi-0 product x W'^T gives the columns
     [N Hi Wi, k k Cout]; their col2im-sum onto the output grid adds the bias and the residual and
-    applies the ReLU (epi 4).  Backward: gp and db from zsb_conv_relu_grad_f32 (gp is the
-    residual's gradient too), then _conv_t_grads at the max |gp| that pass left."""
+    applies the activation (epi 1).  Backward: gp and db from _act_grad (gp is the residual's
+    gradient too), then _conv_t_grads at the max |gp| that pass left."""
 
     @staticmethod
-    def forward(ctx, x, W, b, res, g, relu):
+    def forward(ctx, x, W, b, res, g, act):
         J, Rb = g.Cout, g.N * g.Hb * g.Wb
         dev = W.device
         cols, hpl, wpl = _conv_t_product(x, W, g)
@@ -3059,20 +3014,20 @@ class _Conv2dTransposeTC(torch.autograd.Function):
         r2 = None if res is None else res.detach().reshape(Rb, J).contiguous()
         y = torch.empty((Rb, J), dtype=torch.float32, device=dev)
         amax = torch.zeros(4, dtype=torch.float32, device=dev)
-        _col2im(4, cols, g, J, out=y, bias=bias, residual=r2, relu=relu, amax=amax)
+        _col2im(1, cols, g, J, out=y, bias=bias, residual=r2, act=act, amax=amax)
         del cols
-        ctx.save_for_backward(y if relu else None)
+        ctx.save_for_backward(y if act else None)
         ctx.hpl, ctx.wpl = hpl, wpl
-        ctx.meta = (g, tuple(x.shape), relu)
+        ctx.meta = (g, tuple(x.shape), act)
         return _tag(y.reshape(tuple(x.shape[:-3]) + (g.Hb, g.Wb, J)), amax)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gy):
         y, = ctx.saved_tensors
-        g, x_shape, relu = ctx.meta
+        g, x_shape, act = ctx.meta
         need = ctx.needs_input_grad
-        gp, db, scale = _relu_grad(gy, y, g.N * g.Hb * g.Wb, g.Cout, relu, need[2])
+        gp, db, scale = _act_grad(gy, y, g.N * g.Hb * g.Wb, g.Cout, act, need[2])
         dx = dW = None
         if need[0] or need[1]:
             dx, dW = _conv_t_grads(ctx, gp, scale, g, need[0], need[1], x_shape)
@@ -3081,7 +3036,7 @@ class _Conv2dTransposeTC(torch.autograd.Function):
         return dx, dW, db, dres, None, None
 
 
-def _conv_tc_apply(fn, name, x, W, b, residual, g, lead, relu, out_hw):
+def _conv_tc_apply(fn, name, x, W, b, residual, g, lead, act, out_hw):
     """Check b and residual against the layer's geometry and the channel and weight-operand
     limits, all before any launch; then zero images give an empty result without a launch."""
     out_shape = tuple(lead) + tuple(out_hw) + (g.Cout,)
@@ -3104,7 +3059,7 @@ def _conv_tc_apply(fn, name, x, W, b, residual, g, lead, relu, out_hw):
                          % name)
     if g.N == 0:
         return torch.empty(out_shape, dtype=torch.float32, device=x.device)
-    return fn.apply(x, W, b, residual, g, bool(relu))
+    return fn.apply(x, W, b, residual, g, act)
 
 
 def conv2d_tc(x, W, b=None, stride=1, relu=False, residual=None, padding="SAME"):
@@ -3130,7 +3085,8 @@ def conv2d_tc(x, W, b=None, stride=1, relu=False, residual=None, padding="SAME")
     ValueError before any launch."""
     x = _unwrap(x)
     g, lead = _conv_tc_geom("conv2d_tc", x, W, stride, padding, False, empty_batch=True)
-    return _conv_tc_apply(_Conv2dTC, "conv2d_tc", x, W, b, residual, g, lead, relu, (g.Hs, g.Ws))
+    return _conv_tc_apply(_Conv2dTC, "conv2d_tc", x, W, b, residual, g, lead,
+                          _ACT_RELU if relu else _ACT_NONE, (g.Hs, g.Ws))
 
 
 def conv2d_transpose_tc(x, W, out_shape, stride=1, b=None, relu=False, residual=None,
@@ -3159,4 +3115,4 @@ def conv2d_transpose_tc(x, W, out_shape, stride=1, b=None, relu=False, residual=
         raise ValueError("conv2d_transpose_tc: out_shape has %d channels, W has %d"
                          % (Co, g.Cout))
     return _conv_tc_apply(_Conv2dTransposeTC, "conv2d_transpose_tc", x, W, b, residual, g, lead,
-                          relu, (Ho, Wo))
+                          _ACT_RELU if relu else _ACT_NONE, (Ho, Wo))
